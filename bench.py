@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """
-bench.py -- snowfall (+ wet-ground) augmentation throughput on B200 (BASELINE.json metric: augmented LiDAR points/s).
+bench.py -- snowfall (+ wet-ground) augmentation throughput on H100 (BASELINE.json metric: augmented LiDAR points/s).
 
     python bench.py --gpus 1 --steps 20 --warmup 5                     # our arm (CUDA engine), BASELINE configs[1]
+    python bench.py --dump-outputs DIR                                 # + what the last timed step computed, as DIR/*.npy
     python bench.py --config 2                                         # configs[2]: snowfall + wet ground fused on device
     python bench.py --impl reference --steps 3 --warmup 1              # CPU arm: the oracle port on all host cores
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -16,10 +17,15 @@ compaction, stats (config 2: followed by ground_water_augmentation(water_height 
 device).  With N > 1 every rank augments its own 32 clouds (clouds are independent, no data-path collective) and one
 all-gather reassembles the augmented batch on every rank (configs[3]).
 
-`value`     device-resident inputs.  A bracket = EXACTLY K steps between one CUDA-event pair on the launching stream
-            (barrier + synchronize on both sides, max over ranks); the bracket is repeated until >= 1 s of device time has
-            been measured and the MEDIAN bracket is reported (`repeats`, `ms_per_step_min/max` beside it).  Two input
-            batches alternate so that no step finds its rows in L2.
+`value`     device-resident inputs.  The timed region is EXACTLY K = --steps steps after W = --warmup untimed ones, between
+            CUDA events on the launching stream (barrier + synchronize on both sides, max over ranks); with one stream an
+            event after every step gives each step's duration and the MEDIAN step is reported (`ms_per_step_min/max`
+            beside it), with two streams the mean.  Two input batches alternate so that no step finds its rows in L2.
+`--dump-outputs DIR`
+            after the timed steps, what the last of them returned to the caller: `counts`, `stats` (config 2: `counts`,
+            `passthrough`, `plane`) whole, and of the row array `points` the kept rows of a fixed seeded sample of
+            DUMP_CLOUDS clouds (`sample_clouds` lists them), float32 rows / float64 everything else.  The inputs are
+            seeded, so two builds run with the same arguments can be compared array for array.
 `e2e`       the public API with pinned HOST buffers: H2D of the batch + augment + D2H of the augmented batch, per step
 `roofline`  the beam stage (scan + solve kernels) against the measured HBM copy peak; algorithmic bytes per launch =
             40 B x points + 12 B x table particles (SURVEY.md 8d), durations from CUDA events on the launching stream
@@ -57,19 +63,47 @@ ALGO_BYTES_PER_PARTICLE = 12        # f32 x, y, r once per launch (SURVEY.md 8d)
 FIXED_POLY = (2e-3, -0.3, 12.0)     # only used with --host-threshold
 CPU_CLOUDS_PER_STEP = 32
 CPU_THREADS_PER_CLOUD = 4
-MIN_TIMED_MS = 1000.0
 STEPS_IN_FLIGHT = 1                 # device-resident leg: consecutive steps on alternating streams (1 = strictly serial)
+DUMP_CLOUDS = 8                     # --dump-outputs: clouds whose rows are written (8 x 64 x 2048 rows x 20 B < 64 MB)
+DUMP_SEED = 0
 
 
 def load_peaks():
     p = os.path.join(ROOT, 'MEASURED_PEAKS.json')
     if os.path.exists(p):
         return float(json.load(open(p))['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
-    return 6650.0, 'fallback (B200_PROFILING.md)'
+    return 3350.0, 'H100 SXM data sheet (HBM3), not measured'
+
+
+def dump_outputs(d, r, off):
+    """Write the arrays of one step's result dict `r` to d/<name>.npy (see the module docstring)."""
+    os.makedirs(d, exist_ok=True)
+    n_rows, n_clouds = int(off[-1]), len(off) - 1
+    counts = r['counts'].cpu().numpy().astype(np.int64)
+    pick = np.sort(np.random.default_rng(DUMP_SEED).choice(n_clouds, size=min(DUMP_CLOUDS, n_clouds), replace=False))
+    arrays = {'sample_clouds': pick.astype(np.float64)}
+    for name, t in r.items():
+        a = t.cpu().numpy()
+        if a.shape[0] == n_rows:                           # slot-compacted rows: cloud b's kept rows start at off[b]
+            a = np.concatenate([a[off[b]:off[b] + counts[b]] for b in pick])
+        arrays[name] = a.astype(np.float32 if a.dtype == np.float32 else np.float64)
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(d, f'{name}.npy'), a)
+
+
+def power_limit_w(gpu_index):
+    """The card's power limit (a number measured on it is only meaningful with this beside it), or None."""
+    try:
+        out = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader,nounits', '-i',
+                              str(gpu_index)], capture_output=True, text=True, timeout=30).stdout
+        return float(out.strip())
+    except Exception:
+        return None
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe).  The sampler runs from
+    """nvidia-smi clocks / throttle reasons DURING the timed region.  The sampler runs from
     before the warm-up (nvidia-smi needs ~0.2 s to start); samples are stamped on arrival and the ones that fall inside
     the timed window are reported."""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
@@ -153,8 +187,8 @@ def workload_config(config, n_gpus):
                         + ('' if n_gpus == 1 else f'; x{n_gpus} GPUs + all-gather of the augmented batch (configs[3])'),
             'config': config, 'batch_per_gpu': BATCH_PER_GPU, 'points_per_cloud': 64 * N_AZIMUTH,
             'parallelism': f'clouds sharded x{n_gpus}',
-            'l2': 'no explicit flush: two different input batches alternate (2 x 84 MB of rows + the table index > 126 MB '
-                  'L2); a bracket of K steps is timed with one CUDA-event pair on the launching stream'}
+            'l2': 'no explicit flush: two different input batches alternate (2 x 84 MB of rows + the table index > 50 MB '
+                  'L2); K steps are timed with CUDA events on the launching stream'}
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -298,7 +332,8 @@ def main():
     ap.add_argument('--no-cpu-baseline', action='store_true')
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--no-gather', action='store_true', help='N > 1: replicas only, skip the all-gather (debug)')
-    ap.add_argument('--min-timed-ms', type=float, default=MIN_TIMED_MS)
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the last one computed as DIR/<name>.npy')
     ap.add_argument('--streams', type=int, default=STEPS_IN_FLIGHT, choices=[1, 2],
                     help='steps in flight in the device-resident leg: consecutive steps alternate between this many streams')
     ap.add_argument('--e2e-inflight', type=int, default=3, help='batches in flight in the e2e leg (1..3)')
@@ -328,9 +363,9 @@ def main():
         dist.init_process_group('nccl', device_id=dev)
     assert world == args.gpus or world == 1, f'--gpus {args.gpus} but WORLD_SIZE={world}'
 
-    # e2e leg with several ranks on one box: the host's memory bandwidth is the limiter (tools/e2e_probe_ranks.py), so the
-    # copy-out kernel that moves only the kept rows pays (8 ranks: 5.98 vs 6.84 ms per step); on one GPU the plain D2H copy
-    # is faster (2.06 vs 2.12 ms) and stays the default.  Read by the library when its host pipeline is created.
+    # e2e leg with several ranks on one box: the ranks share the host's memory bandwidth (tools/e2e_probe_ranks.py), so the
+    # copy-out kernel that moves only the kept rows is used; on one GPU the plain D2H copy by the copy engine stays the
+    # default.  Read by the library when its host pipeline is created.
     if world > 1:
         os.environ.setdefault('LSS_PIPE_KERNEL_OUT', '1')
     numa_cpus = None
@@ -347,7 +382,7 @@ def main():
     B = args.batch
     fused_wet = args.config == 2
     # two different batches per rank, used alternately: 2 x 84 MB of rows (+ the index) per pair of steps is more
-    # than the 126 MB L2, so no step finds its inputs cached by the previous one (no explicit flush needed)
+    # than the 50 MB L2, so no step finds its inputs cached by the previous one (no explicit flush needed)
     clouds, orders = make_workload(rank, B)
     clouds2, orders2 = make_workload(rank, B, seed0=500000)
     n_per = [c.shape[0] for c in clouds]
@@ -379,6 +414,7 @@ def main():
     wet_outs = [{}, {}]
     ev_snow = [torch.cuda.Event() for _ in range(2)]
     ev_wet = [None, None]
+    serial = step_streams is None and not fused_wet and gather is None    # every step's work on the launching stream
 
     def step(k):
         """One pass of the augment() pipeline over this rank's batch (config 2: + wet ground on the snow output); with
@@ -432,20 +468,24 @@ def main():
             torch.cuda.synchronize(dev)
 
     def bracket(n_steps, k0=0):
-        """EXACTLY n_steps steps between one CUDA-event pair (the last gathers are inside the bracket)."""
-        e0 = torch.cuda.Event(enable_timing=True)
-        e1 = torch.cuda.Event(enable_timing=True)
+        """EXACTLY n_steps steps between CUDA events (the last gathers are inside the bracket).  Returns the total ms,
+        the ms of every step (when all of a step's work is on the launching stream: an event after each step; else None)
+        and the last step's result."""
+        ev = [torch.cuda.Event(enable_timing=True) for _ in range(n_steps + 1)]
         sync_all()
-        e0.record()
+        ev[0].record()
         if step_streams is not None:
             for st in step_streams:
-                st.wait_event(e0)
+                st.wait_event(ev[0])
         for k in range(n_steps):
-            step(k0 + k)
+            r = step(k0 + k)
+            if serial and k < n_steps - 1:
+                ev[k + 1].record()
         drain()
-        e1.record()
+        ev[n_steps].record()
         sync_all()
-        return float(e0.elapsed_time(e1))
+        per_step = [float(ev[k].elapsed_time(ev[k + 1])) for k in range(n_steps)] if serial else None
+        return float(ev[0].elapsed_time(ev[n_steps])), per_step, r
 
     # ---- device-resident throughput (`value`) ------------------------------------------------------------------------
     clocks = ClockSampler(local_rank)
@@ -454,25 +494,22 @@ def main():
         step(k)
     drain()
     eng.check()
-    est = bracket(args.steps)                               # untimed estimate: how many brackets make >= 1 s
-    repeats = int(min(400, max(3, np.ceil(args.min_timed_ms / max(est, 1e-3)))))
-    if world > 1:
-        t = torch.tensor([repeats], dtype=torch.int64, device=dev)
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)
-        repeats = int(t.item())
     launches0 = eng.launch_count()
     clocks.window_begin()
-    times = [bracket(args.steps) for _ in range(repeats)]
+    total_ms, step_ms, last = bracket(args.steps)
     clocks.window_end()
-    launches = (eng.launch_count() - launches0) // repeats
+    launches = eng.launch_count() - launches0
     clk = clocks.stop()
     eng.check()
-    t = torch.tensor(times, dtype=torch.float64, device=dev)
+    if rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, last, off)
+    t = torch.tensor([total_ms] + (step_ms or []), dtype=torch.float64, device=dev)
     if world > 1:
-        dist.all_reduce(t, op=dist.ReduceOp.MAX)            # every bracket: max over ranks
+        dist.all_reduce(t, op=dist.ReduceOp.MAX)            # the bracket and every step: max over ranks
     times = t.cpu().numpy()
-    total_ms = float(np.median(times))
-    ms_per_step = total_ms / args.steps
+    total_ms = float(times[0])
+    times = times[1:] if step_ms is not None else np.array([total_ms / args.steps])
+    ms_per_step = float(np.median(times))
     points_all = N * world
     value = points_all / (ms_per_step * 1e-3)
 
@@ -549,14 +586,13 @@ def main():
                    'engine.wet_ground_batch on the slot-compacted snow output, device -> pinned host copy of rows + counts, '
                    'synchronize (no pipelining across steps in this configuration)')
 
-        n_e2e = max(args.steps, 20)
+        n_e2e = n_sync = args.steps
         e2e_run(3)
         sync_all()
         t0 = time.perf_counter()
         e2e_run(n_e2e)
         sync_all()
         dt = (time.perf_counter() - t0) / n_e2e
-        n_sync = max(3, args.steps // 2)
         t0 = time.perf_counter()
         e2e_sync(n_sync)
         dt_sync = (time.perf_counter() - t0) / n_sync
@@ -598,16 +634,10 @@ def main():
                 'kernel_ms': k_avg_ms, 'kernel_share_of_step': k_avg_ms / ms_per_step,
                 'frac_over_whole_step': algo_bytes / (ms_per_step * 1e-3) / 1e9 / peak,
                 'kernel_ms_all': per_step,
-                'note': 'latency / issue bound, not HBM bound (DESIGN.md 4, profiles/): durations are CUDA events on the '
+                'note': 'latency / issue bound, not HBM bound (DESIGN.md 4): durations are CUDA events on the '
                         'launching stream in a separate profiled bracket (event pairs around every launch would perturb the '
-                        'timed brackets); the pre-pass runs concurrently on a side stream, so kernel_ms_all sums to more than '
-                        'the step; traffic = dram bytes of the beam-stage launches from the ncu capture in profiles/traffic.json'}
-    prof = os.path.join(ROOT, 'profiles', 'traffic.json')
-    if os.path.exists(prof):
-        try:
-            roofline['traffic'] = json.load(open(prof)).get('beam_stage_dram_bytes_per_launch')
-        except Exception:
-            pass
+                        'timed steps); the pre-pass runs concurrently on a side stream, so kernel_ms_all sums to more than '
+                        'the step; traffic (measured DRAM bytes) is not measured'}
 
     # ---- CPU baseline (oracle port, bounded sample: one warm-up + two timed steps of 32 clouds) ---------------------------
     cpu = None
@@ -631,8 +661,9 @@ def main():
             'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f64', 'data': 'synthetic', 'config': cfg,
             'clouds_per_s': value / (64 * N_AZIMUTH), 'e2e': e2e, 'gpu_launches': int(launches), 'clocks': clk,
             'roofline': roofline, 'cpu_baseline': cpu,
-            'repeats': repeats, 'timed_region_ms': float(np.sum(times)),
-            'ms_per_step_min': float(np.min(times)) / args.steps, 'ms_per_step_max': float(np.max(times)) / args.steps,
+            'timed_steps': args.steps, 'timed_region_ms': total_ms, 'ms_per_step_mean': total_ms / args.steps,
+            'ms_per_step_min': float(np.min(times)), 'ms_per_step_max': float(np.max(times)),
+            'gpu': torch.cuda.get_device_name(dev), 'gpu_power_limit_w': power_limit_w(local_rank),
             'theta_label_mismatch': theta_info, 'steps_in_flight': n_streams,
             'engine': {'prepass': 'device' if device_prepass else 'DEBUG: fixed host-supplied threshold polynomial',
                        'table_particles': tinfo['n_particles'], 'table_index_bytes': tinfo['bytes'],

@@ -1,5 +1,5 @@
 /*
- * lidar_snow_sim.h -- C ABI of the B200-native LiDAR snowfall / wet-ground augmentation engine.
+ * lidar_snow_sim.h -- C ABI of the H100-native (sm_90a) LiDAR snowfall / wet-ground augmentation engine.
  *
  * The reference (SysCV/LiDAR_snow_sim) has no FFI: its boundary is plain Python functions on NumPy arrays
  * (SURVEY.md 8b).  This header is what a binding for that boundary would bind; lidar_snow_sim_b200/_lib.py is the
@@ -309,7 +309,7 @@ LSS_API int64_t lss_voxelize_workspace_bytes(int64_t n_total, int n_clouds, int 
  *   h_peer_points[world], h_peer_counts[world]   host arrays of DEVICE pointers: every rank's gathered buffers as mapped into
  *                       this process (peer mappings of a symmetric allocation; entry `rank` is the local buffer)
  *   d_mc_points / d_mc_counts   multicast (NVLS) mappings of the same allocations, or both NULL: then one store per peer
- *   n_blocks            CTAs to launch (<= 0: a quarter of the SMs with multicast, 64 with per-peer stores: the measured optima)
+ *   n_blocks            CTAs to launch (<= 0: a quarter of the SMs with multicast, 64 with per-peer stores)
  * Stream-ordered on `stream`; a consumer on ANOTHER rank needs a barrier across ranks after this rank's kernel has finished. */
 LSS_API lss_status lss_gather_push(lss_engine *e, const float *d_points, const int32_t *d_counts,
                                    const int64_t *d_cloud_offsets, int n_clouds, int64_t n_rows, int world, int rank,

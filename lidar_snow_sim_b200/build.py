@@ -1,9 +1,9 @@
 """
-Build the engine's shared library IN-TREE with nvcc for sm_100a (cross-compiles without a GPU):
+Build the engine's shared library IN-TREE with nvcc for sm_90a (H100; cross-compiles without a GPU):
 
     python -m lidar_snow_sim_b200.build [--force]
 
-Output: lidar_snow_sim_b200/liblss_b200.so (git-ignored, travels to the GPU box with the snapshot).
+Output: lidar_snow_sim_b200/liblss_b200.so (git-ignored build product).
 """
 import os
 import shutil
@@ -16,7 +16,7 @@ LIB = os.path.join(HERE, 'liblss_b200.so')
 SOURCES = ['api.cu', 'tables.cu', 'snowfall.cu', 'solve.cu', 'prepass.cu', 'wet_ground.cu', 'sampler.cu', 'sampler_gpu.cu', 'host_pipeline.cu', 'fog.cu', 'voxelize.cu', 'lisa.cu', 'gather.cu']
 # -fmad=false: float32/float64 expressions are evaluated as written (mul, then add), like NumPy on the reference host;
 # where a fused multiply-add is wanted the source says fma() / __fma_rn() explicitly.
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17', '-fmad=false',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17', '-fmad=false',
               '-Xcompiler', '-fPIC', '-Xcompiler', '-fvisibility=hidden', '-Xcompiler', '-ffp-contract=off', '--shared', '-cudart', 'static']
 
 

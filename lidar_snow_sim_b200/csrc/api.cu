@@ -73,7 +73,7 @@ lss_status lss_create(int device, lss_engine **out)
     host_phase_table(R, wtab.data());
     int zero = 0;
     cudaDeviceGetAttribute(&e->n_sm, cudaDevAttrMultiProcessorCount, device);
-    if (e->n_sm <= 0) e->n_sm = 148;
+    if (e->n_sm <= 0) e->n_sm = 132;
     if (cudaMalloc(&e->d_R, sizeof(R)) != cudaSuccess || cudaMalloc(&e->d_status, sizeof(int)) != cudaSuccess ||
         cudaMalloc(&e->d_wtab, sizeof(double) * wtab.size()) != cudaSuccess ||
         cudaMemcpy(e->d_wtab, wtab.data(), sizeof(double) * wtab.size(), cudaMemcpyHostToDevice) != cudaSuccess ||

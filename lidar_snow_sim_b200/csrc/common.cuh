@@ -88,7 +88,7 @@ struct lss_engine {
     CameraConst *d_camera = nullptr;
     double *d_R = nullptr;              // range grid, LSS_M_EXT doubles
     double2 *d_wtab = nullptr;          // (sin, cos)(pi R[k] / (c tau)), LSS_M_EXT entries (solve.cu)
-    int n_sm = 148;                     // multiprocessors of the device (persistent grids)
+    int n_sm = 132;                     // multiprocessors of the device (persistent grids); queried by lss_create
     int *d_status = nullptr;            // latched asynchronous device status
     std::map<int, TableSet> tables;
     int next_table_id = 1;
@@ -171,8 +171,7 @@ inline cudaError_t lss_stage_upload(lss_engine *e, void *dst, const void *src, s
 }
 
 // Stream-ordered zero fill of up to 6 device regions in ONE kernel launch.  Not cudaMemsetAsync: memsets may be executed
-// by a copy engine, where they queue behind the host pipeline's multi-megabyte chunk copies (measured: a step next to a
-// saturated H2D stream went from 1.7 ms to 6.4 ms).  Region sizes are multiples of 4 bytes, pointers 4-byte aligned.
+// by a copy engine, where they queue behind the host pipeline's multi-megabyte chunk copies.  Region sizes are multiples of 4 bytes, pointers 4-byte aligned.
 struct ZeroRegions {
     static constexpr int MAX = 6;
     uint32_t *p[MAX];
@@ -192,7 +191,8 @@ inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStrea
     if (r.n == 0) return cudaSuccess;
     unsigned long long mx = 0;
     for (int i = 0; i < r.n; i++) mx = r.words[i] > mx ? r.words[i] : mx;
-    const unsigned blocks = (unsigned)((mx + 1023) / 1024 < 592 ? (mx + 1023) / 1024 : 592);
+    const unsigned long long cap = 4ull * e->n_sm;
+    const unsigned blocks = (unsigned)((mx + 1023) / 1024 < cap ? (mx + 1023) / 1024 : cap);
     k_zero_regions<<<dim3(blocks ? blocks : 1, r.n), 256, 0, stream>>>(r);
     e->launches++;
     return cudaGetLastError();

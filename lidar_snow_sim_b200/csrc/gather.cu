@@ -1,11 +1,10 @@
 // gather.cu -- the exchange step of the sharded batch (BASELINE configs[3], SURVEY.md 8e): every rank pushes the KEPT rows
 // of its slot-compacted augmented batch straight into every peer's gathered buffer over NVLink / NVSwitch.
 //
-// Why a kernel and not ncclAllGather or copy-engine copies (both measured on 8 x B200, profiles/r02_n8_*):
+// Why a kernel and not ncclAllGather or copy-engine copies:
 //   * the payload is known on the DEVICE only: cloud b keeps count[b] of its rows (the threshold filter drops 20-35 %);
 //     a library collective or a cudaMemcpyPeerAsync has to move the whole fixed-stride slot, this kernel reads the counts;
-//   * ncclAllGather's SM-resident channels took 0.1-0.25 ms per step from the latency-bound beam kernels and the
-//     copy engines reached 335 GB/s (one stream) or less (one stream per peer) of the ~900 GB/s a GPU can send;
+//   * ncclAllGather's SM-resident channels compete with the latency-bound beam kernels for SMs;
 //   * the persistent solve kernel leaves 4096 registers per SM: CTAs of 128 threads x 32 registers are the largest that
 //     still find room next to it, so this kernel is built to exactly that size and runs on a high-priority stream.
 // Stores to peer memory are plain 16-byte global stores through the peer mappings of a symmetric allocation, or -- when the
@@ -125,10 +124,8 @@ extern "C" lss_status lss_gather_push(lss_engine *e, const float *d_points, cons
         a.peer_counts[p] = h_peer_counts[p];
     }
     a.mc = d_mc_points; a.mc_counts = d_mc_counts;
-    // Measured on 8 GPUs next to the beam kernels (profiles/r02_n8c_*, r02_n8d_*): multicast 37 CTAs 1.09-1.13 ms per step,
-    // 74 / 148 CTAs 1.22 / 1.34 ms (alone every count takes 0.70 ms); per-peer
-    // stores 64 CTAs 1.07 ms, 148 CTAs 1.57 ms.  A chunk-cursor variant with 148 CTAs was slower on 2 GPUs (0.97 vs 0.93 ms);
-    // four instead of two 16-byte loads in flight per thread (multicast) changed nothing on 2 GPUs and was slower on 8 (1.28 ms).
+    // Default CTA counts: few CTAs, so that the push leaves the SMs to the beam kernels it runs next to (a quarter of the SMs
+    // with multicast stores, at most 64 with per-peer stores); LSS_GATHER_BLOCKS overrides them.
     if (n_blocks <= 0) n_blocks = d_mc_points ? std::max(1, e->n_sm / 4) : std::min(e->n_sm, 64);
     cudaStream_t st = (cudaStream_t)stream;
     if (d_mc_points) k_gather_push<true><<<n_blocks, GATHER_TPB, 0, st>>>(a);

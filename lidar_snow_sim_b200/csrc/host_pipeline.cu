@@ -208,9 +208,9 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
     cudaError_t ce = cudaSuccess;
     std::vector<int64_t> loc_off;
     // Copy-out: by default a cudaMemcpyAsync of the whole slot on the copy engine.  LSS_PIPE_KERNEL_OUT=1 (and a page-locked
-    // result buffer, i.e. one the device can address) selects k_copy_rows_out, which moves only the kept rows: measured on one
-    // B200 it does NOT pay (2.12 vs 2.06 ms per step: SM-issued PCIe writes are slower than the copy engine by more than
-    // the 25 % of bytes saved); it is kept for hosts whose memory write bandwidth is the limiter (8 ranks on one box).
+    // result buffer, i.e. one the device can address) selects k_copy_rows_out, which moves only the kept rows (about 25 % fewer
+    // bytes, but written by SMs over PCIe instead of the copy engine); it is meant for hosts whose memory write bandwidth is
+    // the limiter (several ranks on one box).
     float *h_out_dev = nullptr;
     {
         static const bool kernel_out = getenv("LSS_PIPE_KERNEL_OUT") && getenv("LSS_PIPE_KERNEL_OUT")[0] == '1';

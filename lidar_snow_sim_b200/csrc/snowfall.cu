@@ -30,7 +30,7 @@
 namespace {
 
 // Cold or bulky pieces are kept out of line and data-dependent loops are not unrolled: the beam kernel is
-// instruction-fetch sensitive (profiles/: `no_inst` stalls grow with its SASS size), every instruction that is not
+// instruction-fetch sensitive (`no_inst` stalls grow with its SASS size), every instruction that is not
 // on the common path costs fetch bandwidth for all resident warps.
 // one waveform sample: sum over the pulses q0..q1 whose window contains k, in dict order (simulation.py:148-149)
 __device__ __noinline__ double waveform_sample(int k, double Rk, int q0, int q1, const double *amp, const double *r,
@@ -801,8 +801,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
                                 !s.h_thresh_poly && !s.d_thresh_poly;
     // Where to fork it: the persistent solve kernel holds every SM's registers until its last tile, so a chain forked
     // AFTER the scan (which would let the scan kernel compact the mounting-window points as a by-product,
-    // PrepassIO::window_staged) finds no room for its 1024-thread CTAs and becomes the critical path (measured: step
-    // 1.07 ms instead of 1.01).  Default: fork before the scan, whose CTAs retire continuously; LSS_FUSE_WINDOW=1 selects
+    // PrepassIO::window_staged) finds no room for its 1024-thread CTAs and becomes the critical path.  Default: fork before the scan, whose CTAs retire continuously; LSS_FUSE_WINDOW=1 selects
     // the other order for experiments.
     static const bool fuse_window_env = getenv("LSS_FUSE_WINDOW") && getenv("LSS_FUSE_WINDOW")[0] == '1';
     const bool fuse_window = fuse_window_env && !s.h_plane_in;

@@ -85,7 +85,7 @@ __device__ __forceinline__ bool exact_hit(const ParticleRec *rp, const Beam &bm,
 // ---------------------------------------------------------------------------------------------------------------------
 // Two phases per warp (32 consecutive rows), because a thread-per-beam loop that tests a candidate exactly as soon as it
 // finds one pays the latency of that dependent record load in EVERY iteration in which any lane of the warp has a
-// candidate (measured: the exact tests ran at 5 of 32 lanes and dominated the kernel):
+// candidate (few lanes of the warp do exact tests at a time):
 //   A  each lane walks its beam's bucket prefix with the float32 broad phase only -- a streaming read of 8-byte
 //      entries, four loads in flight -- and notes the particle indices of the survivors (shared memory, SURV_CAP per lane);
 //   B  the survivors of all 32 beams are tested exactly by ALL lanes, one survivor per lane and round (owner by a

@@ -11,7 +11,8 @@
 //
 // Size (round 2): 8-byte quantised broad-phase entries (common.cuh: BroadEntry) + 24-byte exact records + 16-byte
 // tangent angles that only hits touch = 8 * 2.2 + 40 = 58 bytes per particle, of which 42 are on the scan kernel's path
-// (round 1: 80): at 18 k disks per plane the scan's working set is 48 MB of the 126 MB L2, next to the streamed rows.
+// (round 1: 80): at 18 k disks per plane the scan's working set is 48 MB, about the size of an H100's 50 MB L2, so the
+// streamed rows evict part of it.
 #include "common.cuh"
 
 namespace {

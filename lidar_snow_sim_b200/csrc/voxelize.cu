@@ -252,7 +252,7 @@ VoxLayout vox_layout(int64_t n_total, int n_clouds, int max_points, int max_voxe
 cudaError_t fill32(lss_engine *e, void *p, unsigned long long words, uint32_t v, cudaStream_t st)
 {
     if (!words) return cudaSuccess;
-    const unsigned blocks = (unsigned)std::min<unsigned long long>((words + 1023) / 1024, 148 * 16);
+    const unsigned blocks = (unsigned)std::min<unsigned long long>((words + 1023) / 1024, (unsigned long long)e->n_sm * 16);
     k_fill32<<<blocks, 256, 0, st>>>((uint32_t *)p, words, v);
     e->launches++;
     return cudaGetLastError();

@@ -141,10 +141,9 @@ class BatchGather:
                 rank writes the KEPT rows of its batch into every rank's buffer with the engine's own kernel
                 (lss_gather_push, csrc/gather.cu: peer-to-peer stores over NVLink, or one multicast store per 16 bytes
                 when the allocation has an NVLS mapping) on a high-priority side stream.  Needs `cloud_offsets`.
-    kind 'ce'   the same buffers, whole slots pushed with peer-to-peer device copies (copy engines, no SM): 8 GPUs reached
-                335 GB/s per rank on one stream and less on one stream per peer (profiles/r02_n8*_bench_ce.json).
+    kind 'ce'   the same buffers, whole slots pushed with peer-to-peer device copies (copy engines, no SM).
     kind 'nccl' dist.all_gather_into_tensor(async_op=True) on NCCL's stream (also what the gloo CPU tests exercise); its
-                SM-resident channels slowed the latency-bound beam kernels by up to 20 % at 8 GPUs (round 1).
+                SM-resident channels compete with the latency-bound beam kernels.
 
     Completion: `wait(j)` makes the caller's stream wait for THIS rank's outgoing copies of buffer j; a consumer that
     reads a gathered buffer needs a barrier across ranks first (bench.py brackets end with one).  LSS_GATHER=nccl|ce
@@ -201,8 +200,7 @@ class BatchGather:
                                    for r in range(self.world)])
             self._mc.append((int(getattr(hp, 'multicast_ptr', 0) or 0), int(getattr(hc, 'multicast_ptr', 0) or 0)))
         # one side stream per peer: the world - 1 pushes of a step run on different copy engines at the same time (one
-        # stream serialised them: 8 GPUs, 587 MB out per rank and step took 1.75 ms, i.e. 335 GB/s of the ~770 GB/s a
-        # GPU can send over NVLink)
+        # stream would serialise them)
         self._side = [torch.cuda.Stream(device=self.device) for _ in range(max(1, self.world))]
         self._done = [[torch.cuda.Event() for _ in range(max(1, self.world))] for _ in range(self.depth)]
         self._ready = torch.cuda.Event()

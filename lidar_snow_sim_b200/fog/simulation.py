@@ -1,6 +1,6 @@
 """
 Drop-in mirror of the reference's fog simulation API (lib/LiDAR_fog_sim/fog_simulation.py): `ParameterSet` (:52-171) and
-`simulate_fog(p, pc, noise, gain, noise_variant, hard, soft)` (:299-316), computed by the B200 engine (csrc/fog.cu).
+`simulate_fog(p, pc, noise, gain, noise_variant, hard, soft)` (:299-316), computed by the CUDA engine (csrc/fog.cu).
 Caller in the reference: DenseDataset.foggify, lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:990-1009.
 
 Like the reference, the noise draws come from a module-level `RNG = np.random.default_rng(seed=42)` (:15) unless the

@@ -258,8 +258,10 @@ def calculate_plane(pointcloud, standart_height=-1.55):
 
 
 def estimate_laser_parameters(pointcloud_planes, calculated_indicent_angle, power_factor=15, noise_floor=0.7,
-                              estimation_method='linear', least_populated='argpartition'):
-    """tools/wet_ground/augmentation.py:195-266, 'linear' branch, with the idx1[0] shim (NumPy >= 1.23)."""
+                              estimation_method='linear', least_populated='argpartition', fits=None):
+    """tools/wet_ground/augmentation.py:195-266, 'linear' branch, with the idx1[0] shim (NumPy >= 1.23).
+    `fits` ((slope, intercept) of the two linregress calls, :216 and :249) replays what a reference run computed on ITS
+    host (tests/golden/*: 'fits'): linregress sums through BLAS, whose kernel -- and so the last bits -- depends on the CPU."""
     from scipy.stats import linregress
     normalized_intensitites = pointcloud_planes[:, 3] / np.cos(calculated_indicent_angle)
     distance = np.linalg.norm(pointcloud_planes[:, :3], axis=1)
@@ -269,6 +271,8 @@ def estimate_laser_parameters(pointcloud_planes, calculated_indicent_angle, powe
         raise NotImplementedError("oracle restates estimation_method='linear' only")
     reg = linregress(distance, normalized_intensitites)
     p = [reg[0], reg[1]]
+    if fits is not None:
+        p = [np.float64(fits[0][0]), np.float64(fits[0][1])]
     stat_values = reg[2:]
     relative_output_intensity = power_factor * (p[0] * distance + p[1])
     hist, xedges, yedges = np.histogram2d(distance, normalized_intensitites, bins=(50, 2555),
@@ -292,7 +296,7 @@ def estimate_laser_parameters(pointcloud_planes, calculated_indicent_angle, powe
     idx1 = [i + 1 for i in idx]
     x = (xedges[idx] + xedges[idx1[0]]) / 2
     if len(min_vals) > 3:
-        pmin = linregress(x, min_vals)
+        pmin = linregress(x, min_vals) if fits is None else (np.float64(fits[1][0]), np.float64(fits[1][1]))
     else:
         pmin = p
     adaptive_noise_threshold = noise_floor * (pmin[0] * distance + pmin[1])
@@ -409,8 +413,9 @@ def total_transmittance_from_ground(ain, nair=1.0003, nw=1.33, rho=0.9):
 
 def ground_water_augmentation(pointcloud, water_height=0.001, pavement_depth=0.0012, noise_floor=0.7, power_factor=15,
                               estimation_method='linear', flat_earth=False, delta=0.5, replace=True, plane=None,
-                              return_internals=False, least_populated='argpartition'):
-    """tools/wet_ground/augmentation.py:25-161 (debug plots dropped; `plane` lets a test inject the RANSAC result)."""
+                              return_internals=False, least_populated='argpartition', fits=None):
+    """tools/wet_ground/augmentation.py:25-161 (debug plots dropped; `plane` lets a test inject the RANSAC result, `fits`
+    the regressions, see estimate_laser_parameters)."""
     w, h = calculate_plane(pointcloud) if plane is None else plane
     height_over_ground = np.matmul(pointcloud[:, :3], np.asarray(w))
     height_over_ground = height_over_ground.reshape((len(height_over_ground), 1))
@@ -428,7 +433,7 @@ def ground_water_augmentation(pointcloud, water_height=0.001, pavement_depth=0.0
                                    np.linalg.norm(pointcloud_planes[:, :3], axis=1) * np.linalg.norm([0, 0, 1])))
     relative_output_intensity, adaptive_noise_threshold, pfit, _ = estimate_laser_parameters(
         pointcloud_planes, ang, noise_floor=noise_floor, estimation_method=estimation_method,
-        power_factor=power_factor, least_populated=least_populated)
+        power_factor=power_factor, least_populated=least_populated, fits=fits)
     reflectivities = pointcloud_planes[:, 3] / np.cos(ang) / relative_output_intensity
     rs, ts, rp, tp, aaout = total_transmittance_from_ground(ang, rho=np.clip(reflectivities, 0.05, 1))
     t = np.maximum(tp, ts)

@@ -11,7 +11,7 @@ GOLD = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run on the B200 box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: test needs a CUDA device (run on an H100 with -m gpu)')
 
 
 @pytest.fixture(scope='session')

@@ -1,5 +1,7 @@
-"""The exchange step on real peers: needs at least two GPUs on the box (skipped otherwise); the single-GPU test of the
-push kernel is tests/test_snowfall_gpu.py::test_gather_push_writes_kept_rows_into_every_peer_buffer."""
+"""The exchange step through torch.distributed, one rank per GPU: 8 ranks on a box with eight or more GPUs, 2 on a smaller
+multi-GPU box, and 1 on a single GPU, where every kind still runs end to end (symmetric allocation and rendezvous, push
+kernel, peer copies, NCCL all-gather) with the rank as its own only peer.  The push kernel alone, with several mapped
+destinations on one GPU, is tests/test_snowfall_gpu.py::test_gather_push_writes_kept_rows_into_every_peer_buffer."""
 import json
 import os
 import subprocess
@@ -14,9 +16,9 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 @pytest.mark.gpu
 def test_every_gather_kind_reassembles_the_batch_on_every_rank():
     n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip('needs two GPUs')
-    n = 2 if n < 8 else 8
+    if n < 1:
+        pytest.skip('no CUDA device')
+    n = 8 if n >= 8 else min(n, 2)
     cmd = [sys.executable, '-m', 'torch.distributed.run', '--nnodes=1', f'--nproc-per-node={n}', '--master-addr', '127.0.0.1',
            '--master-port', '29533', os.path.join(ROOT, 'tools', 'check_gather_ranks.py')]
     p = subprocess.run(cmd, capture_output=True, text=True, timeout=600, cwd=ROOT)

@@ -95,12 +95,16 @@ def test_augment_full_size(oracle, gold_dir):
 
 
 def test_wet_ground(oracle, gold_dir):
+    """Bit for bit with the reference host's RANSAC plane, bin picks and regression fits replayed (linregress sums
+    through BLAS, whose last bits depend on the CPU); the oracle's own fits agree to rounding."""
     g = np.load(os.path.join(gold_dir, 'wet_ground.npz'))
     pc = synthetic_cloud(seed=int(g['seed']), n_azimuth=int(g['n_azimuth']))
     assert sha(pc) == str(g['cloud_sha'])
-    out = oracle.ground_water_augmentation(pc, water_height=0.001, plane=(g['plane_w'], float(g['plane_h'])),
-                                           least_populated=g['ymins'])
+    kw = dict(water_height=0.001, plane=(g['plane_w'], float(g['plane_h'])), least_populated=g['ymins'])
+    out = oracle.ground_water_augmentation(pc, fits=g['fits'], **kw)
     assert out.dtype == np.float64 and np.array_equal(out, g['out'])
+    own = oracle.ground_water_augmentation(pc, **kw)
+    assert own.shape == out.shape and np.allclose(own, g['out'], rtol=1e-13, atol=0)
 
 
 def test_config1_and_config2(oracle, gold_dir):

@@ -1,77 +1,59 @@
-"""Cross-check of the CPU oracle against the LIVE reference on seeds the frozen fixtures do not contain.
-
-Runs only where /root/reference is mounted (the build container); skipped on the GPU box and anywhere else.  The
-frozen fixtures under tests/golden/ pin the oracle on fixed cases; this test keeps the pin honest on fresh random cases
-every time the CPU suite runs here: snowfall per-channel solve, wet ground, fog simulation.  CPU only."""
+"""Cross-check of the CPU oracle against the reference on seeds the other fixtures do not contain: snowfall per-channel
+solve, wet ground, fog simulation.  The reference's outputs for these seeded cases are frozen in
+tests/golden/fresh_seeds.npz by tools/make_golden_fresh.py, which runs the unmodified reference.  CPU only."""
 import os
 import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from oracle import ref_harness as rh                            # noqa: E402
-
-pytestmark = pytest.mark.skipif(not rh.available(), reason='reference tree not mounted (build container only)')
+from tools.make_golden_fresh import FOG_CASES, WET_KW, WET_SEED, channel_case, nan_sha  # noqa: E402
+from helpers import sha                                                              # noqa: E402
 
 DIV = float(np.degrees(3e-3))
 
 
+@pytest.fixture(scope='module')
+def gold(gold_dir):
+    return np.load(os.path.join(gold_dir, 'fresh_seeds.npz'))
+
+
 @pytest.mark.parametrize('seed,ch', [(101, 7), (102, 58)])
-def test_snowfall_channel_fresh_seed(seed, ch):
+def test_snowfall_channel_fresh_seed(seed, ch, gold):
     from oracle import oracle as orc
-    from tools.make_golden import channel_infos, write_tables
-    from lidar_snow_sim_b200.synthetic import synthetic_particles
     from lidar_snow_sim_b200.calib.hdl64e_s3 import sensor_arrays
-    ns = rh.load()
-    rng = np.random.default_rng(seed)
-    M = 96
-    table = synthetic_particles(seed, 22000)
-    az = rng.uniform(-np.pi, np.pi, M)
-    az[:16] = rng.uniform(-0.004, 0.004, 16)                     # seam beams
-    d = rng.uniform(1.2, 110.0, M)
-    el = rng.uniform(-0.4, 0.03, M)
-    pts = np.stack([d * np.cos(el) * np.cos(az), d * np.cos(el) * np.sin(az), d * np.sin(el),
-                    np.round(rng.uniform(1, 255, M)), np.full(M, ch)], axis=1).astype(np.float32)
-    root = tempfile.mkdtemp()
-    write_tables(root, 'g', [table] * 64)
-    s, idx, out = ns.sim.process_single_channel(root, 'g', pts, DIV, list(range(64)), channel_infos(), ch)
+    pts, table = channel_case(seed, ch)
+    assert np.array_equal(pts, gold[f'chan_{seed}_{ch}_pts']), 'numpy RNG stream changed: regenerate tests/golden'
+    out, s = gold[f'chan_{seed}_{ch}_out'], float(gold[f'chan_{seed}_{ch}_sum'])
     sensor = sensor_arrays()
     o_out, o_s, o_n, _ = orc.snow_channel(pts, table, DIV, sensor[0][ch], sensor[1][ch], sensor[2][ch], sensor[3][ch],
                                           theta=np.arctan2(pts[:, 1], pts[:, 0]))
-    assert np.array_equal(out, o_out) and float(s) == o_s
+    assert np.array_equal(out, o_out) and s == o_s
     assert (o_out[:, 4] > 0).sum() > 5                           # the case exercises attenuated / scattered beams
 
 
-def test_fog_fresh_seeds():
-    sys.path.insert(0, os.path.join(rh.REF_ROOT, 'lib', 'LiDAR_fog_sim'))
-    import fog_simulation as ref
+def test_fog_fresh_seeds(gold):
     from oracle import fog as ofog
     from lidar_snow_sim_b200.synthetic import synthetic_cloud
-    for seed, alpha, variant, noise, gain in ((5, 0.03, 'v1', 10, False), (6, 0.12, 'v3', 7, True), (7, 0.1, 'v4', 10, False)):
+    for seed, alpha, variant, noise, gain in FOG_CASES:
         pc = synthetic_cloud(seed=seed, n_azimuth=12)
-        p_ref = ref.ParameterSet(alpha=alpha, gamma=0.000001)
-        d = ref.get_integral_dict(p_ref)
-        lut = np.array([[float(d[k][0]), float(d[k][1])] for k in sorted(d.keys())])
-        ref.RNG = np.random.default_rng(seed)
-        w_aug, w_fog, w_info = ref.simulate_fog(p_ref, pc=pc, noise=noise, gain=gain, noise_variant=variant)
         rng = np.random.default_rng(seed)
-        aug, fog, info = ofog.simulate_fog(ofog.ParameterSet(alpha=alpha, gamma=0.000001), pc, noise, lut, rng, gain=gain,
-                                           noise_variant=variant)
-        assert np.array_equal(aug, w_aug, equal_nan=True), (seed, variant)
-        assert (fog is None and w_fog is None) or np.array_equal(fog, w_fog)
-        assert info['num_fog_responses'] == w_info['num_fog_responses']
-        assert np.array_equal(rng.random(2), ref.RNG.random(2))
+        aug, fog, info = ofog.simulate_fog(ofog.ParameterSet(alpha=alpha, gamma=0.000001), pc, noise, gold[f'fog_{seed}_lut'],
+                                           rng, gain=gain, noise_variant=variant)
+        shape, digest = nan_sha(aug)                                 # == np.array_equal(aug, ref, equal_nan=True)
+        assert aug.dtype == np.float64 and np.array_equal(shape, gold[f'fog_{seed}_aug_shape'])
+        assert np.array_equal(digest, gold[f'fog_{seed}_aug_sha']), (seed, variant)
+        shape, digest = nan_sha(np.zeros((0, 5)) if fog is None else fog)
+        assert np.array_equal(shape, gold[f'fog_{seed}_fog_shape']) and np.array_equal(digest, gold[f'fog_{seed}_fog_sha'])
+        assert info['num_fog_responses'] == int(gold[f'fog_{seed}_num_fog_responses'])
+        assert np.array_equal(rng.random(2), gold[f'fog_{seed}_next_u'])
 
 
-def test_wet_ground_fresh_seed():
+def test_wet_ground_fresh_seed(gold):
     from oracle import oracle as orc
     from lidar_snow_sim_b200.synthetic import synthetic_cloud
-    ns = rh.load()
-    pc = synthetic_cloud(seed=321, n_azimuth=128)
-    kw = dict(water_height=0.0008, pavement_depth=0.0012, noise_floor=0.7, power_factor=15, flat_earth=True, delta=0.5)
-    want = ns.wet_aug.ground_water_augmentation(pc.copy(), estimation_method='linear', debug=False, replace=True, **kw)
-    got = orc.ground_water_augmentation(pc.copy(), replace=True, **kw)
-    assert got.shape == want.shape and np.array_equal(got, want)
+    pc = synthetic_cloud(seed=WET_SEED, n_azimuth=128)
+    got = orc.ground_water_augmentation(pc.copy(), replace=True, **WET_KW)
+    assert got.shape == tuple(gold['wet_shape']) and sha(got) == str(gold['wet_sha'])

@@ -1,5 +1,5 @@
 """
-GPU parity tests (run on the B200 box with `-m gpu`): the CUDA path, called through the C ABI, against
+GPU parity tests (run on an H100 with `-m gpu`): the CUDA path, called through the C ABI, against
   (1) the golden vectors frozen from the unmodified reference (tests/golden/),
   (2) the CPU oracle on the same seeded inputs at sizes it finishes in seconds,
   (3) size-independent properties at BASELINE.json's full batch size.

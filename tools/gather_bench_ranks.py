@@ -38,11 +38,11 @@ def main():
     d_pts = torch.randn((n_rows, 5), dtype=torch.float32, device=dev)
     d_cnt = torch.from_numpy(cnt).to(dev)
     res = {'world': world, 'rows_per_rank': n_rows, 'kept_fraction': float(cnt.sum() / n_rows)}
-    variants = [('push_mc_b37', 'push', {'LSS_GATHER_BLOCKS': '37'}), ('push_mc_b74', 'push', {'LSS_GATHER_BLOCKS': '74'}),
-                ('push_mc_b148', 'push', {'LSS_GATHER_BLOCKS': '148'}), ('push_mc_b296', 'push', {'LSS_GATHER_BLOCKS': '296'}),
+    variants = [('push_mc_b33', 'push', {'LSS_GATHER_BLOCKS': '33'}), ('push_mc_b66', 'push', {'LSS_GATHER_BLOCKS': '66'}),
+                ('push_mc_b132', 'push', {'LSS_GATHER_BLOCKS': '132'}), ('push_mc_b264', 'push', {'LSS_GATHER_BLOCKS': '264'}),
                 ('push_uni_b32', 'push', {'LSS_GATHER_MULTICAST': '0', 'LSS_GATHER_BLOCKS': '32'}),
                 ('push_uni_b64', 'push', {'LSS_GATHER_MULTICAST': '0', 'LSS_GATHER_BLOCKS': '64'}),
-                ('push_uni_b148', 'push', {'LSS_GATHER_MULTICAST': '0', 'LSS_GATHER_BLOCKS': '148'}),
+                ('push_uni_b132', 'push', {'LSS_GATHER_MULTICAST': '0', 'LSS_GATHER_BLOCKS': '132'}),
                 ('ce', 'ce', {}), ('nccl', 'nccl', {})]
     for name, kind, env in variants:
         for k, v in env.items():

@@ -1,7 +1,7 @@
 """
 BASELINE.json configs[4]: snowfall-rate x terminal-velocity sweep -- throughput versus particle density.
 
-    python tools/sweep.py [--batch 32] [--steps 5] [--out profiles/r01_sweep.json]
+    python tools/sweep.py [--batch 32] [--steps 5] [--out sweep.json]
     python -m torch.distributed.run --nproc-per-node N ... tools/sweep.py     # batch sharded over N GPUs (weak scaling)
 
 For every (snowfall_rate, terminal_velocity) the 64 snowflake planes are drawn ON THE DEVICE by the engine's sampler,
