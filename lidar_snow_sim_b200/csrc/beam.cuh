@@ -60,17 +60,24 @@ struct DevArgs {
     unsigned long long *list_out;
     int *count_out;
     int cap_out;
-    // solve list (scan kernel -> sort -> solve kernel); hdr = the list header ints (LIST_HDR_BYTES)
-    SolveItem *items_out;
-    const SolveItem *items_in;
-    int *hdr;                    // [0] listed beams, [1] overflow beams, [2] tile cursor, [3] hit positions used, class counts ...
-    int items_cap;
+    // solve list, bucketed by work class as the scan kernel writes it (no sort pass): the beams of class c are numbered
+    // 0, 1, ... in the order the scan appends them, and beam j sits in chunk j / LIST_CHUNK of the class, which is
+    // items + (chunk_tab[c * chunks_per_class + j / LIST_CHUNK] - 1) * LIST_CHUNK (0 = chunk not allocated yet).
+    // hdr = the list header ints (LIST_HDR_BYTES)
+    SolveItem *items;
+    int *chunk_tab;
+    int chunks_per_class;
+    int *hdr;                    // [0] chunks allocated, [1] overflow beams, [2] tile cursor, [3] hit positions used, class counts
     int *hit_idx;                // particle indices of the hits of the listed beams
     int hit_cap;
     // optional by-product of the scan kernel for the concurrent pre-pass: the mounting-window points of calculate_plane
     // (tools/wet_ground/planes.py:21-27) compacted per 32-row tile (prepass.cu, PrepassIO::window_staged)
     float *win_stage;
     int *win_tile_cnt;
+    // plane-major schedule of the scan kernel: warp tile s of the launch is (cloud, first row) = sched[s] (cloud << 32 | row;
+    // bits 48.. hold the sort key), warp tiles of the whole batch sorted by plane
+    const unsigned long long *sched;
+    int n_wtiles;
 };
 
 namespace {
@@ -83,8 +90,14 @@ constexpr int POOL = 128;                           // pulses a warp publishes p
 constexpr int CCAP = 512;                           // candidate samples a warp evaluates per cooperative batch
 constexpr int SLOW_CAP = 128;                       // occluders per beam held by the overflow kernel (per-thread lists)
 constexpr int OVF_LIST_CAP = 1 << 16;               // beams the overflow kernel can take per call
-constexpr int LIST_HDR_BYTES = 2048;  // ints: [0] solve count, [1] overflow count, [C..2C) class counts, [2C..3C) cursors
-constexpr int LIST_CLASSES = 128;  // solve list is counting-sorted by work class (occluder count) before the solve kernel
+constexpr int LIST_HDR_BYTES = 1024;  // ints: [0] chunks allocated, [1] overflow count, [2] tile cursor, [3] hit positions,
+                                      // [C..2C) class counts
+constexpr int LIST_CLASSES = 128;     // solve list bucketed by work class (occluder count), costliest class first
+constexpr int LIST_CHUNK = 1024;      // solve items per chunk of a class (a multiple of 32: a solve tile is in one chunk)
+// scan schedule: warp tiles counting-sorted by the plane (mod SCHED_PLANES) of their first row's channel; rows without a
+// valid channel get the last bin.  Only locality depends on the bins, never a result.
+constexpr int SCHED_PLANES = 64;
+constexpr int SCHED_BINS = SCHED_PLANES + 1;
 
 __device__ __forceinline__ void raise_status(int *status, int code) { atomicMax(status, code); }
 
@@ -175,5 +188,5 @@ __device__ __forceinline__ float azimuth32(float yf, float xf)
 
 // solve.cu: the dense solve kernel over the (sorted) solve list; beams it cannot take (more than SOLVE_LCAP occluders or
 // a bucket prefix longer than it tracks) go to list_out for the overflow kernel.  hdr[2] is its tile cursor (zeroed).
-void lss_launch_scan(const DevArgs &a, int64_t max_rows, int n_clouds, cudaStream_t stream);
+void lss_launch_scan(const DevArgs &a, cudaStream_t stream);
 void lss_launch_solve(const DevArgs &a, int *tile_cursor, int n_sm, cudaStream_t stream);

@@ -3,9 +3,12 @@
 // Pipeline per call (on the caller's stream; the pre-pass is forked onto an engine side stream and joined before k_keep):
 //   [pre-pass]       ground plane + noise-threshold polynomial (prepass.cu), concurrent with the beam kernels
 //                                                                                 (tools/snowfall/simulation.py:449-467)
-//   k_scan           (solve.cu) every beam, rows in INPUT order: range / azimuth, walk of ONE azimuth bucket of the channel's
-//                    snowflake plane; un-occluded beams are finished, the others pushed to the solve list with their hits
-//   k_list_sort      counting sort of the solve list by work class (a solve warp runs as long as its slowest lane)
+//   k_sched_key      scan schedule: the warp tiles (32 input rows) of the batch keyed by plane; k_sched_sort orders them,
+//                    so that the resident scan warps read the tables of a few planes at a time
+//   k_scan           (solve.cu) every beam, warp tiles in schedule order, rows at their input positions: range / azimuth,
+//                    walk of ONE azimuth bucket of the channel's snowflake plane; un-occluded beams are finished, the
+//                    others appended, with their hits, to the solve list's bucket of their work class (a solve warp runs
+//                    as long as its slowest lane, so a solve tile takes beams of one class)
 //   k_solve          (solve.cu) the listed beams: nearest-first claiming of the beam's angular sub-intervals, summed
 //                    sin^2 waveform + argmax, relabel / move the point, label-1 statistics  (simulation.py:50-194, 231-424)
 //   k_overflow       beams with more than 63 occluders (rare): one beam per thread, per-thread lists of up to 128 hits
@@ -409,64 +412,86 @@ __global__ void __launch_bounds__(SNOW_TPB, 1) k_overflow(DevArgs a)
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// counting sort of the solve list by work class, so that the 32 beams of a solve-kernel warp cost about the same
-// (the warp runs as long as its slowest lane).  hdr: [0] entries, [LIST_CLASSES + c] class counts (from the scan kernel),
-// [2 * LIST_CLASSES + c] class cursors.  Order inside a class is arbitrary: the results do not depend on list order.
+// plane-major schedule of the scan kernel.  Every cloud maps its 64 channels onto the planes through order[], so in input
+// order the resident scan warps read the bucket prefixes of all planes at once -- tens of MB of index and records, more
+// than the H100's L2 keeps next to the streamed rows.  Sorted by plane, the warps resident at any moment read the tables
+// of two or three planes.  k_sched_key writes each warp tile's entry (plane bin << 48 | cloud << 32 | first row; 32 rows
+// of one cloud, the scan's unit of work) and the bin histogram hist[0, SCHED_BINS); k_sched_sort orders the entries.
+// ---------------------------------------------------------------------------------------------------------------------
+constexpr int SCHED_KEY_TPB = 128;
+
+__global__ void __launch_bounds__(SCHED_KEY_TPB) k_sched_key(const float *__restrict__ pts, const int64_t *__restrict__ cloud_off,
+                                                            const int32_t *__restrict__ order, const int32_t *__restrict__ wtile_base,
+                                                            unsigned long long *ent, int *hist)
+{
+    const int b = blockIdx.y, t = blockIdx.x * SCHED_KEY_TPB + threadIdx.x;
+    const int64_t beg = cloud_off[b];
+    const int n = (int)(cloud_off[b + 1] - beg);
+    if (blockIdx.x * SCHED_KEY_TPB * 32 >= n) return;
+    const int w0 = 32 * t;
+    const bool on = w0 < n;
+    int bin = -1;
+    if (on) {
+        const int ch = channel_bin(pts[(beg + w0) * 5 + 4]);
+        bin = ch < LSS_N_CHANNELS ? order[b * LSS_N_CHANNELS + ch] % SCHED_PLANES : SCHED_PLANES;
+        ent[wtile_base[b] + t] = ((unsigned long long)bin << 48) | ((unsigned long long)b << 32) | (unsigned)w0;
+    }
+    const unsigned m = __match_any_sync(0xffffffffu, bin);
+    if (on && (threadIdx.x & 31) == __ffs(m) - 1) atomicAdd(&hist[bin], __popc(m));
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// counting sort of the schedule entries by bin (k_sched_key's histogram, then the bin cursors in hist[SCHED_BINS ..]):
+// block-local ranks in shared memory, one global cursor update per bin and block.  Order inside a bin is arbitrary.
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int HIT_POS_PER_BEAM = 6;                 // capacity of the hit-position array per beam of the batch
-constexpr int SORT_PER_THREAD = 8;
-__global__ void __launch_bounds__(256) k_list_sort(const SolveItem *__restrict__ in, SolveItem *out, int *hdr, int cap)
+constexpr int SCHED_PER_THREAD = 2;
+__global__ void __launch_bounds__(256) k_sched_sort(const unsigned long long *__restrict__ in, unsigned long long *out,
+                                                    int *hist, int n)
 {
-    __shared__ int base[LIST_CLASSES], hist[LIST_CLASSES], blk[LIST_CLASSES];
-    const int cnt = min(hdr[0], cap);
-    const int first = blockIdx.x * (256 * SORT_PER_THREAD);
-    if (first >= cnt) return;
-    for (int c = threadIdx.x; c < LIST_CLASSES; c += 256) hist[c] = 0;
-    if (threadIdx.x < 32) {                                  // exclusive scan of the class counts, one warp
+    __shared__ int base[SCHED_BINS], cnt[SCHED_BINS], blk[SCHED_BINS];
+    const int first = blockIdx.x * (256 * SCHED_PER_THREAD);
+    for (int c = threadIdx.x; c < SCHED_BINS; c += 256) cnt[c] = 0;
+    if (threadIdx.x < 32) {                                  // exclusive scan of the bin counts, one warp
         int run = 0;
-        for (int c0 = 0; c0 < LIST_CLASSES; c0 += 32) {
-            const int v = hdr[LIST_CLASSES + c0 + threadIdx.x];
+        for (int c0 = 0; c0 < SCHED_BINS; c0 += 32) {
+            const int c = c0 + (int)threadIdx.x;
+            const int v = c < SCHED_BINS ? hist[c] : 0;
             int incl = v;
 #pragma unroll
             for (int s = 1; s < 32; s <<= 1) {
                 const int t = __shfl_up_sync(0xffffffffu, incl, s);
                 if ((int)threadIdx.x >= s) incl += t;
             }
-            base[c0 + threadIdx.x] = run + incl - v;
+            if (c < SCHED_BINS) base[c] = run + incl - v;
             run += __shfl_sync(0xffffffffu, incl, 31);
         }
     }
     __syncthreads();
-    // rank inside the block (shared-memory counters, warp-aggregated), then ONE global cursor update per class and
-    // block: the neighbouring beams of a cloud fall into few classes, per-entry global atomics would serialise
     const int lane = threadIdx.x & 31;
-    int cls_of[SORT_PER_THREAD], rank[SORT_PER_THREAD];
+    int bin_of[SCHED_PER_THREAD], rank[SCHED_PER_THREAD];
+    unsigned long long e[SCHED_PER_THREAD];
 #pragma unroll
-    for (int k = 0; k < SORT_PER_THREAD; k++) {
-        const int slot = first + k * 256 + threadIdx.x;
-        const bool on = slot < cnt;
-        const int cls = on ? (int)(in[slot].key >> 48) : -1;
-        cls_of[k] = cls;
-        const unsigned m = __match_any_sync(0xffffffffu, cls);
+    for (int k = 0; k < SCHED_PER_THREAD; k++) {
+        const int s = first + k * 256 + threadIdx.x;
+        const bool on = s < n;
+        e[k] = on ? in[s] : 0ull;
+        const int bin = on ? (int)(e[k] >> 48) : -1;
+        bin_of[k] = bin;
+        const unsigned m = __match_any_sync(0xffffffffu, bin);
         const int leader = __ffs(m) - 1;
         int r = 0;
-        if (on && lane == leader) r = atomicAdd(&hist[cls], __popc(m));
+        if (on && lane == leader) r = atomicAdd(&cnt[bin], __popc(m));
         r = __shfl_sync(0xffffffffu, r, leader);
         rank[k] = r + __popc(m & ((1u << lane) - 1u));
     }
     __syncthreads();
-    for (int c = threadIdx.x; c < LIST_CLASSES; c += 256)
-        blk[c] = hist[c] ? atomicAdd(&hdr[2 * LIST_CLASSES + c], hist[c]) : 0;
+    for (int c = threadIdx.x; c < SCHED_BINS; c += 256)
+        blk[c] = cnt[c] ? atomicAdd(&hist[SCHED_BINS + c], cnt[c]) : 0;
     __syncthreads();
 #pragma unroll
-    for (int k = 0; k < SORT_PER_THREAD; k++)
-        if (cls_of[k] >= 0) {
-            const int slot = first + k * 256 + threadIdx.x;
-            const uint4 *src = reinterpret_cast<const uint4 *>(in + slot);
-            uint4 *dst = reinterpret_cast<uint4 *>(out + base[cls_of[k]] + blk[cls_of[k]] + rank[k]);
-            dst[0] = src[0];
-            dst[1] = src[1];
-        }
+    for (int k = 0; k < SCHED_PER_THREAD; k++)
+        if (bin_of[k] >= 0) out[base[bin_of[k]] + blk[bin_of[k]] + rank[k]] = e[k];
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -647,13 +672,14 @@ inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
 struct WsLayout {
     int64_t aug, code_keep, code_all, nocc, hist_keep, hist_all, hist_rows, cloud_off, tile_base, order, thresh, counters,
-        counters_bytes, ovf, prepass, prepass_bytes, total;
+        counters_bytes, ovf, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
 };
 
 WsLayout ws_layout(int64_t n_total, int n_clouds)
 {
     WsLayout w;
     w.hist_rows = n_total / TILE + (int64_t)n_clouds + 1;          // >= sum over clouds of ceil(n_b / TILE)
+    w.sched_tiles = n_total / 32 + (int64_t)n_clouds + 1;          // >= sum over clouds of ceil(n_b / 32)
     int64_t o = 0;
     w.aug = o;        o = align_up(o + n_total * 5 * 4, 256);
     w.code_keep = o;  o = align_up(o + n_total, 256);
@@ -662,17 +688,24 @@ WsLayout ws_layout(int64_t n_total, int n_clouds)
     w.hist_keep = o;  o = align_up(o + w.hist_rows * NBINS * 4, 256);
     w.hist_all = o;   o = align_up(o + w.hist_rows * NBINS * 4, 256);
     w.cloud_off = o;  o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    w.tile_base = o;  o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
+    w.tile_base = o;  o = align_up(o + (int64_t)(n_clouds + 1) * 2 * 4, 256);   // scatter tiles, then warp tiles
     w.order = o;      o = align_up(o + (int64_t)n_clouds * LSS_N_CHANNELS * 4, 256);
     w.thresh = o;     o = align_up(o + (int64_t)n_clouds * 3 * 8, 256);
     // counters: int[B*2] | unsigned att_cnt[B*64] | unsigned long long att_sum[B]
     w.counters_bytes = align_up((int64_t)n_clouds * 2 * 4, 8) + (int64_t)n_clouds * LSS_N_CHANNELS * 4 + (int64_t)n_clouds * 8;
     w.counters = o;   o = align_up(o + w.counters_bytes, 256);
-    // list header | overflow list | solve list, unsorted + sorted (every beam may have occluders)
+    // list header | overflow list | solve list chunks (every beam may have occluders; each class leaves at most one chunk
+    // partly filled)
     //   | hit particle indices (int32; HIT_POS_PER_BEAM per beam of the batch on average: the surveyed densities give 1-5 occluders
     //   on a third of the beams)
-    w.ovf = o;        o = align_up(o + LIST_HDR_BYTES + (int64_t)OVF_LIST_CAP * 8 + 2 * n_total * (int64_t)sizeof(SolveItem) +
+    w.chunks_per_class = (n_total + LIST_CHUNK - 1) / LIST_CHUNK;
+    w.ovf = o;        o = align_up(o + LIST_HDR_BYTES + (int64_t)OVF_LIST_CAP * 8 +
+                                   (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK * (int64_t)sizeof(SolveItem) +
                                    (n_total * HIT_POS_PER_BEAM + 4096) * 4, 256);
+    // chunk table of the solve list: LIST_CLASSES x chunks_per_class ids
+    w.chunk_tab = o;  o = align_up(o + (int64_t)LIST_CLASSES * w.chunks_per_class * 4, 256);
+    // scan schedule: bin counts and cursors | warp-tile entries, unsorted + sorted
+    w.sched = o;      o = align_up(o + (int64_t)SCHED_BINS * 2 * 4 + 2 * w.sched_tiles * 8, 256);
     w.prepass_bytes = lss_prepass_ws_bytes(n_total, n_clouds);
     w.prepass = o;    o = align_up(o + w.prepass_bytes, 256);
     w.total = o;
@@ -714,9 +747,15 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     if (!(div_rad > 0) || div_rad > s.ts->max_div_rad * (1 + 1e-12))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "beam_divergence exceeds the value the table set was built for");
     const int max_tiles = (int)((max_n + TILE - 1) / TILE);
-    std::vector<int32_t> h_tile_base(B + 1, 0);
-    for (int b = 0; b < B; b++)
-        h_tile_base[b + 1] = h_tile_base[b] + (int32_t)((s.h_cloud_offsets[b + 1] - s.h_cloud_offsets[b] + TILE - 1) / TILE);
+    // [0, B] first scatter tile (TILE rows) of each cloud, [B + 1, 2 B + 1] first warp tile (32 rows) of each cloud
+    std::vector<int32_t> h_tile_base(2 * (B + 1), 0);
+    int32_t *h_wtile_base = h_tile_base.data() + B + 1;
+    for (int b = 0; b < B; b++) {
+        const int64_t n = s.h_cloud_offsets[b + 1] - s.h_cloud_offsets[b];
+        h_tile_base[b + 1] = h_tile_base[b] + (int32_t)((n + TILE - 1) / TILE);
+        h_wtile_base[b + 1] = h_wtile_base[b] + (int32_t)((n + 31) / 32);
+    }
+    const int n_wtiles = h_wtile_base[B];
     if ((s.d_out_perm || s.d_out_nocc) && !s.d_out_full)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "d_out_perm / d_out_nocc need d_out_full");
 
@@ -737,11 +776,11 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     unsigned long long *d_att_sum = (unsigned long long *)((char *)d_att_cnt + (int64_t)B * LSS_N_CHANNELS * 4);
 
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, s.h_cloud_offsets, sizeof(int64_t) * (B + 1), stream));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_tile_base, h_tile_base.data(), sizeof(int32_t) * (B + 1), stream));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_tile_base, h_tile_base.data(), sizeof(int32_t) * 2 * (B + 1), stream));
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS, stream));
     if (s.h_thresh_poly && !s.d_thresh_poly)
         LSS_CUDA_CHECK(e, lss_stage_upload(e, d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B, stream));
-    int *d_counts2 = (int *)(ws + w.ovf);                                   // [0] solve list, [1] overflow list
+    int *d_counts2 = (int *)(ws + w.ovf);                                   // list header (LIST_HDR_BYTES)
     {
         ZeroRegions z;
         z.add(d_counters, w.counters_bytes);
@@ -752,6 +791,8 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             return LSS_OK;
         }
         z.add(d_counts2, LIST_HDR_BYTES);                 // (the tile histograms are written whole by k_keep)
+        z.add(ws + w.chunk_tab, (size_t)LIST_CLASSES * w.chunks_per_class * 4);
+        z.add(ws + w.sched, (size_t)SCHED_BINS * 2 * 4);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
     }
 
@@ -791,9 +832,8 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.att_sum = d_att_sum;
     a.status = e->d_status;
     unsigned long long *d_ovf_list = (unsigned long long *)(ws + w.ovf + LIST_HDR_BYTES);
-    SolveItem *d_solve_list = (SolveItem *)(d_ovf_list + OVF_LIST_CAP);
-    SolveItem *d_sorted_list = d_solve_list + N;
-    a.hit_idx = (int *)(d_sorted_list + N);
+    SolveItem *d_solve_list = (SolveItem *)(d_ovf_list + OVF_LIST_CAP);   // (chunks_per_class + LIST_CLASSES) chunks
+    a.hit_idx = (int *)(d_solve_list + (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK);
     // Device pre-pass: plane + laser parameters + threshold polynomial (simulation.py:449-467), on the cloud as given.
     // Only k_keep needs its result, so it runs on one of the engine's high-priority side streams next to the beam kernels (a
     // chain of small latency-bound kernels).
@@ -833,21 +873,32 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.hit_cap = (int)std::min<int64_t>(N * HIT_POS_PER_BEAM + 4096, 0x7fffffff);
     {
         KernelTimer kt(e, LSS_K_SNOWFALL, stream);
-        const int items_cap = (int)std::min<int64_t>(N, 0x7fffffff);
         // 1. scan: all beams; the ones without occluders are finished, the others go to the solve list with their hit masks
         a.list_in = nullptr; a.count_in = nullptr; a.cap_in = 0;
         a.list_out = nullptr; a.count_out = nullptr; a.cap_out = 0;
         a.hdr = d_counts2;
-        a.items_out = d_solve_list; a.items_in = nullptr; a.items_cap = items_cap;
+        a.items = d_solve_list;
+        a.chunk_tab = (int *)(ws + w.chunk_tab);
+        a.chunks_per_class = (int)w.chunks_per_class;
+        {   // plane-major order of the warp tiles
+            int *d_sched_hist = (int *)(ws + w.sched);
+            unsigned long long *d_ent = (unsigned long long *)(d_sched_hist + 2 * SCHED_BINS);
+            unsigned long long *d_sched = d_ent + w.sched_tiles;
+            const int max_wtiles = (int)((max_n + 31) / 32);
+            k_sched_key<<<dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B), SCHED_KEY_TPB, 0, stream>>>(
+                s.d_points, d_off, d_order, d_tile_base + B + 1, d_ent, d_sched_hist);
+            k_sched_sort<<<(unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)), 256, 0, stream>>>(
+                d_ent, d_sched, d_sched_hist, n_wtiles);
+            e->launches += 2;
+            a.sched = d_sched;
+            a.n_wtiles = n_wtiles;
+        }
         {
             KernelTimer ks(e, LSS_K_SCAN, stream);
-            lss_launch_scan(a, max_n, B, stream);
+            lss_launch_scan(a, stream);
         }
         if (device_prepass && fuse_window) LSS_CHECK_STATUS(fork_prepass());
-        // 2. solve: the listed beams, sorted by work class, one warp per tile of 32 (persistent grid)
-        k_list_sort<<<(unsigned)((N + 256 * SORT_PER_THREAD - 1) / (256 * SORT_PER_THREAD)), 256, 0, stream>>>(d_solve_list, d_sorted_list, d_counts2, items_cap);
-        a.items_in = d_sorted_list; a.items_out = nullptr;
-        a.count_in = d_counts2; a.cap_in = items_cap;
+        // 2. solve: the listed beams, class by class, one warp per tile of 32 (persistent grid)
         a.list_out = d_ovf_list; a.count_out = d_counts2 + 1; a.cap_out = OVF_LIST_CAP;
         {
             KernelTimer ks(e, LSS_K_SOLVE, stream);
@@ -856,8 +907,8 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
         // 3. overflow: beams with more occluders than the solve kernel's arena takes per beam (rare), round-1 list kernel
         a.list_in = d_ovf_list; a.count_in = d_counts2 + 1; a.cap_in = OVF_LIST_CAP;
         a.list_out = nullptr; a.count_out = nullptr; a.cap_out = 0;
-        k_overflow<<<OVF_LIST_CAP / SNOW_TPB, SNOW_TPB, 0, stream>>>(a);
-        e->launches += 1;           // (+ one each from the three KernelTimer brackets = 4 launches)
+        k_overflow<<<OVF_LIST_CAP / SNOW_TPB, SNOW_TPB, 0, stream>>>(a);   // (scan, solve, overflow: one launch counted
+                                                                            // by each of the three KernelTimer brackets)
     }
     if (ev_join) LSS_CUDA_CHECK(e, cudaStreamWaitEvent(stream, ev_join, 0));
     {

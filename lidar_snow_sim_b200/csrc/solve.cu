@@ -1,19 +1,20 @@
 // solve.cu -- the two per-beam kernels of the snowfall path.
 //
-//   k_scan   every beam of the batch, one thread per beam, rows in INPUT order: float32 range / azimuth, walk of the
+//   k_scan   every beam of the batch, one thread per beam, warps of 32 input rows taken in plane-major order (the schedule
+//            of snowfall.cu, k_sched_key), rows read and written at their input positions: float32 range / azimuth, walk of the
 //            beam's azimuth bucket of its channel's snowflake plane (float32 broad phase, exact float64 disk / wedge test)
 //            over the WHOLE prefix of entries nearer than the target.  Beams without occluder (~2/3) are finished here;
 //            the others are pushed to the solve list together with what the walk found: the particle indices of the
 //            hits (in prefix order) and the azimuth.                         (tools/snowfall/simulation.py:80-101, 329-390)
-//   k_solve  the listed beams, sorted by work class: tangent angles of the hits, nearest-first claiming of the beam's
+//   k_solve  the listed beams, class by class: tangent angles of the hits, nearest-first claiming of the beam's
 //            angular sub-intervals, summed sin^2 waveform + argmax, relabel / move the point, label-1 statistics.
 //                                                                              (simulation.py:118-188, 231-295, 391-424)
 //
 // Design of k_solve (round 2; the round-1 kernel kept per-thread lists in local memory -- 180 MB of it across the
 // resident threads, thrashing L2 --, walked the bucket a second time, published one descriptor per waveform sample
 // lane-serially and evaluated a float64 sinpi per sample and pulse):
-//   * persistent grid, one warp = one tile of 32 listed beams, tiles handed out by an atomic cursor (the list is sorted
-//     costliest class first, so the tail is cheap tiles);
+//   * persistent grid, one warp = one tile of 32 listed beams of one work class, tiles handed out by an atomic cursor
+//     costliest class first (so the tail is cheap tiles);
 //   * NO local memory: the beams of a warp share a shared-memory arena of ARENA slots, allocated exactly
 //     (occluders + 1 per beam) with a warp scan of the counts the scan kernel delivered;
 //   * the hits are loaded COOPERATIVELY: arena slot s is filled by lane s mod 32, whatever beam it belongs to (owner by
@@ -113,14 +114,17 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     __shared__ int s_idx[SNOW_WARPS][32][SURV_CAP];                // plane-local particle index of each lane's survivors
     __shared__ unsigned s_hit[SNOW_WARPS][32];                     // bit r: survivor r of this lane is a hit
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int b = blockIdx.y, blk0 = blockIdx.x * SNOW_TPB, i = blk0 + threadIdx.x;
+    // this warp's tile from the plane-major schedule: the warps of a CTA may belong to different clouds (no block-wide
+    // barrier below)
+    const int st = blockIdx.x * SNOW_WARPS + wid;
+    if (st >= a.n_wtiles) return;
+    const unsigned long long se = a.sched[st];
+    const int b = (int)((se >> 32) & 0xffffu), w0 = (int)(unsigned)se;  // cloud, first row of this warp
     const int64_t beg = a.cloud_off[b];
     const int n = (int)(a.cloud_off[b + 1] - beg);
-    if (blk0 >= n) return;
+    const int i = w0 + lane;
     const bool active = i < n;
-    const int w0 = blk0 + 32 * wid;                                 // first row of this warp
-    const int nf_w = max(0, min(32, n - w0)) * 5;                   // floats of this warp's rows
-    if (nf_w <= 0) return;                                          // (whole warps only; no block-wide barrier below)
+    const int nf_w = min(32, n - w0) * 5;                           // floats of this warp's rows
     float px = 0, py = 0, pz = 0, pint = 0, pch = 0;
     {   // coalesced load of the warp's 32 rows (160 floats)
         const float *src = a.pts + (beg + w0) * 5;
@@ -253,13 +257,9 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
         }
         const int ltotal = __shfl_sync(FULL, lincl, 31);
         if (pm) {
-            int base = 0, hbase = 0;
+            int hbase = 0;
             const int leader = __ffs(pm) - 1;
-            if (lane == leader) {
-                base = atomicAdd(a.hdr, __popc(pm));
-                hbase = atomicAdd(a.hdr + 3, ltotal);
-            }
-            base = __shfl_sync(FULL, base, leader);
+            if (lane == leader) hbase = atomicAdd(a.hdr + 3, ltotal);
             hbase = __shfl_sync(FULL, hbase, leader);
             if (push) {
                 // work class = number of occluders (then far / near target): what a beam costs the solve kernel -- claiming,
@@ -271,10 +271,23 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
 #else
                 const int cls = LIST_CLASSES - 1 - min(LIST_CLASSES - 1, 2 * min(L, 63) + (d32 > 40.0f ? 1 : 0));
 #endif
-                const int slot = base + __popc(pm & ((1u << lane) - 1u));
+                // append to the class's bucket: number j in the class, warp-aggregated per class
+                const unsigned cm = __match_any_sync(pm, cls);
+                const int cl = __ffs(cm) - 1;
+                int j = 0;
+                if (lane == cl) j = atomicAdd(a.hdr + LIST_CLASSES + cls, __popc(cm));
+                j = __shfl_sync(cm, j, cl) + __popc(cm & ((1u << lane) - 1u));
+                // the beam that takes the first number of a chunk allocates it; the others wait for its id.  Every
+                // lane of the warp stores its allocations before any lane waits, and a warp allocates right after
+                // its numbers were handed out, so every awaited store is already on its way.
+                int *ct = a.chunk_tab + (int64_t)cls * a.chunks_per_class + j / LIST_CHUNK;
+                if (j % LIST_CHUNK == 0) atomicExch(ct, atomicAdd(a.hdr, 1) + 1);
+                __syncwarp(pm);
+                int chunk;
+                while ((chunk = *(volatile int *)ct) == 0) {}
                 const int hoff = hbase + lincl - L;
                 const bool fits = hoff + L <= a.hit_cap;        // position array full: the beam goes to the overflow kernel
-                if (slot < a.items_cap) {
+                {
                     SolveItem it;
                     it.key = ((unsigned long long)cls << 48) | ((unsigned long long)b << 32) | (unsigned)i;
                     it.hit_off = hoff;
@@ -282,7 +295,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
                     it.th32 = th32;
                     it.pad0 = 0;
                     it.pad1 = 0;
-                    a.items_out[slot] = it;
+                    a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK] = it;
                 }
                 if (fits) {
                     int *hp = a.hit_idx + hoff;                 // particle indices of the hits, in prefix (~ range) order
@@ -303,8 +316,6 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
                         }
                     }
                 }
-                const unsigned cm = __match_any_sync(pm, cls);
-                if (lane == __ffs(cm) - 1) atomicAdd(a.hdr + LIST_CLASSES + cls, __popc(cm));
             }
         }
     }
@@ -363,8 +374,27 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
     double *A0 = s_arena[wid][0], *A1 = s_arena[wid][1], *A2 = s_arena[wid][2], *A3 = s_arena[wid][3];
     unsigned long long *W = reinterpret_cast<unsigned long long *>(A2);
 
-    const int cnt = min(*a.count_in, a.cap_in);
-    const int n_tiles = (cnt + 31) >> 5;
+    // tiles in class order, costliest class first; a tile holds beams of one class only.  s_tile0[c] = first tile of
+    // class c, s_tile0[LIST_CLASSES] = number of tiles.
+    __shared__ int s_tile0[LIST_CLASSES + 1];
+    const int *cls_cnt = a.hdr + LIST_CLASSES;
+    if (wid == 0) {
+        int run = 0;
+        for (int c0 = 0; c0 < LIST_CLASSES; c0 += 32) {
+            const int v = (cls_cnt[c0 + lane] + 31) >> 5;
+            int incl = v;
+#pragma unroll
+            for (int sft = 1; sft < 32; sft <<= 1) {
+                const int t = __shfl_up_sync(FULL, incl, sft);
+                if (lane >= sft) incl += t;
+            }
+            s_tile0[c0 + lane] = run + incl - v;
+            run += __shfl_sync(FULL, incl, 31);
+        }
+        if (lane == 0) s_tile0[LIST_CLASSES] = run;
+    }
+    __syncthreads();
+    const int n_tiles = s_tile0[LIST_CLASSES];
     const double ctau = 299792458.0 * 1e-8;
     const double inv_step = (double)(LSS_M_EXT - 1) / (120 + ctau);
 
@@ -373,11 +403,18 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         if (lane == 0) tile = atomicAdd(tile_cursor, 1);
         tile = __shfl_sync(FULL, tile, 0);
         if (tile >= n_tiles) break;
-        const int slot = tile * 32 + lane;
-        const bool active = slot < cnt;
+        int cls = 0;                                        // the tile's class: last c with s_tile0[c] <= tile
+#pragma unroll
+        for (int step = LIST_CLASSES / 2; step; step >>= 1)
+            if (s_tile0[cls + step] <= tile) cls += step;
+        const int j = (tile - s_tile0[cls]) * 32 + lane;    // number of this lane's beam in its class
+        const bool active = j < cls_cnt[cls];
         SolveItem it;
         it.key = 0ull; it.hit_off = 0; it.L = 0; it.th32 = 0.0f; it.pad0 = 0; it.pad1 = 0;
-        if (active) it = a.items_in[slot];
+        if (active) {
+            const int chunk = a.chunk_tab[(int64_t)cls * a.chunks_per_class + j / LIST_CHUNK];
+            it = a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK];
+        }
         const int b = (int)((it.key >> 32) & 0xffffu);
         const int i = (int)(it.key & 0xffffffffu);
         const int64_t beg = a.cloud_off[b];
@@ -765,10 +802,9 @@ extern "C" lss_status lss_debug_azimuth(lss_engine *e, const float *d_y, const f
     return LSS_OK;
 }
 
-void lss_launch_scan(const DevArgs &a, int64_t max_rows, int n_clouds, cudaStream_t stream)
+void lss_launch_scan(const DevArgs &a, cudaStream_t stream)
 {
-    const dim3 grid((unsigned)((max_rows + SNOW_TPB - 1) / SNOW_TPB), (unsigned)n_clouds);
-    k_scan<<<grid, SNOW_TPB, 0, stream>>>(a);
+    k_scan<<<(unsigned)((a.n_wtiles + SNOW_WARPS - 1) / SNOW_WARPS), SNOW_TPB, 0, stream>>>(a);
 }
 
 void lss_launch_solve(const DevArgs &a, int *tile_cursor, int n_sm, cudaStream_t stream)
