@@ -5,14 +5,14 @@
 
 // One beam of the solve list, written by the scan kernel (32 bytes).  The scan has already walked the beam's whole
 // bucket prefix and tested every candidate exactly, so it hands over WHICH particles hit (their indices, in prefix
-// order, in the hit array) and the azimuth it used.
+// order, in the hit array), the azimuth it used and the beam's point and channel: the solve kernel never reads the
+// input row.
 struct __align__(16) SolveItem {
-    unsigned long long key;       // work class << 48 | cloud << 32 | row
+    unsigned long long key;       // channel << 56 | work class << 48 | cloud << 32 | row
     int hit_off;                  // first of the beam's L entries of hit_idx[]
     int L;                        // occluders
     float th32;                   // beam azimuth in [0, 2 pi) as the scan used it
-    int pad0;
-    long long pad1;
+    float px, py, pz;             // the input point
 };
 
 // argument block of the per-beam kernels (global type: it crosses translation units)
@@ -41,6 +41,11 @@ struct DevArgs {
     double div_rad;              // radians(beam_divergence)
     uint32_t flags;
     float *aug;                  // [N*5] augmented rows, input order
+    // keep record, input order: what k_keep decides on, so that it does not read whole rows.  The scan kernel writes all
+    // three for every row, the solve and overflow kernels rewrite keep_i / keep_tag of the beams they change.
+    float *keep_d;               // [N] original range d32
+    float *keep_i;               // [N] output intensity, rounded
+    uint8_t *keep_tag;           // [N] keep_tag_of(channel bin, label)
     uint8_t *code_keep;          // [N] channel bin of a kept row, 255 = dropped
     uint8_t *code_all;           // optional [N] channel bin of every row (un-filtered debug output)
     int32_t *nocc;               // optional [N], input order
@@ -106,6 +111,17 @@ __device__ __forceinline__ int channel_bin(float ch)
     int c = (int)ch;
     return (ch >= 0.0f && ch < 64.0f && (float)c == ch) ? c : LSS_N_CHANNELS;
 }
+
+// keep record tag: channel bin (0 .. 64) + NBINS * label, 195 values.  The label is that of the output row: 0, 1 or 2
+// for a valid channel.  A row with an invalid channel keeps its channel value as label; channel_bin() maps every integer
+// in [0, 64) -- 1.0f and 2.0f among them -- to a valid bin, so such a value is never 1.0f or 2.0f and the row is tagged
+// with label 0, which k_keep's tests (label == 1, label == 2) treat alike.
+__device__ __forceinline__ uint8_t keep_tag_of(int bin, float label)
+{
+    return (uint8_t)(bin + NBINS * (label == 2.0f ? 2 : (label == 1.0f ? 1 : 0)));
+}
+
+__device__ __forceinline__ int keep_tag_label(int tag) { return tag >= 2 * NBINS ? 2 : (tag >= NBINS ? 1 : 0); }
 
 __device__ __forceinline__ bool within(double diff, double tol)
 {

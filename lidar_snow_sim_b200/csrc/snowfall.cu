@@ -12,8 +12,8 @@
 //   k_solve          (solve.cu) the listed beams: nearest-first claiming of the beam's angular sub-intervals, summed
 //                    sin^2 waveform + argmax, relabel / move the point, label-1 statistics  (simulation.py:50-194, 231-424)
 //   k_overflow       beams with more than 63 occluders (rare): one beam per thread, per-thread lists of up to 128 hits
-//   k_keep           threshold (original range) + FOV keep flag, per-tile channel histogram of the kept rows,
-//                    num_attenuated / num_removed                                 (simulation.py:516-540)
+//   k_keep           threshold (original range) + FOV keep flag from the keep record the beam kernels wrote, per-tile
+//                    channel histogram of the kept rows, num_attenuated / num_removed   (simulation.py:516-540)
 //   k_tile_scan      per cloud: exclusive scan of the tile histograms -> destination of every (tile, channel) run;
 //                    kept-row count and stats (num_attenuated, num_removed, avg_intensity_diff)  (simulation.py:525-542)
 //   k_scatter        stable scatter of the kept rows to "sorted by channel, compacted" order -- the reference's
@@ -399,6 +399,8 @@ __global__ void __launch_bounds__(SNOW_TPB, 1) k_overflow(DevArgs a)
     if (counted) {
         float *row = a.aug + (beg + i) * 5;
         row[0] = out_x; row[1] = out_y; row[2] = out_z; row[3] = out_i; row[4] = out_l;
+        a.keep_i[beg + i] = out_i;                  // (keep_d, the original range, is the scan's)
+        a.keep_tag[beg + i] = keep_tag_of(ch, out_l);
     }
     // label-1 beams per channel and the sum of their new intensities (simulation.py:170): integer atomics, order
     // independent => bit-reproducible
@@ -498,9 +500,15 @@ __global__ void __launch_bounds__(256) k_sched_sort(const unsigned long long *__
 // keep pass: threshold filter on the ORIGINAL range (simulation.py:518-523), camera FOV filter (:532-537), per-tile
 // channel histograms for the scatter pass, num_attenuated / num_removed.  One CTA per tile of 1024 rows: the tile's
 // histogram rows are written, not accumulated, so they need no zero fill.  Runs after the beam kernels AND the
-// pre-pass (which may have run concurrently with them on another stream).
+// pre-pass (which may have run concurrently with them on another stream).  It reads the keep record the beam kernels
+// wrote (9 B per row instead of the input and the augmented row, 40 B); only the camera FOV filter reads the output
+// xyz from the augmented row.  KEEP_ROWS rows per thread (strided by the CTA: coalesced), all loaded before any is
+// decided, so that enough bytes are in flight for a pass this short.
 // ---------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(TILE) k_keep(DevArgs a)
+constexpr int KEEP_TPB = 256;
+constexpr int KEEP_ROWS = TILE / KEEP_TPB;
+
+__global__ void __launch_bounds__(KEEP_TPB) k_keep(DevArgs a)
 {
     __shared__ unsigned h_keep[NBINS], h_all[NBINS];
     __shared__ int s_cnt[2];
@@ -510,47 +518,60 @@ __global__ void __launch_bounds__(TILE) k_keep(DevArgs a)
     if (tile * TILE >= n) return;
     if (threadIdx.x < NBINS) { h_keep[threadIdx.x] = 0; h_all[threadIdx.x] = 0; }
     if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0;
-    __syncthreads();
-    const int i = tile * TILE + threadIdx.x;
-    const int lane = threadIdx.x & 31;
-    const bool active = i < n;
-    bool keep = false, att = false;
-    int ch = -1;
-    if (active) {
-        const float *in = a.pts + (beg + i) * 5;
-        const float *row = a.aug + (beg + i) * 5;
-        const float px = __ldcs(in), py = __ldcs(in + 1), pz = __ldcs(in + 2);
-        ch = channel_bin(__ldcs(in + 4));
-        const float out_x = row[0], out_y = row[1], out_z = row[2], out_i = row[3], out_l = row[4];
-        keep = true;
-        if (a.flags & LSS_FLAG_THRESHOLD_FILTER) {
-            const float d32 = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
-            const double d = (double)d32;
-            const double *p = a.thresh + 3 * b;
-            const double d2 = (double)__fmul_rn(d32, d32);
-            const double thr = __dadd_rn(__dadd_rn(__dmul_rn(p[0], d2), __dmul_rn(p[1], d)), p[2]);
-            keep = (out_l == 2.0f) || ((double)out_i > thr);
+    const bool thr_on = a.flags & LSS_FLAG_THRESHOLD_FILTER;
+    int tags[KEEP_ROWS];
+    float d32s[KEEP_ROWS], out_is[KEEP_ROWS];
+#pragma unroll
+    for (int k = 0; k < KEEP_ROWS; k++) {
+        const int i = tile * TILE + k * KEEP_TPB + threadIdx.x;
+        tags[k] = 0; d32s[k] = 0.0f; out_is[k] = 0.0f;
+        if (i < n) {
+            tags[k] = __ldcs(a.keep_tag + beg + i);
+            if (thr_on) { d32s[k] = __ldcs(a.keep_d + beg + i); out_is[k] = __ldcs(a.keep_i + beg + i); }
         }
-        att = keep && out_l == 1.0f && ch < LSS_N_CHANNELS;   // num_attenuated is counted BEFORE the FOV filter (:525)
-        if (keep && (a.flags & LSS_FLAG_CAMERA_FOV)) {
-            const float *M = a.camera->M, *P2 = a.camera->P2;
-            float rx = fmaf(out_z, M[6], fmaf(out_y, M[3], out_x * M[0])) + M[9];
-            float ry = fmaf(out_z, M[7], fmaf(out_y, M[4], out_x * M[1])) + M[10];
-            float rz = fmaf(out_z, M[8], fmaf(out_y, M[5], out_x * M[2])) + M[11];
-            float u = fmaf(rz, P2[2], fmaf(ry, P2[1], rx * P2[0])) + P2[3];
-            float v = fmaf(rz, P2[6], fmaf(ry, P2[5], rx * P2[4])) + P2[7];
-            float wd = fmaf(rz, P2[10], fmaf(ry, P2[9], rx * P2[8])) + P2[11];
-            u = u / rz;
-            v = v / rz;
-            const float depth = wd - P2[11];
-            keep = (u >= 0.0f) && (u < (float)a.camera->img_w) && (v >= 0.0f) && (v < (float)a.camera->img_h) &&
-                   (depth >= 0.0f);
-        }
-        a.code_keep[beg + i] = keep ? (uint8_t)ch : (uint8_t)255;
-        if (a.code_all) a.code_all[beg + i] = (uint8_t)ch;
     }
-    // warp-aggregated shared-memory histograms
-    {
+    double p0 = 0.0, p1 = 0.0, p2 = 0.0;
+    if (thr_on) { p0 = a.thresh[3 * b]; p1 = a.thresh[3 * b + 1]; p2 = a.thresh[3 * b + 2]; }
+    __syncthreads();
+    const int lane = threadIdx.x & 31;
+#pragma unroll
+    for (int k = 0; k < KEEP_ROWS; k++) {
+        const int i = tile * TILE + k * KEEP_TPB + threadIdx.x;
+        const bool active = i < n;
+        bool keep = false, att = false;
+        int ch = -1;
+        if (active) {
+            const int label = keep_tag_label(tags[k]);
+            ch = tags[k] - NBINS * label;
+            keep = true;
+            if (thr_on) {
+                const float d32 = d32s[k];
+                const double d = (double)d32;
+                const double d2 = (double)__fmul_rn(d32, d32);
+                const double thr = __dadd_rn(__dadd_rn(__dmul_rn(p0, d2), __dmul_rn(p1, d)), p2);
+                keep = (label == 2) || ((double)out_is[k] > thr);
+            }
+            att = keep && label == 1 && ch < LSS_N_CHANNELS;  // num_attenuated is counted BEFORE the FOV filter (:525)
+            if (keep && (a.flags & LSS_FLAG_CAMERA_FOV)) {
+                const float *row = a.aug + (beg + i) * 5;
+                const float out_x = row[0], out_y = row[1], out_z = row[2];
+                const float *M = a.camera->M, *P2 = a.camera->P2;
+                float rx = fmaf(out_z, M[6], fmaf(out_y, M[3], out_x * M[0])) + M[9];
+                float ry = fmaf(out_z, M[7], fmaf(out_y, M[4], out_x * M[1])) + M[10];
+                float rz = fmaf(out_z, M[8], fmaf(out_y, M[5], out_x * M[2])) + M[11];
+                float u = fmaf(rz, P2[2], fmaf(ry, P2[1], rx * P2[0])) + P2[3];
+                float v = fmaf(rz, P2[6], fmaf(ry, P2[5], rx * P2[4])) + P2[7];
+                float wd = fmaf(rz, P2[10], fmaf(ry, P2[9], rx * P2[8])) + P2[11];
+                u = u / rz;
+                v = v / rz;
+                const float depth = wd - P2[11];
+                keep = (u >= 0.0f) && (u < (float)a.camera->img_w) && (v >= 0.0f) && (v < (float)a.camera->img_h) &&
+                       (depth >= 0.0f);
+            }
+            a.code_keep[beg + i] = keep ? (uint8_t)ch : (uint8_t)255;
+            if (a.code_all) a.code_all[beg + i] = (uint8_t)ch;
+        }
+        // warp-aggregated shared-memory histograms
         const int ck = (active && keep) ? ch : -1;
         const unsigned mk = __match_any_sync(0xffffffffu, ck);
         if (ck >= 0 && lane == __ffs(mk) - 1) atomicAdd(&h_keep[ck], (unsigned)__popc(mk));
@@ -576,27 +597,46 @@ __global__ void __launch_bounds__(TILE) k_keep(DevArgs a)
 
 // ---------------------------------------------------------------------------------------------------------------------
 // tile scan: hist[tile][bin] -> exclusive destination offsets in (bin-major, tile-minor) order.  One CTA per cloud,
-// one warp per bin at a time, tiles scanned 32 at a time.
+// one warp per bin at a time, TSCAN_PER_LANE consecutive tiles per lane (one round of loads covers 128 tiles, a cloud
+// of 131 072 rows).  The kernel is a chain of dependent L2 round trips, so every phase issues its loads together: the
+// stats' per-channel terms are staged in shared memory next to the bin scans (thread 0 then sums them in channel order:
+// bit-reproducible), and the final pass loads TSCAN_ADD entries per thread before it stores any.
 // ---------------------------------------------------------------------------------------------------------------------
+constexpr int TSCAN_PER_LANE = 4;
+constexpr int TSCAN_ADD = 8;
+
 __global__ void __launch_bounds__(1024) k_tile_scan(unsigned *hist, const int32_t *__restrict__ tile_base,
                                                      int32_t *counts /* or null */, double *stats, const int *counters,
                                                      const unsigned *att_cnt, const unsigned long long *att_sum,
                                                      const SensorConst *sensor)
 {
     __shared__ unsigned bin_total[NBINS];
+    __shared__ double att_term[LSS_N_CHANNELS];
     const int b = blockIdx.x;
     const int n_tiles = tile_base[b + 1] - tile_base[b];
     unsigned *h = hist + (size_t)tile_base[b] * NBINS;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (stats && threadIdx.x < LSS_N_CHANNELS)
+        att_term[threadIdx.x] = (double)att_cnt[b * LSS_N_CHANNELS + threadIdx.x] * (0.9 * sensor->max_intensity[threadIdx.x]);
     for (int c = warp; c < NBINS; c += 32) {
         unsigned run = 0;
-        for (int t0 = 0; t0 < n_tiles; t0 += 32) {
-            const int t = t0 + lane;
-            const unsigned v = t < n_tiles ? h[(size_t)t * NBINS + c] : 0u;
-            unsigned incl = v;
+        for (int t0 = 0; t0 < n_tiles; t0 += 32 * TSCAN_PER_LANE) {
+            const int t = t0 + lane * TSCAN_PER_LANE;
+            unsigned v[TSCAN_PER_LANE], sum = 0;
+#pragma unroll
+            for (int q = 0; q < TSCAN_PER_LANE; q++) {
+                v[q] = t + q < n_tiles ? h[(size_t)(t + q) * NBINS + c] : 0u;
+                sum += v[q];
+            }
+            unsigned incl = sum;
 #pragma unroll
             for (int s = 1; s < 32; s <<= 1) { const unsigned o = __shfl_up_sync(0xffffffffu, incl, s); if (lane >= s) incl += o; }
-            if (t < n_tiles) h[(size_t)t * NBINS + c] = run + incl - v;
+            unsigned ex = run + incl - sum;
+#pragma unroll
+            for (int q = 0; q < TSCAN_PER_LANE; q++) {
+                if (t + q < n_tiles) h[(size_t)(t + q) * NBINS + c] = ex;
+                ex += v[q];
+            }
             run += __shfl_sync(0xffffffffu, incl, 31);
         }
         if (lane == 0) bin_total[c] = run;
@@ -610,8 +650,7 @@ __global__ void __launch_bounds__(1024) k_tile_scan(unsigned *hist, const int32_
             const int n_att = counters[2 * b], n_rem = counters[2 * b + 1];
             // intensity_diff_sum = sum over attenuated beams of (0.9 * max_intensity - new_i)   (simulation.py:140,170)
             double sum = 0.0;
-            for (int c = 0; c < LSS_N_CHANNELS; c++)
-                sum += (double)att_cnt[b * LSS_N_CHANNELS + c] * (0.9 * sensor->max_intensity[c]);
+            for (int c = 0; c < LSS_N_CHANNELS; c++) sum += att_term[c];
             sum -= (double)att_sum[b];
             stats[4 * b + 3] = sum;
             stats[4 * b + 0] = (double)n_att;
@@ -620,7 +659,20 @@ __global__ void __launch_bounds__(1024) k_tile_scan(unsigned *hist, const int32_
         }
     }
     __syncthreads();
-    for (int k = threadIdx.x; k < n_tiles * NBINS; k += blockDim.x) h[k] += bin_total[k % NBINS];
+    const int total = n_tiles * NBINS;
+    for (int k0 = threadIdx.x; k0 < total; k0 += TSCAN_ADD * blockDim.x) {
+        unsigned v[TSCAN_ADD];
+#pragma unroll
+        for (int q = 0; q < TSCAN_ADD; q++) {
+            const int k = k0 + q * blockDim.x;
+            v[q] = k < total ? h[k] : 0u;
+        }
+#pragma unroll
+        for (int q = 0; q < TSCAN_ADD; q++) {
+            const int k = k0 + q * blockDim.x;
+            if (k < total) h[k] = v[q] + bin_total[k % NBINS];
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -671,8 +723,8 @@ __global__ void __launch_bounds__(TILE) k_scatter(const float *__restrict__ aug,
 inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
 struct WsLayout {
-    int64_t aug, code_keep, code_all, nocc, hist_keep, hist_all, hist_rows, cloud_off, tile_base, order, thresh, counters,
-        counters_bytes, ovf, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
+    int64_t aug, keep_d, keep_i, keep_tag, code_keep, code_all, nocc, hist_keep, hist_all, hist_rows, cloud_off, tile_base,
+        order, thresh, counters, counters_bytes, ovf, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
 };
 
 WsLayout ws_layout(int64_t n_total, int n_clouds)
@@ -682,6 +734,9 @@ WsLayout ws_layout(int64_t n_total, int n_clouds)
     w.sched_tiles = n_total / 32 + (int64_t)n_clouds + 1;          // >= sum over clouds of ceil(n_b / 32)
     int64_t o = 0;
     w.aug = o;        o = align_up(o + n_total * 5 * 4, 256);
+    w.keep_d = o;     o = align_up(o + n_total * 4, 256);           // keep record: range | intensity | tag
+    w.keep_i = o;     o = align_up(o + n_total * 4, 256);
+    w.keep_tag = o;   o = align_up(o + n_total, 256);
     w.code_keep = o;  o = align_up(o + n_total, 256);
     w.code_all = o;   o = align_up(o + n_total, 256);
     w.nocc = o;       o = align_up(o + n_total * 4, 256);
@@ -820,6 +875,9 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.div_rad = div_rad;
     a.flags = s.flags;
     a.aug = d_aug;
+    a.keep_d = (float *)(ws + w.keep_d);
+    a.keep_i = (float *)(ws + w.keep_i);
+    a.keep_tag = (uint8_t *)(ws + w.keep_tag);
     a.code_keep = d_code_keep;
     a.code_all = d_code_all;
     a.nocc = d_nocc_tmp;
@@ -913,7 +971,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     if (ev_join) LSS_CUDA_CHECK(e, cudaStreamWaitEvent(stream, ev_join, 0));
     {
         KernelTimer kt(e, LSS_K_FINALIZE, stream);
-        k_keep<<<dim3(max_tiles, B), TILE, 0, stream>>>(a);
+        k_keep<<<dim3(max_tiles, B), KEEP_TPB, 0, stream>>>(a);
     }
     {
         KernelTimer kt(e, LSS_K_SORT, stream);

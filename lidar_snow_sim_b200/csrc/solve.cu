@@ -288,13 +288,15 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
                 const int hoff = hbase + lincl - L;
                 const bool fits = hoff + L <= a.hit_cap;        // position array full: the beam goes to the overflow kernel
                 {
-                    SolveItem it;
-                    it.key = ((unsigned long long)cls << 48) | ((unsigned long long)b << 32) | (unsigned)i;
+                    SolveItem it;           // (only beams with a valid channel walk a bucket: ch < 64)
+                    it.key = ((unsigned long long)ch << 56) | ((unsigned long long)cls << 48) |
+                             ((unsigned long long)b << 32) | (unsigned)i;
                     it.hit_off = hoff;
                     it.L = fits ? L : 0x7fff;
                     it.th32 = th32;
-                    it.pad0 = 0;
-                    it.pad1 = 0;
+                    it.px = px;
+                    it.py = py;
+                    it.pz = pz;
                     a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK] = it;
                 }
                 if (fits) {
@@ -319,13 +321,18 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
             }
         }
     }
-    // ---- rows back through shared memory (coalesced store); the listed beams' rows are rewritten by the solve kernel ------
+    // ---- rows back through shared memory (coalesced store) and the keep record; the listed beams' rows and records are
+    // rewritten by the solve kernel where it changes them ---------------------------------------------------------------
     __syncwarp();
     if (active) {
         float *row = &s_rows[wid][5 * lane];
-        row[3] = rintf(pint);                                       // np.round of the intensity column (simulation.py:516)
+        const float out_i = rintf(pint);                            // np.round of the intensity column (simulation.py:516)
+        row[3] = out_i;
         row[4] = out_l;
         if (a.nocc) a.nocc[beg + i] = 0;
+        a.keep_d[beg + i] = d32;
+        a.keep_i[beg + i] = out_i;
+        a.keep_tag[beg + i] = (uint8_t)ch;      // = keep_tag_of(ch, out_l): label 0 here (out_l is 0 or an invalid channel)
     }
     __syncwarp();
     {
@@ -410,24 +417,22 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         const int j = (tile - s_tile0[cls]) * 32 + lane;    // number of this lane's beam in its class
         const bool active = j < cls_cnt[cls];
         SolveItem it;
-        it.key = 0ull; it.hit_off = 0; it.L = 0; it.th32 = 0.0f; it.pad0 = 0; it.pad1 = 0;
+        it.key = 0ull; it.hit_off = 0; it.L = 0; it.th32 = 0.0f; it.px = 0.0f; it.py = 0.0f; it.pz = 0.0f;
         if (active) {
             const int chunk = a.chunk_tab[(int64_t)cls * a.chunks_per_class + j / LIST_CHUNK];
             it = a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK];
         }
+        // the item holds all the solve needs of the input row (the intensity only matters if the waveform is solved,
+        // and then it is replaced)
         const int b = (int)((it.key >> 32) & 0xffffu);
         const int i = (int)(it.key & 0xffffffffu);
-        const int64_t beg = a.cloud_off[b];
-        float px = 0, py = 0, pz = 0, pint = 0, pch = 0;
-        if (active) {
-            const float *row = a.pts + (beg + i) * 5;
-            px = row[0]; py = row[1]; pz = row[2]; pint = row[3]; pch = row[4];
-        }
+        const int ch = (int)(it.key >> 56);
+        const int64_t beg = a.cloud_off[b];                 // (issued here, its latency hides behind the solve)
+        const float px = it.px, py = it.py, pz = it.pz;
         // np.linalg.norm([x, y, z], axis=0) in float32: sqrt((x*x + y*y) + z*z), no FMA   (simulation.py:89)
         const float d32 = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
-        const int ch = channel_bin(pch);
 
-        float out_x = px, out_y = py, out_z = pz, out_i = pint, out_l = active ? 0.0f : pch;
+        float out_x = px, out_y = py, out_z = pz, out_i = 0.0f, out_l = 0.0f;
         long long att_new_i = -1;
         int n_claim = 0;
 
@@ -765,8 +770,15 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         // ---- np.round of the intensity column (simulation.py:516), store, label-1 statistics (simulation.py:170) ----------
         const bool counted = active && !deferred;          // a deferred beam is written by the overflow kernel
         if (counted) {
-            float *row = a.aug + (beg + i) * 5;
-            row[0] = out_x; row[1] = out_y; row[2] = out_z; row[3] = rintf(out_i); row[4] = out_l;
+            // label 1 or 2 <=> the waveform was solved; otherwise (no claiming particle, or a range-index error raised)
+            // the row and the record the scan wrote are final
+            if (out_l != 0.0f) {
+                const float ri = rintf(out_i);
+                float *row = a.aug + (beg + i) * 5;
+                row[0] = out_x; row[1] = out_y; row[2] = out_z; row[3] = ri; row[4] = out_l;
+                a.keep_i[beg + i] = ri;
+                a.keep_tag[beg + i] = keep_tag_of(ch, out_l);
+            }
             if (a.nocc) a.nocc[beg + i] = n_claim;
         }
         {
