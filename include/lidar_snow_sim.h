@@ -39,7 +39,7 @@ typedef enum {
     LSS_ERR_RANGE_INDEX = 4,      /* IndexError analogue: a waveform sample index >= 1230, i.e. a return beyond
                                      ~120 m on a beam that has occluders (simulation.py:149) */
     LSS_ERR_NEGATIVE_INTENSITY = 5,  /* AssertionError analogue (simulation.py:184) */
-    LSS_ERR_OCCLUDER_OVERFLOW = 6,   /* more than 128 occluders on one beam (or > 65536 beams with more than 24) */
+    LSS_ERR_OCCLUDER_OVERFLOW = 6,   /* more than 128 occluders on one beam */
     LSS_ERR_WORKSPACE = 7,        /* caller-supplied workspace too small */
     LSS_ERR_NO_SENSOR = 8,        /* AssertionError analogue: sensor constants missing (simulation.py:35,474-480) */
     LSS_ERR_TOO_FEW_GROUND = 9    /* TypeError analogue: fewer than 3 ground points, estimate_laser_parameters returns

@@ -1,5 +1,5 @@
 // beam.cuh -- argument block, constants and small device helpers shared by the per-beam kernels
-// (snowfall.cu: scan / overflow / keep / scatter; solve.cu: the dense solve kernel).
+// (snowfall.cu: schedule / keep / scatter; solve.cu: the scan and solve kernels).
 #pragma once
 #include "common.cuh"
 
@@ -9,7 +9,8 @@
 // input row.
 struct __align__(16) SolveItem {
     unsigned long long key;       // channel << 56 | work class << 48 | cloud << 32 | row
-    int hit_off;                  // first of the beam's L entries of hit_idx[]
+    int hit_off;                  // first of the beam's L entries of hit_idx[]; -1: the hit array was full, the solve
+                                  // kernel walks the bucket prefix again
     int L;                        // occluders
     float th32;                   // beam azimuth in [0, 2 pi) as the scan used it
     float px, py, pz;             // the input point
@@ -42,7 +43,7 @@ struct DevArgs {
     uint32_t flags;
     float *aug;                  // [N*5] augmented rows, input order
     // keep record, input order: what k_keep decides on, so that it does not read whole rows.  The scan kernel writes all
-    // three for every row, the solve and overflow kernels rewrite keep_i / keep_tag of the beams they change.
+    // three for every row, the solve kernel rewrites keep_i / keep_tag of the beams it changes.
     float *keep_d;               // [N] original range d32
     float *keep_i;               // [N] output intensity, rounded
     uint8_t *keep_tag;           // [N] keep_tag_of(channel bin, label)
@@ -57,28 +58,16 @@ struct DevArgs {
     unsigned *att_cnt;           // [B*64] label-1 beams per channel (all of them, simulation.py:170)
     unsigned long long *att_sum; // [B] sum of their new integer intensities
     int *status;
-    // work lists (cloud << 32 | row): the scan kernel defers every beam that has occluders to the dense solve kernel,
-    // which in turn defers beams with more than SOLVE_LCAP occluders to the overflow kernel
-    const unsigned long long *list_in;
-    const int *count_in;
-    int cap_in;
-    unsigned long long *list_out;
-    int *count_out;
-    int cap_out;
-    // solve list, bucketed by work class as the scan kernel writes it (no sort pass): the beams of class c are numbered
+    // solve list (every beam that has occluders), bucketed by work class as the scan kernel writes it (no sort pass): the beams of class c are numbered
     // 0, 1, ... in the order the scan appends them, and beam j sits in chunk j / LIST_CHUNK of the class, which is
     // items + (chunk_tab[c * chunks_per_class + j / LIST_CHUNK] - 1) * LIST_CHUNK (0 = chunk not allocated yet).
     // hdr = the list header ints (LIST_HDR_BYTES)
     SolveItem *items;
     int *chunk_tab;
     int chunks_per_class;
-    int *hdr;                    // [0] chunks allocated, [1] overflow beams, [2] tile cursor, [3] hit positions used, class counts
+    int *hdr;                    // [0] chunks allocated, [1] tile cursor, [2] hit positions used, class counts
     int *hit_idx;                // particle indices of the hits of the listed beams
     int hit_cap;
-    // optional by-product of the scan kernel for the concurrent pre-pass: the mounting-window points of calculate_plane
-    // (tools/wet_ground/planes.py:21-27) compacted per 32-row tile (prepass.cu, PrepassIO::window_staged)
-    float *win_stage;
-    int *win_tile_cnt;
     // plane-major schedule of the scan kernel: warp tile s of the launch is (cloud, first row) = sched[s] (cloud << 32 | row;
     // bits 48.. hold the sort key), warp tiles of the whole batch sorted by plane
     const unsigned long long *sched;
@@ -91,12 +80,7 @@ constexpr int SNOW_TPB = 128;
 constexpr int SNOW_WARPS = SNOW_TPB / 32;
 constexpr int TILE = 1024;                          // rows per scatter tile
 constexpr int NBINS = LSS_N_CHANNELS + 1;           // + "not a valid channel" (sorted last)
-constexpr int POOL = 128;                           // pulses a warp publishes per cooperative batch
-constexpr int CCAP = 512;                           // candidate samples a warp evaluates per cooperative batch
-constexpr int SLOW_CAP = 128;                       // occluders per beam held by the overflow kernel (per-thread lists)
-constexpr int OVF_LIST_CAP = 1 << 16;               // beams the overflow kernel can take per call
-constexpr int LIST_HDR_BYTES = 1024;  // ints: [0] chunks allocated, [1] overflow count, [2] tile cursor, [3] hit positions,
-                                      // [C..2C) class counts
+constexpr int LIST_HDR_BYTES = 1024;  // ints: [0] chunks allocated, [1] tile cursor, [2] hit positions, [C..2C) class counts
 constexpr int LIST_CLASSES = 128;     // solve list bucketed by work class (occluder count), costliest class first
 constexpr int LIST_CHUNK = 1024;      // solve items per chunk of a class (a multiple of 32: a solve tile is in one chunk)
 // scan schedule: warp tiles counting-sorted by the plane (mod SCHED_PLANES) of their first row's channel; rows without a
@@ -202,7 +186,7 @@ __device__ __forceinline__ float azimuth32(float yf, float xf)
 
 }  // namespace
 
-// solve.cu: the dense solve kernel over the (sorted) solve list; beams it cannot take (more than SOLVE_LCAP occluders or
-// a bucket prefix longer than it tracks) go to list_out for the overflow kernel.  hdr[2] is its tile cursor (zeroed).
+// solve.cu: the scan kernel over every beam, then the solve kernel over the class-bucketed solve list (tile_cursor: a
+// zeroed int, hdr[1]).
 void lss_launch_scan(const DevArgs &a, cudaStream_t stream);
 void lss_launch_solve(const DevArgs &a, int *tile_cursor, int n_sm, cudaStream_t stream);

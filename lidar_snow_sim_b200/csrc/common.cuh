@@ -301,21 +301,7 @@ struct PrepassIO {
     double *d_fit_out = nullptr;            // device [B*8]: lin slope, lin intercept, pmin slope, pmin intercept, ymax,
                                             //               n_ground, n_window, flat-earth fallback taken
     int32_t *d_ymins_out = nullptr;         // device [B*50] the picks used (-1: fewer than 3 ground points)
-    bool window_staged = false;             // the mounting-window points were compacted per 32-row tile by the caller's
-                                            // kernel already (snowfall scan kernel): skip k_window_tiles
 };
-// where the scan kernel of snowfall.cu has to put the per-tile compacted window points for `window_staged`
-void lss_prepass_window_staging(void *d_ws, int64_t n_total, int n_clouds, float **stage, int **tile_cnt);
-// the mounting window of calculate_plane (tools/wet_ground/planes.py:21-27); float32 comparisons, python floats are weak
-// scalars under NumPy 2
-__device__ __forceinline__ bool lss_in_window(float x, float y, float z)
-{
-    const float lim = __fsub_rn(-1.86f, __fmul_rn(0.01f, x));
-    return (z < -1.55f) && (z > lim) && (x > 10.0f) && (x < 70.0f) && (y > -3.0f) && (y < 3.0f);
-}
-// 32-row tiles of the window compaction: cloud b owns tiles [off[b] / 32 + b, ... + ceil(n_b / 32)) -- disjoint for
-// ragged clouds without a per-cloud table
-__device__ __forceinline__ int64_t lss_window_tile0(int64_t cloud_begin, int b) { return cloud_begin / 32 + b; }
 lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_cloud_off, const int32_t *d_cloud_cnt,
                            const int64_t *h_cloud_off, int n_clouds, double delta, double noise_floor, int flat_earth,
                            int range64, int raise_few_ground, const PrepassIO &io, void *d_ws, int64_t ws_bytes,

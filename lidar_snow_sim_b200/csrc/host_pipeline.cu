@@ -8,7 +8,7 @@
 // A batch is cut into chunks of whole clouds.  Per chunk, in stream order:
 //
 //   copy-in stream    H2D of the chunk's rows                                    (PCIe, ~50 GB/s)
-//   beam streams      scan / solve / overflow / keep / tile scan / scatter (snowfall.cu), chunks in order, lower
+//   beam streams      schedule / scan / solve / keep / tile scan / scatter (snowfall.cu), chunks in order, lower
 //                     priority; the pre-pass (prepass.cu) is forked by lss_snowfall_run onto the engine's high-priority
 //                     side streams and runs next to the beam kernels
 //   copy-out stream   D2H of the chunk's augmented rows, counts, stats

@@ -92,8 +92,18 @@ __device__ void block_sum(double (&v)[NV], double *smem /* [NV * warps] */)
 // k_window_gather (one CTA per cloud): scans the tile counts and gathers the few thousand points contiguously.
 constexpr int WTILE = 1024;
 
-// every warp compacts the window points of its 32 rows into the staging slot of those rows and writes their number:
-// 32-row tiles, the layout the snowfall scan kernel produces as a by-product (PrepassIO::window_staged)
+// the mounting window of calculate_plane (tools/wet_ground/planes.py:21-27); float32 comparisons, python floats are weak
+// scalars under NumPy 2
+__device__ __forceinline__ bool lss_in_window(float x, float y, float z)
+{
+    const float lim = __fsub_rn(-1.86f, __fmul_rn(0.01f, x));
+    return (z < -1.55f) && (z > lim) && (x > 10.0f) && (x < 70.0f) && (y > -3.0f) && (y < 3.0f);
+}
+// 32-row tiles of the window compaction: cloud b owns tiles [off[b] / 32 + b, ... + ceil(n_b / 32)) -- disjoint for
+// ragged clouds without a per-cloud table
+__device__ __forceinline__ int64_t lss_window_tile0(int64_t cloud_begin, int b) { return cloud_begin / 32 + b; }
+
+// every warp compacts the window points of its 32 rows into the staging slot of those rows and writes their number
 __global__ void __launch_bounds__(WTILE) k_window_tiles(PreArgs a)
 {
     const int b = blockIdx.y;
@@ -643,13 +653,6 @@ static PrepassLayout prepass_layout(int64_t n_total, int n_clouds)
 
 int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds) { return prepass_layout(n_total, n_clouds).total; }
 
-void lss_prepass_window_staging(void *d_ws, int64_t n_total, int n_clouds, float **stage, int **tile_cnt)
-{
-    const PrepassLayout L = prepass_layout(n_total, n_clouds);
-    *stage = (float *)((char *)d_ws + L.stage);
-    *tile_cnt = (int *)((char *)d_ws + L.tile_cnt);
-}
-
 // Runs the whole pre-pass for a batch.  d_poly_out / d_plane_out: device [B*3] / [B*4] (either may be null).
 // h_plane_in: optional host [B*4] (w0, w1, w2, h) to use instead of the RANSAC estimate.
 // d_cloudpre_out: optional device pointer receiving the address of the per-cloud CloudPre records (for wet ground).
@@ -711,10 +714,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
             k_set_plane<<<(B + 127) / 128, 128, 0, stream>>>(a, d_plane);
         } else {
             const int max_tiles = (int)std::max<int64_t>(1, (max_n + WTILE - 1) / WTILE);
-            if (!io.window_staged) {
-                k_window_tiles<<<dim3(max_tiles, B), WTILE, 0, stream>>>(a);
-                e->launches++;
-            }
+            k_window_tiles<<<dim3(max_tiles, B), WTILE, 0, stream>>>(a);
             const size_t gather_smem = sizeof(int) * ((size_t)max_tiles * (WTILE / 32) + 2);
             if (gather_smem > 48 * 1024)
                 LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_window_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gather_smem));
@@ -722,7 +722,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
             k_window_mad<<<B, 1024, 0, stream>>>(a);
             k_ransac_trials<<<dim3(RANSAC_T, B), PP_TPB, 0, stream>>>(a);
             k_ransac_refit<<<B, PP_TPB, 0, stream>>>(a);
-            e->launches += 3;
+            e->launches += 4;
         }
         k_ground_stats<<<dim3(nblk, B), PP_TPB, 0, stream>>>(a);
         k_ground_stats_final<<<B, 32, 0, stream>>>(a, nblk);

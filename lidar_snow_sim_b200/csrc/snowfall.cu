@@ -11,7 +11,6 @@
 //                    as long as its slowest lane, so a solve tile takes beams of one class)
 //   k_solve          (solve.cu) the listed beams: nearest-first claiming of the beam's angular sub-intervals, summed
 //                    sin^2 waveform + argmax, relabel / move the point, label-1 statistics  (simulation.py:50-194, 231-424)
-//   k_overflow       beams with more than 63 occluders (rare): one beam per thread, per-thread lists of up to 128 hits
 //   k_keep           threshold (original range) + FOV keep flag from the keep record the beam kernels wrote, per-tile
 //                    channel histogram of the kept rows, num_attenuated / num_removed   (simulation.py:516-540)
 //   k_tile_scan      per cloud: exclusive scan of the tile histograms -> destination of every (tile, channel) run;
@@ -26,392 +25,8 @@
 // waveform window and r^2) is computed in float32 with round-to-nearest, non-fused intrinsics so it is bit-identical;
 // the geometric narrow phase, the occlusion ratios and the waveform run in float64.
 #include "beam.cuh"
-#include <cstdlib>
-
-#define LSS_CHECK_STATUS(call) do { const lss_status _st = (call); if (_st != LSS_OK) return _st; } while (0)
 
 namespace {
-
-// Cold or bulky pieces are kept out of line and data-dependent loops are not unrolled: the beam kernel is
-// instruction-fetch sensitive (`no_inst` stalls grow with its SASS size), every instruction that is not
-// on the common path costs fetch bandwidth for all resident warps.
-// one waveform sample: sum over the pulses q0..q1 whose window contains k, in dict order (simulation.py:148-149)
-__device__ __noinline__ double waveform_sample(int k, double Rk, int q0, int q1, const double *amp, const double *r,
-                                               const int *ks, const int *ke)
-{
-    const double inv_ctau = 1.0 / (299792458.0 * 1e-8);
-    double v = 0.0;
-#pragma unroll 1
-    for (int q = q0; q <= q1; q++)
-        if (k >= ks[q] && k < ke[q]) {
-            const double sn = sinpi((Rk - r[q]) * inv_ctau);
-            v += amp[q] * (sn * sn);
-        }
-    return v;
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// overflow kernel: the beams the solve kernel's shared-memory arena cannot take (more than 63 occluders).  This is round
-// 1's per-beam kernel reduced to its list mode: it walks the bucket again, keeps per-thread lists (local memory) and
-// evaluates whole windows with a sinpi per sample -- slow, general, and only ever run on a handful of beams.
-// ---------------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(SNOW_TPB, 1) k_overflow(DevArgs a)
-{
-    constexpr int CAP = SLOW_CAP;
-    __shared__ double s_amp[SNOW_WARPS][POOL];
-    __shared__ double s_r[SNOW_WARPS][POOL];
-    __shared__ int s_win[SNOW_WARPS][POOL];
-    __shared__ unsigned s_cand[SNOW_WARPS][CCAP];                   // sample | first pulse << 11 | last pulse << 18 | lane << 25
-    __shared__ double s_best[SNOW_WARPS][32];
-    __shared__ int s_kbest[SNOW_WARPS][32];
-
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    // one listed beam per thread: the lanes of a warp may belong to different clouds
-    const int slot = blockIdx.x * SNOW_TPB + threadIdx.x;
-    const int cnt = min(*a.count_in, a.cap_in);
-    if (blockIdx.x * SNOW_TPB >= cnt) return;
-    const bool active = slot < cnt;
-    const unsigned long long it = active ? a.list_in[slot] : 0ull;
-    const int b = (int)((it >> 32) & 0xffffu);
-    const int i = (int)(it & 0xffffffffu);
-    const int64_t beg = a.cloud_off[b];
-    float px = 0, py = 0, pz = 0, pint = 0, pch = 0;
-    if (active) {
-        const float *row = a.pts + (beg + i) * 5;
-        px = row[0]; py = row[1]; pz = row[2]; pint = row[3]; pch = row[4];
-    }
-    // np.linalg.norm([x, y, z], axis=0) in float32: sqrt((x*x + y*y) + z*z), no FMA   (simulation.py:89)
-    const float d32 = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
-    const double d = (double)d32;
-
-    float out_x = px, out_y = py, out_z = pz, out_i = pint, out_l = pch;
-    long long att_new_i = -1;    // >= 0: this beam was attenuated (label 1) to this integer intensity
-    int n_claim = 0;
-    const int ch = channel_bin(pch);
-    const double ctau = 299792458.0 * 1e-8;
-
-    // per-beam lists (local memory): hits (a1, a2, range) -> after claiming: pulses (amplitude, range, window)
-    double ha1[CAP + 1], ha2[CAP], hr[CAP + 1];
-    int ks[CAP + 1], ke[CAP + 1];
-    bool deferred = false;       // only with a further overflow list (a.list_out): not used by the engine's launcher
-    int n_pulses = 0;            // > 0: this beam has a waveform to solve (claiming particles + hard target)
-
-    if (active && ch < LSS_N_CHANNELS) {
-        out_l = 0.0f;
-        // ---- beam limits (simulation.py:91-101) -------------------------------------------------------------------
-        float th32 = a.theta ? a.theta[beg + i] : azimuth32(py, px);
-        if (th32 < 0.0f) th32 = __fadd_rn(th32, 6.2831855f);
-        const double thd = (double)th32;
-        double right = thd - a.half_div, left = thd + a.half_div;
-        if (right < 0) right += LSS_TWO_PI;
-        if (left < 0) left += LSS_TWO_PI;
-        if (right > LSS_TWO_PI) right -= LSS_TWO_PI;
-        if (left > LSS_TWO_PI) left -= LSS_TWO_PI;
-        const bool straddle = right > left;
-
-        // ---- candidate scan: one azimuth bucket of this channel's plane -------------------------------------------
-        int L = 0;
-        bool overflow = false;
-        const int plane = a.order[b * LSS_N_CHANNELS + ch];
-        if (plane >= 0 && plane < a.n_planes && thd == thd) {
-            double thm = thd >= LSS_TWO_PI ? thd - LSS_TWO_PI : thd;
-            int bk = (int)(thm * a.inv_w);
-            bk = bk < 0 ? 0 : (bk >= a.n_buckets ? a.n_buckets - 1 : bk);
-            const float th_rel = (float)(thm - (bk + 0.5) * a.w);
-            const int32_t *bs = a.bucket_start + (int64_t)plane * (a.n_buckets + 1) + bk;
-            const int e0 = bs[0], e1 = bs[1];
-#pragma unroll 1
-            for (int e = e0; e < e1; e++) {
-                const EntryView en = lss_decode(__ldg(&a.entries[e]), a.zbase);
-                if (!(en.x < d32)) break;                       // sorted by range: nothing nearer follows
-                if (!(fabsf(en.y - th_rel) <= en.z)) continue;   // float32 broad phase (conservative)
-                const long long pi = a.plane_off[plane] + en.idx;
-                const ParticleRec *rp = a.rec + pi;
-                const double rho = rp->rho;
-                if (!(rho < d)) continue;                        // simulation.py:345 (strict, float64)
-                const double phi = rp->phi, alpha = rp->alpha;
-                // simulation.py:359-365 centre inside the beam
-                bool inside = (right <= phi) && (phi <= left);
-                if (straddle) inside = inside || ((right - LSS_TWO_PI <= phi) && (phi <= left)) ||
-                                       ((right <= phi) && (phi <= left + LSS_TWO_PI));
-                // simulation.py:371-385: disk crosses a limit ray  <=>  |phi - limit| < asin(r/rho)  (mod 2 pi)
-                const bool right_hit = within(right - phi, alpha);
-                const bool left_hit = within(left - phi, alpha);
-                if (!(inside || right_hit || left_hit)) continue;
-                if (L == CAP) { overflow = true; break; }
-                const double a1 = right_hit ? right : a.tan[pi].t_right;   // geometry.py:26-27
-                const double a2 = left_hit ? left : a.tan[pi].t_left;
-                int j = L - 1;                                   // insertion by range (np.argsort, :416)
-#pragma unroll 1
-                while (j >= 0 && hr[j] > rho) { ha1[j + 1] = ha1[j]; ha2[j + 1] = ha2[j]; hr[j + 1] = hr[j]; j--; }
-                ha1[j + 1] = a1; ha2[j + 1] = a2; hr[j + 1] = rho;
-                L++;
-            }
-        }
-        if (overflow) {
-            if (a.list_out == nullptr) {
-                raise_status(a.status, LSS_ERR_OCCLUDER_OVERFLOW);
-            } else {
-                const int slot = atomicAdd(a.count_out, 1);
-                if (slot < a.cap_out) a.list_out[slot] = ((unsigned long long)b << 32) | (unsigned)i;
-                else raise_status(a.status, LSS_ERR_OCCLUDER_OVERFLOW);
-                deferred = slot < a.cap_out;
-            }
-        }
-        if (L > 0 && !overflow) {
-            // ---- compute_occlusion_dict (simulation.py:231-295) ---------------------------------------------------
-            // The reference splits the beam into elementary sub-intervals between all sorted end points and lets the
-            // particles claim, nearest first, every still-unclaimed piece inside their own interval.  Equivalent
-            // formulation used here: keep the union of the intervals claimed so far as a list of disjoint, non-touching
-            // intervals; a particle claims |[a1,a2]| - |[a1,a2] n union| and is dropped iff [a1,a2] is contained in
-            // one union interval (or a1 >= a2, the reference's empty range(i1, i2)).  The hard target gets what is left
-            // between the smallest and the largest end point -- including the ~2 pi gap of the seam quirk.
-            double rb = right;
-            if (straddle) {
-                rb = right - LSS_TWO_PI;
-#pragma unroll 1
-                for (int j = 0; j < L; j++) if (ha1[j] > ha2[j]) ha1[j] -= LSS_TWO_PI;
-            }
-            double ulo[CAP], uhi[CAP];
-            int nu = 0;
-            double ep_min = fmin(rb, left), ep_max = fmax(rb, left), claimed_total = 0.0;
-            int P = 0;          // pulses: claiming particles in range order, then the hard target
-#pragma unroll 1
-            for (int j = 0; j < L; j++) {
-                const double lo = ha1[j], hi = ha2[j];
-                ep_min = fmin(ep_min, fmin(lo, hi));
-                ep_max = fmax(ep_max, fmax(lo, hi));
-                if (!(lo < hi)) continue;
-                bool contained = false;
-                double cov = 0.0;
-#pragma unroll 1
-                for (int u = 0; u < nu; u++) {
-                    contained |= (ulo[u] <= lo) && (hi <= uhi[u]);
-                    const double ov = fmin(hi, uhi[u]) - fmax(lo, ulo[u]);
-                    if (ov > 0.0) cov += ov;
-                }
-                if (contained) continue;
-                const double claimed = (hi - lo) - cov;
-                claimed_total += claimed;
-                double nlo = lo, nhi = hi;      // merge [lo, hi] into the union (absorb overlapping / touching pieces)
-                int w = 0;
-#pragma unroll 1
-                for (int u = 0; u < nu; u++) {
-                    if (ulo[u] <= hi && uhi[u] >= lo) {
-                        nlo = fmin(nlo, ulo[u]);
-                        nhi = fmax(nhi, uhi[u]);
-                    } else {
-                        ulo[w] = ulo[u]; uhi[w] = uhi[u]; w++;
-                    }
-                }
-                ulo[w] = nlo; uhi[w] = nhi;
-                nu = w + 1;
-                double ratio = claimed / a.div_rad;
-                ratio = ratio < 0 ? 0 : (ratio > 1 ? 1 : ratio);
-                hr[P] = hr[j];          // P <= j: safe in place
-                ha1[P] = ratio;
-                P++;
-            }
-            n_claim = P;
-            double ratio_hard = ((ep_max - ep_min) - claimed_total) / a.div_rad;
-            ratio_hard = ratio_hard < 0 ? 0 : (ratio_hard > 1 ? 1 : ratio_hard);
-
-            if (P > 0) {
-                // ---- pulses of the waveform (simulation.py:137-149) -------------------------------------------------
-                const double beta_0 = 1 * 1e-06 / LSS_PI;
-                const double i_orig = 0.9 * a.sensor->max_intensity[ch];
-                const double A = (i_orig / beta_0) * beta_0;        // CA_P0 * beta_0 (quirk: every pulse uses it)
-                double *amp = ha1, *rj = hr;                         // reuse the hit arrays
-                bool bad = false;
-#pragma unroll 1
-                for (int j = 0; j < P; j++) {
-                    const double r = rj[j];
-                    ks[j] = (int)ceil(r * 10);
-                    ke[j] = (int)(floor((r + ctau) * 10) + 1);
-                    amp[j] = (A * amp[j] * xsi64(r)) / (r * r);
-                    bad |= (ke[j] > LSS_M_EXT) || (ks[j] < 0);
-                }
-                {   // hard target: r_j is float32 => float32 index arithmetic and r^2 (SURVEY.md App. D)
-                    ks[P] = (int)ceilf(__fmul_rn(d32, 10.0f));
-                    ke[P] = (int)(floorf(__fmul_rn(__fadd_rn(d32, (float)ctau), 10.0f)) + 1.0f);
-                    rj[P] = d;
-                    amp[P] = (A * ratio_hard * xsi32(d32)) / (double)__fmul_rn(d32, d32);
-                    bad |= (ke[P] > LSS_M_EXT) || (ks[P] < 0);
-                }
-                if (bad) raise_status(a.status, LSS_ERR_RANGE_INDEX);
-                else n_pulses = P + 1;
-            }
-        }
-    }
-
-    // ---- argmax of the summed waveform (simulation.py:148-153), warp-cooperative ------------------------------------
-    // Only samples inside some pulse window are non-zero.  Pulses whose windows overlap form a group whose samples are
-    // summed in full (in dict order, like the reference's i[k] +=); an isolated pulse A sin^2(pi (R - r)/(c tau)) is
-    // unimodal and symmetric about r + c tau / 2, so its maximum over the grid is at one of the three samples around
-    // the sample nearest to the peak.  Every lane publishes its pulses and one descriptor per candidate sample in the
-    // warp's pool; the candidates of all beams of the warp are then evaluated 32 at a time and reduced per beam with a
-    // segmented scan (first maximum wins, np.argmax).
-    const double inv_step = (double)(LSS_M_EXT - 1) / (120 + ctau);
-    const double inv_ctau = 1.0 / ctau;
-    // candidate segments of this beam: calls f(k_lo, k_hi, first pulse, last pulse) in ascending sample order
-    auto for_each_segment = [&](auto &&f) {
-        int j = 0;
-        while (j < n_pulses) {
-            int g1 = j, k_lo = ks[j], k_hi = ke[j];
-            while (g1 + 1 < n_pulses && ks[g1 + 1] < k_hi) {
-                g1++;
-                k_lo = min(k_lo, ks[g1]);
-                k_hi = max(k_hi, ke[g1]);
-            }
-            if (g1 == j) {
-                const int k0 = (int)rint((hr[j] + ctau / 2) * inv_step);
-                k_lo = max(k_lo, k0 - 1);
-                k_hi = min(k_hi, k0 + 2);
-            }
-            if (k_hi > k_lo) f(k_lo, k_hi, j, g1);
-            j = g1 + 1;
-        }
-    };
-    int T_all = 0;
-    if (n_pulses > 0) for_each_segment([&](int k_lo, int k_hi, int, int) { T_all += k_hi - k_lo; });
-    double best = 0.0;
-    int kbest = 0;
-    bool coop = n_pulses > 0;
-    if (T_all > CCAP || n_pulses > POOL) {   // pathological beam (dozens of overlapping pulses): solve it in this thread
-        coop = false;
-        for_each_segment([&](int k_lo, int k_hi, int j0, int j1) {
-#pragma unroll 1
-            for (int k = k_lo; k < k_hi; k++) {
-                const double v = waveform_sample(k, __ldg(&a.R[k]), j0, j1, ha1, hr, ks, ke);
-                if (v > best) { best = v; kbest = k; }
-            }
-        });
-    }
-    s_best[wid][lane] = 0.0;
-    s_kbest[wid][lane] = 0;
-    unsigned remaining = __ballot_sync(0xffffffffu, coop);
-    while (remaining) {
-        const bool rem = (remaining >> lane) & 1u;
-        const int mine = rem ? n_pulses : 0, myT = rem ? T_all : 0;
-        int incl = mine, cincl = myT;
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) {
-            const int t = __shfl_up_sync(0xffffffffu, incl, s);
-            const int u = __shfl_up_sync(0xffffffffu, cincl, s);
-            if (lane >= s) { incl += t; cincl += u; }
-        }
-        // a prefix of the remaining lanes (each has <= 49 pulses and <= CCAP candidates)
-        const bool in_batch = rem && incl <= POOL && cincl <= CCAP;
-        const unsigned batch = __ballot_sync(0xffffffffu, in_batch);
-        remaining &= ~batch;
-        const int total = __shfl_sync(0xffffffffu, cincl, 31 - __clz(batch));
-        if (in_batch) {
-            const int poff = incl - mine;
-            int coff = cincl - myT;
-#pragma unroll 1
-            for (int j = 0; j < mine; j++) {
-                s_amp[wid][poff + j] = ha1[j];
-                s_r[wid][poff + j] = hr[j];
-                s_win[wid][poff + j] = ks[j] | (ke[j] << 16);
-            }
-            for_each_segment([&](int k_lo, int k_hi, int j0, int j1) {
-                const unsigned hi_bits = ((unsigned)(poff + j0) << 11) | ((unsigned)(poff + j1) << 18) | ((unsigned)lane << 25);
-#pragma unroll 4
-                for (int k = k_lo; k < k_hi; k++) s_cand[wid][coff++] = (unsigned)k | hi_bits;
-            });
-        }
-        __syncwarp();
-        for (int base = 0; base < total; base += 32) {
-            const int c = base + lane;
-            int owner = -1, k = 0;
-            double v = 0.0;
-            if (c < total) {
-                const unsigned desc = s_cand[wid][c];
-                k = desc & 2047u;
-                owner = desc >> 25;
-                const int q0 = (desc >> 11) & 127u, q1 = (desc >> 18) & 127u;
-                const double Rk = __ldg(&a.R[k]);
-#pragma unroll 1
-                for (int q = q0; q <= q1; q++) {
-                    const int wn = s_win[wid][q];
-                    if (k >= (wn & 0xffff) && k < (wn >> 16)) {
-                        // sin(pi (R - r) / (c tau)) of simulation.py:549, as sinpi of the normalised offset
-                        const double sn = sinpi((Rk - s_r[wid][q]) * inv_ctau);
-                        v += s_amp[wid][q] * (sn * sn);      // pulses in dict order, like the reference's i[k] +=
-                    }
-                }
-            }
-            // per-beam argmax over the lanes holding candidates of the same beam: peer groups by beam, then three
-            // integer reductions (non-negative doubles order like their bit patterns): max high word, max low word
-            // among those, min sample index among the exact ties -> the first maximum, like np.argmax
-            const unsigned peers = __match_any_sync(0xffffffffu, owner);
-            const unsigned long long vb = (unsigned long long)__double_as_longlong(v);
-            const unsigned vhi = (unsigned)(vb >> 32), vlo = (unsigned)vb;
-            const unsigned mhi = __reduce_max_sync(peers, vhi);
-            const unsigned mlo = __reduce_max_sync(peers, vhi == mhi ? vlo : 0u);
-            const bool is_max = (vhi == mhi) && (vlo == mlo);
-            const unsigned kmin = __reduce_min_sync(peers, is_max ? (unsigned)k : 0xffffffffu);
-            if (owner >= 0 && lane == __ffs(peers) - 1) {
-                const double vmax = __longlong_as_double((long long)(((unsigned long long)mhi << 32) | mlo));
-                if (vmax > s_best[wid][owner]) { s_best[wid][owner] = vmax; s_kbest[wid][owner] = (int)kmin; }
-            }
-            __syncwarp();
-        }
-    }
-    if (coop) {
-        best = s_best[wid][lane];
-        kbest = best > 0.0 ? s_kbest[wid][lane] : 0;
-    }
-
-    if (n_pulses > 0) {
-        // ---- new range / intensity / label (simulation.py:151-188) -------------------------------------------------
-        const double max_i = a.sensor->max_intensity[ch];
-        const double min_i = a.sensor->min_intensity[ch];
-        const double d_max = ((double)kbest / 10) - (ctau / 2);
-        const double q1 = 1 - d_max / 120;
-        double i_max = best + max_i * a.sensor->focal_slope[ch] * fabs(a.sensor->focal_offset[ch] - q1 * q1);
-        i_max = i_max < min_i ? min_i : (i_max > max_i ? max_i : i_max);
-        const long long new_i = (long long)i_max;       // int(): truncation
-        if (fabs(d_max - d) < 2 * (1.0 / 10)) {
-            out_l = 1.0f;
-            att_new_i = new_i;                          // intensity_diff_sum += i_orig - new_i   (simulation.py:170)
-        } else {
-            out_l = 2.0f;
-            const double sc = d_max / d;
-            out_x = (float)((double)px * sc);
-            out_y = (float)((double)py * sc);
-            out_z = (float)((double)pz * sc);
-        }
-        if (new_i < 0) raise_status(a.status, LSS_ERR_NEGATIVE_INTENSITY);
-        double ci = (double)new_i;
-        ci = ci < min_i ? min_i : (ci > max_i ? max_i : ci);
-        out_i = (float)ci;
-    }
-
-    // ---- np.round of the intensity column (simulation.py:516); the threshold / FOV filters, which need the pre-pass
-    // polynomial, are applied by k_keep so that the pre-pass can run next to the beam kernels -------------------------
-    if (active) {
-        out_i = rintf(out_i);
-        if (!deferred && a.nocc) a.nocc[beg + i] = n_claim;
-    }
-    const bool counted = active && !deferred;      // a deferred beam is accounted for by the overflow kernel
-    // one unrelated beam per thread: plain stores; integer atomics aggregated over lanes hitting the same counter
-    if (counted) {
-        float *row = a.aug + (beg + i) * 5;
-        row[0] = out_x; row[1] = out_y; row[2] = out_z; row[3] = out_i; row[4] = out_l;
-        a.keep_i[beg + i] = out_i;                  // (keep_d, the original range, is the scan's)
-        a.keep_tag[beg + i] = keep_tag_of(ch, out_l);
-    }
-    // label-1 beams per channel and the sum of their new intensities (simulation.py:170): integer atomics, order
-    // independent => bit-reproducible
-    const bool on = counted && att_new_i >= 0;
-    const int key = b * LSS_N_CHANNELS + (ch < LSS_N_CHANNELS ? ch : 0);
-    const unsigned mk = __match_any_sync(0xffffffffu, on ? key : -1);
-    if (on && lane == __ffs(mk) - 1) atomicAdd(a.att_cnt + key, (unsigned)__popc(mk));
-    const unsigned m = __match_any_sync(0xffffffffu, on ? b : -1);
-    const unsigned sum = __reduce_add_sync(m, on ? (unsigned)att_new_i : 0u);
-    if (on && lane == __ffs(m) - 1) atomicAdd(&a.att_sum[b], (unsigned long long)sum);
-}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // plane-major schedule of the scan kernel.  Every cloud maps its 64 channels onto the planes through order[], so in input
@@ -724,7 +339,7 @@ inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
 struct WsLayout {
     int64_t aug, keep_d, keep_i, keep_tag, code_keep, code_all, nocc, hist_keep, hist_all, hist_rows, cloud_off, tile_base,
-        order, thresh, counters, counters_bytes, ovf, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
+        order, thresh, counters, counters_bytes, list, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
 };
 
 WsLayout ws_layout(int64_t n_total, int n_clouds)
@@ -749,12 +364,11 @@ WsLayout ws_layout(int64_t n_total, int n_clouds)
     // counters: int[B*2] | unsigned att_cnt[B*64] | unsigned long long att_sum[B]
     w.counters_bytes = align_up((int64_t)n_clouds * 2 * 4, 8) + (int64_t)n_clouds * LSS_N_CHANNELS * 4 + (int64_t)n_clouds * 8;
     w.counters = o;   o = align_up(o + w.counters_bytes, 256);
-    // list header | overflow list | solve list chunks (every beam may have occluders; each class leaves at most one chunk
-    // partly filled)
+    // list header | solve list chunks (every beam may have occluders; each class leaves at most one chunk partly filled)
     //   | hit particle indices (int32; HIT_POS_PER_BEAM per beam of the batch on average: the surveyed densities give 1-5 occluders
     //   on a third of the beams)
     w.chunks_per_class = (n_total + LIST_CHUNK - 1) / LIST_CHUNK;
-    w.ovf = o;        o = align_up(o + LIST_HDR_BYTES + (int64_t)OVF_LIST_CAP * 8 +
+    w.list = o;       o = align_up(o + LIST_HDR_BYTES +
                                    (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK * (int64_t)sizeof(SolveItem) +
                                    (n_total * HIT_POS_PER_BEAM + 4096) * 4, 256);
     // chunk table of the solve list: LIST_CLASSES x chunks_per_class ids
@@ -835,7 +449,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS, stream));
     if (s.h_thresh_poly && !s.d_thresh_poly)
         LSS_CUDA_CHECK(e, lss_stage_upload(e, d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B, stream));
-    int *d_counts2 = (int *)(ws + w.ovf);                                   // list header (LIST_HDR_BYTES)
+    int *d_list_hdr = (int *)(ws + w.list);                                 // (LIST_HDR_BYTES)
     {
         ZeroRegions z;
         z.add(d_counters, w.counters_bytes);
@@ -845,7 +459,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
             return LSS_OK;
         }
-        z.add(d_counts2, LIST_HDR_BYTES);                 // (the tile histograms are written whole by k_keep)
+        z.add(d_list_hdr, LIST_HDR_BYTES);                 // (the tile histograms are written whole by k_keep)
         z.add(ws + w.chunk_tab, (size_t)LIST_CLASSES * w.chunks_per_class * 4);
         z.add(ws + w.sched, (size_t)SCHED_BINS * 2 * 4);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
@@ -889,35 +503,26 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.att_cnt = d_att_cnt;
     a.att_sum = d_att_sum;
     a.status = e->d_status;
-    unsigned long long *d_ovf_list = (unsigned long long *)(ws + w.ovf + LIST_HDR_BYTES);
-    SolveItem *d_solve_list = (SolveItem *)(d_ovf_list + OVF_LIST_CAP);   // (chunks_per_class + LIST_CLASSES) chunks
+    SolveItem *d_solve_list = (SolveItem *)(ws + w.list + LIST_HDR_BYTES);   // (chunks_per_class + LIST_CLASSES) chunks
     a.hit_idx = (int *)(d_solve_list + (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK);
     // Device pre-pass: plane + laser parameters + threshold polynomial (simulation.py:449-467), on the cloud as given.
     // Only k_keep needs its result, so it runs on one of the engine's high-priority side streams next to the beam kernels (a
-    // chain of small latency-bound kernels).
+    // chain of small latency-bound kernels).  It is forked before the scan, whose CTAs retire continuously: the persistent
+    // solve kernel holds every SM's registers until its last tile, so a chain forked after the scan would find no room for
+    // its 1024-thread CTAs and become the critical path.
     const bool device_prepass = (s.flags & LSS_FLAG_THRESHOLD_FILTER) && (s.flags & LSS_FLAG_DEVICE_PREPASS) &&
                                 !s.h_thresh_poly && !s.d_thresh_poly;
-    // Where to fork it: the persistent solve kernel holds every SM's registers until its last tile, so a chain forked
-    // AFTER the scan (which would let the scan kernel compact the mounting-window points as a by-product,
-    // PrepassIO::window_staged) finds no room for its 1024-thread CTAs and becomes the critical path.  Default: fork before the scan, whose CTAs retire continuously; LSS_FUSE_WINDOW=1 selects
-    // the other order for experiments.
-    static const bool fuse_window_env = getenv("LSS_FUSE_WINDOW") && getenv("LSS_FUSE_WINDOW")[0] == '1';
-    const bool fuse_window = fuse_window_env && !s.h_plane_in;
-    a.win_stage = nullptr;
-    a.win_tile_cnt = nullptr;
-    if (device_prepass && fuse_window) lss_prepass_window_staging(ws + w.prepass, N, B, &a.win_stage, &a.win_tile_cnt);
     cudaEvent_t ev_join = nullptr;
-    auto fork_prepass = [&]() -> lss_status {
+    if (device_prepass) {
         cudaStream_t side = nullptr;
         cudaEvent_t ev_fork = nullptr;
         LSS_CUDA_CHECK(e, lss_side_stream(e, &side, &ev_fork, &ev_join));
-        LSS_CUDA_CHECK(e, cudaEventRecord(ev_fork, stream));        // (with fuse_window: after the scan has staged the window points)
+        LSS_CUDA_CHECK(e, cudaEventRecord(ev_fork, stream));
         LSS_CUDA_CHECK(e, cudaStreamWaitEvent(side, ev_fork, 0));
         PrepassIO io;
         io.h_plane_in = s.h_plane_in;
         io.h_ymins_in = s.h_ymins_in;
         io.d_poly_out = d_thresh;
-        io.window_staged = a.win_stage != nullptr;
         lss_status ps = lss_prepass_run(e, s.d_points, d_off, nullptr, s.h_cloud_offsets, B, 0.5, s.noise_floor, 0, 0, 1,
                                 io, ws + w.prepass, w.prepass_bytes, nullptr, side);
         const cudaError_t je = cudaEventRecord(ev_join, side);
@@ -925,16 +530,12 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             cudaStreamWaitEvent(stream, ev_join, 0);                // never leave the side stream dangling
             return ps != LSS_OK ? ps : lss_fail(e, LSS_ERR_CUDA, "event record failed");
         }
-        return LSS_OK;
-    };
-    if (device_prepass && !fuse_window) LSS_CHECK_STATUS(fork_prepass());
+    }
     a.hit_cap = (int)std::min<int64_t>(N * HIT_POS_PER_BEAM + 4096, 0x7fffffff);
     {
         KernelTimer kt(e, LSS_K_SNOWFALL, stream);
-        // 1. scan: all beams; the ones without occluders are finished, the others go to the solve list with their hit masks
-        a.list_in = nullptr; a.count_in = nullptr; a.cap_in = 0;
-        a.list_out = nullptr; a.count_out = nullptr; a.cap_out = 0;
-        a.hdr = d_counts2;
+        // 1. scan: all beams; the ones without occluders are finished, the others go to the solve list with their hits
+        a.hdr = d_list_hdr;
         a.items = d_solve_list;
         a.chunk_tab = (int *)(ws + w.chunk_tab);
         a.chunks_per_class = (int)w.chunks_per_class;
@@ -947,7 +548,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
                 s.d_points, d_off, d_order, d_tile_base + B + 1, d_ent, d_sched_hist);
             k_sched_sort<<<(unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)), 256, 0, stream>>>(
                 d_ent, d_sched, d_sched_hist, n_wtiles);
-            e->launches += 2;
+            e->launches++;                                  // (the other one is counted by the LSS_K_SNOWFALL bracket)
             a.sched = d_sched;
             a.n_wtiles = n_wtiles;
         }
@@ -955,18 +556,11 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             KernelTimer ks(e, LSS_K_SCAN, stream);
             lss_launch_scan(a, stream);
         }
-        if (device_prepass && fuse_window) LSS_CHECK_STATUS(fork_prepass());
         // 2. solve: the listed beams, class by class, one warp per tile of 32 (persistent grid)
-        a.list_out = d_ovf_list; a.count_out = d_counts2 + 1; a.cap_out = OVF_LIST_CAP;
         {
             KernelTimer ks(e, LSS_K_SOLVE, stream);
-            lss_launch_solve(a, d_counts2 + 2, e->n_sm, stream);
+            lss_launch_solve(a, d_list_hdr + 1, e->n_sm, stream);
         }
-        // 3. overflow: beams with more occluders than the solve kernel's arena takes per beam (rare), round-1 list kernel
-        a.list_in = d_ovf_list; a.count_in = d_counts2 + 1; a.cap_in = OVF_LIST_CAP;
-        a.list_out = nullptr; a.count_out = nullptr; a.cap_out = 0;
-        k_overflow<<<OVF_LIST_CAP / SNOW_TPB, SNOW_TPB, 0, stream>>>(a);   // (scan, solve, overflow: one launch counted
-                                                                            // by each of the three KernelTimer brackets)
     }
     if (ev_join) LSS_CUDA_CHECK(e, cudaStreamWaitEvent(stream, ev_join, 0));
     {

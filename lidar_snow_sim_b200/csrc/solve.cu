@@ -30,8 +30,8 @@
 //     dict order like the reference's i[k] +=; first maximum wins, np.argmax -- instead of whole windows; the pieces of
 //     all 32 beams are handled one per lane, with uniform code.
 //
-// Beams the arena cannot take (more than SOLVE_LCAP occluders) go to the overflow list and are redone by the
-// overflow kernel (snowfall.cu, k_overflow: round 1's list kernel), which has no such limit below 128.
+// A beam takes up to SOLVE_LCAP = 128 occluders, the engine's hard cap: more raise LSS_ERR_OCCLUDER_OVERFLOW.  A beam
+// whose hit indices the scan could not store (hit array full) has its bucket prefix walked again by its own lane.
 #include "beam.cuh"
 
 namespace {
@@ -46,7 +46,8 @@ constexpr int SOLVE_WARPS = SOLVE_TPB / 32;
 #endif
 constexpr int SOLVE_CTAS_PER_SM = LSS_SOLVE_CTAS;
 constexpr int ARENA = LSS_SOLVE_ARENA;                 // slots per warp: sum over the 32 beams of (occluders + 1); more -> extra round
-constexpr int SOLVE_LCAP = 63;             // occluders per beam handled here (needs LCAP + 1 <= ARENA)
+constexpr int SOLVE_LCAP = 128;            // occluders per beam (LSS_ERR_OCCLUDER_OVERFLOW above)
+static_assert(SOLVE_LCAP + 1 <= ARENA, "a beam with SOLVE_LCAP occluders must fit a round of the arena on its own");
 constexpr unsigned FULL = 0xffffffffu;
 
 struct Beam {                              // what the narrow phase needs of a beam
@@ -81,6 +82,48 @@ __device__ __forceinline__ bool exact_hit(const ParticleRec *rp, const Beam &bm,
     return inside || right_hit || left_hit;
 }
 
+// the beam's azimuth bucket of its channel's plane: entries e0 .. e1 of the index (sorted by range), the azimuth
+// relative to the bucket's centre (float32 broad phase), the plane's first particle (entries hold plane-local indices)
+struct Bucket {
+    int e0, e1;
+    float th_rel;
+    long long pbase;
+};
+
+__device__ __forceinline__ Bucket beam_bucket(const DevArgs &a, int plane, float th32)
+{
+    const double thd = (double)th32;
+    const double thm = thd >= LSS_TWO_PI ? thd - LSS_TWO_PI : thd;
+    int bk = (int)(thm * a.inv_w);
+    bk = bk < 0 ? 0 : (bk >= a.n_buckets ? a.n_buckets - 1 : bk);
+    const int32_t *bs = a.bucket_start + (int64_t)plane * (a.n_buckets + 1) + bk;
+    Bucket k;
+    k.e0 = bs[0];
+    k.e1 = bs[1];
+    k.th_rel = (float)(thm - (bk + 0.5) * a.w);
+    k.pbase = a.plane_off[plane];
+    return k;
+}
+
+// serial walk of the beam's bucket prefix (the entries nearer than the target): f(particle, rho, right_hit, left_hit)
+// for every exact hit, in prefix order.  Returns the number of hits.
+template <class F>
+__device__ __forceinline__ int for_each_hit(const DevArgs &a, const Bucket &k, const Beam &bm, float d32, F &&f)
+{
+    int n = 0;
+#pragma unroll 1
+    for (int e = k.e0; e < k.e1; e++) {
+        const EntryView en = lss_decode(__ldg(&a.entries[e]), a.zbase);
+        if (!(en.x < d32)) break;                                   // sorted by range: nothing nearer follows
+        if (!(fabsf(en.y - k.th_rel) <= en.z)) continue;            // float32 broad phase (conservative)
+        const long long pi = k.pbase + en.idx;
+        double rho;
+        bool rh, lh;
+        if (exact_hit(a.rec + pi, bm, rho, rh, lh)) { f((int)pi, rho, rh, lh); n++; }
+    }
+    return n;
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // scan: all beams
 // ---------------------------------------------------------------------------------------------------------------------
@@ -102,9 +145,6 @@ __device__ __forceinline__ double shfl_f64(double v, int src)
     return __longlong_as_double(((long long)hi << 32) | (unsigned)lo);
 }
 
-#ifndef LSS_CLASS_BY_RANGE
-#define LSS_CLASS_BY_RANGE 0
-#endif
 #ifndef LSS_SCAN_CTAS
 #define LSS_SCAN_CTAS 10
 #endif
@@ -139,23 +179,15 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
             px = row[0]; py = row[1]; pz = row[2]; pint = row[3]; pch = row[4];
         }
     }
-    if (a.win_stage) {      // by-product for the pre-pass: this warp's mounting-window points, compacted (planes.py:21-27)
-        const bool in = active && lss_in_window(px, py, pz);
-        const unsigned m = __ballot_sync(FULL, in);
-        if (in) {
-            float *o = a.win_stage + (beg + w0 + __popc(m & ((1u << lane) - 1u))) * 3;
-            o[0] = px; o[1] = py; o[2] = pz;
-        }
-        if (lane == 0) a.win_tile_cnt[lss_window_tile0(beg, b) + w0 / 32] = __popc(m);
-    }
     // np.linalg.norm([x, y, z], axis=0) in float32: sqrt((x*x + y*y) + z*z), no FMA   (simulation.py:89)
     const float d32 = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(px, px), __fmul_rn(py, py)), __fmul_rn(pz, pz)));
     const int ch = channel_bin(pch);
     float out_l = pch;
-    int e0 = 0, e1 = 0, ns = 0;
-    long long pbase = 0;                                            // first particle of the beam's plane
+    int ns = 0;
+    Bucket bkt;
+    bkt.e0 = bkt.e1 = 0; bkt.th_rel = 0.0f; bkt.pbase = 0;
     bool slow = false;
-    float th32 = 0.0f, th_rel = 0.0f;
+    float th32 = 0.0f;
     Beam bm;
     bm.d = (double)d32; bm.right = bm.left = 0.0; bm.straddle = false;
     if (active && ch < LSS_N_CHANNELS) {
@@ -163,22 +195,15 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
         th32 = a.theta ? a.theta[beg + i] : azimuth32(py, px);
         if (th32 < 0.0f) th32 = __fadd_rn(th32, 6.2831855f);
         beam_limits(th32, a.half_div, bm);
-        const double thd = (double)th32;
         const int plane = a.order[b * LSS_N_CHANNELS + ch];
-        if (plane >= 0 && plane < a.n_planes && thd == thd) {
-            const double thm = thd >= LSS_TWO_PI ? thd - LSS_TWO_PI : thd;
-            int bk = (int)(thm * a.inv_w);
-            bk = bk < 0 ? 0 : (bk >= a.n_buckets ? a.n_buckets - 1 : bk);
-            th_rel = (float)(thm - (bk + 0.5) * a.w);
-            const int32_t *bs = a.bucket_start + (int64_t)plane * (a.n_buckets + 1) + bk;
-            e0 = bs[0];
-            e1 = bs[1];
-            pbase = a.plane_off[plane];
+        if (plane >= 0 && plane < a.n_planes && th32 == th32) {
+            bkt = beam_bucket(a, plane, th32);
+            const int e1 = bkt.e1;
             // ---- phase A: broad phase over the prefix of entries nearer than the target, four loads in flight --------------
             int *pos = s_idx[wid][lane];
             bool stop = false;
 #pragma unroll 1
-            for (int e = e0; e < e1 && !stop; e += 4) {
+            for (int e = bkt.e0; e < e1 && !stop; e += 4) {
                 BroadEntry raw[4];
 #pragma unroll
                 for (int q = 0; q < 4; q++) raw[q] = __ldg(&a.entries[min(e + q, e1 - 1)]);
@@ -187,7 +212,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
                     if (stop || e + q >= e1) continue;
                     const EntryView en = lss_decode(raw[q], a.zbase);
                     if (!(en.x < d32)) { stop = true; continue; }               // sorted by range: nothing nearer follows
-                    if (!(fabsf(en.y - th_rel) <= en.z)) continue;               // float32 broad phase (conservative)
+                    if (!(fabsf(en.y - bkt.th_rel) <= en.z)) continue;           // float32 broad phase (conservative)
                     if (ns < SURV_CAP) pos[ns] = en.idx;
                     else slow = true;
                     ns++;
@@ -218,7 +243,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
             if (c < 32 && oc <= s) j = c;
         }
         const int r = s - __shfl_sync(FULL, off, j);
-        const long long pbj = __shfl_sync(FULL, pbase, j);
+        const long long pbj = __shfl_sync(FULL, bkt.pbase, j);
         Beam bj;
         bj.d = shfl_f64(bm.d, j);
         bj.right = shfl_f64(bm.right, j);
@@ -233,18 +258,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     __syncwarp();
     unsigned hits = s_hit[wid][lane];
     int L = __popc(hits);
-    if (slow) {                                                 // serial fallback: count the hits of the whole prefix
-        L = 0;
-#pragma unroll 1
-        for (int e = e0; e < e1; e++) {
-            const EntryView en = lss_decode(__ldg(&a.entries[e]), a.zbase);
-            if (!(en.x < d32)) break;
-            if (!(fabsf(en.y - th_rel) <= en.z)) continue;
-            double rho;
-            bool rh, lh;
-            if (exact_hit(a.rec + pbase + en.idx, bm, rho, rh, lh)) L++;
-        }
-    }
+    if (slow) L = for_each_hit(a, bkt, bm, d32, [](int, double, bool, bool) {});   // serial fallback: count the hits
     // ---- beams with occluders: warp-aggregated push to the solve list, hit positions to the position array -------------------
     {
         const bool push = L > 0;
@@ -259,18 +273,14 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
         if (pm) {
             int hbase = 0;
             const int leader = __ffs(pm) - 1;
-            if (lane == leader) hbase = atomicAdd(a.hdr + 3, ltotal);
+            if (lane == leader) hbase = atomicAdd(a.hdr + 2, ltotal);
             hbase = __shfl_sync(FULL, hbase, leader);
             if (push) {
                 // work class = number of occluders (then far / near target): what a beam costs the solve kernel -- claiming,
                 // pulses, the sweep over the window ends -- is per-beam serial work proportional to it, and a warp runs as long as
                 // its slowest lane, so the 32 beams of a tile should have the same count.  The costliest class comes first so
-                // that the kernel's tail is cheap tiles.  (Round 1 sorted by target range: the cost was the window samples then.)
-#if LSS_CLASS_BY_RANGE
-                const int cls = LIST_CLASSES - 1 - min(LIST_CLASSES - 1, (int)(d32 * (LIST_CLASSES / 100.0f)));
-#else
+                // that the kernel's tail is cheap tiles; beams with 64 .. 128 occluders (rare) share the costliest class.
                 const int cls = LIST_CLASSES - 1 - min(LIST_CLASSES - 1, 2 * min(L, 63) + (d32 > 40.0f ? 1 : 0));
-#endif
                 // append to the class's bucket: number j in the class, warp-aggregated per class
                 const unsigned cm = __match_any_sync(pm, cls);
                 const int cl = __ffs(cm) - 1;
@@ -286,13 +296,13 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
                 int chunk;
                 while ((chunk = *(volatile int *)ct) == 0) {}
                 const int hoff = hbase + lincl - L;
-                const bool fits = hoff + L <= a.hit_cap;        // position array full: the beam goes to the overflow kernel
+                const bool fits = hoff + L <= a.hit_cap;        // position array full: the solve kernel walks the prefix
                 {
                     SolveItem it;           // (only beams with a valid channel walk a bucket: ch < 64)
                     it.key = ((unsigned long long)ch << 56) | ((unsigned long long)cls << 48) |
                              ((unsigned long long)b << 32) | (unsigned)i;
-                    it.hit_off = hoff;
-                    it.L = fits ? L : 0x7fff;
+                    it.hit_off = fits ? hoff : -1;
+                    it.L = L;
                     it.th32 = th32;
                     it.px = px;
                     it.py = py;
@@ -304,18 +314,9 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
                     if (!slow) {
                         const int *pos = s_idx[wid][lane];
 #pragma unroll 1
-                        for (int k = 0; hits; hits &= hits - 1) hp[k++] = (int)pbase + pos[__ffs(hits) - 1];
+                        for (int k = 0; hits; hits &= hits - 1) hp[k++] = (int)bkt.pbase + pos[__ffs(hits) - 1];
                     } else {
-                        int k = 0;
-#pragma unroll 1
-                        for (int e = e0; e < e1 && k < L; e++) {
-                            const EntryView en = lss_decode(__ldg(&a.entries[e]), a.zbase);
-                            if (!(en.x < d32)) break;
-                            if (!(fabsf(en.y - th_rel) <= en.z)) continue;
-                            double rho;
-                            bool rh, lh;
-                            if (exact_hit(a.rec + pbase + en.idx, bm, rho, rh, lh)) hp[k++] = (int)pbase + en.idx;
-                        }
+                        for_each_hit(a, bkt, bm, d32, [&](int pi, double, bool, bool) { *hp++ = pi; });
                     }
                 }
             }
@@ -442,13 +443,10 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         bm.d = (double)d32;
         beam_limits(it.th32, a.half_div, bm);
 
-        const bool deferred = L > SOLVE_LCAP;
-        if (deferred) {
-            const int s2 = atomicAdd(a.count_out, 1);
-            if (s2 < a.cap_out) a.list_out[s2] = ((unsigned long long)b << 32) | (unsigned)i;
-            else raise_status(a.status, LSS_ERR_OCCLUDER_OVERFLOW);
-        }
-        const int need = (L > 0 && !deferred) ? L + 1 : 0;
+        // more than SOLVE_LCAP occluders: an error, and the beam is not solved (n_claim = 0, out_l = 0: its row, record
+        // and occluder count stay as the scan wrote them)
+        if (L > SOLVE_LCAP) raise_status(a.status, LSS_ERR_OCCLUDER_OVERFLOW);
+        const int need = (L > 0 && L <= SOLVE_LCAP) ? L + 1 : 0;
 
         // ---- rounds: as many beams of the tile as fit into the arena (normally all of them) ---------------------------
         unsigned remaining = __ballot_sync(FULL, need > 0);
@@ -490,7 +488,8 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 bj.right = shfl_f64(bm.right, j);
                 bj.left = shfl_f64(bm.left, j);
                 bj.straddle = bj.right > bj.left;
-                if (s < total && inr && r < Lj) {                   // (slot L of a beam is its hard target: filled later)
+                // (slot L of a beam is its hard target: filled later; a beam without stored hits is filled below)
+                if (s < total && inr && r < Lj && hoj >= 0) {
                     const int pi = a.hit_idx[hoj + r];
                     const ParticleTan tn = a.tan[pi];               // (both records requested before either is used)
                     double rho;
@@ -500,6 +499,18 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                     A1[s] = lh ? bj.left : tn.t_left;
                     A2[s] = rho;
                 }
+            }
+            if (in_round && it.hit_off < 0) {
+                // the scan could not store this beam's hits (hit array full, rare): its lane walks the bucket prefix
+                // again and fills its slots in prefix order, the order the scan would have stored them in
+                const Bucket bkt = beam_bucket(a, a.order[b * LSS_N_CHANNELS + ch], it.th32);
+                int s = off;
+                for_each_hit(a, bkt, bm, d32, [&](int pi, double rho, bool rh, bool lh) {
+                    A0[s] = rh ? bm.right : a.tan[pi].t_right;
+                    A1[s] = lh ? bm.left : a.tan[pi].t_left;
+                    A2[s] = rho;
+                    s++;
+                });
             }
             __syncwarp();
 
@@ -518,9 +529,12 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 }
 
                 // ---- compute_occlusion_dict (simulation.py:231-295) ------------------------------------------------------
-                // Union-list formulation (see snowfall.cu): a particle claims |[a1,a2]| - |[a1,a2] n union of the claims so
-                // far| and is dropped iff its interval is contained in one union interval (or is empty); the hard target
-                // gets what is left between the smallest and the largest end point -- seam quirk included.
+                // The reference splits the beam into elementary sub-intervals between all sorted end points and lets the
+                // particles claim, nearest first, every still-unclaimed piece inside their own interval.  Equivalent
+                // union-list formulation: keep the union of the intervals claimed so far as a list of disjoint, non-touching
+                // intervals; a particle claims |[a1,a2]| - |[a1,a2] n union| and is dropped iff its interval is contained
+                // in one union interval (or a1 >= a2, the reference's empty range(i1, i2)); the hard target gets what is
+                // left between the smallest and the largest end point -- including the ~2 pi gap of the seam quirk.
                 double rb = bm.right;
                 if (bm.straddle) rb = bm.right - LSS_TWO_PI;
                 int nu = 0, P = 0;
@@ -768,8 +782,7 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         }
 
         // ---- np.round of the intensity column (simulation.py:516), store, label-1 statistics (simulation.py:170) ----------
-        const bool counted = active && !deferred;          // a deferred beam is written by the overflow kernel
-        if (counted) {
+        if (active) {
             // label 1 or 2 <=> the waveform was solved; otherwise (no claiming particle, or a range-index error raised)
             // the row and the record the scan wrote are final
             if (out_l != 0.0f) {
@@ -782,7 +795,7 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
             if (a.nocc) a.nocc[beg + i] = n_claim;
         }
         {
-            const bool on = counted && att_new_i >= 0;
+            const bool on = att_new_i >= 0;                 // (only a solved beam has one)
             const int key = b * LSS_N_CHANNELS + (ch < LSS_N_CHANNELS ? ch : 0);
             const unsigned mk = __match_any_sync(FULL, on ? key : -1);
             if (on && lane == __ffs(mk) - 1) atomicAdd(a.att_cnt + key, (unsigned)__popc(mk));

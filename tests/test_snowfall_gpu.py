@@ -416,7 +416,7 @@ def test_degenerate_rows(engine, oracle, tables18k):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# (4) many occluders on one beam: the solve kernel's deferral to the overflow kernel, and the hard cap
+# (4) many occluders on one beam, a full hit array, and the hard cap
 # ----------------------------------------------------------------------------------------------------------------------
 def _column_of_flakes(n, seed):
     """n small disks strung along azimuth ~0 between 2 and 45 m, plus background flakes elsewhere."""
@@ -427,18 +427,25 @@ def _column_of_flakes(n, seed):
 
 
 def test_beams_with_dozens_of_occluders_match_the_oracle(engine, oracle):
-    """40 and 100 occluders on one beam: more than the solve kernel's shared-memory arena takes per beam (63), so the
-    second case is deferred to the overflow kernel -- both must equal the oracle (labels, intensities, occluder counts)."""
+    """40 and 100 occluders on one beam (the solve kernel takes up to 128 per beam), and 400 beams under the 100-flake
+    column: more hits than the scan's hit array holds for the batch (6 per beam + 4096), so the solve kernel walks the
+    bucket prefixes of the beams it could not store again -- every case must equal the oracle (labels, intensities,
+    occluder counts)."""
     fd, fs, mi, mx = sensor_arrays()
-    for n_col, seed in ((40, 21), (100, 22)):
+    fan_az = np.concatenate(([0.0, 1e-4, -2e-4, 3e-4], np.linspace(-np.pi, np.pi, 60, endpoint=False)))
+    fan_d = np.concatenate(([50.0, 48.0, 60.0, 30.0], np.full(60, 35.0)))
+    rng = np.random.default_rng(24)
+    crowd_az, crowd_d = rng.uniform(-3e-4, 3e-4, 400), rng.uniform(30.0, 60.0, 400)
+    for n_col, seed, az, d, hit_array_full in ((40, 21, fan_az, fan_d, False), (100, 22, fan_az, fan_d, False),
+                                               (100, 22, crowd_az, crowd_d, True)):
         table = _column_of_flakes(n_col, seed)
-        az = np.concatenate(([0.0, 1e-4, -2e-4, 3e-4], np.linspace(-np.pi, np.pi, 60, endpoint=False)))
-        d = np.concatenate(([50.0, 48.0, 60.0, 30.0], np.full(60, 35.0)))
         pts = np.stack([d * np.cos(az), d * np.sin(az), np.zeros_like(d), np.full_like(d, 90.0), np.full_like(d, 5.0)],
                        axis=1).astype(np.float32)
         theta = np.arctan2(pts[:, 1], pts[:, 0])
         want, s, nocc, _ = oracle.snow_channel(pts, table, DIV, fd[5], fs[5], mi[5], mx[5], theta=theta)
         assert nocc.max() >= n_col * 0.6, 'test set-up: most flakes of the column must claim a piece of the first beams'
+        if hit_array_full:      # claiming occluders never outnumber hits
+            assert nocc.sum() > 6 * len(d) + 4096, 'test set-up: the hits must overflow the hit array'
         tid = engine.upload_tables([table] * 64)
         r = run_full(engine, tid, pts, list(range(64)), theta=theta)
         engine.free_tables(tid)
