@@ -296,6 +296,38 @@ LSS_API lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int 
                                       int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_voxelize_workspace_bytes(int64_t n_total, int n_clouds, int max_points_per_voxel, int max_voxels);
 
+/* ---- DROR snow removal ------------------------------------------------------------------------------------------------
+ * Dynamic Radius Outlier Removal, dynamic_radius_outlier_filter (lib/cadc_devkit/other/dror.py:288-334), for every cloud of
+ * a batch, as the dataset applies it under its DROR / DROR++ keys (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:588-616).
+ * Point i is kept iff c_i >= k_min + 1, c_i = the number of points j of its cloud (i included) with
+ *     d_ij = ((dx*dx) + dy*dy) + dz*dz in float32 (flann::L2_Simple, PCL's KdTreeFLANN), dx = x_j - x_i, and
+ *     (double)sqrtf(d_ij) < sr_i         when sr_i = ((alpha * beta) * pi) / 180 * sqrt(x_i*x_i + y_i*y_i) (float64) >= sr_min
+ *     sqrtf(d_ij) < (float)sr_min         otherwise (the reference compares np.float32 with a Python float: float32)
+ * which is exactly the reference's k-nearest count with k = k_min + 1.  Clouds of fewer than k_min + 1 points come out all
+ * snow; a row with a non-finite x, y or z is snow and is nobody's neighbour (both left undefined by the reference).
+ *   d_points        float32[n_total * n_features], n_features >= 3 (x, y, z, ...); cloud b starts at row h_cloud_offsets[b]
+ *   d_cloud_counts  int32[n_clouds] device or NULL: valid rows per cloud slot (the slot-compacted output of
+ *                   lss_snowfall_batch / lss_wet_ground_batch); NULL: h_cloud_offsets[b+1] - h_cloud_offsets[b]
+ *   alpha_deg, beta, k_min, sr_min   the reference's parameters (defaults 0.16, 3, 3, 0.04); all >= 0
+ *   flags           LSS_DROR_CUBE: only rows inside get_cube_mask's box take part (the reference's crop variant); the
+ *                   others get code 2 and are nobody's neighbour.  LSS_DROR_WORK_STATS: diagnostic, the first 32 bytes of
+ *                   the workspace receive uint64 {queries, cells visited, candidates tested, queries that exited early}
+ *   d_out_keep      uint8[n_total]: per valid row 1 keep, 0 snow, 2 outside the cube; rows behind a cloud's count untouched
+ *   d_out_points    float32[n_total * n_features] or NULL: the rows with code 1, whole and in input order, compacted to the
+ *                   front of their cloud's slot; rows behind that are unspecified.  Must not alias d_points.
+ *   d_out_counts    int32[n_clouds] rows kept per cloud;  d_out_n_snow  int32[n_clouds] rows with code 0 per cloud
+ *   d_workspace     lss_dror_workspace_bytes(n_total, n_clouds) bytes; that query needs a CUDA device (the size of the
+ *                   radix sort's scratch depends on it) and returns -1 without one
+ * Results are deterministic and exact (integer counts of an exact per-pair test).  No allocation, no synchronisation.   */
+#define LSS_DROR_CUBE 0x1u          /* only rows inside get_cube_mask's box take part (dror.py:73-84, z ignored) */
+#define LSS_DROR_WORK_STATS 0x100u  /* diagnostic work counters into the workspace's first 32 bytes */
+LSS_API lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                  const int32_t *d_cloud_counts, int n_clouds, double alpha_deg, double beta, int k_min,
+                                  double sr_min, uint32_t flags, uint8_t *d_out_keep /* 1 keep / 0 snow / 2 outside cube */,
+                                  float *d_out_points /* or NULL */, int32_t *d_out_counts, int32_t *d_out_n_snow,
+                                  void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_dror_workspace_bytes(int64_t n_total, int n_clouds);
+
 /* ---- exchange step of the sharded batch (SURVEY.md 8e, BASELINE.json configs[3]) ------------------------------------------
  * The reference has no multi-GPU augmentation; its collectives are OpenPCDet's result merging
  * (lib/OpenPCDet/pcdet/utils/commu_utils.py:77,90: all_gather of pickled, variable-size objects).  The sharded engine

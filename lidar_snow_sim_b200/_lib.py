@@ -26,6 +26,7 @@ FLAG_CAMERA_FOV = 0x2
 FLAG_DEVICE_PREPASS = 0x4
 FLAG_ASSUME_SORTED = 0x8
 FOG_HARD, FOG_SOFT, FOG_GAIN = 0x1, 0x2, 0x4
+DROR_CUBE, DROR_WORK_STATS = 0x1, 0x100
 
 # status -> exception type the reference would have raised at the corresponding place (SURVEY.md 8b "Errors")
 _EXC = {
@@ -84,6 +85,9 @@ SIGNATURES = [
     ('lss_voxelize_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P,
                                       _P, _P, _c.c_int64, _P]),
     ('lss_voxelize_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int]),
+    ('lss_dror_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_int, _c.c_double,
+                                  _c.c_uint32, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_dror_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_gather_push', _c.c_int, [_P, _P, _P, _P, _c.c_int, _c.c_int64, _c.c_int, _c.c_int, _P, _P, _P, _P, _c.c_int, _P]),
     ('lss_dart_throwing', _c.c_int, [_c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _P, _c.c_int64,
                                      _c.POINTER(_c.c_int64)]),

@@ -407,6 +407,49 @@ class SnowfallEngine:
         _lib.check(st, self.h)
         return out
 
+    def dror_batch(self, points, cloud_offsets, alpha=0.16, beta=3.0, k_min=3, sr_min=0.04, counts=None, crop=False,
+                   want_points=True, work_stats=False, out=None):
+        """
+        Batched DROR snow removal (dynamic_radius_outlier_filter, lib/cadc_devkit/other/dror.py:288-334) on
+        device-resident clouds (current stream, no synchronisation).  points: CUDA float32 (N, F), F >= 3; counts:
+        optional CUDA int32 (B,) valid rows per cloud slot (e.g. the output of snowfall_batch); crop: only rows inside
+        get_cube_mask's box take part (dror.py:73-84).  Returns dict(keep uint8 (N,) = 1 keep / 0 snow / 2 outside the
+        cube, counts int32 (B,) kept rows, n_snow int32 (B,) [, points (N, F) kept rows slot-compacted in input order]
+        [, work: uint64 CUDA tensor (4,) = queries, cells visited, candidates tested, early exits]).
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        N = int(off[-1])
+        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
+        assert points.dim() == 2
+        F = int(points.shape[1])
+        if counts is not None:
+            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        flags = (_lib.DROR_CUBE if crop else 0) | (_lib.DROR_WORK_STATS if work_stats else 0)
+        with torch.cuda.device(self.device):
+            if out is None:
+                out = {}
+            if 'keep' not in out:
+                out.update(keep=torch.empty((N,), dtype=torch.uint8, device=self.device),
+                           counts=torch.empty((B,), dtype=torch.int32, device=self.device),
+                           n_snow=torch.empty((B,), dtype=torch.int32, device=self.device))
+            if want_points and 'points' not in out:
+                out['points'] = torch.empty((N, F), dtype=torch.float32, device=self.device)
+            need = self.lib.lss_dror_workspace_bytes(N, B)
+            if need < 0:
+                raise RuntimeError('lss_dror_workspace_bytes failed (no usable CUDA device?)')
+            if getattr(self, '_ws_dror', None) is None or self._ws_dror.numel() < need:
+                self._ws_dror = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_dror_batch(self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, float(alpha), float(beta),
+                                         int(k_min), float(sr_min), flags, _ptr(out['keep']),
+                                         _ptr(out['points']) if want_points else None, _ptr(out['counts']),
+                                         _ptr(out['n_snow']), _ptr(self._ws_dror), int(self._ws_dror.numel()),
+                                         self._stream())
+            _lib.check(st, self.h)
+            if work_stats:
+                out['work'] = self._ws_dror[:32].view(torch.int64).clone()
+        return out
+
     def gather_push(self, points, counts, d_cloud_offsets, n_rows, world, rank, peer_points, peer_counts, mc_points=0,
                     mc_counts=0, blocks=0):
         """lss_gather_push on the current stream: write the kept rows of this rank's slot-compacted batch (+ counts) into
@@ -438,11 +481,12 @@ class SnowfallEngine:
     def kernel_times(self, reset=True):
         """{kernel name: (total ms, launches)} measured with CUDA events on the launching stream (synchronises)."""
         torch.cuda.synchronize(self.device)
-        n = 10
+        n = 16                                        # every id the library can have; unused ids have no name
         ms = np.zeros(n, dtype=np.float64)
         calls = np.zeros(n, dtype=np.int64)
         _lib.check(self.lib.lss_kernel_times(self.h, 1 if reset else 0, _ptr(ms), _ptr(calls), n), self.h)
-        return {self.lib.lss_kernel_name(k).decode(): (float(ms[k]), int(calls[k])) for k in range(n)}
+        names = [self.lib.lss_kernel_name(k).decode() for k in range(n)]
+        return {names[k]: (float(ms[k]), int(calls[k])) for k in range(n) if names[k]}
 
 
 _default_engines = {}

@@ -145,3 +145,25 @@ def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None)
     points, _, _ = simulate_fog(p, pc=points, noise=10, gain=gain, noise_variant=fog_noise_variant, soft=soft, hard=hard,
                                 engine=engine, lut_dir=lut_dir, rng=rng)
     return points
+
+
+def dror_filter(points, dataset_cfg, split, engine=None):
+    """The DROR / DROR++ block of `DenseDataset.__getitem__` (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:588-616)
+    without the pre-computed index files: the snow indices the reference reads from
+    `DROR/alpha_<alpha>/all/<sensor>/<signal>/full/<id>.pkl` are computed by the engine on the raw cloud (full variant,
+    beta 3, k_min 3, sr_min 0.04, alpha = the config value).  As in the reference, `DROR++` applies only when 'snow' is in
+    the split, and with both keys the second index list -- computed on the RAW cloud -- is applied to the already filtered
+    cloud (raising IndexError where an index falls outside it)."""
+    from ..dror import snow_indices
+    raw = points
+    if 'DROR' in dataset_cfg:
+        snow = snow_indices(raw, float(dataset_cfg['DROR']), crop=False, engine=engine)
+        keep_indices = np.ones(len(points), dtype=bool)
+        keep_indices[snow] = False
+        points = points[keep_indices]
+    if 'DROR++' in dataset_cfg and 'snow' in split:
+        snow = snow_indices(raw, float(dataset_cfg['DROR++']), crop=False, engine=engine)
+        keep_indices = np.ones(len(points), dtype=bool)
+        keep_indices[snow] = False
+        points = points[keep_indices]
+    return points
