@@ -164,7 +164,8 @@ LSS_API lss_status lss_snowfall_batch_host_wait(lss_engine *e, int ticket);
 LSS_API int lss_host_pipe_trace(lss_engine *e, float *out, int cap_chunks);
 /* Synchronises `stream`, then returns and clears the latched asynchronous device status.                          */
 LSS_API lss_status lss_check_async(lss_engine *e, void *stream);
-/* number of kernel launches the engine has enqueued since creation (bench.py's gpu_launches) */
+/* number of kernel launches the engine has enqueued since creation (bench.py's gpu_launches); one CUB sort (DROR),
+ * which enqueues several kernels, counts as one launch */
 LSS_API int64_t lss_launch_count(const lss_engine *e);
 /* ---- per-cloud pre-pass ----------------------------------------------------------------------------------------------
  * Ground plane (calculate_plane, tools/wet_ground/planes.py:12-50), ground mask + incident angle

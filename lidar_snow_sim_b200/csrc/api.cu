@@ -249,8 +249,7 @@ lss_status lss_snowfall_batch(lss_engine *e, int table_id, const float *d_points
     if (!e) return LSS_ERR_INVALID_ARG;
     if (!h_cloud_offsets || !h_order || n_clouds < 0 || !d_out_points || !d_out_counts || !d_out_stats)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    if (n_clouds > 65535) return lss_fail(e, LSS_ERR_INVALID_ARG, "at most 65535 clouds per call");
-    if (!d_points && h_cloud_offsets[n_clouds] > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
+    if (!d_points && n_clouds <= 65535 && h_cloud_offsets[n_clouds] > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
     if (!e->has_sensor) return lss_fail(e, LSS_ERR_NO_SENSOR, "sensor constants not set (lss_set_sensor)");
     auto it = e->tables.find(table_id);
     if (it == e->tables.end()) return lss_fail(e, LSS_ERR_NO_TABLE, "unknown table id");
@@ -291,13 +290,13 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
                                     void *d_workspace, int64_t workspace_bytes, void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
-    if (!d_points || !h_cloud_offsets || n_clouds <= 0 || !d_poly_out || !d_workspace)
-        return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
+    if (!d_points || n_clouds <= 0 || !d_poly_out || !d_workspace) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
+    BatchGeometry geo;
+    if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, 0, geo)) return rc;
     DeviceGuard g(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t off_bytes = ((int64_t)(n_clouds + 1) * 8 + 255) / 256 * 256;
-    if (workspace_bytes < off_bytes + lss_prepass_ws_bytes(h_cloud_offsets[n_clouds], n_clouds))
+    const int64_t off_bytes = align_up((int64_t)(n_clouds + 1) * 8, 256);
+    if (workspace_bytes < off_bytes + lss_prepass_ws_bytes(geo.n, n_clouds))
         return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     int64_t *d_off = (int64_t *)d_workspace;
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), st));
@@ -339,7 +338,7 @@ lss_status lss_set_profiling(lss_engine *e, int enable)
 }
 
 static const char *kernel_names[LSS_K_COUNT] = {"channel_sort", "prepass", "snowfall", "compact", "keep", "wet_ground", "fog",
-                                                "snowfall_scan", "snowfall_solve", "voxelize", "dror"};
+                                                "snowfall_scan", "snowfall_solve", "voxelize", "dror", "lisa"};
 
 const char *lss_kernel_name(int kernel) { return (kernel >= 0 && kernel < LSS_K_COUNT) ? kernel_names[kernel] : ""; }
 

@@ -188,5 +188,5 @@ __device__ __forceinline__ float azimuth32(float yf, float xf)
 
 // solve.cu: the scan kernel over every beam, then the solve kernel over the class-bucketed solve list (tile_cursor: a
 // zeroed int, hdr[1]).
-void lss_launch_scan(const DevArgs &a, cudaStream_t stream);
-void lss_launch_solve(const DevArgs &a, int *tile_cursor, int n_sm, cudaStream_t stream);
+cudaError_t lss_launch_scan(lss_engine *e, const DevArgs &a, cudaStream_t stream);
+cudaError_t lss_launch_solve(lss_engine *e, const DevArgs &a, int *tile_cursor, cudaStream_t stream);

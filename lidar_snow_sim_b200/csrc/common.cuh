@@ -7,6 +7,7 @@
 #include <vector>
 #include <cstring>
 #include <map>
+#include <utility>
 
 #include "../../include/lidar_snow_sim.h"
 
@@ -115,6 +116,18 @@ struct lss_engine {
 };
 void lss_host_pipe_free(lss_engine *e);
 
+inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
+
+// Every kernel launch of the library goes through here, so that lss_launch_count() counts exactly what is enqueued.
+template <typename... P, typename... A>
+[[nodiscard]] inline cudaError_t lss_launch(lss_engine *e, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem,
+                                            cudaStream_t stream, A &&...args)
+{
+    kernel<<<grid, block, smem, stream>>>(std::forward<A>(args)...);
+    e->launches++;
+    return cudaGetLastError();
+}
+
 // next side stream + a (fork, join) event pair, round robin; created on first use
 inline cudaError_t lss_side_stream(lss_engine *e, cudaStream_t *stream, cudaEvent_t *ev_fork, cudaEvent_t *ev_join)
 {
@@ -164,9 +177,9 @@ inline cudaError_t lss_stage_upload(lss_engine *e, void *dst, const void *src, s
     memcpy(sl.host, src, bytes);
     const int n_words = (int)(bytes / 4);
     const int blocks = n_words >= 1 << 16 ? 64 : (n_words + 1023) / 1024;
-    k_stage_copy<<<blocks, 256, 0, stream>>>((uint32_t *)dst, (const uint32_t *)sl.host, n_words);
-    e->launches++;
-    if ((err = cudaGetLastError()) != cudaSuccess) return err;
+    if ((err = lss_launch(e, k_stage_copy, blocks, 256, 0, stream, (uint32_t *)dst, (const uint32_t *)sl.host, n_words)) !=
+        cudaSuccess)
+        return err;
     return cudaEventRecord(sl.done, stream);
 }
 
@@ -193,18 +206,16 @@ inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStrea
     for (int i = 0; i < r.n; i++) mx = r.words[i] > mx ? r.words[i] : mx;
     const unsigned long long cap = 4ull * e->n_sm;
     const unsigned blocks = (unsigned)((mx + 1023) / 1024 < cap ? (mx + 1023) / 1024 : cap);
-    k_zero_regions<<<dim3(blocks ? blocks : 1, r.n), 256, 0, stream>>>(r);
-    e->launches++;
-    return cudaGetLastError();
+    return lss_launch(e, k_zero_regions, dim3(blocks ? blocks : 1, r.n), 256, 0, stream, r);
 }
 
 enum { LSS_K_SORT = 0, LSS_K_PREPASS = 1, LSS_K_SNOWFALL = 2, LSS_K_COMPACT = 3, LSS_K_FINALIZE = 4, LSS_K_WET = 5,
-       LSS_K_FOG = 6, LSS_K_SCAN = 7, LSS_K_SOLVE = 8, LSS_K_VOXEL = 9, LSS_K_DROR = 10, LSS_K_COUNT = 11 };   // 7, 8: inside the LSS_K_SNOWFALL bracket
+       LSS_K_FOG = 6, LSS_K_SCAN = 7, LSS_K_SOLVE = 8, LSS_K_VOXEL = 9, LSS_K_DROR = 10, LSS_K_LISA = 11,
+       LSS_K_COUNT = 12 };   // 7, 8: inside the LSS_K_SNOWFALL bracket
 
-struct KernelTimer {        // RAII: records begin/end events when profiling is on
+struct KernelTimer {        // RAII: records begin/end events around the launches of its scope when profiling is on
     lss_engine *e; cudaStream_t s; int idx = -1;
     KernelTimer(lss_engine *e_, int kernel, cudaStream_t s_) : e(e_), s(s_) {
-        e->launches++;
         if (!e->profiling) return;
         lss_engine::TimedLaunch t; t.kernel = kernel;
         cudaEventCreate(&t.beg); cudaEventCreate(&t.end);
@@ -238,6 +249,44 @@ static inline lss_status lss_fail(lss_engine *e, lss_status s, const char *msg)
     return s;
 }
 
+// Host-side geometry of a batch of clouds: n = off[B] rows in all, max_n = rows of the largest cloud, tile_base[b] =
+// first tile of cloud b when every cloud is cut into tiles of `tile` rows (tile_base[B] = tiles in all; empty for tile 0).
+struct BatchGeometry {
+    int64_t n = 0, max_n = 0;
+    std::vector<int32_t> tile_base;
+};
+
+// Checks the host cloud offsets of a batch entry point and returns its geometry.  The offsets must start at 0 and not
+// decrease; a batch has at most 65535 clouds (the kernels' grid y dimension) of fewer than 2^31 rows each.
+inline lss_status lss_batch_geometry(lss_engine *e, const int64_t *h_cloud_offsets, int n_clouds, int tile,
+                                     BatchGeometry &g)
+{
+    if (!h_cloud_offsets || n_clouds < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
+    if (n_clouds > 65535) return lss_fail(e, LSS_ERR_INVALID_ARG, "at most 65535 clouds per call");
+    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
+    g.max_n = 0;
+    g.tile_base.assign(tile > 0 ? n_clouds + 1 : 0, 0);
+    for (int b = 0; b < n_clouds; b++) {
+        const int64_t n = h_cloud_offsets[b + 1] - h_cloud_offsets[b];
+        if (n < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets must be non-decreasing");
+        if (n >= (1LL << 31)) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud too large");
+        g.max_n = n > g.max_n ? n : g.max_n;
+        if (tile > 0) g.tile_base[b + 1] = g.tile_base[b] + (int32_t)((n + tile - 1) / tile);
+    }
+    g.n = h_cloud_offsets[n_clouds];
+    return LSS_OK;
+}
+
+// Stream-ordered upload of a batch's cloud offsets [B + 1] and tile bases (any number of int32) to the device.
+inline cudaError_t lss_stage_geometry(lss_engine *e, const int64_t *h_cloud_offsets, int n_clouds,
+                                      const std::vector<int32_t> &tile_base, int64_t *d_off, int32_t *d_tile_base,
+                                      cudaStream_t stream)
+{
+    const cudaError_t err = lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), stream);
+    if (err != cudaSuccess) return err;
+    return lss_stage_upload(e, d_tile_base, tile_base.data(), sizeof(int32_t) * tile_base.size(), stream);
+}
+
 // implemented in tables.cu
 lss_status lss_build_tables(lss_engine *e, TableSet &ts, const double *d_xyr, const int64_t *h_plane_offsets,
                             cudaStream_t stream);
@@ -251,7 +300,6 @@ struct SnowfallArgs {
     double beam_divergence_deg;
     const float *d_theta;
     const double *h_thresh_poly;
-    const double *d_thresh_poly = nullptr;      // device-resident polynomials (host pipeline: pre-pass on another stream)
     const double *h_plane_in = nullptr;         // device pre-pass: injected plane / bin picks (PrepassIO)
     const int32_t *h_ymins_in = nullptr;
     double noise_floor;

@@ -31,9 +31,10 @@
 // outward from the query's own sorted position, and the walk stops once c_i reaches k_min + 1.
 //
 // Kernels (one profiling id, LSS_K_DROR): k_dror_key -> cub::DeviceRadixSort::SortPairs (scratch from the caller's
-// workspace) -> k_dror_seg -> k_dror_pack -> k_dror_query -> k_dror_tile_count -> k_dror_tile_scan [-> k_dror_scatter].
+// workspace) -> k_dror_seg -> k_dror_pack -> k_dror_query -> k_seg_count_codes -> k_seg_scan [-> k_dror_scatter]
+// (segments.cuh; class 0 = snow, class 1 = kept).
 // No allocation or synchronisation inside the call; results are deterministic (counts do not depend on visiting order).
-#include "common.cuh"
+#include "segments.cuh"
 #include <cfloat>
 #include <cub/device/device_radix_sort.cuh>
 
@@ -62,17 +63,10 @@ struct DrorArgs {
     float4 *packed;                  // [N] (x, y, z, row bits) in sorted order
     float2 *thr;                     // [N] (distance threshold, neighbour bound R) in sorted order
     uint8_t *keep;                   // [N] output codes
-    const int32_t *tile_base;        // [B+1]
-    int32_t *tile_keep, *tile_snow, *tile_off;
+    SegTiles tiles;                  // compaction tiles of DTILE rows; totals: snow rows, kept rows
     float *out_pts;
-    int32_t *out_counts, *out_snow;
     unsigned long long *stats;       // optional: queries, cells visited, candidates tested, early exits
 };
-
-__device__ __forceinline__ int cloud_rows(const DrorArgs &a, int b)
-{
-    return a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - a.cloud_off[b]);
-}
 
 __device__ __forceinline__ unsigned long long spread3(unsigned long long v)     // 16 bits -> every third bit
 {
@@ -116,7 +110,7 @@ __global__ void __launch_bounds__(256) k_dror_key(DrorArgs a)
     if (i >= slot) return;
     const int64_t row = beg + i;
     unsigned long long key = (unsigned long long)a.n_clouds << 48;
-    if (i < cloud_rows(a, b)) {
+    if (i < seg_rows(a.cloud_off, a.cloud_cnt, b)) {
         const float *p = a.pts + row * a.F;
         const float x = p[0], y = p[1], z = p[2];
         if (a.cube && !in_cube(x, y)) {
@@ -255,81 +249,19 @@ __global__ void __launch_bounds__(QBLOCK) k_dror_query(DrorArgs a)
     }
 }
 
-__global__ void __launch_bounds__(DTILE) k_dror_tile_count(DrorArgs a)
-{
-    __shared__ int ck, cs;
-    const int b = blockIdx.y, tile = blockIdx.x;
-    if (tile >= a.tile_base[b + 1] - a.tile_base[b]) return;
-    if (threadIdx.x == 0) { ck = 0; cs = 0; }
-    __syncthreads();
-    const int i = tile * DTILE + threadIdx.x;
-    int code = 2;
-    if (i < cloud_rows(a, b)) code = a.keep[a.cloud_off[b] + i];
-    const unsigned mk = __ballot_sync(0xffffffffu, code == 1), ms = __ballot_sync(0xffffffffu, code == 0);
-    if ((threadIdx.x & 31) == 0) {
-        if (mk) atomicAdd(&ck, __popc(mk));
-        if (ms) atomicAdd(&cs, __popc(ms));
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        a.tile_keep[a.tile_base[b] + tile] = ck;
-        a.tile_snow[a.tile_base[b] + tile] = cs;
-    }
-}
-
-// per cloud: exclusive scan of the tiles' kept counts, totals of kept and snow rows
-__global__ void __launch_bounds__(256) k_dror_tile_scan(DrorArgs a)
-{
-    __shared__ int wsum[8];
-    __shared__ int run, snow;
-    const int b = blockIdx.x;
-    const int t0 = a.tile_base[b], nt = a.tile_base[b + 1] - t0;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) { run = 0; snow = 0; }
-    __syncthreads();
-    for (int base = 0; base < nt; base += 256) {
-        const int t = base + tid;
-        const int v = t < nt ? a.tile_keep[t0 + t] : 0;
-        int sn = t < nt ? a.tile_snow[t0 + t] : 0;
-        int incl = v;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, d); if (lane >= d) incl += u; }
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) sn += __shfl_down_sync(0xffffffffu, sn, d);
-        if (lane == 31) wsum[warp] = incl;
-        if (lane == 0 && sn) atomicAdd(&snow, sn);
-        __syncthreads();
-        int o = run;
-        for (int w = 0; w < warp; w++) o += wsum[w];
-        if (t < nt) a.tile_off[t0 + t] = o + incl - v;
-        __syncthreads();
-        if (tid == 255) run = o + incl;
-        __syncthreads();
-    }
-    if (tid == 0) { a.out_counts[b] = run; a.out_snow[b] = snow; }
-}
-
 __global__ void __launch_bounds__(DTILE) k_dror_scatter(DrorArgs a)
 {
-    __shared__ int wcnt[DTILE / 32];
     const int b = blockIdx.y, tile = blockIdx.x;
-    if (tile >= a.tile_base[b + 1] - a.tile_base[b]) return;
+    if (tile >= a.tiles.tile_base[b + 1] - a.tiles.tile_base[b]) return;
     const int64_t beg = a.cloud_off[b];
     const int i = tile * DTILE + threadIdx.x;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const bool k = i < cloud_rows(a, b) && a.keep[beg + i] == 1;
-    const unsigned m = __ballot_sync(0xffffffffu, k);
-    if (lane == 0) wcnt[warp] = __popc(m);
-    __syncthreads();
+    const bool k = i < seg_rows(a.cloud_off, a.cloud_cnt, b) && a.keep[beg + i] == 1;
+    const int dst = seg_rank<2, DTILE>(k ? 1 : -1, a.tiles, b, tile);
     if (!k) return;
-    int dst = a.tile_off[a.tile_base[b] + tile] + __popc(m & ((1u << lane) - 1u));
-    for (int w = 0; w < warp; w++) dst += wcnt[w];
     const float *src = a.pts + (beg + i) * a.F;
     float *o = a.out_pts + (beg + dst) * a.F;
     for (int f = 0; f < a.F; f++) o[f] = src[f];
 }
-
-inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
 
 int end_bit(int n_clouds)
 {
@@ -347,16 +279,15 @@ cudaError_t sort_bytes(int64_t n, int n_clouds, size_t *bytes)
                                            (int)n, 0, end_bit(n_clouds));
 }
 
-struct DrorLayout { int64_t stats, off, tile_base, seg, keys, rows, skeys, srows, packed, thr, tiles, sort, total, n_tiles; };
+struct DrorLayout { int64_t stats, off, tiles, seg, keys, rows, skeys, srows, packed, thr, sort, total; };
 
 DrorLayout dror_layout(int64_t n, int n_clouds, size_t sort_tmp)
 {
     DrorLayout L;
-    L.n_tiles = n / DTILE + n_clouds + 1;
     int64_t o = 0;
     L.stats = o;     o = align_up(o + 32, 256);
     L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.tile_base = o; o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
+    L.tiles = o;     o += seg_ws_bytes(n, n_clouds, DTILE, 2);
     L.seg = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
     L.keys = o;      o = align_up(o + n * 8, 256);
     L.rows = o;      o = align_up(o + n * 4, 256);
@@ -364,7 +295,6 @@ DrorLayout dror_layout(int64_t n, int n_clouds, size_t sort_tmp)
     L.srows = o;     o = align_up(o + n * 4, 256);
     L.packed = o;    o = align_up(o + n * 16, 256);
     L.thr = o;       o = align_up(o + n * 8, 256);
-    L.tiles = o;     o = align_up(o + L.n_tiles * 12, 256);
     L.sort = o;      o = align_up(o + (int64_t)sort_tmp, 256);
     L.total = o;
     return L;
@@ -389,28 +319,19 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
                           void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
-    if (!h_cloud_offsets || n_clouds < 0 || !d_out_keep || !d_out_counts || !d_out_n_snow || !d_workspace)
-        return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
+    BatchGeometry g;
+    if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, DTILE, g)) return rc;
+    if (!d_out_keep || !d_out_counts || !d_out_n_snow || !d_workspace) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
     if (n_features < 3) return lss_fail(e, LSS_ERR_INVALID_ARG, "n_features >= 3 required");
     if (k_min < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "k_min must be >= 0");
     if (!(alpha_deg >= 0) || !(beta >= 0) || !(sr_min >= 0))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "alpha, beta and sr_min must be >= 0");
-    if (n_clouds > 65535) return lss_fail(e, LSS_ERR_INVALID_ARG, "at most 65535 clouds per call");
     if (flags & ~(LSS_DROR_CUBE | LSS_DROR_WORK_STATS)) return lss_fail(e, LSS_ERR_INVALID_ARG, "unknown flag");
-    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
     const int B = n_clouds;
-    const int64_t N = h_cloud_offsets[B];
+    const int64_t N = g.n;
     if (N >= (1LL << 31)) return lss_fail(e, LSS_ERR_INVALID_ARG, "batch too large");
     if (N > 0 && !d_points) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
-    std::vector<int32_t> h_tb(B + 1, 0);
-    int64_t max_n = 0;
-    for (int b = 0; b < B; b++) {
-        const int64_t nb = h_cloud_offsets[b + 1] - h_cloud_offsets[b];
-        if (nb < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets must be non-decreasing");
-        max_n = std::max(max_n, nb);
-        h_tb[b + 1] = h_tb[b] + (int32_t)((nb + DTILE - 1) / DTILE);
-    }
-    DeviceGuard g(e->device);
+    DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     size_t sort_tmp = 0;
     LSS_CUDA_CHECK(e, sort_bytes(N, B, &sort_tmp));
@@ -437,17 +358,14 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
     a.packed = (float4 *)(ws + L.packed);
     a.thr = (float2 *)(ws + L.thr);
     a.keep = d_out_keep;
-    a.tile_base = (const int32_t *)(ws + L.tile_base);
-    a.tile_keep = (int32_t *)(ws + L.tiles);
-    a.tile_snow = a.tile_keep + L.n_tiles;
-    a.tile_off = a.tile_snow + L.n_tiles;
+    a.tiles = seg_tiles(ws + L.tiles, B);
+    a.tiles.total[0] = d_out_n_snow;
+    a.tiles.total[1] = d_out_counts;
     a.out_pts = d_out_points;
-    a.out_counts = d_out_counts;
-    a.out_snow = d_out_n_snow;
     a.stats = (flags & LSS_DROR_WORK_STATS) ? (unsigned long long *)(ws + L.stats) : nullptr;
 
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.tile_base, h_tb.data(), sizeof(int32_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
+                                         (int32_t *)a.tiles.tile_base, st));
     if (a.stats) {
         ZeroRegions z;
         z.add(a.stats, 32);
@@ -455,25 +373,23 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
     }
     {
         KernelTimer kt(e, LSS_K_DROR, st);
-        if (max_n > 0) {
-            const dim3 g256((unsigned)((max_n + 255) / 256), B), gt((unsigned)((max_n + DTILE - 1) / DTILE), B);
-            k_dror_key<<<g256, 256, 0, st>>>(a);
+        if (g.max_n > 0) {
+            const dim3 g256((unsigned)((g.max_n + 255) / 256), B), gt((unsigned)((g.max_n + DTILE - 1) / DTILE), B);
+            LSS_CUDA_CHECK(e, lss_launch(e, k_dror_key, g256, 256, 0, st, a));
             size_t tmp = sort_tmp;
             LSS_CUDA_CHECK(e, cub::DeviceRadixSort::SortPairs(ws + L.sort, tmp, (const unsigned long long *)a.keys,
                                                               (unsigned long long *)a.skeys, (const int32_t *)a.rows,
                                                               (int32_t *)a.srows, (int)N, 0, end_bit(B), st));
-            k_dror_seg<<<(B + 1 + 127) / 128, 128, 0, st>>>(a, (int)N);
+            e->launches++;                                   // the sort's kernels count as one launch
+            LSS_CUDA_CHECK(e, lss_launch(e, k_dror_seg, (B + 1 + 127) / 128, 128, 0, st, a, (int)N));
             const unsigned qblocks = (unsigned)((N + QBLOCK - 1) / QBLOCK);
-            k_dror_pack<<<(unsigned)std::min<int64_t>((N + 255) / 256, (int64_t)e->n_sm * 16), 256, 0, st>>>(a);
-            if (a.stats) k_dror_query<true><<<qblocks, QBLOCK, 0, st>>>(a);
-            else k_dror_query<false><<<qblocks, QBLOCK, 0, st>>>(a);
-            k_dror_tile_count<<<gt, DTILE, 0, st>>>(a);
-            k_dror_tile_scan<<<B, 256, 0, st>>>(a);
-            e->launches += 6;
-            if (d_out_points) {
-                k_dror_scatter<<<gt, DTILE, 0, st>>>(a);
-                e->launches++;
-            }
+            LSS_CUDA_CHECK(e, lss_launch(e, k_dror_pack, (unsigned)std::min<int64_t>((N + 255) / 256, (int64_t)e->n_sm * 16),
+                                         256, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, a.stats ? k_dror_query<true> : k_dror_query<false>, qblocks, QBLOCK, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_seg_count_codes<2, DTILE>, gt, DTILE, 0, st, a.keep, a.cloud_off, a.cloud_cnt,
+                                         a.tiles));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.tiles));
+            if (d_out_points) LSS_CUDA_CHECK(e, lss_launch(e, k_dror_scatter, gt, DTILE, 0, st, a));
         } else {
             ZeroRegions z;
             z.add(d_out_counts, sizeof(int32_t) * B);
@@ -481,7 +397,6 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
             LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
         }
     }
-    LSS_CUDA_CHECK(e, cudaGetLastError());
     return LSS_OK;
 }
 

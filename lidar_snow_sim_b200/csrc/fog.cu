@@ -9,16 +9,17 @@
 //
 // Kernels (one thread per point, tiles of 256 points staged through shared memory for coalesced I/O, HBM bound: reads F x 4 B, writes F x 8 B + 1 B per point):
 //   k_fog_count   fog mask per point -> fog points per tile
-//   k_fog_scan    per cloud: exclusive scan of the tile counts (rank of a fog point in POINT ORDER = position of its draw
-//                 in the generator's stream), num_fog_responses
-//   k_fog_apply   everything: hard, soft, noise (k-th PCG64 output by jump-ahead), min / max response, max intensity
+//   k_seg_scan    per cloud: exclusive scan of the tile counts (rank of a fog point in POINT ORDER = position of its draw
+//                 in the generator's stream), fog points per cloud (segments.cuh)
+//   k_fog_apply   everything: hard, soft, noise (k-th PCG64 output by jump-ahead), min / max response, max intensity,
+//                 num_fog_responses
 //   k_fog_gain    intensity *= 255 / ceil(max intensity)                                            (:282-285)
 //
 // Numerics: float32 where NumPy 2 computes in float32 (r_0, exp, the hard-target product, r_0 ** 2, r_0 -/+ noise),
 // float64 elsewhere, no FMA contraction.  Two places are host-defined in the reference and therefore parity by
 // tolerance, not by bits (DESIGN.md 8): the float32 np.exp and the scalar float32 power r_0 ** 2 (neither is correctly
 // rounded on every host; the device uses the correctly rounded values), and pow() of the v2 / v3 noise factors.
-#include "common.cuh"
+#include "segments.cuh"
 
 namespace {
 
@@ -30,7 +31,6 @@ struct FogArgs {
     const float *pts;            // [N * F]
     int F;
     const int64_t *cloud_off;    // [B + 1] device
-    const int32_t *tile_base;    // [B + 1] device
     const double *lut;           // [LUT_N * 2] (fog_distance, fog_response)
     double alpha, beta, beta_0;
     int hard, soft, gain;
@@ -40,9 +40,9 @@ struct FogArgs {
     double *out;                 // [N * F]
     uint8_t *mask;               // [N]
     int32_t *rank;               // [N] or null
-    int *tile_cnt;               // [tiles]
-    int *tile_off;               // [tiles] exclusive, per cloud
-    unsigned long long *info;    // [B * 4] bit patterns: min response, max response, count, max intensity (ordered)
+    SegTiles seg;                // tiles of FOG_TILE rows, one class: fog points
+    unsigned long long *info;    // [B * 4] zero-filled; bit patterns: ~min response, max response, count, max intensity
+                                 // (ordered; the minimum is kept complemented so that 0 is the neutral value of both)
 };
 
 // correctly rounded float32 exp via float64 (np.exp on float32 is a host SIMD kernel, < 1 ulp but host defined)
@@ -104,53 +104,14 @@ __device__ __forceinline__ const float *stage_rows(const FogArgs &a, int64_t fir
 __global__ void __launch_bounds__(FOG_TILE) k_fog_count(FogArgs a)
 {
     __shared__ float s_in[FOG_TILE * FOG_STAGE_F];
-    __shared__ int cnt;
     const int b = blockIdx.y, tile = blockIdx.x;
     const int64_t beg = a.cloud_off[b];
     const int n = (int)(a.cloud_off[b + 1] - beg);
     if (tile * FOG_TILE >= n) return;
-    if (threadIdx.x == 0) cnt = 0;
     const int i = tile * FOG_TILE + threadIdx.x;
     const float *row = stage_rows(a, beg + (int64_t)tile * FOG_TILE, min(FOG_TILE, n - tile * FOG_TILE), s_in);
-    __syncthreads();
-    bool fog = false;
-    if (i < n) fog = soft_target(a, row).fog;
-    const unsigned m = __ballot_sync(0xffffffffu, fog);
-    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
-    __syncthreads();
-    if (threadIdx.x == 0) a.tile_cnt[a.tile_base[b] + tile] = cnt;
-}
-
-__global__ void __launch_bounds__(1024) k_fog_scan(FogArgs a)
-{
-    __shared__ int warp_tot[32];
-    __shared__ int carry;
-    const int b = blockIdx.x;
-    const int t0 = a.tile_base[b], nt = a.tile_base[b + 1] - t0;
-    if (threadIdx.x == 0) carry = 0;
-    __syncthreads();
-    for (int base = 0; base < nt; base += 1024) {
-        const int t = base + threadIdx.x;
-        const int v = t < nt ? a.tile_cnt[t0 + t] : 0;
-        int incl = v;
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, incl, s);
-            if ((threadIdx.x & 31) >= s) incl += u;
-        }
-        if ((threadIdx.x & 31) == 31) warp_tot[threadIdx.x >> 5] = incl;
-        __syncthreads();
-        int woff = 0;
-        for (int w = 0; w < (int)(threadIdx.x >> 5); w++) woff += warp_tot[w];
-        if (t < nt) a.tile_off[t0 + t] = carry + woff + incl - v;
-        __syncthreads();
-        if (threadIdx.x == 1023) carry += woff + incl;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) {
-        a.info[4 * b + 2] = (unsigned long long)carry;       // num_fog_responses
-        a.info[4 * b] = ~0ull;                                // running minimum of the responses
-    }
+    const bool fog = i < n && soft_target(a, row).fog;
+    seg_count<1>(fog ? 0 : -1, a.seg, b, tile);
 }
 
 // PCG64 (XSL-RR 128/64, numpy's default bit generator): the (k+1)-th state after `st` by jump-ahead, then its output
@@ -201,7 +162,6 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
 {
     __shared__ float s_in[FOG_TILE * FOG_STAGE_F];
     __shared__ double s_out[FOG_TILE * FOG_STAGE_F];
-    __shared__ int warp_cnt[FOG_TILE / 32];
     __shared__ unsigned long long s_min, s_max, s_imax;
     const int b = blockIdx.y, tile = blockIdx.x;
     const int64_t beg = a.cloud_off[b];
@@ -209,7 +169,6 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
     if (tile * FOG_TILE >= n) return;
     if (threadIdx.x == 0) { s_min = ~0ull; s_max = 0ull; s_imax = 0ull; }
     const int i = tile * FOG_TILE + threadIdx.x;
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
     const bool active = i < n;
     const int rows = min(FOG_TILE, n - tile * FOG_TILE);
     const bool staged = a.F <= FOG_STAGE_F;
@@ -217,9 +176,7 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
     s.fog = false;
     const float *row = stage_rows(a, beg + (int64_t)tile * FOG_TILE, rows, s_in);
     if (active) s = soft_target(a, row);
-    const unsigned m = __ballot_sync(0xffffffffu, active && s.fog);
-    if (lane == 0) warp_cnt[wid] = __popc(m);
-    __syncthreads();
+    const int rank = seg_rank<1, FOG_TILE>(active && s.fog ? 0 : -1, a.seg, b, tile);
     double out_i = 0.0;
     if (active) {
         double *o = staged ? s_out + threadIdx.x * a.F : a.out + (beg + i) * a.F;
@@ -235,8 +192,6 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
             a.mask[beg + i] = 0;
             if (a.rank) a.rank[beg + i] = -1;
         } else {
-            int rank = a.tile_off[a.tile_base[b] + tile] + __popc(m & ((1u << lane) - 1u));
-            for (int w = 0; w < wid; w++) rank += warp_cnt[w];
             const double scaling = __ddiv_rn(s.fog_distance, (double)s.r0);                  // :227
             double px = __dmul_rn((double)row[0], scaling), py = __dmul_rn((double)row[1], scaling),
                    pz = __dmul_rn((double)row[2], scaling);
@@ -289,8 +244,9 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
         for (int f = threadIdx.x; f < nf; f += FOG_TILE) __stcs(dst + f, s_out[f]);
     }
     if (threadIdx.x == 0) {
-        if (s_min != ~0ull) { atomicMin(&a.info[4 * b], s_min); atomicMax(&a.info[4 * b + 1], s_max); }
+        if (s_min != ~0ull) { atomicMax(&a.info[4 * b], ~s_min); atomicMax(&a.info[4 * b + 1], s_max); }
         if (a.gain) atomicMax(&a.info[4 * b + 3], s_imax);
+        if (a.soft && tile == 0) a.info[4 * b + 2] = (unsigned long long)a.seg.total[0][b];   // (0 for an empty cloud)
     }
 }
 
@@ -314,25 +270,22 @@ __global__ void k_fog_info(FogArgs a, int B, double *info_out)
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
     const unsigned long long cnt = a.info[4 * b + 2];
-    info_out[3 * b] = cnt ? ord_to(a.info[4 * b]) : __longlong_as_double(0x7ff0000000000000LL);
+    info_out[3 * b] = cnt ? ord_to(~a.info[4 * b]) : __longlong_as_double(0x7ff0000000000000LL);
     info_out[3 * b + 1] = cnt ? ord_to(a.info[4 * b + 1]) : 0.0;
     info_out[3 * b + 2] = (double)cnt;
 }
 
-struct FogLayout { int64_t off, tile_base, tile_cnt, tile_off, info, rng, total; };
+struct FogLayout { int64_t off, seg, seg_total, info, rng, total; };
 
 FogLayout fog_layout(int64_t n_total, int n_clouds)
 {
     FogLayout L;
-    const int64_t tiles = n_total / FOG_TILE + n_clouds + 1;
     int64_t o = 0;
-    auto take = [&](int64_t bytes) { const int64_t at = o; o = (o + bytes + 255) / 256 * 256; return at; };
-    L.off = take((int64_t)(n_clouds + 1) * 8);
-    L.tile_base = take((int64_t)(n_clouds + 1) * 4);
-    L.tile_cnt = take(tiles * 4);
-    L.tile_off = take(tiles * 4);
-    L.info = take((int64_t)n_clouds * 4 * 8);
-    L.rng = take((int64_t)n_clouds * 4 * 8);
+    L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
+    L.seg = o;       o += seg_ws_bytes(n_total, n_clouds, FOG_TILE, 1);
+    L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 4, 256);
+    L.info = o;      o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
+    L.rng = o;       o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
     L.total = o;
     return L;
 }
@@ -353,31 +306,21 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
                                     void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
-    if (!h_cloud_offsets || n_clouds < 0 || !d_out || !d_out_fog_mask || !d_out_info || !d_workspace)
-        return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
+    BatchGeometry g;
+    if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, FOG_TILE, g)) return rc;
+    if (!d_out || !d_out_fog_mask || !d_out_info || !d_workspace) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
     if (n_features < 4 || n_features > 16) return lss_fail(e, LSS_ERR_INVALID_ARG, "n_features must be in 4..16");
-    if (n_clouds > 65535) return lss_fail(e, LSS_ERR_INVALID_ARG, "at most 65535 clouds per call");
-    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
     const bool soft = flags & LSS_FOG_SOFT;
     if (soft && !d_lut) return lss_fail(e, LSS_ERR_INVALID_ARG, "the soft target needs the integral look-up table");
     if (noise > 0 && soft && (noise_variant < 1 || noise_variant > 4))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "noise variant must be 1..4 (NotImplementedError in the reference)");
     const int B = n_clouds;
-    const int64_t N = h_cloud_offsets[B];
-    int64_t max_n = 0;
-    std::vector<int32_t> h_tb(B + 1, 0);
-    for (int b = 0; b < B; b++) {
-        const int64_t n = h_cloud_offsets[b + 1] - h_cloud_offsets[b];
-        if (n < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets must be non-decreasing");
-        if (n >= (1LL << 31)) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud too large");
-        max_n = std::max(max_n, n);
-        h_tb[b + 1] = h_tb[b] + (int32_t)((n + FOG_TILE - 1) / FOG_TILE);
-    }
+    const int64_t N = g.n;
     if (!d_points && N > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
     const FogLayout L = fog_layout(N, B);
     if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
-    DeviceGuard g(e->device);
+    DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)d_workspace;
 
@@ -385,7 +328,8 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
     a.pts = d_points;
     a.F = n_features;
     a.cloud_off = (const int64_t *)(ws + L.off);
-    a.tile_base = (const int32_t *)(ws + L.tile_base);
+    a.seg = seg_tiles(ws + L.seg, B);
+    a.seg.total[0] = (int32_t *)(ws + L.seg_total);
     a.lut = d_lut;
     a.alpha = alpha; a.beta = beta; a.beta_0 = beta_0;
     a.hard = (flags & LSS_FOG_HARD) ? 1 : 0;
@@ -398,12 +342,10 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
     a.out = d_out;
     a.mask = d_out_fog_mask;
     a.rank = d_out_rank;
-    a.tile_cnt = (int *)(ws + L.tile_cnt);
-    a.tile_off = (int *)(ws + L.tile_off);
     a.info = (unsigned long long *)(ws + L.info);
 
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.tile_base, h_tb.data(), sizeof(int32_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
+                                         (int32_t *)a.seg.tile_base, st));
     if (h_rng_state && soft && noise > 0 && noise_variant != 4 && !d_ext_noise) {
         LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.rng, h_rng_state, sizeof(uint64_t) * 4 * B, st));
         a.rng = (const unsigned long long *)(ws + L.rng);
@@ -413,19 +355,16 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
         z.add(ws + L.info, (size_t)B * 4 * 8);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
-    const int max_tiles = (int)((max_n + FOG_TILE - 1) / FOG_TILE);
+    const dim3 grid((unsigned)((g.max_n + FOG_TILE - 1) / FOG_TILE), B);
     if (N > 0) {
         KernelTimer kt(e, LSS_K_FOG, st);
         if (soft) {
-            k_fog_count<<<dim3(max_tiles, B), FOG_TILE, 0, st>>>(a);
-            k_fog_scan<<<B, 1024, 0, st>>>(a);
-            e->launches += 2;
+            LSS_CUDA_CHECK(e, lss_launch(e, k_fog_count, grid, FOG_TILE, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<1>, B, SEG_SCAN_TPB, 0, st, a.seg));
         }
-        k_fog_apply<<<dim3(max_tiles, B), FOG_TILE, 0, st>>>(a);
-        if (a.gain) { k_fog_gain<<<dim3(max_tiles, B), FOG_TILE, 0, st>>>(a); e->launches++; }
+        LSS_CUDA_CHECK(e, lss_launch(e, k_fog_apply, grid, FOG_TILE, 0, st, a));
+        if (a.gain) LSS_CUDA_CHECK(e, lss_launch(e, k_fog_gain, grid, FOG_TILE, 0, st, a));
     }
-    k_fog_info<<<(B + 127) / 128, 128, 0, st>>>(a, B, d_out_info);
-    e->launches++;
-    LSS_CUDA_CHECK(e, cudaGetLastError());
+    LSS_CUDA_CHECK(e, lss_launch(e, k_fog_info, (B + 127) / 128, 128, 0, st, a, B, d_out_info));
     return LSS_OK;
 }

@@ -128,9 +128,6 @@ extern "C" lss_status lss_gather_push(lss_engine *e, const float *d_points, cons
     // with multicast stores, at most 64 with per-peer stores); LSS_GATHER_BLOCKS overrides them.
     if (n_blocks <= 0) n_blocks = d_mc_points ? std::max(1, e->n_sm / 4) : std::min(e->n_sm, 64);
     cudaStream_t st = (cudaStream_t)stream;
-    if (d_mc_points) k_gather_push<true><<<n_blocks, GATHER_TPB, 0, st>>>(a);
-    else k_gather_push<false><<<n_blocks, GATHER_TPB, 0, st>>>(a);
-    e->launches++;
-    LSS_CUDA_CHECK(e, cudaGetLastError());
+    LSS_CUDA_CHECK(e, lss_launch(e, d_mc_points ? k_gather_push<true> : k_gather_push<false>, n_blocks, GATHER_TPB, 0, st, a));
     return LSS_OK;
 }

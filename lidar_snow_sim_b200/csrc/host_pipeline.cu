@@ -165,15 +165,12 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
                                                      double *h_out_stats, int *ticket_out)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
-    if (!h_cloud_offsets || !h_order || n_clouds <= 0 || !h_out_points || !h_out_counts || !h_out_stats || !ticket_out)
+    if (!h_order || n_clouds <= 0 || !h_out_points || !h_out_counts || !h_out_stats || !ticket_out)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument / empty batch");
-    if (n_clouds > 65535) return lss_fail(e, LSS_ERR_INVALID_ARG, "at most 65535 clouds per call");
-    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
-    for (int b = 0; b < n_clouds; b++)
-        if (h_cloud_offsets[b + 1] < h_cloud_offsets[b])
-            return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets must be non-decreasing");
+    BatchGeometry geo;
+    if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, 0, geo)) return rc;
     const int B = n_clouds;
-    const int64_t N = h_cloud_offsets[B];
+    const int64_t N = geo.n;
     if (!h_points && N > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
     if (!e->has_sensor) return lss_fail(e, LSS_ERR_NO_SENSOR, "sensor constants not set (lss_set_sensor)");
     auto it = e->tables.find(table_id);
@@ -253,7 +250,6 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
         a.beam_divergence_deg = beam_divergence_deg;
         a.d_theta = nullptr;
         a.h_thresh_poly = h_thresh_poly ? h_thresh_poly + 3 * (size_t)b0 : nullptr;
-        a.d_thresh_poly = nullptr;
         a.noise_floor = noise_floor;
         a.flags = flags;
         a.d_out_points = sl.d_out + r0 * 5;
@@ -276,10 +272,8 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
             if (h_out_dev) {        // page-locked result buffer: only the kept rows travel (see k_copy_rows_out)
                 // cloud offsets of this chunk on the device: the snowfall stage uploaded them to the head of its workspace
                 const int64_t *d_off_chunk = (const int64_t *)(ws + lss_snowfall_ws_cloud_off(nr, nb));
-                k_copy_rows_out<<<dim3(COPY_OUT_BLOCKS, nb), 256, 0, p->s_d2h>>>(sl.d_out + r0 * 5, d_off_chunk, sl.d_counts + b0,
-                                                                               h_out_dev + r0 * 5);
-                e->launches++;
-                ce = cudaGetLastError();
+                ce = lss_launch(e, k_copy_rows_out, dim3(COPY_OUT_BLOCKS, nb), 256, 0, p->s_d2h, sl.d_out + r0 * 5,
+                                d_off_chunk, sl.d_counts + b0, h_out_dev + r0 * 5);
             } else {
                 ce = cudaMemcpyAsync(h_out_points + r0 * 5, sl.d_out + r0 * 5, (size_t)nr * 5 * sizeof(float),
                                      cudaMemcpyDeviceToHost, p->s_d2h);

@@ -248,10 +248,7 @@ extern "C" lss_status lss_lisa_batch(lss_engine *e, const double *d_points, int 
     a.status = e->d_status;
     const long long warps = n_points;
     const unsigned blocks = (unsigned)std::min<long long>((warps + 7) / 8, (long long)e->n_sm * 64);
-    {
-        KernelTimer kt(e, LSS_K_FOG, (cudaStream_t)stream);
-        k_lisa<<<blocks, 256, 0, (cudaStream_t)stream>>>(a);
-    }
-    LSS_CUDA_CHECK(e, cudaGetLastError());
+    KernelTimer kt(e, LSS_K_LISA, (cudaStream_t)stream);
+    LSS_CUDA_CHECK(e, lss_launch(e, k_lisa, blocks, 256, 0, (cudaStream_t)stream, a));
     return LSS_OK;
 }

@@ -625,8 +625,6 @@ __global__ void k_poly_solve(PreArgs a, int n_blocks, double *poly_out /* [B*3] 
     if (ymins_out) for (int k = 0; k < HIST_NX; k++) ymins_out[b * HIST_NX + k] = cp.n_ground >= 3 ? a.ymins[b * HIST_NX + k] : -1;
 }
 
-inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
-
 }  // namespace
 
 struct PrepassLayout { int64_t cp, win, stage, tile_cnt, tile_base, hist, trial, partial, plane_in, ymins, ymins_in, total; int max_blocks; };
@@ -711,26 +709,24 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
         if (h_plane_in) {
             double *d_plane = (double *)(ws + L.plane_in);
             LSS_CUDA_CHECK(e, lss_stage_upload(e, d_plane, h_plane_in, sizeof(double) * 4 * B, stream));
-            k_set_plane<<<(B + 127) / 128, 128, 0, stream>>>(a, d_plane);
+            LSS_CUDA_CHECK(e, lss_launch(e, k_set_plane, (B + 127) / 128, 128, 0, stream, a, d_plane));
         } else {
             const int max_tiles = (int)std::max<int64_t>(1, (max_n + WTILE - 1) / WTILE);
-            k_window_tiles<<<dim3(max_tiles, B), WTILE, 0, stream>>>(a);
+            LSS_CUDA_CHECK(e, lss_launch(e, k_window_tiles, dim3(max_tiles, B), WTILE, 0, stream, a));
             const size_t gather_smem = sizeof(int) * ((size_t)max_tiles * (WTILE / 32) + 2);
             if (gather_smem > 48 * 1024)
                 LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_window_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gather_smem));
-            k_window_gather<<<B, 1024, gather_smem, stream>>>(a);
-            k_window_mad<<<B, 1024, 0, stream>>>(a);
-            k_ransac_trials<<<dim3(RANSAC_T, B), PP_TPB, 0, stream>>>(a);
-            k_ransac_refit<<<B, PP_TPB, 0, stream>>>(a);
-            e->launches += 4;
+            LSS_CUDA_CHECK(e, lss_launch(e, k_window_gather, B, 1024, gather_smem, stream, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_window_mad, B, 1024, 0, stream, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_ransac_trials, dim3(RANSAC_T, B), PP_TPB, 0, stream, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_ransac_refit, B, PP_TPB, 0, stream, a));
         }
-        k_ground_stats<<<dim3(nblk, B), PP_TPB, 0, stream>>>(a);
-        k_ground_stats_final<<<B, 32, 0, stream>>>(a, nblk);
-        k_ground_hist<<<dim3(nblk, B), PP_TPB, 0, stream>>>(a);
-        k_hist_minima<<<B, 1024, 0, stream>>>(a);
-        k_poly_solve<<<B, 32, 0, stream>>>(a, nblk, d_poly_out, d_plane_out, io.d_fit_out, io.d_ymins_out);
-        e->launches += 4;
+        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats, dim3(nblk, B), PP_TPB, 0, stream, a));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats_final, B, 32, 0, stream, a, nblk));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_hist, dim3(nblk, B), PP_TPB, 0, stream, a));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_hist_minima, B, 1024, 0, stream, a));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_poly_solve, B, 32, 0, stream, a, nblk, d_poly_out, d_plane_out, io.d_fit_out,
+                                     io.d_ymins_out));
     }
-    LSS_CUDA_CHECK(e, cudaGetLastError());
     return LSS_OK;
 }

@@ -255,8 +255,6 @@ __global__ void __launch_bounds__(1024) k_count(SampArgs a)
     if (tid == 0) a.counts[p] = run_cnt;
 }
 
-inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
-
 struct SampLayout { int64_t cand, state, conf, hkey, hhead, next, undecided, flags, total; int H, U; };
 
 SampLayout samp_layout(int n_planes, int64_t M)
@@ -340,12 +338,14 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
             break;
         }
         const dim3 grid((unsigned)((n_candidates + 255) / 256), n_planes);
-        k_darts<<<grid, 256, 0, st>>>(a);
-        k_conflicts<<<grid, 256, 0, st>>>(a);
-        k_resolve<<<(n_planes + 63) / 64, 64, 0, st>>>(a);
-        k_cut<<<n_planes, 1024, 0, st>>>(a);
-        k_count<<<n_planes, 1024, 0, st>>>(a);
-        e->launches += 5;
+        if (lss_launch(e, k_darts, grid, 256, 0, st, a) != cudaSuccess ||
+            lss_launch(e, k_conflicts, grid, 256, 0, st, a) != cudaSuccess ||
+            lss_launch(e, k_resolve, (n_planes + 63) / 64, 64, 0, st, a) != cudaSuccess ||
+            lss_launch(e, k_cut, n_planes, 1024, 0, st, a) != cudaSuccess ||
+            lss_launch(e, k_count, n_planes, 1024, 0, st, a) != cudaSuccess) {
+            rc = lss_fail(e, LSS_ERR_CUDA, "sampler launch failed");
+            break;
+        }
         if (d_candidates_out)
             cudaMemcpyAsync(d_candidates_out, a.cand, sizeof(double) * 3 * (size_t)n_planes * n_candidates,
                             cudaMemcpyDeviceToDevice, st);

@@ -335,8 +335,6 @@ __global__ void __launch_bounds__(TILE) k_scatter(const float *__restrict__ aug,
     }
 }
 
-inline int64_t align_up(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
-
 struct WsLayout {
     int64_t aug, keep_d, keep_i, keep_tag, code_keep, code_all, nocc, hist_keep, hist_all, hist_rows, cloud_off, tile_base,
         order, thresh, counters, counters_bytes, list, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
@@ -394,21 +392,17 @@ int64_t lss_snowfall_ws_cloud_off(int64_t n_total, int n_clouds) { return ws_lay
 lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t stream)
 {
     const int B = s.n_clouds;
-    const int64_t N = s.h_cloud_offsets[B] - s.h_cloud_offsets[0];
-    if (s.h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
-    int64_t max_n = 0;
-    for (int b = 0; b < B; b++) {
-        int64_t n = s.h_cloud_offsets[b + 1] - s.h_cloud_offsets[b];
-        if (n < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets must be non-decreasing");
-        if (n >= (1LL << 31)) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud too large");
-        max_n = n > max_n ? n : max_n;
-    }
+    // scatter tiles (TILE rows) and warp tiles (32 rows) of each cloud
+    BatchGeometry g, wg;
+    if (lss_status rc = lss_batch_geometry(e, s.h_cloud_offsets, B, TILE, g)) return rc;
+    if (lss_status rc = lss_batch_geometry(e, s.h_cloud_offsets, B, 32, wg)) return rc;
+    const int64_t N = g.n, max_n = g.max_n;
     for (int k = 0; k < B * LSS_N_CHANNELS; k++)
         if (s.h_order[k] < 0 || s.h_order[k] >= s.ts->n_planes)
             return lss_fail(e, LSS_ERR_NO_TABLE, "order[] names a plane that is not in the table set");
     const WsLayout w = ws_layout(N, B);
     if (s.workspace_bytes < w.total || !s.d_workspace) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
-    if ((s.flags & LSS_FLAG_THRESHOLD_FILTER) && !s.h_thresh_poly && !s.d_thresh_poly && !(s.flags & LSS_FLAG_DEVICE_PREPASS))
+    if ((s.flags & LSS_FLAG_THRESHOLD_FILTER) && !s.h_thresh_poly && !(s.flags & LSS_FLAG_DEVICE_PREPASS))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "threshold filter needs h_thresh_poly or LSS_FLAG_DEVICE_PREPASS");
     if ((s.flags & LSS_FLAG_CAMERA_FOV) && !e->has_camera)
         return lss_fail(e, LSS_ERR_NO_SENSOR, "camera calibration not set");
@@ -416,15 +410,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     if (!(div_rad > 0) || div_rad > s.ts->max_div_rad * (1 + 1e-12))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "beam_divergence exceeds the value the table set was built for");
     const int max_tiles = (int)((max_n + TILE - 1) / TILE);
-    // [0, B] first scatter tile (TILE rows) of each cloud, [B + 1, 2 B + 1] first warp tile (32 rows) of each cloud
-    std::vector<int32_t> h_tile_base(2 * (B + 1), 0);
-    int32_t *h_wtile_base = h_tile_base.data() + B + 1;
-    for (int b = 0; b < B; b++) {
-        const int64_t n = s.h_cloud_offsets[b + 1] - s.h_cloud_offsets[b];
-        h_tile_base[b + 1] = h_tile_base[b] + (int32_t)((n + TILE - 1) / TILE);
-        h_wtile_base[b + 1] = h_wtile_base[b] + (int32_t)((n + 31) / 32);
-    }
-    const int n_wtiles = h_wtile_base[B];
+    const int n_wtiles = wg.tile_base[B];
     if ((s.d_out_perm || s.d_out_nocc) && !s.d_out_full)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "d_out_perm / d_out_nocc need d_out_full");
 
@@ -444,10 +430,11 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     unsigned *d_att_cnt = (unsigned *)(ws + w.counters + align_up((int64_t)B * 2 * 4, 8));
     unsigned long long *d_att_sum = (unsigned long long *)((char *)d_att_cnt + (int64_t)B * LSS_N_CHANNELS * 4);
 
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, s.h_cloud_offsets, sizeof(int64_t) * (B + 1), stream));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_tile_base, h_tile_base.data(), sizeof(int32_t) * 2 * (B + 1), stream));
+    // d_tile_base: [0, B] first scatter tile of each cloud, [B + 1, 2 B + 1] first warp tile of each cloud
+    g.tile_base.insert(g.tile_base.end(), wg.tile_base.begin(), wg.tile_base.end());
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, s.h_cloud_offsets, B, g.tile_base, d_off, d_tile_base, stream));
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS, stream));
-    if (s.h_thresh_poly && !s.d_thresh_poly)
+    if (s.h_thresh_poly)
         LSS_CUDA_CHECK(e, lss_stage_upload(e, d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B, stream));
     int *d_list_hdr = (int *)(ws + w.list);                                 // (LIST_HDR_BYTES)
     {
@@ -480,7 +467,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.theta = s.d_theta;
     a.cloud_off = d_off;
     a.order = d_order;
-    a.thresh = s.d_thresh_poly ? s.d_thresh_poly : d_thresh;
+    a.thresh = d_thresh;
     a.sensor = e->d_sensor;
     a.camera = e->d_camera;
     a.R = e->d_R;
@@ -511,7 +498,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     // solve kernel holds every SM's registers until its last tile, so a chain forked after the scan would find no room for
     // its 1024-thread CTAs and become the critical path.
     const bool device_prepass = (s.flags & LSS_FLAG_THRESHOLD_FILTER) && (s.flags & LSS_FLAG_DEVICE_PREPASS) &&
-                                !s.h_thresh_poly && !s.d_thresh_poly;
+                                !s.h_thresh_poly;
     cudaEvent_t ev_join = nullptr;
     if (device_prepass) {
         cudaStream_t side = nullptr;
@@ -532,6 +519,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
         }
     }
     a.hit_cap = (int)std::min<int64_t>(N * HIT_POS_PER_BEAM + 4096, 0x7fffffff);
+    cudaError_t ce;                                 // (checked after the join: never leave the side stream dangling)
     {
         KernelTimer kt(e, LSS_K_SNOWFALL, stream);
         // 1. scan: all beams; the ones without occluders are finished, the others go to the solve list with their hits
@@ -544,46 +532,46 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             unsigned long long *d_ent = (unsigned long long *)(d_sched_hist + 2 * SCHED_BINS);
             unsigned long long *d_sched = d_ent + w.sched_tiles;
             const int max_wtiles = (int)((max_n + 31) / 32);
-            k_sched_key<<<dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B), SCHED_KEY_TPB, 0, stream>>>(
-                s.d_points, d_off, d_order, d_tile_base + B + 1, d_ent, d_sched_hist);
-            k_sched_sort<<<(unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)), 256, 0, stream>>>(
-                d_ent, d_sched, d_sched_hist, n_wtiles);
-            e->launches++;                                  // (the other one is counted by the LSS_K_SNOWFALL bracket)
+            ce = lss_launch(e, k_sched_key, dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B),
+                            SCHED_KEY_TPB, 0, stream, s.d_points, d_off, d_order, d_tile_base + B + 1, d_ent, d_sched_hist);
+            if (ce == cudaSuccess)
+                ce = lss_launch(e, k_sched_sort, (unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)),
+                                256, 0, stream, d_ent, d_sched, d_sched_hist, n_wtiles);
             a.sched = d_sched;
             a.n_wtiles = n_wtiles;
         }
-        {
+        if (ce == cudaSuccess) {
             KernelTimer ks(e, LSS_K_SCAN, stream);
-            lss_launch_scan(a, stream);
+            ce = lss_launch_scan(e, a, stream);
         }
         // 2. solve: the listed beams, class by class, one warp per tile of 32 (persistent grid)
-        {
+        if (ce == cudaSuccess) {
             KernelTimer ks(e, LSS_K_SOLVE, stream);
-            lss_launch_solve(a, d_list_hdr + 1, e->n_sm, stream);
+            ce = lss_launch_solve(e, a, d_list_hdr + 1, stream);
         }
     }
     if (ev_join) LSS_CUDA_CHECK(e, cudaStreamWaitEvent(stream, ev_join, 0));
+    LSS_CUDA_CHECK(e, ce);
     {
         KernelTimer kt(e, LSS_K_FINALIZE, stream);
-        k_keep<<<dim3(max_tiles, B), KEEP_TPB, 0, stream>>>(a);
+        LSS_CUDA_CHECK(e, lss_launch(e, k_keep, dim3(max_tiles, B), KEEP_TPB, 0, stream, a));
     }
     {
         KernelTimer kt(e, LSS_K_SORT, stream);
-        k_tile_scan<<<B, 1024, 0, stream>>>(d_hist_keep, d_tile_base, s.d_out_counts, s.d_out_stats, d_counters,
-                                            d_att_cnt, d_att_sum, e->d_sensor);
+        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, d_hist_keep, d_tile_base, s.d_out_counts,
+                                     s.d_out_stats, d_counters, d_att_cnt, d_att_sum, e->d_sensor));
     }
     {
         KernelTimer kt(e, LSS_K_COMPACT, stream);
-        k_scatter<<<dim3(max_tiles, B), TILE, 0, stream>>>(d_aug, d_code_keep, d_hist_keep, d_off, d_tile_base,
-                                                           s.d_out_points, nullptr, nullptr, nullptr);
+        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, d_aug, d_code_keep, d_hist_keep, d_off,
+                                     d_tile_base, s.d_out_points, nullptr, nullptr, nullptr));
     }
     if (want_all) {     // un-filtered, channel-sorted debug views (tests): full rows, original index, occluder counts
         KernelTimer kt(e, LSS_K_COMPACT, stream);
-        k_tile_scan<<<B, 1024, 0, stream>>>(d_hist_all, d_tile_base, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
-        k_scatter<<<dim3(max_tiles, B), TILE, 0, stream>>>(d_aug, d_code_all, d_hist_all, d_off, d_tile_base, s.d_out_full,
-                                                           d_nocc_tmp, s.d_out_nocc, s.d_out_perm);
-        e->launches++;
+        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, d_hist_all, d_tile_base, nullptr, nullptr, nullptr,
+                                     nullptr, nullptr, nullptr));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, d_aug, d_code_all, d_hist_all, d_off,
+                                     d_tile_base, s.d_out_full, d_nocc_tmp, s.d_out_nocc, s.d_out_perm));
     }
-    LSS_CUDA_CHECK(e, cudaGetLastError());
     return LSS_OK;
 }

@@ -821,18 +821,17 @@ extern "C" lss_status lss_debug_azimuth(lss_engine *e, const float *d_y, const f
     if (!e || !d_y || !d_x || !d_out || n < 0) return LSS_ERR_INVALID_ARG;
     if (n == 0) return LSS_OK;
     DeviceGuard g(e->device);
-    k_debug_azimuth<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_y, d_x, d_out, n);
-    e->launches++;
-    LSS_CUDA_CHECK(e, cudaGetLastError());
+    LSS_CUDA_CHECK(e, lss_launch(e, k_debug_azimuth, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, d_y, d_x,
+                                 d_out, n));
     return LSS_OK;
 }
 
-void lss_launch_scan(const DevArgs &a, cudaStream_t stream)
+cudaError_t lss_launch_scan(lss_engine *e, const DevArgs &a, cudaStream_t stream)
 {
-    k_scan<<<(unsigned)((a.n_wtiles + SNOW_WARPS - 1) / SNOW_WARPS), SNOW_TPB, 0, stream>>>(a);
+    return lss_launch(e, k_scan, (unsigned)((a.n_wtiles + SNOW_WARPS - 1) / SNOW_WARPS), SNOW_TPB, 0, stream, a);
 }
 
-void lss_launch_solve(const DevArgs &a, int *tile_cursor, int n_sm, cudaStream_t stream)
+cudaError_t lss_launch_solve(lss_engine *e, const DevArgs &a, int *tile_cursor, cudaStream_t stream)
 {
-    k_solve<<<(unsigned)(n_sm * SOLVE_CTAS_PER_SM), SOLVE_TPB, 0, stream>>>(a, tile_cursor);
+    return lss_launch(e, k_solve, (unsigned)(e->n_sm * SOLVE_CTAS_PER_SM), SOLVE_TPB, 0, stream, a, tile_cursor);
 }

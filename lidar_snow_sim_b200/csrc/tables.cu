@@ -247,8 +247,7 @@ lss_status lss_build_tables(lss_engine *e, TableSet &ts, const double *d_xyr, co
 
     const int tpb = 256;
     const unsigned grid = (unsigned)((np + tpb - 1) / tpb);
-    k_particle_records<<<grid, tpb, 0, stream>>>(bp);
-    e->launches++;
+    LSS_CUDA_CHECK(e, lss_launch(e, k_particle_records, grid, tpb, 0, stream, bp));
     std::vector<int32_t> counts((size_t)n_planes * nb), starts((size_t)n_planes * (nb + 1));
     LSS_CUDA_CHECK(e, cudaMemcpyAsync(counts.data(), d_counts, sizeof(int32_t) * counts.size(),
                                       cudaMemcpyDeviceToHost, stream));
@@ -267,11 +266,9 @@ lss_status lss_build_tables(lss_engine *e, TableSet &ts, const double *d_xyr, co
     LSS_CUDA_CHECK(e, cudaMemcpyAsync(ts.d_bucket_start, starts.data(), sizeof(int32_t) * starts.size(),
                                       cudaMemcpyHostToDevice, stream));
     bp.entries = ts.d_entries;
-    k_fill_entries<<<grid, tpb, 0, stream>>>(bp);
+    LSS_CUDA_CHECK(e, lss_launch(e, k_fill_entries, grid, tpb, 0, stream, bp));
     const unsigned grid_b = (unsigned)((n_planes * nb + 127) / 128);
-    k_sort_buckets<<<grid_b, 128, 0, stream>>>(bp);
-    e->launches += 2;
-    LSS_CUDA_CHECK(e, cudaGetLastError());
+    LSS_CUDA_CHECK(e, lss_launch(e, k_sort_buckets, grid_b, 128, 0, stream, bp));
     LSS_CUDA_CHECK(e, cudaStreamSynchronize(stream));
     ts.d_plane_off = d_off;
     cudaFree(d_span_lo);

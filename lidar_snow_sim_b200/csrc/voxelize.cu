@@ -16,14 +16,14 @@
 // first appearance) and the max_points smallest point indices (= the points kept).  Both are order-independent
 // reductions:
 //   k_vox_insert    hash table per cloud (open addressing, 64-bit voxel key): atomicMin of the point index, count
-//   k_vox_flags / k_vox_scan / k_vox_assign   a point is "first of its voxel" iff the table's minimum is its own index;
-//                   exclusive scan of those flags in point order = the voxel number; coordinates, counts
+//   k_vox_flags / k_seg_scan / k_vox_assign   a point is "first of its voxel" iff the table's minimum is its own index;
+//                   exclusive scan of those flags in point order (segments.cuh) = the voxel number; coordinates, counts
 //   k_vox_cascade   the max_points smallest indices of every kept voxel: a cascade of atomicMin over max_points levels
 //                   (the value displaced from / rejected by level t moves on to level t + 1: level t ends up with the
 //                   (t+1)-th smallest index whatever the interleaving)
 //   k_vox_write     every point finds its rank in its voxel's level list and copies its row there
 // Everything is integer / float32 arithmetic without reassociation: bit-identical to the sequential rule.
-#include "common.cuh"
+#include "segments.cuh"
 #include <climits>
 
 namespace {
@@ -42,19 +42,13 @@ struct VoxArgs {
     unsigned long long *h_key;     // [2N + B] hash slots; cloud b owns [2 off[b] + b, 2 off[b+1] + b + 1)
     int *h_first, *h_count, *h_vid;
     int *slot_of;                  // [N] slot of each point's voxel, -1 = point not in the grid
-    int *tile_cnt, *tile_off;
-    const int32_t *tile_base;      // [B+1]
+    SegTiles seg;                  // tiles of VTILE rows, one class: first point of its voxel
     int *top;                      // [B * max_voxels * max_points]
     float *out_vox;                // [B * max_voxels * max_points * F]
     int32_t *out_coords;           // [B * max_voxels * 4]  (batch index, z, y, x)
     int32_t *out_num;              // [B * max_voxels]
     int32_t *out_nvox;             // [B]
 };
-
-__device__ __forceinline__ int cloud_rows(const VoxArgs &a, int b)
-{
-    return a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - a.cloud_off[b]);
-}
 
 // voxel coordinate of a point, or false if it is masked / outside the grid
 __device__ __forceinline__ bool voxel_of(const VoxArgs &a, const float *row, int &cx, int &cy, int &cz)
@@ -80,7 +74,7 @@ __global__ void __launch_bounds__(256) k_vox_insert(VoxArgs a)
 {
     const int b = blockIdx.y;
     const int64_t beg = a.cloud_off[b];
-    const int n = cloud_rows(a, b);
+    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     int cx, cy, cz, slot = -1;
@@ -101,80 +95,38 @@ __global__ void __launch_bounds__(256) k_vox_insert(VoxArgs a)
     a.slot_of[beg + i] = slot;
 }
 
+__device__ __forceinline__ bool first_of_voxel(const VoxArgs &a, int b, int i, int &slot)
+{
+    slot = -1;
+    if (i >= seg_rows(a.cloud_off, a.cloud_cnt, b)) return false;
+    slot = a.slot_of[a.cloud_off[b] + i];
+    return slot >= 0 && a.h_first[slot] == i;
+}
+
 __global__ void __launch_bounds__(VTILE) k_vox_flags(VoxArgs a)
 {
-    __shared__ int cnt;
     const int b = blockIdx.y, tile = blockIdx.x;
-    const int n = cloud_rows(a, b);
-    const int n_tiles = a.tile_base[b + 1] - a.tile_base[b];
-    if (tile >= n_tiles) return;
-    if (threadIdx.x == 0) cnt = 0;
-    __syncthreads();
-    const int i = tile * VTILE + threadIdx.x;
-    bool first = false;
-    if (i < n) {
-        const int slot = a.slot_of[a.cloud_off[b] + i];
-        first = slot >= 0 && a.h_first[slot] == i;
-    }
-    const unsigned m = __ballot_sync(0xffffffffu, first);
-    if ((threadIdx.x & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
-    __syncthreads();
-    if (threadIdx.x == 0) a.tile_cnt[a.tile_base[b] + tile] = cnt;
+    if (tile >= a.seg.tile_base[b + 1] - a.seg.tile_base[b]) return;
+    int slot;
+    const bool first = first_of_voxel(a, b, tile * VTILE + threadIdx.x, slot);
+    seg_count<1>(first ? 0 : -1, a.seg, b, tile);
 }
 
-__global__ void __launch_bounds__(1024) k_vox_scan(VoxArgs a)
-{
-    __shared__ int wsum[32];
-    __shared__ int run;
-    const int b = blockIdx.x;
-    const int t0 = a.tile_base[b], nt = a.tile_base[b + 1] - t0;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) run = 0;
-    __syncthreads();
-    for (int base = 0; base < nt; base += 1024) {
-        const int t = base + tid;
-        const int v = t < nt ? a.tile_cnt[t0 + t] : 0;
-        int incl = v;
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) { const int u = __shfl_up_sync(0xffffffffu, incl, s); if (lane >= s) incl += u; }
-        if (lane == 31) wsum[warp] = incl;
-        __syncthreads();
-        int o = run;
-        for (int wv = 0; wv < warp; wv++) o += wsum[wv];
-        if (t < nt) a.tile_off[t0 + t] = o + incl - v;
-        __syncthreads();
-        if (tid == 1023) run = o + incl;
-        __syncthreads();
-    }
-    if (tid == 0) a.out_nvox[b] = run < a.max_voxels ? run : a.max_voxels;
-}
-
+// Tile 0 of every cloud also writes the cloud's voxel count.
 __global__ void __launch_bounds__(VTILE) k_vox_assign(VoxArgs a)
 {
-    __shared__ int wcnt[VTILE / 32];
     const int b = blockIdx.y, tile = blockIdx.x;
-    const int n = cloud_rows(a, b);
-    const int n_tiles = a.tile_base[b + 1] - a.tile_base[b];
-    if (tile >= n_tiles) return;
-    const int64_t beg = a.cloud_off[b];
+    if (tile == 0 && threadIdx.x == 0) a.out_nvox[b] = min(a.seg.total[0][b], a.max_voxels);
+    if (tile >= a.seg.tile_base[b + 1] - a.seg.tile_base[b]) return;
     const int i = tile * VTILE + threadIdx.x;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int slot = -1;
-    bool first = false;
-    if (i < n) {
-        slot = a.slot_of[beg + i];
-        first = slot >= 0 && a.h_first[slot] == i;
-    }
-    const unsigned m = __ballot_sync(0xffffffffu, first);
-    if (lane == 0) wcnt[warp] = __popc(m);
-    __syncthreads();
+    int slot;
+    const bool first = first_of_voxel(a, b, i, slot);
+    const int vid = seg_rank<1, VTILE>(first ? 0 : -1, a.seg, b, tile);
     if (!first) return;
-    int vid = a.tile_off[a.tile_base[b] + tile] + __popc(m & ((1u << lane) - 1u));
-    for (int wv = 0; wv < warp; wv++) vid += wcnt[wv];
     if (vid >= a.max_voxels) { a.h_vid[slot] = -1; return; }          // later voxels are skipped (and their points)
     a.h_vid[slot] = vid;
     int cx, cy, cz;
-    voxel_of(a, a.pts + (beg + i) * a.F, cx, cy, cz);
+    voxel_of(a, a.pts + (a.cloud_off[b] + i) * a.F, cx, cy, cz);
     int32_t *c = a.out_coords + ((size_t)b * a.max_voxels + vid) * 4;
     c[0] = b; c[1] = cz; c[2] = cy; c[3] = cx;                         // collate_batch's batch index + spconv's (z, y, x)
     const int cnt = a.h_count[slot];
@@ -185,7 +137,7 @@ __global__ void __launch_bounds__(256) k_vox_cascade(VoxArgs a)
 {
     const int b = blockIdx.y;
     const int64_t beg = a.cloud_off[b];
-    const int n = cloud_rows(a, b);
+    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     const int slot = a.slot_of[beg + i];
@@ -205,7 +157,7 @@ __global__ void __launch_bounds__(256) k_vox_write(VoxArgs a)
 {
     const int b = blockIdx.y;
     const int64_t beg = a.cloud_off[b];
-    const int n = cloud_rows(a, b);
+    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     const int slot = a.slot_of[beg + i];
@@ -225,15 +177,12 @@ __global__ void __launch_bounds__(256) k_vox_write(VoxArgs a)
     }
 }
 
-inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
-
-struct VoxLayout { int64_t off, key, first, count, vid, slot_of, tile_base, tile_cnt, tile_off, top, total, n_slots, n_tiles; };
+struct VoxLayout { int64_t off, key, first, count, vid, slot_of, seg, seg_total, top, total, n_slots; };
 
 VoxLayout vox_layout(int64_t n_total, int n_clouds, int max_points, int max_voxels)
 {
     VoxLayout L;
     L.n_slots = 2 * n_total + n_clouds + 1;
-    L.n_tiles = n_total / VTILE + n_clouds + 1;
     int64_t o = 0;
     L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
     L.key = o;       o = align_up(o + L.n_slots * 8, 256);
@@ -241,9 +190,8 @@ VoxLayout vox_layout(int64_t n_total, int n_clouds, int max_points, int max_voxe
     L.count = o;     o = align_up(o + L.n_slots * 4, 256);
     L.vid = o;       o = align_up(o + L.n_slots * 4, 256);
     L.slot_of = o;   o = align_up(o + n_total * 4, 256);
-    L.tile_base = o; o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
-    L.tile_cnt = o;  o = align_up(o + L.n_tiles * 4, 256);
-    L.tile_off = o;  o = align_up(o + L.n_tiles * 4, 256);
+    L.seg = o;       o += seg_ws_bytes(n_total, n_clouds, VTILE, 1);
+    L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 4, 256);
     L.top = o;       o = align_up(o + (int64_t)n_clouds * max_voxels * max_points * 4, 256);
     L.total = o;
     return L;
@@ -253,9 +201,7 @@ cudaError_t fill32(lss_engine *e, void *p, unsigned long long words, uint32_t v,
 {
     if (!words) return cudaSuccess;
     const unsigned blocks = (unsigned)std::min<unsigned long long>((words + 1023) / 1024, (unsigned long long)e->n_sm * 16);
-    k_fill32<<<blocks, 256, 0, st>>>((uint32_t *)p, words, v);
-    e->launches++;
-    return cudaGetLastError();
+    return lss_launch(e, k_fill32, blocks, 256, 0, st, (uint32_t *)p, words, v);
 }
 
 }  // namespace
@@ -275,16 +221,17 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
                               int32_t *d_out_n_voxels, void *d_workspace, int64_t workspace_bytes, void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
-    if (!h_cloud_offsets || n_clouds < 0 || !h_point_cloud_range || !h_voxel_size || !d_out_voxels || !d_out_coords ||
+    BatchGeometry g;
+    if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, VTILE, g)) return rc;
+    if (!h_point_cloud_range || !h_voxel_size || !d_out_voxels || !d_out_coords ||
         !d_out_num_points || !d_out_n_voxels || !d_workspace)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
     if (n_features < 3 || max_points_per_voxel <= 0 || max_voxels <= 0)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "n_features >= 3, max_points_per_voxel > 0, max_voxels > 0 required");
-    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
     const int B = n_clouds;
-    const int64_t N = h_cloud_offsets[B];
+    const int64_t N = g.n;
     if (N >= (1LL << 30)) return lss_fail(e, LSS_ERR_INVALID_ARG, "batch too large");
-    DeviceGuard g(e->device);
+    DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     const VoxLayout L = vox_layout(N, B, max_points_per_voxel, max_voxels);
     if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
@@ -314,9 +261,8 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
     a.h_count = (int *)(ws + L.count);
     a.h_vid = (int *)(ws + L.vid);
     a.slot_of = (int *)(ws + L.slot_of);
-    a.tile_base = (const int32_t *)(ws + L.tile_base);
-    a.tile_cnt = (int *)(ws + L.tile_cnt);
-    a.tile_off = (int *)(ws + L.tile_off);
+    a.seg = seg_tiles(ws + L.seg, B);
+    a.seg.total[0] = (int32_t *)(ws + L.seg_total);
     a.top = (int *)(ws + L.top);
     a.out_vox = d_out_voxels;
     a.out_coords = d_out_coords;
@@ -325,16 +271,7 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
 
     const size_t n_vox_all = (size_t)B * max_voxels;
     if (B == 0) return LSS_OK;
-    std::vector<int32_t> h_tb(B + 1, 0);
-    int64_t max_n = 0;
-    for (int b = 0; b < B; b++) {
-        const int64_t nb = h_cloud_offsets[b + 1] - h_cloud_offsets[b];
-        if (nb < 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets must be non-decreasing");
-        max_n = std::max(max_n, nb);
-        h_tb[b + 1] = h_tb[b] + (int32_t)((nb + VTILE - 1) / VTILE);
-    }
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.tile_base, h_tb.data(), sizeof(int32_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)a.seg.tile_base, st));
     {
         KernelTimer kt(e, LSS_K_VOXEL, st);
         LSS_CUDA_CHECK(e, fill32(e, a.h_key, (unsigned long long)L.n_slots * 2, 0xffffffffu, st));
@@ -344,20 +281,18 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
         LSS_CUDA_CHECK(e, fill32(e, d_out_voxels, (unsigned long long)n_vox_all * max_points_per_voxel * n_features, 0u, st));
         LSS_CUDA_CHECK(e, fill32(e, d_out_coords, (unsigned long long)n_vox_all * 4, 0u, st));
         LSS_CUDA_CHECK(e, fill32(e, d_out_num_points, (unsigned long long)n_vox_all, 0u, st));
-        if (max_n > 0) {
-            const dim3 g256((unsigned)((max_n + 255) / 256), B), gt((unsigned)((max_n + VTILE - 1) / VTILE), B);
-            k_vox_insert<<<g256, 256, 0, st>>>(a);
-            k_vox_flags<<<gt, VTILE, 0, st>>>(a);
-            k_vox_scan<<<B, 1024, 0, st>>>(a);
-            k_vox_assign<<<gt, VTILE, 0, st>>>(a);
-            k_vox_cascade<<<g256, 256, 0, st>>>(a);
-            k_vox_write<<<g256, 256, 0, st>>>(a);
-            e->launches += 5;
+        if (g.max_n > 0) {
+            const dim3 g256((unsigned)((g.max_n + 255) / 256), B), gt((unsigned)((g.max_n + VTILE - 1) / VTILE), B);
+            LSS_CUDA_CHECK(e, lss_launch(e, k_vox_insert, g256, 256, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_vox_flags, gt, VTILE, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<1>, B, SEG_SCAN_TPB, 0, st, a.seg));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_vox_assign, gt, VTILE, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_vox_cascade, g256, 256, 0, st, a));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_vox_write, g256, 256, 0, st, a));
         } else {
             LSS_CUDA_CHECK(e, fill32(e, d_out_n_voxels, (unsigned long long)B, 0u, st));
         }
     }
-    LSS_CUDA_CHECK(e, cudaGetLastError());
     return LSS_OK;
 }
 

@@ -3,17 +3,18 @@
 //   pre-pass (prepass.cu)   plane, ground band |p.w + h| < delta, incident angle, estimate_laser_parameters
 //   k_wet_points            per ground point: reflectivity, two Fresnel interfaces air->water->ground->water->air
 //                           (tools/wet_ground/phy_equations.py:35-108), wet/dry mixing, clipped new intensity, drop test
-//   k_wet_tile_count / k_wet_tile_scan / k_wet_scatter
+//   k_seg_count_codes / k_seg_scan / k_wet_scatter
 //                           output order of the reference: all non-ground rows first, then the kept ground rows
-//                           (augmentation.py:150-159), column 4 rewritten; stable, tile parallel
+//                           (augmentation.py:150-159), column 4 rewritten; stable, tile parallel (segments.cuh)
 //
 // All per-point physics in float64, as the reference (its ground array is float64, augmentation.py:50).
 // A cloud with fewer than 1000 ground points is passed through unchanged (augmentation.py:51-52).
-#include "common.cuh"
+#include "segments.cuh"
 
 namespace {
 
 constexpr int WET_TPB = 256;
+constexpr int WET_TILE = 1024;
 
 struct WetArgs {
     const float *pts;
@@ -28,9 +29,7 @@ struct WetArgs {
     double *out_i64;              // optional [N] float64 intensity of the output rows
     int32_t *out_counts;          // [B]
     int32_t *out_passthrough;     // [B] 1 = cloud returned unchanged
-    const int32_t *tile_base;     // [B+1] tiles of 1024 rows per cloud slot
-    int *tile_cnt;                // [tiles*2] rows of class 0 / class 1 per tile
-    int *tile_off;                // [tiles*2] exclusive scans per cloud
+    SegTiles seg;                 // tiles of WET_TILE rows; class 0 = not ground, 1 = ground kept
 };
 
 struct Fresnel { double rs, ts, rp, tp, aout; };
@@ -56,17 +55,12 @@ __device__ __forceinline__ Fresnel fresnel_power(double ain, double nair, double
     return f;
 }
 
-__device__ __forceinline__ int cloud_n(const WetArgs &a, int b)
-{
-    return a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - a.cloud_off[b]);
-}
-
 __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
 {
     const int b = blockIdx.y;
     const CloudPre cp = a.cp[b];
     const int64_t beg = a.cloud_off[b];
-    const int n = cloud_n(a, b);
+    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
     const bool pass = cp.n_ground < 1000;                                  // augmentation.py:51-52
     for (int i = blockIdx.x * WET_TPB + threadIdx.x; i < n; i += gridDim.x * WET_TPB) {
         const float *r = a.pts + (beg + i) * 5;
@@ -100,98 +94,27 @@ __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
     }
 }
 
-// Stable two-stream compaction [not ground ...][kept ground ...] (augmentation.py:150-153), tile parallel:
-//   k_wet_tile_count   per tile of 1024 points: rows of class 0 (not ground) and class 1 (ground kept)
-//   k_wet_tile_scan    per cloud: exclusive scan of both tile counts, output count, pass-through flag
-//   k_wet_scatter      per tile: destination = stream base + tile offset + rank inside the tile
-constexpr int WET_TILE = 1024;
-
-__global__ void __launch_bounds__(WET_TILE) k_wet_tile_count(WetArgs a)
-{
-    __shared__ int ca, cb;
-    const int b = blockIdx.y, tile = blockIdx.x;
-    const int n = cloud_n(a, b);
-    if (tile * WET_TILE >= n) {
-        if (threadIdx.x == 0 && tile < a.tile_base[b + 1] - a.tile_base[b]) {
-            a.tile_cnt[2 * (a.tile_base[b] + tile)] = 0;              // tile of the slot beyond the valid rows
-            a.tile_cnt[2 * (a.tile_base[b] + tile) + 1] = 0;
-        }
-        return;
-    }
-    if (threadIdx.x == 0) { ca = 0; cb = 0; }
-    __syncthreads();
-    const int i = tile * WET_TILE + threadIdx.x;
-    const int c = i < n ? a.cls[a.cloud_off[b] + i] : 3;
-    const unsigned ma = __ballot_sync(0xffffffffu, c == 0), mb = __ballot_sync(0xffffffffu, c == 1);
-    if ((threadIdx.x & 31) == 0) {
-        if (ma) atomicAdd(&ca, __popc(ma));
-        if (mb) atomicAdd(&cb, __popc(mb));
-    }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        a.tile_cnt[2 * (a.tile_base[b] + tile)] = ca;
-        a.tile_cnt[2 * (a.tile_base[b] + tile) + 1] = cb;
-    }
-}
-
-__global__ void __launch_bounds__(1024) k_wet_tile_scan(WetArgs a)
-{
-    __shared__ int wa[32], wb[32];
-    __shared__ int run_a, run_b;
-    const int b = blockIdx.x;
-    const int t0 = a.tile_base[b], nt = a.tile_base[b + 1] - t0;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) { run_a = 0; run_b = 0; }
-    __syncthreads();
-    for (int base = 0; base < nt; base += 1024) {
-        const int t = base + tid;
-        const int va = t < nt ? a.tile_cnt[2 * (t0 + t)] : 0, vb = t < nt ? a.tile_cnt[2 * (t0 + t) + 1] : 0;
-        int ia = va, ib = vb;
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) {
-            const int ua = __shfl_up_sync(0xffffffffu, ia, s), ub = __shfl_up_sync(0xffffffffu, ib, s);
-            if (lane >= s) { ia += ua; ib += ub; }
-        }
-        if (lane == 31) { wa[warp] = ia; wb[warp] = ib; }
-        __syncthreads();
-        int oa = run_a, ob = run_b;
-        for (int wv = 0; wv < warp; wv++) { oa += wa[wv]; ob += wb[wv]; }
-        if (t < nt) {
-            a.tile_off[2 * (t0 + t)] = oa + ia - va;
-            a.tile_off[2 * (t0 + t) + 1] = ob + ib - vb;
-        }
-        __syncthreads();
-        if (tid == 1023) { run_a = oa + ia; run_b = ob + ib; }
-        __syncthreads();
-    }
-    if (tid == 0) {
-        a.out_counts[b] = run_a + run_b;
-        if (a.out_passthrough) a.out_passthrough[b] = (a.cp[b].n_ground < 1000) ? 1 : 0;
-    }
-}
-
+// Stable two-stream compaction [not ground ...][kept ground ...] (augmentation.py:150-153): destination = stream base +
+// rank inside the class.  Tile 0 of every cloud also writes the output count and the pass-through flag.
 __global__ void __launch_bounds__(WET_TILE) k_wet_scatter(WetArgs a)
 {
-    __shared__ int wa[WET_TILE / 32], wb[WET_TILE / 32];
     const int b = blockIdx.y, tile = blockIdx.x;
-    const int n = cloud_n(a, b);
-    if (tile * WET_TILE >= n) return;
     const CloudPre &cp = a.cp[b];
-    const int64_t beg = a.cloud_off[b];
     const bool pass = cp.n_ground < 1000;
+    if (tile == 0 && threadIdx.x == 0) {
+        a.out_counts[b] = a.seg.total[0][b] + a.seg.total[1][b];
+        if (a.out_passthrough) a.out_passthrough[b] = pass ? 1 : 0;
+    }
+    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
+    if (tile * WET_TILE >= n) return;
+    const int64_t beg = a.cloud_off[b];
     const int n_non = pass ? n : n - cp.n_ground;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const int i = tile * WET_TILE + tid;
-    const int c = i < n ? a.cls[beg + i] : 3;
-    const unsigned ma = __ballot_sync(0xffffffffu, c == 0), mb = __ballot_sync(0xffffffffu, c == 1);
-    if (lane == 0) { wa[warp] = __popc(ma); wb[warp] = __popc(mb); }
-    __syncthreads();
-    if (c == 0 || c == 1) {
-        int oa = a.tile_off[2 * (a.tile_base[b] + tile)], ob = a.tile_off[2 * (a.tile_base[b] + tile) + 1];
-        for (int wv = 0; wv < warp; wv++) { oa += wa[wv]; ob += wb[wv]; }
+    const int i = tile * WET_TILE + threadIdx.x;
+    const int c = i < n ? a.cls[beg + i] : 2;
+    const int r = seg_rank<2, WET_TILE>(c < 2 ? c : -1, a.seg, b, tile);
+    if (r >= 0) {
         const float *s = a.pts + (beg + i) * 5;
-        const int dst = (c == 0) ? oa + __popc(ma & ((1u << lane) - 1u))
-                                 : n_non + ob + __popc(mb & ((1u << lane) - 1u));
+        const int dst = (c == 0) ? r : n_non + r;
         float *o = a.out + (beg + dst) * 5;
         o[0] = s[0]; o[1] = s[1]; o[2] = s[2];
         const double inten = (c == 1) ? a.new_i[beg + i] : (double)s[3];
@@ -201,9 +124,7 @@ __global__ void __launch_bounds__(WET_TILE) k_wet_scatter(WetArgs a)
     }
 }
 
-inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
-
-struct WetLayout { int64_t off, cls, new_i, tile_base, tile_cnt, tile_off, prepass, prepass_bytes, total; };
+struct WetLayout { int64_t off, cls, new_i, seg, seg_total, prepass, prepass_bytes, total; };
 
 WetLayout wet_layout(int64_t n_total, int n_clouds)
 {
@@ -212,10 +133,8 @@ WetLayout wet_layout(int64_t n_total, int n_clouds)
     L.off = o;      o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
     L.cls = o;      o = align_up(o + n_total, 256);
     L.new_i = o;    o = align_up(o + n_total * 8, 256);
-    const int64_t tiles = n_total / 1024 + n_clouds + 1;
-    L.tile_base = o; o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
-    L.tile_cnt = o;  o = align_up(o + tiles * 2 * 4, 256);
-    L.tile_off = o;  o = align_up(o + tiles * 2 * 4, 256);
+    L.seg = o;      o += seg_ws_bytes(n_total, n_clouds, WET_TILE, 2);
+    L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 2 * 4, 256);
     L.prepass_bytes = lss_prepass_ws_bytes(n_total, n_clouds);
     L.prepass = o;  o = align_up(o + L.prepass_bytes, 256);
     L.total = o;
@@ -240,91 +159,67 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
                                 double *d_out_plane, void *d_workspace, int64_t workspace_bytes, void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
-    if (!h_cloud_offsets || n_clouds < 0 || !d_out_points || !d_out_counts || !d_workspace)
-        return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    if (n_clouds > 65535) return lss_fail(e, LSS_ERR_INVALID_ARG, "at most 65535 clouds per call");
-    if (h_cloud_offsets[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "cloud_offsets[0] must be 0");
+    BatchGeometry g;
+    if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, WET_TILE, g)) return rc;
+    if (!d_out_points || !d_out_counts || !d_workspace) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
     const int B = n_clouds;
-    const int64_t N = h_cloud_offsets[B];
+    const int64_t N = g.n;
+    DeviceGuard dg(e->device);
+    cudaStream_t st = (cudaStream_t)stream;
     if (B == 0 || N == 0) {
         ZeroRegions z;
         z.add(d_out_counts, sizeof(int32_t) * B);
-        lss_zero_async(e, z, (cudaStream_t)stream);
+        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
         return LSS_OK;
     }
     if (!d_points) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
-    int dev_prev = -1;
-    cudaGetDevice(&dev_prev);
-    if (dev_prev != e->device) cudaSetDevice(e->device);
-    cudaStream_t st = (cudaStream_t)stream;
     const WetLayout L = wet_layout(N, B);
-    lss_status rc = LSS_OK;
-    do {
-        if (workspace_bytes < L.total) { rc = lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small"); break; }
-        char *ws = (char *)d_workspace;
-        int64_t *d_off = (int64_t *)(ws + L.off);
-        if (lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st) != cudaSuccess) {
-            rc = lss_fail(e, LSS_ERR_CUDA, "memcpy failed");
-            break;
-        }
-        void *cp_ptr = nullptr;
-        // the plane is fitted on the cloud as given; laser parameters over the |p.w+h| < delta band, float64 ranges
-        PrepassIO io;
-        io.h_plane_in = h_plane_in;
-        io.h_ymins_in = h_ymins_in;
-        io.d_plane_out = d_out_plane;
-        rc = lss_prepass_run(e, d_points, d_off, d_cloud_counts, h_cloud_offsets, B, delta, noise_floor, flat_earth, 1, 0,
-                             io, ws + L.prepass, L.prepass_bytes, &cp_ptr, st);
-        if (rc != LSS_OK) break;
-        WetArgs a;
-        a.pts = d_points;
-        a.cloud_off = d_off;
-        a.cloud_cnt = d_cloud_counts;
-        a.cp = (const CloudPre *)cp_ptr;
-        a.delta = delta;
-        a.noise_floor = noise_floor;
-        a.power_factor = power_factor;
-        double f = water_height / pavement_depth;                             // augmentation.py:122
-        a.f_wet = f < 0 ? 0 : (f > 1 ? 1 : f);
-        a.flat_earth = flat_earth;
-        a.replace = replace;
-        a.cls = (uint8_t *)(ws + L.cls);
-        a.new_i = (double *)(ws + L.new_i);
-        a.out = d_out_points;
-        a.out_i64 = d_out_intensity64;
-        a.out_counts = d_out_counts;
-        a.out_passthrough = d_out_passthrough;
-        int64_t max_n = 0;
-        std::vector<int32_t> h_tb(B + 1, 0);
-        for (int b = 0; b < B; b++) {
-            const int64_t nb = h_cloud_offsets[b + 1] - h_cloud_offsets[b];
-            max_n = std::max<int64_t>(max_n, nb);
-            h_tb[b + 1] = h_tb[b] + (int32_t)((nb + WET_TILE - 1) / WET_TILE);
-        }
-        if (lss_stage_upload(e, ws + L.tile_base, h_tb.data(), sizeof(int32_t) * (B + 1), st) != cudaSuccess) {
-            rc = lss_fail(e, LSS_ERR_CUDA, "upload failed");
-            break;
-        }
-        a.tile_base = (const int32_t *)(ws + L.tile_base);
-        a.tile_cnt = (int *)(ws + L.tile_cnt);
-        a.tile_off = (int *)(ws + L.tile_off);
-        const int max_tiles = (int)std::max<int64_t>(1, (max_n + WET_TILE - 1) / WET_TILE);
-        const int nblk = (int)std::max<int64_t>(1, std::min<int64_t>(1024, (max_n + WET_TPB * 4 - 1) / (WET_TPB * 4)));
-        {
-            KernelTimer kt(e, LSS_K_WET, st);
-            k_wet_points<<<dim3(nblk, B), WET_TPB, 0, st>>>(a);
-        }
-        {
-            KernelTimer kt(e, LSS_K_COMPACT, st);
-            k_wet_tile_count<<<dim3(max_tiles, B), WET_TILE, 0, st>>>(a);
-            k_wet_tile_scan<<<B, 1024, 0, st>>>(a);
-            k_wet_scatter<<<dim3(max_tiles, B), WET_TILE, 0, st>>>(a);
-            e->launches += 2;
-        }
-        if (cudaGetLastError() != cudaSuccess) rc = lss_fail(e, LSS_ERR_CUDA, "wet-ground launch failed");
-    } while (0);
-    if (dev_prev != e->device && dev_prev >= 0) cudaSetDevice(dev_prev);
-    return rc;
+    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    char *ws = (char *)d_workspace;
+    WetArgs a;
+    a.seg = seg_tiles(ws + L.seg, B);
+    a.seg.total[0] = (int32_t *)(ws + L.seg_total);
+    a.seg.total[1] = a.seg.total[0] + B;
+    int64_t *d_off = (int64_t *)(ws + L.off);
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)a.seg.tile_base, st));
+    void *cp_ptr = nullptr;
+    // the plane is fitted on the cloud as given; laser parameters over the |p.w+h| < delta band, float64 ranges
+    PrepassIO io;
+    io.h_plane_in = h_plane_in;
+    io.h_ymins_in = h_ymins_in;
+    io.d_plane_out = d_out_plane;
+    if (lss_status rc = lss_prepass_run(e, d_points, d_off, d_cloud_counts, h_cloud_offsets, B, delta, noise_floor,
+                                        flat_earth, 1, 0, io, ws + L.prepass, L.prepass_bytes, &cp_ptr, st))
+        return rc;
+    a.pts = d_points;
+    a.cloud_off = d_off;
+    a.cloud_cnt = d_cloud_counts;
+    a.cp = (const CloudPre *)cp_ptr;
+    a.delta = delta;
+    a.noise_floor = noise_floor;
+    a.power_factor = power_factor;
+    double f = water_height / pavement_depth;                                 // augmentation.py:122
+    a.f_wet = f < 0 ? 0 : (f > 1 ? 1 : f);
+    a.flat_earth = flat_earth;
+    a.replace = replace;
+    a.cls = (uint8_t *)(ws + L.cls);
+    a.new_i = (double *)(ws + L.new_i);
+    a.out = d_out_points;
+    a.out_i64 = d_out_intensity64;
+    a.out_counts = d_out_counts;
+    a.out_passthrough = d_out_passthrough;
+    const int max_tiles = (int)std::max<int64_t>(1, (g.max_n + WET_TILE - 1) / WET_TILE);
+    const int nblk = (int)std::max<int64_t>(1, std::min<int64_t>(1024, (g.max_n + WET_TPB * 4 - 1) / (WET_TPB * 4)));
+    {
+        KernelTimer kt(e, LSS_K_WET, st);
+        LSS_CUDA_CHECK(e, lss_launch(e, k_wet_points, dim3(nblk, B), WET_TPB, 0, st, a));
+    }
+    KernelTimer kt(e, LSS_K_COMPACT, st);
+    LSS_CUDA_CHECK(e, lss_launch(e, k_seg_count_codes<2, WET_TILE>, dim3(max_tiles, B), WET_TILE, 0, st, a.cls, a.cloud_off,
+                                 a.cloud_cnt, a.seg));
+    LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.seg));
+    LSS_CUDA_CHECK(e, lss_launch(e, k_wet_scatter, dim3(max_tiles, B), WET_TILE, 0, st, a));
+    return LSS_OK;
 }
 
 }  // extern "C"

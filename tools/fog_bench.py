@@ -57,7 +57,7 @@ def main():
     algo = 60 * N
     out = {'metric': 'fog-augmented LiDAR points/sec', 'workload': f'{B} clouds x 131072 points, 5 features, alpha 0.06',
            'cases': res,
-           'roofline': {'bound': 'hbm', 'kernel': 'k_fog_count + k_fog_scan + k_fog_apply', 'algorithmic_bytes': algo,
+           'roofline': {'bound': 'hbm', 'kernel': 'k_fog_count + k_seg_scan + k_fog_apply', 'algorithmic_bytes': algo,
                         'achieved': algo / (k_ms * 1e-3) / 1e9, 'peak': peak, 'unit': 'GB/s',
                         'frac': algo / (k_ms * 1e-3) / 1e9 / peak, 'peak_source': src,
                         'note': '20 B/point read + 40 B/point written (float64 rows like the reference); the count pass '
