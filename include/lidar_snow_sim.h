@@ -245,6 +245,47 @@ LSS_API lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_fea
                                  const double *d_ext_noise, double *d_out, uint8_t *d_out_fog_mask, int32_t *d_out_rank,
                                  double *d_out_info, void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_fog_workspace_bytes(int64_t n_total, int n_clouds);
+/* Per-cloud fog parameters: lss_fog_batch with alpha, beta, beta_0 and the integral table chosen per cloud, e.g. the
+ * dataset's fog curriculum drawing a density per sample (dense_dataset.py:618-675), in one call.
+ *   h_alpha, h_beta, h_beta_0   float64[n_clouds] host
+ *   h_table_index               int32[n_clouds] host: cloud b uses the table d_luts + h_table_index[b] * 2001 * 2; must be
+ *                               in [0, n_tables) (LSS_ERR_INVALID_ARG otherwise).  May be NULL without LSS_FOG_SOFT.
+ *   d_luts                      float64[n_tables * 2001 * 2] device: a stack of tables in lss_fog_batch's layout (e.g. the
+ *                               output of lss_fog_integral_tables)
+ * Everything else as lss_fog_batch; a cloud's results are bit-identical to lss_fog_batch called with its parameters and
+ * table.  Workspace: lss_fog_batch_params_workspace_bytes.                                                            */
+LSS_API lss_status lss_fog_batch_params(lss_engine *e, const float *d_points, int n_features,
+                                        const int64_t *h_cloud_offsets, int n_clouds, const double *h_alpha,
+                                        const double *h_beta, const double *h_beta_0, const int32_t *h_table_index,
+                                        const double *d_luts, int n_tables, uint32_t flags, int noise, int noise_variant,
+                                        const uint64_t *h_rng_state, const double *d_ext_noise, double *d_out,
+                                        uint8_t *d_out_fog_mask, int32_t *d_out_rank, double *d_out_info,
+                                        void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_fog_batch_params_workspace_bytes(int64_t n_total, int n_clouds);
+
+/* ---- fog integral look-up tables ---------------------------------------------------------------------------------------
+ * The tables lss_fog_batch reads, generated on the device: generate_integral_lookup_table.py (lib/LiDAR_fog_sim/, :52-99)
+ * with theory.P_R_fog_soft (theory.py:622-644) for any parameter set, instead of the nine shipped pickles.  Row k is the
+ * generator's entry for r_0 = round(k * granularity, 2): with f(R) = P_R_fog_soft(p, R) on R = linspace(0, r_range, n),
+ * (R[argmax], f[argmax] / (c_a * p_0 * beta)) over the grid points R <= r_0 (the first index of the maximum; 0 when all
+ * are 0), R - tau_h * c / 2 with `shift`.  The integral is the old SciPy simps(y, x) (even='avg') over
+ * t = linspace(0, 2 tau_h, n).  Rows: int(r_0_max / granularity) + 1; the shipped grid is n = 2000, r_range = r_0_max =
+ * 200, granularity = 0.1 (2001 rows).
+ * Fields: the ParameterSet fields the generator reads (fog_simulation.py:52-171; GAMMA_T / GAMMA_R in radians), the grid,
+ * and shift != 0 for the `shifted` variant.  The tables of one call share n, r_range, r_0_max and granularity.
+ * Invalid values (non-finite, tau_h <= 0, alpha < 0, n outside 3..8192, not 0 <= r_1 < r_2, c_a * p_0 * beta <= 0, a
+ * geometric overlap with D, ROH_T or ROH_R <= 0, a row count that does not fit) fail with LSS_ERR_INVALID_ARG.       */
+typedef struct lss_fog_table_params {
+    double alpha, tau_h, r_1, r_2, D, ROH_T, ROH_R, GAMMA_T, GAMMA_R;
+    double c_a, p_0, beta;                  /* the response's scale c_a * p_0 * beta, divided out again (:92) */
+    double r_range, r_0_max, granularity;
+    int32_t n, linear_xsi, shift, reserved;
+} lss_fog_table_params;
+/*   d_out   float64[n_tables * rows * 2]: table t, row k = (fog_distance, fog_integral)
+ *   d_workspace  lss_fog_integral_tables_workspace_bytes(n, n_tables) bytes.  No allocation, no synchronisation. */
+LSS_API lss_status lss_fog_integral_tables(lss_engine *e, const lss_fog_table_params *h_params, int n_tables,
+                                           double *d_out, void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_fog_integral_tables_workspace_bytes(int n, int n_tables);
 
 /* ---- LISA Monte-Carlo rain / snow augmenter ("next" row, SURVEY.md 8f-3) ----------------------------------------------
  * LISA.monte_carlo_augment (lib/LISA/python/lisa.py:293-341) with the per-return experiment monte_carlo_lisa (:34-190) on

@@ -28,6 +28,15 @@ FLAG_ASSUME_SORTED = 0x8
 FOG_HARD, FOG_SOFT, FOG_GAIN = 0x1, 0x2, 0x4
 DROR_CUBE, DROR_WORK_STATS = 0x1, 0x100
 
+
+
+class FogTableParams(ctypes.Structure):
+    """lss_fog_table_params of include/lidar_snow_sim.h"""
+    _fields_ = [(f, ctypes.c_double) for f in ('alpha', 'tau_h', 'r_1', 'r_2', 'D', 'ROH_T', 'ROH_R', 'GAMMA_T',
+                                                'GAMMA_R', 'c_a', 'p_0', 'beta', 'r_range', 'r_0_max', 'granularity')]
+    _fields_ += [(f, ctypes.c_int32) for f in ('n', 'linear_xsi', 'shift', 'reserved')]
+
+
 # status -> exception type the reference would have raised at the corresponding place (SURVEY.md 8b "Errors")
 _EXC = {
     LSS_ERR_INVALID_ARG: ValueError,
@@ -80,6 +89,11 @@ SIGNATURES = [
     ('lss_fog_batch', _c.c_int, [_P, _P, _c.c_int, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _P, _c.c_uint32,
                                  _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_fog_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_fog_batch_params', _c.c_int, [_P, _P, _c.c_int, _P, _c.c_int, _P, _P, _P, _P, _P, _c.c_int, _c.c_uint32,
+                                        _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_fog_batch_params_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_fog_integral_tables', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int64, _P]),
+    ('lss_fog_integral_tables_workspace_bytes', _c.c_int64, [_c.c_int, _c.c_int]),
     ('lss_lisa_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int64, _c.c_double, _c.c_int, _c.c_double, _c.c_double, _c.c_double,
                                   _c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _c.c_int, _c.c_uint64, _P, _P]),
     ('lss_voxelize_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P,

@@ -14,6 +14,8 @@
 //   k_fog_apply   everything: hard, soft, noise (k-th PCG64 output by jump-ahead), min / max response, max intensity,
 //                 num_fog_responses
 //   k_fog_gain    intensity *= 255 / ceil(max intensity)                                            (:282-285)
+// k_fog_count / k_fog_apply take their fog parameters (alpha, beta, beta_0, table) either once for the whole batch
+// (lss_fog_batch) or per cloud (lss_fog_batch_params, PER_CLOUD = true); the arithmetic is the same.
 //
 // Numerics: float32 where NumPy 2 computes in float32 (r_0, exp, the hard-target product, r_0 ** 2, r_0 -/+ noise),
 // float64 elsewhere, no FMA contraction.  Two places are host-defined in the reference and therefore parity by
@@ -33,6 +35,8 @@ struct FogArgs {
     const int64_t *cloud_off;    // [B + 1] device
     const double *lut;           // [LUT_N * 2] (fog_distance, fog_response)
     double alpha, beta, beta_0;
+    const double *cloud_par;     // [B * 3] per-cloud alpha, beta, beta_0 (PER_CLOUD kernels)
+    const int32_t *cloud_lut;    // [B] per-cloud table index: the table at lut + index * LUT_N * 2 (PER_CLOUD kernels)
     int hard, soft, gain;
     int noise, variant;          // variant 1..4; 4 = externally drawn values (ext_noise, by rank)
     const unsigned long long *rng;   // [B * 4] PCG64 state_hi, state_lo, inc_hi, inc_lo per cloud, or null
@@ -62,7 +66,17 @@ __device__ __forceinline__ double ord_to(unsigned long long o)
 
 struct Soft { bool fog; double resp, fog_distance; float r0, hard_i; };
 
-__device__ __forceinline__ Soft soft_target(const FogArgs &a, const float *row)
+struct FogCloud { const double *lut; double alpha, beta, beta_0; };
+
+template <bool PER_CLOUD>
+__device__ __forceinline__ FogCloud fog_cloud(const FogArgs &a, int b)
+{
+    if (!PER_CLOUD) return FogCloud{a.lut, a.alpha, a.beta, a.beta_0};
+    return FogCloud{a.lut ? a.lut + (int64_t)a.cloud_lut[b] * (LUT_N * 2) : nullptr, a.cloud_par[3 * b],
+                    a.cloud_par[3 * b + 1], a.cloud_par[3 * b + 2]};
+}
+
+__device__ __forceinline__ Soft soft_target(const FogArgs &a, const FogCloud &c, const float *row)
 {
     Soft s;
     const float x = row[0], y = row[1], z = row[2], I = row[3];
@@ -71,7 +85,7 @@ __device__ __forceinline__ Soft soft_target(const FogArgs &a, const float *row)
     s.hard_i = I;
     if (a.hard) {
         // np.round(np.exp(-2 * alpha * r_0) * I): -2*alpha is a Python float (weak), the array op runs in float32
-        const float coef = (float)(-2.0 * a.alpha);
+        const float coef = (float)(-2.0 * c.alpha);
         s.hard_i = rintf(__fmul_rn(exp32(__fmul_rn(coef, s.r0)), I));
     }
     s.fog = false; s.resp = 0.0; s.fog_distance = 0.0;
@@ -80,10 +94,10 @@ __device__ __forceinline__ Soft soft_target(const FogArgs &a, const float *row)
         const float k10 = rintf(__fmul_rn(s.r0, 10.0f));
         int k = (k10 >= (float)(LUT_N - 1)) ? LUT_N - 1 : (int)k10;
         k = k < 0 ? 0 : k;
-        s.fog_distance = a.lut[2 * k];
-        double r = __dmul_rn(a.lut[2 * k + 1], (double)I);                  // * original intensity       (:216)
+        s.fog_distance = c.lut[2 * k];
+        double r = __dmul_rn(c.lut[2 * k + 1], (double)I);                  // * original intensity       (:216)
         r = __dmul_rn(r, (double)__fmul_rn(s.r0, s.r0));                    // * r_0 ** 2 (float32)
-        r = __ddiv_rn(__dmul_rn(r, a.beta), a.beta_0);
+        r = __ddiv_rn(__dmul_rn(r, c.beta), c.beta_0);
         s.resp = fmin(r, 255.0);                                            // :219
         s.fog = s.resp > (double)s.hard_i;                                  // :221
     }
@@ -101,6 +115,7 @@ __device__ __forceinline__ const float *stage_rows(const FogArgs &a, int64_t fir
     return s_in + threadIdx.x * a.F;
 }
 
+template <bool PER_CLOUD>
 __global__ void __launch_bounds__(FOG_TILE) k_fog_count(FogArgs a)
 {
     __shared__ float s_in[FOG_TILE * FOG_STAGE_F];
@@ -110,7 +125,7 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_count(FogArgs a)
     if (tile * FOG_TILE >= n) return;
     const int i = tile * FOG_TILE + threadIdx.x;
     const float *row = stage_rows(a, beg + (int64_t)tile * FOG_TILE, min(FOG_TILE, n - tile * FOG_TILE), s_in);
-    const bool fog = i < n && soft_target(a, row).fog;
+    const bool fog = i < n && soft_target(a, fog_cloud<PER_CLOUD>(a, b), row).fog;
     seg_count<1>(fog ? 0 : -1, a.seg, b, tile);
 }
 
@@ -158,6 +173,7 @@ __device__ double pcg64_kth_double(const unsigned long long *st, unsigned long l
     return (double)(out >> 11) * (1.0 / 9007199254740992.0);
 }
 
+template <bool PER_CLOUD>
 __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
 {
     __shared__ float s_in[FOG_TILE * FOG_STAGE_F];
@@ -175,7 +191,7 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
     Soft s;
     s.fog = false;
     const float *row = stage_rows(a, beg + (int64_t)tile * FOG_TILE, rows, s_in);
-    if (active) s = soft_target(a, row);
+    if (active) s = soft_target(a, fog_cloud<PER_CLOUD>(a, b), row);
     const int rank = seg_rank<1, FOG_TILE>(active && s.fog ? 0 : -1, a.seg, b, tile);
     double out_i = 0.0;
     if (active) {
@@ -275,9 +291,10 @@ __global__ void k_fog_info(FogArgs a, int B, double *info_out)
     info_out[3 * b + 2] = (double)cnt;
 }
 
-struct FogLayout { int64_t off, seg, seg_total, info, rng, total; };
+struct FogLayout { int64_t off, seg, seg_total, info, rng, par, total; };
 
-FogLayout fog_layout(int64_t n_total, int n_clouds)
+// per_cloud: room for the per-cloud parameters of lss_fog_batch_params behind lss_fog_batch's regions
+FogLayout fog_layout(int64_t n_total, int n_clouds, bool per_cloud = false)
 {
     FogLayout L;
     int64_t o = 0;
@@ -286,24 +303,23 @@ FogLayout fog_layout(int64_t n_total, int n_clouds)
     L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 4, 256);
     L.info = o;      o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
     L.rng = o;       o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
+    L.par = o;       if (per_cloud) o = align_up(o + (int64_t)n_clouds * (3 * 8 + 4), 256);
     L.total = o;
     return L;
 }
 
-}  // namespace
+// per-cloud fog parameters of lss_fog_batch_params (host arrays); null for lss_fog_batch
+struct FogPerCloud {
+    const double *alpha, *beta, *beta_0;
+    const int32_t *table_index;
+    int n_tables;
+};
 
-int64_t lss_fog_workspace_bytes(int64_t n_total, int n_clouds)
-{
-    if (n_total < 0 || n_clouds < 0) return -1;
-    return fog_layout(n_total, n_clouds).total;
-}
-
-lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
-                                    int n_clouds, double alpha, double beta, double beta_0, const double *d_lut,
-                                    uint32_t flags, int noise, int noise_variant, const uint64_t *h_rng_state,
-                                    const double *d_ext_noise, double *d_out, uint8_t *d_out_fog_mask,
-                                    int32_t *d_out_rank, double *d_out_info, void *d_workspace, int64_t workspace_bytes,
-                                    void *stream)
+lss_status fog_run(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets, int n_clouds,
+                   double alpha, double beta, double beta_0, const double *d_lut, const FogPerCloud *pc, uint32_t flags,
+                   int noise, int noise_variant, const uint64_t *h_rng_state, const double *d_ext_noise, double *d_out,
+                   uint8_t *d_out_fog_mask, int32_t *d_out_rank, double *d_out_info, void *d_workspace,
+                   int64_t workspace_bytes, void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
     BatchGeometry g;
@@ -315,9 +331,24 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
     if (noise > 0 && soft && (noise_variant < 1 || noise_variant > 4))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "noise variant must be 1..4 (NotImplementedError in the reference)");
     const int B = n_clouds;
+    std::vector<char> par;                                      // per cloud: B x (alpha, beta, beta_0), then B table indices
+    if (pc) {
+        if (B > 0 && (!pc->alpha || !pc->beta || !pc->beta_0)) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
+        if (soft && B > 0 && !pc->table_index) return lss_fail(e, LSS_ERR_INVALID_ARG, "null table index");
+        if (soft && pc->n_tables <= 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "n_tables must be > 0");
+        par.assign((size_t)B * (3 * 8 + 4), 0);
+        double *p = (double *)par.data();
+        int32_t *ti = (int32_t *)(par.data() + (size_t)B * 3 * 8);
+        for (int b = 0; b < B; b++) {
+            p[3 * b] = pc->alpha[b]; p[3 * b + 1] = pc->beta[b]; p[3 * b + 2] = pc->beta_0[b];
+            ti[b] = pc->table_index ? pc->table_index[b] : 0;
+            if (soft && (ti[b] < 0 || ti[b] >= pc->n_tables))
+                return lss_fail(e, LSS_ERR_INVALID_ARG, "table index outside [0, n_tables)");
+        }
+    }
     const int64_t N = g.n;
     if (!d_points && N > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
-    const FogLayout L = fog_layout(N, B);
+    const FogLayout L = fog_layout(N, B, pc != nullptr);
     if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
@@ -332,6 +363,8 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
     a.seg.total[0] = (int32_t *)(ws + L.seg_total);
     a.lut = d_lut;
     a.alpha = alpha; a.beta = beta; a.beta_0 = beta_0;
+    a.cloud_par = pc ? (const double *)(ws + L.par) : nullptr;
+    a.cloud_lut = pc ? (const int32_t *)(ws + L.par + (int64_t)B * 3 * 8) : nullptr;
     a.hard = (flags & LSS_FOG_HARD) ? 1 : 0;
     a.soft = soft ? 1 : 0;
     a.gain = (soft && (flags & LSS_FOG_GAIN)) ? 1 : 0;
@@ -346,6 +379,7 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
 
     LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
                                          (int32_t *)a.seg.tile_base, st));
+    if (pc) LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.par, par.data(), par.size(), st));
     if (h_rng_state && soft && noise > 0 && noise_variant != 4 && !d_ext_noise) {
         LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.rng, h_rng_state, sizeof(uint64_t) * 4 * B, st));
         a.rng = (const unsigned long long *)(ws + L.rng);
@@ -359,12 +393,53 @@ lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, c
     if (N > 0) {
         KernelTimer kt(e, LSS_K_FOG, st);
         if (soft) {
-            LSS_CUDA_CHECK(e, lss_launch(e, k_fog_count, grid, FOG_TILE, 0, st, a));
+            LSS_CUDA_CHECK(e, pc ? lss_launch(e, k_fog_count<true>, grid, FOG_TILE, 0, st, a)
+                                 : lss_launch(e, k_fog_count<false>, grid, FOG_TILE, 0, st, a));
             LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<1>, B, SEG_SCAN_TPB, 0, st, a.seg));
         }
-        LSS_CUDA_CHECK(e, lss_launch(e, k_fog_apply, grid, FOG_TILE, 0, st, a));
+        LSS_CUDA_CHECK(e, pc ? lss_launch(e, k_fog_apply<true>, grid, FOG_TILE, 0, st, a)
+                             : lss_launch(e, k_fog_apply<false>, grid, FOG_TILE, 0, st, a));
         if (a.gain) LSS_CUDA_CHECK(e, lss_launch(e, k_fog_gain, grid, FOG_TILE, 0, st, a));
     }
     LSS_CUDA_CHECK(e, lss_launch(e, k_fog_info, (B + 127) / 128, 128, 0, st, a, B, d_out_info));
     return LSS_OK;
+}
+
+}  // namespace
+
+int64_t lss_fog_workspace_bytes(int64_t n_total, int n_clouds)
+{
+    if (n_total < 0 || n_clouds < 0) return -1;
+    return fog_layout(n_total, n_clouds).total;
+}
+
+int64_t lss_fog_batch_params_workspace_bytes(int64_t n_total, int n_clouds)
+{
+    if (n_total < 0 || n_clouds < 0) return -1;
+    return fog_layout(n_total, n_clouds, true).total;
+}
+
+lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                    int n_clouds, double alpha, double beta, double beta_0, const double *d_lut,
+                                    uint32_t flags, int noise, int noise_variant, const uint64_t *h_rng_state,
+                                    const double *d_ext_noise, double *d_out, uint8_t *d_out_fog_mask,
+                                    int32_t *d_out_rank, double *d_out_info, void *d_workspace, int64_t workspace_bytes,
+                                    void *stream)
+{
+    return fog_run(e, d_points, n_features, h_cloud_offsets, n_clouds, alpha, beta, beta_0, d_lut, nullptr, flags, noise,
+                   noise_variant, h_rng_state, d_ext_noise, d_out, d_out_fog_mask, d_out_rank, d_out_info, d_workspace,
+                   workspace_bytes, stream);
+}
+
+lss_status lss_fog_batch_params(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                int n_clouds, const double *h_alpha, const double *h_beta, const double *h_beta_0,
+                                const int32_t *h_table_index, const double *d_luts, int n_tables, uint32_t flags,
+                                int noise, int noise_variant, const uint64_t *h_rng_state, const double *d_ext_noise,
+                                double *d_out, uint8_t *d_out_fog_mask, int32_t *d_out_rank, double *d_out_info,
+                                void *d_workspace, int64_t workspace_bytes, void *stream)
+{
+    const FogPerCloud pc{h_alpha, h_beta, h_beta_0, h_table_index, n_tables};
+    return fog_run(e, d_points, n_features, h_cloud_offsets, n_clouds, 0.0, 0.0, 0.0, d_luts, &pc, flags, noise,
+                   noise_variant, h_rng_state, d_ext_noise, d_out, d_out_fog_mask, d_out_rank, d_out_info, d_workspace,
+                   workspace_bytes, stream);
 }

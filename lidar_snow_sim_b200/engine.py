@@ -375,6 +375,73 @@ class SnowfallEngine:
         _lib.check(st, self.h)
         return out
 
+    def fog_batch_params(self, points, cloud_offsets, luts, alpha, beta, beta_0, table_index=None, hard=True, soft=True,
+                         gain=False, noise=0, noise_variant=1, rng_states=None, ext_noise=None, want_rank=False):
+        """
+        fog_batch with the fog parameters chosen per cloud (lss_fog_batch_params): alpha, beta, beta_0 and table_index
+        are length-B host sequences; luts: CUDA float64 (T, 2001, 2) stack of integral tables (e.g. fog_integral_tables);
+        cloud b uses luts[table_index[b]].  A cloud's results are bit-identical to fog_batch with its own parameters.
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        N = int(off[-1])
+        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
+        F = int(points.shape[1])
+        T = 0
+        if luts is not None:
+            assert luts.is_cuda and luts.dtype == torch.float64 and luts.is_contiguous()
+            assert luts.dim() == 3 and tuple(luts.shape[1:]) == (2001, 2)
+            T = int(luts.shape[0])
+        per = [np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (B,))) for v in (alpha, beta, beta_0)]
+        ti = None if table_index is None else np.ascontiguousarray(table_index, dtype=np.int32).reshape(B)
+        rs = None if rng_states is None else np.ascontiguousarray(rng_states, dtype=np.uint64).reshape(B, 4)
+        if ext_noise is not None:
+            assert ext_noise.is_cuda and ext_noise.dtype == torch.float64 and ext_noise.numel() >= N
+        flags = (_lib.FOG_HARD if hard else 0) | (_lib.FOG_SOFT if soft else 0) | (_lib.FOG_GAIN if gain else 0)
+        with torch.cuda.device(self.device):
+            out = dict(points=torch.empty((N, F), dtype=torch.float64, device=self.device),
+                       fog_mask=torch.empty((N,), dtype=torch.uint8, device=self.device),
+                       info=torch.empty((B, 3), dtype=torch.float64, device=self.device))
+            if want_rank:
+                out['rank'] = torch.empty((N,), dtype=torch.int32, device=self.device)
+            need = self.lib.lss_fog_batch_params_workspace_bytes(N, B)
+            ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_fog_batch_params(
+                self.h, _ptr(points), F, _ptr(off), B, *[_ptr(v) for v in per], _ptr(ti), _ptr(luts), T, flags,
+                int(noise), int(noise_variant), _ptr(rs), _ptr(ext_noise), _ptr(out['points']), _ptr(out['fog_mask']),
+                _ptr(out.get('rank')), _ptr(out['info']), _ptr(ws), int(ws.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out
+
+    def fog_integral_tables(self, params, shift=False, n=2000, r_range=200, r_0_max=200, granularity=None):
+        """
+        The fog integral look-up tables of `params` (a sequence of fog ParameterSets, or one), generated on the device
+        (lss_fog_integral_tables, current stream, no synchronisation): the reference generator's table for each
+        parameter set (generate_integral_lookup_table.py), row k = (fog_distance, fog_integral) at r_0 =
+        round(k * granularity, 2).  The defaults are the shipped grid (n_steps = 2000 over 200 m, 2001 rows; the
+        generator sets n = n_steps and r_range = r_0_max).  Returns a CUDA float64 tensor (T, rows, 2).
+        """
+        if not isinstance(params, (list, tuple)):
+            params = [params]
+        granularity = r_0_max / n if granularity is None else granularity
+        T = len(params)
+        arr = (_lib.FogTableParams * max(T, 1))()
+        for t, p in enumerate(params):
+            q = arr[t]
+            for f in ('alpha', 'tau_h', 'r_1', 'r_2', 'D', 'ROH_T', 'ROH_R', 'GAMMA_T', 'GAMMA_R', 'c_a', 'p_0', 'beta'):
+                setattr(q, f, float(getattr(p, f)))
+            q.r_range, q.r_0_max, q.granularity = float(r_range), float(r_0_max), float(granularity)
+            q.n, q.linear_xsi, q.shift = int(n), 1 if p.linear_xsi else 0, 1 if shift else 0
+        steps = float(r_0_max) / float(granularity)
+        rows = int(steps) + 1 if np.isfinite(steps) and 0 <= steps < 2 ** 24 else 0
+        with torch.cuda.device(self.device):
+            out = torch.empty((T, rows, 2), dtype=torch.float64, device=self.device)
+            need = self.lib.lss_fog_integral_tables_workspace_bytes(int(n), T)
+            ws = torch.empty(max(int(need), 0) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_fog_integral_tables(self.h, ctypes.cast(arr, ctypes.c_void_p), T, _ptr(out), _ptr(ws), int(ws.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out
+
     def voxelize_batch(self, points, cloud_offsets, point_cloud_range, voxel_size, max_points_per_voxel, max_voxels,
                        counts=None, mask_xy_range=True):
         """

@@ -1,1 +1,2 @@
-from .simulation import ParameterSet, simulate_fog, load_integral_table, get_available_alphas  # noqa: F401
+from .simulation import (ParameterSet, simulate_fog, simulate_fog_batch, load_integral_table,  # noqa: F401
+                         get_available_alphas, integral_table, generate_integral_lookup_tables)

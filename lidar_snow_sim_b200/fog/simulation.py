@@ -7,8 +7,13 @@ Like the reference, the noise draws come from a module-level `RNG = np.random.de
 caller passes `rng=`; the generator's stream is consumed exactly as the reference consumes it (one `integers` draw per
 call, then one draw per fog point in point order), so a run is reproducible against the reference draw for draw.
 
-The integral look-up tables are the reference's data files (`integral_lookup_tables/original/*.pickle`, 1.7 MB, :19);
-point `LSS_FOG_LUT_DIR` (or `lut_dir=`) at that directory, or pass `lut=` a (2001, 2) float64 array directly.
+The integral look-up tables are by default the reference's data files (`integral_lookup_tables/original/*.pickle`,
+1.7 MB, :19); point `LSS_FOG_LUT_DIR` (or `lut_dir=`) at that directory, or pass `lut=` a (2001, 2) float64 array
+directly.  `lut='device'` generates the table on the device instead (csrc/fog_lut.cu, the reference's generator
+generate_integral_lookup_table.py), at exactly `p.alpha` and for any pulse width and sensor geometry.  The reference
+ships tables for nine alphas only and snaps every other alpha to the nearest of them (get_integral_dict, :174-180), so
+for an alpha it does not ship the device table -- the one its generator would make -- differs from what the reference
+uses; at the shipped alphas both agree (fog distances exactly, responses to ~1e-15 relative).
 """
 import math
 import os
@@ -129,6 +134,59 @@ def load_integral_table(p, lut_dir=None):
     return np.array([[float(integral_dict[k][0]), float(integral_dict[k][1])] for k in keys], dtype=np.float64)
 
 
+_TABLE_FIELDS = ('alpha', 'tau_h', 'r_1', 'r_2', 'linear_xsi', 'D', 'ROH_T', 'ROH_R', 'GAMMA_T', 'GAMMA_R', 'c_a', 'p_0',
+                 'beta')
+
+
+def _table_key(p):
+    """The ParameterSet fields a fog integral table depends on (two sets with equal keys share a table)."""
+    return tuple(bool(getattr(p, f)) if f == 'linear_xsi' else float(getattr(p, f)) for f in _TABLE_FIELDS)
+
+
+def integral_table(p, shift=False, engine=None):
+    """The integral look-up table of ParameterSet `p`, generated on the device: what the reference's generator
+    (generate_integral_lookup_table.py:52-99, n_steps = 2000 over 200 m) writes for p, as a (2001, 2) float64 array
+    (fog_distance, fog_integral); row k is the entry of key k / 10.  shift: the `shifted` variant (fog_distance -
+    tau_h c / 2).  simulate_fog reads unshifted tables."""
+    eng = engine or default_engine()
+    out = eng.fog_integral_tables([p], shift=shift)
+    return out[0].cpu().numpy()
+
+
+def generate_integral_lookup_tables(alphas=None, r_0_max=200, n_steps=None, shift=True,
+                                    save_path='integral_lookup_tables', engine=None):
+    """
+    generate_integral_lookup_table.py (:52-99) on the device: one pickle per alpha in `save_path`, with the reference's
+    file names and format -- {round(r_0, 2): (np.float64 fog_distance, np.float64 fog_integral)} for r_0 = 0, granularity,
+    ... r_0_max with granularity = r_0_max / n_steps -- for ParameterSet(n=n_steps, r_range=r_0_max, alpha=alpha), as the
+    script builds it.  Defaults as the script's: its nine alphas, n_steps = 10 r_0_max, shift=True.  (The reference's
+    `original` tables, the ones fog simulation reads, are the shift=False variant.)  Returns the paths written.
+    """
+    if alphas is None:
+        alphas = [0.005, 0.01, 0.02, 0.03, 0.06, 0.1, 0.12, 0.15, 0.2]
+    n = 10 * r_0_max if n_steps is None else n_steps
+    granularity = r_0_max / n
+    eng = engine or default_engine()
+    ps = [ParameterSet(n=n, r_range=r_0_max, alpha=alpha) for alpha in alphas]
+    tables = eng.fog_integral_tables(ps, shift=shift, n=n, r_range=r_0_max, r_0_max=r_0_max,
+                                     granularity=granularity).cpu().numpy()
+    # the script's keys: r_0 accumulated by += granularity, rounded to 2 decimals (:71-96)
+    keys, r_0 = [], 0
+    for _ in range(int(r_0_max / granularity) + 1):
+        keys.append(round(r_0, 2))
+        r_0 += granularity
+    save_path = Path(save_path)
+    save_path.mkdir(parents=True, exist_ok=True)
+    paths = []
+    for alpha, table in zip(alphas, tables):
+        integral = {k: (np.float64(table[i, 0]), np.float64(table[i, 1])) for i, k in enumerate(keys)}
+        filepath = save_path / f'integral_0m_to_{r_0_max}m_stepsize_{granularity}m_tau_h_20ns_alpha_{alpha}.pickle'
+        with open(filepath, 'wb') as f:
+            pickle.dump(integral, f, protocol=pickle.HIGHEST_PROTOCOL)
+        paths.append(filepath)
+    return paths
+
+
 def _pcg64_state(rng):
     st = rng.bit_generator.state
     if st['bit_generator'] != 'PCG64':
@@ -160,6 +218,8 @@ def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=T
     fog_simulation.py:299-316.  pc: (N, F >= 4) array (x, y, z, intensity, ...).  Returns
     (augmented_pc, simulated_fog_pc or None, info_dict or None) with the reference's dtypes: float64 (N, F) when `soft`,
     the input's float32 when only `hard`.
+    lut: None = the pickled table of the nearest shipped alpha (LSS_FOG_LUT_DIR / lut_dir), a (2001, 2) array, or
+    'device' = the table of exactly p.alpha (and p's pulse width and geometry) generated on the device.
     """
     variants = {'v1': 1, 'v2': 2, 'v3': 3, 'v4': 4}
     if soft and noise > 0 and noise_variant not in variants:
@@ -172,8 +232,13 @@ def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=T
     d_pts = torch.from_numpy(pc32).to(eng.device)
     d_lut = None
     if soft:
-        table = load_integral_table(p, lut_dir) if lut is None else np.ascontiguousarray(lut, dtype=np.float64)
-        d_lut = torch.from_numpy(table).to(eng.device)
+        if isinstance(lut, str):
+            if lut != 'device':
+                raise ValueError(f"lut must be None, an array or 'device', not {lut!r}")
+            d_lut = eng.fog_integral_tables([p])[0]
+        else:
+            table = load_integral_table(p, lut_dir) if lut is None else np.ascontiguousarray(lut, dtype=np.float64)
+            d_lut = torch.from_numpy(table).to(eng.device)
         rng.integers(low=1, high=20, size=1)                # :207 (the value is overwritten by 10 at :208)
     variant = variants.get(noise_variant, 1)
     kw = dict(hard=hard, soft=soft, gain=gain, noise=int(noise), noise_variant=variant)
@@ -203,3 +268,93 @@ def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=T
                  'max_fog_response': float(info[1]) if cnt else 0,
                  'num_fog_responses': cnt}
     return aug, simulated_fog_pc, info_dict
+
+
+def simulate_fog_batch(ps, pcs, noise, gain=False, noise_variant='v1', hard=True, soft=True, *, engine=None, rngs=None):
+    """
+    simulate_fog for a batch of clouds in one engine call (lss_fog_batch_params), each with its own ParameterSet and
+    generator: ps a sequence of B ParameterSets (or one for all), pcs B (N_b, F) arrays of the same F, rngs B numpy
+    Generators (None: the module-level RNG for every cloud).  The integral tables are generated on the device, one per
+    distinct parameter set, as with lut='device'.  Returns B triples, each identical to
+    simulate_fog(ps[b], pcs[b], noise, ..., rng=rngs[b], lut='device') called for b = 0, 1, ... in turn -- the generators
+    are left where those calls leave them, also when clouds share one.
+    """
+    variants = {'v1': 1, 'v2': 2, 'v3': 3, 'v4': 4}
+    if soft and noise > 0 and noise_variant not in variants:
+        raise NotImplementedError(f"noise variant '{noise_variant}' is not implemented (yet)")      # :264-266
+    B = len(pcs)
+    ps = list(ps) if isinstance(ps, (list, tuple)) else [ps] * B
+    rngs = [RNG] * B if rngs is None else list(rngs)
+    if len(ps) != B or len(rngs) != B:
+        raise ValueError('ps, pcs and rngs must have one entry per cloud')
+    if B == 0:
+        return []
+    eng = engine or default_engine()
+    pc32 = [np.ascontiguousarray(pc, dtype=np.float32) for pc in pcs]
+    F = pc32[0].shape[1]
+    if any(pc.ndim != 2 or pc.shape[1] != F for pc in pc32):
+        raise ValueError('every cloud of a batch needs the same number of features')
+    off = np.concatenate([[0], np.cumsum([pc.shape[0] for pc in pc32])]).astype(np.int64)
+    N = int(off[-1])
+    d_pts = torch.from_numpy(np.concatenate(pc32)).to(eng.device)
+    alpha = np.array([p.alpha for p in ps], dtype=np.float64)
+    beta = np.array([p.beta for p in ps], dtype=np.float64)
+    beta_0 = np.array([p.beta_0 for p in ps], dtype=np.float64)
+    luts, index = None, None
+    if soft:
+        keys, index, unique = {}, np.zeros(B, dtype=np.int32), []
+        for b, p in enumerate(ps):
+            k = _table_key(p)
+            if k not in keys:
+                keys[k] = len(unique)
+                unique.append(p)
+            index[b] = keys[k]
+        luts = eng.fog_integral_tables(unique)
+    variant = variants.get(noise_variant, 1)
+    kw = dict(hard=hard, soft=soft, gain=gain, noise=int(noise), noise_variant=variant)
+
+    def run(**extra):
+        return eng.fog_batch_params(d_pts, off, luts, alpha, beta, beta_0, index, **dict(kw, **extra))
+
+    draws = soft and noise > 0
+    if not draws:
+        res = run()
+        if soft:
+            for g in rngs:
+                g.integers(low=1, high=20, size=1)          # :207, one per call
+    else:
+        # the fog counts do not depend on the noise: a first pass gives every cloud's count, so each generator can be
+        # stepped exactly as the sequential calls step it (integers draw, then one draw per fog point), shared or not
+        cnt = run(noise=0)['info'][:, 2].cpu().numpy().astype(np.int64)
+        if variant == 4:
+            ext = torch.zeros((max(N, 1),), dtype=torch.float64)
+            for b, g in enumerate(rngs):
+                g.integers(low=1, high=20, size=1)
+                if cnt[b]:
+                    ext[off[b]:off[b] + cnt[b]] = torch.from_numpy(g.beta(a=2, b=20, size=int(cnt[b])))
+            res = run(ext_noise=ext.to(eng.device))
+        else:
+            states = np.zeros((B, 4), dtype=np.uint64)
+            for b, g in enumerate(rngs):
+                g.integers(low=1, high=20, size=1)
+                states[b] = _pcg64_state(g)
+                if cnt[b]:
+                    _pcg64_advance(g, int(cnt[b]))
+            res = run(rng_states=states)
+    eng.check()
+    aug_all = res['points'].cpu().numpy()
+    info_all = res['info'].cpu().numpy()
+    mask_all = res['fog_mask'].cpu().numpy().astype(bool)
+    out = []
+    for b in range(B):
+        aug = aug_all[off[b]:off[b + 1]]
+        if not soft:
+            out.append((aug.astype(np.float32), None, None))
+            continue
+        info = info_all[b]
+        c = int(info[2])
+        fog_pc = aug[mask_all[off[b]:off[b + 1]]] if c > 0 else None
+        out.append((aug, fog_pc, {'min_fog_response': float(info[0]) if c else np.inf,
+                                  'max_fog_response': float(info[1]) if c else 0,
+                                  'num_fog_responses': c}))
+    return out

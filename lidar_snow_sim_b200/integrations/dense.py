@@ -126,10 +126,12 @@ class OnTheFlyWeather:
         return points
 
 
-def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None):
+def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None, lut=None):
     """The 'CVL' branch of `DenseDataset.foggify` (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:988-1009): fog
     simulation with attenuation `alpha` (a string like '0.060' in the reference's curriculum; '0.000' = clear) and the
-    optional config keys FOG_GAIN / FOG_NOISE_VARIANT / FOG_SOFT / FOG_HARD, computed by the engine."""
+    optional config keys FOG_GAIN / FOG_NOISE_VARIANT / FOG_SOFT / FOG_HARD, computed by the engine.
+    lut='device': the integral table of exactly `alpha` is generated on the device instead of read from the pickled
+    tables (no LSS_FOG_LUT_DIR needed; see simulate_fog)."""
     if alpha == '0.000' or float(alpha) == 0.0:
         return points
     p = ParameterSet(alpha=float(alpha), gamma=0.000001)
@@ -143,7 +145,7 @@ def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None)
     if 'FOG_HARD' in dataset_cfg:
         hard = dataset_cfg['FOG_HARD']
     points, _, _ = simulate_fog(p, pc=points, noise=10, gain=gain, noise_variant=fog_noise_variant, soft=soft, hard=hard,
-                                engine=engine, lut_dir=lut_dir, rng=rng)
+                                engine=engine, lut=lut, lut_dir=lut_dir, rng=rng)
     return points
 
 
