@@ -40,9 +40,13 @@ struct PreArgs {
     CloudPre *cp;
     float *win;              // [N*3] compacted window points of each cloud at its own offset
     float *stage;            // [N*3] per-tile staging of the window compaction
-    int *tile_cnt;           // [sum of tiles] window points per 1024-row tile
+    int *tile_cnt;           // [sum of tiles] window points per 32-row tile
     const int32_t *tile_base;   // [B+1] first tile of each cloud
-    unsigned *hist;          // [B*50*2555]
+    // histogram records of the ground pass, each cloud's list at its own row offset (the staging region, dead after the
+    // window gather): I/cos and range bin of every ground point that falls inside the 50 x 2555 histogram
+    double *rec_norm;        // [N]
+    unsigned char *rec_bin;  // [N]
+    int *rec_cnt;            // [B] records per cloud
     double *trial;           // [B*RANSAC_T*8]: n_inl, score, a, b, c, valid
     double *partial;         // [B * max_blocks * 16]
     int max_blocks;
@@ -88,9 +92,10 @@ __device__ void block_sum(double (&v)[NV], double *smem /* [NV * warps] */)
 }
 
 // ---- 1. mounting-window compaction (planes.py:21-27): stable, two kernels ----------------------------------------------
-// k_window_tiles (grid tiles x clouds): every 1024-row tile compacts its window points into its own staging slot;
-// k_window_gather (one CTA per cloud): scans the tile counts and gathers the few thousand points contiguously.
-constexpr int WTILE = 1024;
+// k_window_tiles (grid tiles x clouds): every 32-row tile compacts its window points into its own staging slot;
+// k_window_gather_mad (one CTA per cloud): scans the tile counts, gathers the few thousand points contiguously and takes
+// their median / MAD.  Small CTAs for the tile pass: it runs next to the scan kernel and should find room beside it.
+constexpr int WTILE = 256;
 
 // the mounting window of calculate_plane (tools/wet_ground/planes.py:21-27); float32 comparisons, python floats are weak
 // scalars under NumPy 2
@@ -117,7 +122,7 @@ __global__ void __launch_bounds__(WTILE) k_window_tiles(PreArgs a)
     bool in = false;
     if (i < n) {
         const float *r = a.pts + (beg + i) * 5;
-        x = r[0]; y = r[1]; z = r[2];
+        x = __ldcs(r); y = __ldcs(r + 1); z = __ldcs(r + 2);
         in = lss_in_window(x, y, z);
     }
     const unsigned m = __ballot_sync(0xffffffffu, in);
@@ -126,46 +131,6 @@ __global__ void __launch_bounds__(WTILE) k_window_tiles(PreArgs a)
         o[0] = x; o[1] = y; o[2] = z;
     }
     if (lane == 0) a.tile_cnt[lss_window_tile0(beg, b) + w0 / 32] = __popc(m);
-}
-
-__global__ void __launch_bounds__(1024) k_window_gather(PreArgs a)
-{
-    extern __shared__ int prefix[];            // [n_tiles + 1]
-    __shared__ int wsum[32];
-    __shared__ int run_s;
-    const int b = blockIdx.x;
-    const int64_t beg = a.cloud_off[b];
-    const int n = (a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - beg));
-    const int n_tiles = (n + 31) / 32;
-    const int *cnt = a.tile_cnt + lss_window_tile0(beg, b);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) run_s = 0;
-    __syncthreads();
-    for (int base = 0; base < n_tiles; base += 1024) {          // exclusive scan of the tile counts
-        const int t = base + tid;
-        const int v = t < n_tiles ? cnt[t] : 0;
-        int incl = v;
-#pragma unroll
-        for (int s = 1; s < 32; s <<= 1) { const int o = __shfl_up_sync(0xffffffffu, incl, s); if (lane >= s) incl += o; }
-        if (lane == 31) wsum[warp] = incl;
-        __syncthreads();
-        int o = run_s;
-        for (int wv = 0; wv < warp; wv++) o += wsum[wv];
-        if (t < n_tiles) prefix[t] = o + incl - v;
-        __syncthreads();
-        if (tid == 1023) run_s = o + incl;
-        __syncthreads();
-    }
-    if (tid == 0) { prefix[n_tiles] = run_s; a.cp[b].n_window = run_s; }
-    __syncthreads();
-    const int K = prefix[n_tiles];
-    for (int o = tid; o < K; o += blockDim.x) {
-        int lo = 0, hi = n_tiles;              // largest tile with prefix[tile] <= o
-        while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (prefix[mid] <= o) lo = mid; else hi = mid; }
-        const float *src = a.stage + (beg + (int64_t)lo * 32 + (o - prefix[lo])) * 3;
-        float *dst = a.win + (beg + o) * 3;
-        dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
-    }
 }
 
 // ---- 2. median / MAD of the window heights: exact k-th element by 4-pass radix select ------------------------------------
@@ -224,14 +189,49 @@ __device__ float block_median(const float *win, int K, int mode, float centre, u
     return __fmul_rn(__fadd_rn(lo, hi), 0.5f);
 }
 
-__global__ void __launch_bounds__(1024) k_window_mad(PreArgs a)
+__global__ void __launch_bounds__(1024) k_window_gather_mad(PreArgs a)
 {
+    extern __shared__ int prefix[];            // [n_tiles + 1]
+    __shared__ int wsum[32];
+    __shared__ int run_s;
     __shared__ unsigned hist[256];
     __shared__ unsigned bcast[2];
     const int b = blockIdx.x;
-    const int K = a.cp[b].n_window;
+    const int64_t beg = a.cloud_off[b];
+    const int n = (a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - beg));
+    const int n_tiles = (n + 31) / 32;
+    const int *cnt = a.tile_cnt + lss_window_tile0(beg, b);
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    if (tid == 0) run_s = 0;
+    __syncthreads();
+    for (int base = 0; base < n_tiles; base += 1024) {          // exclusive scan of the tile counts
+        const int t = base + tid;
+        const int v = t < n_tiles ? cnt[t] : 0;
+        int incl = v;
+#pragma unroll
+        for (int s = 1; s < 32; s <<= 1) { const int o = __shfl_up_sync(0xffffffffu, incl, s); if (lane >= s) incl += o; }
+        if (lane == 31) wsum[warp] = incl;
+        __syncthreads();
+        int o = run_s;
+        for (int wv = 0; wv < warp; wv++) o += wsum[wv];
+        if (t < n_tiles) prefix[t] = o + incl - v;
+        __syncthreads();
+        if (tid == 1023) run_s = o + incl;
+        __syncthreads();
+    }
+    if (tid == 0) { prefix[n_tiles] = run_s; a.cp[b].n_window = run_s; }
+    __syncthreads();
+    const int K = prefix[n_tiles];
+    float *win = a.win + beg * 3;
+    for (int o = tid; o < K; o += blockDim.x) {
+        int lo = 0, hi = n_tiles;              // largest tile with prefix[tile] <= o
+        while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (prefix[mid] <= o) lo = mid; else hi = mid; }
+        const float *src = a.stage + (beg + (int64_t)lo * 32 + (o - prefix[lo])) * 3;
+        float *dst = win + (int64_t)o * 3;
+        dst[0] = src[0]; dst[1] = src[1]; dst[2] = src[2];
+    }
     if (K <= 5) return;                       // planes.py:29: flat-earth default, handled in k_ransac_refit
-    const float *win = a.win + a.cloud_off[b] * 3;
+    __syncthreads();                          // the gathered window is read back by the whole CTA
     const float med = block_median(win, K, 0, 0.0f, hist, bcast);
     const float mad = block_median(win, K, 1, med, hist, bcast);     // sklearn: median(|y - median(y)|)
     if (threadIdx.x == 0) { a.cp[b].z_med = med; a.cp[b].mad = mad; }
@@ -406,7 +406,25 @@ __device__ __forceinline__ GroundPt ground_point(const PreArgs &a, const CloudPr
     return g;
 }
 
-// ---- 5. ground pass 1: count, max(I/cos), first regression sums; grid (blocks, cloud) ---------------------------------------
+// ---- histogram binning (augmentation.py:232-233) ------------------------------------------------------------------------------
+__device__ __forceinline__ int edge_bin(double v, double lo, double hi, int nb)
+{
+    // np.histogramdd: searchsorted(edges, v, 'right') - 1 with edges = linspace(lo, hi, nb + 1); the last bin is closed
+    if (!(v >= lo) || !(v <= hi)) return -1;
+    const double step = (hi - lo) / nb;
+    int k = (int)((v - lo) / step);
+    k = k < 0 ? 0 : (k > nb ? nb : k);
+    // fix up against the edges as linspace produces them (k * step + lo; the last edge is exactly hi)
+    while (k > 0 && v < ((k == nb) ? hi : (k * step + lo))) k--;
+    while (k < nb && v >= ((k + 1 == nb) ? hi : ((k + 1) * step + lo))) k++;
+    if (k >= nb) k = nb - 1;            // v == hi belongs to the last bin
+    return k;
+}
+
+// ---- 5. the ground pass: count, max(I/cos), regression and moment sums; histogram records; grid (blocks, cloud) --------------
+// A ground point goes into the 50 x 2555 histogram when its range bin exists (10 <= d <= 70) and 5 <= I/cos <= ymax.
+// ymax is the maximum of I/cos over the ground points, so I/cos <= ymax holds for all of them once I/cos >= 5: the
+// record needs only the range bin and I/cos, and the intensity bin is taken once ymax is known (k_ground_hist).
 __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
 {
     __shared__ double red[15 * (PP_TPB / 32)];
@@ -415,20 +433,44 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
     const CloudPre cp = a.cp[b];
     const int64_t beg = a.cloud_off[b];
     const int n = (a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - beg));
+    const int lane = threadIdx.x & 31;
     // 0 n, 1-4 first regression (shifted), 5-8 S t .. S t^4, 9-11 S cos t^k, 12-14 S d cos t^k
     double v[15] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     double vmax = -1e300;
-    for (int i = blockIdx.x * PP_TPB + threadIdx.x; i < n; i += gridDim.x * PP_TPB) {
-        const GroundPt g = ground_point(a, cp, a.pts + (beg + i) * 5);
-        if (!g.ground) continue;
-        const double dd = g.d - 30.0, yy = g.norm_i - 50.0;              // shifted sums (conditioning)
-        v[0] += 1.0; v[1] += dd; v[2] += yy; v[3] += dd * dd; v[4] += dd * yy;
-        vmax = fmax(vmax, g.norm_i);
-        const double t = (g.d - 40.0) / 30.0, t2 = t * t;
-        const double c = g.cosang, dc = g.d * g.cosang;
-        v[5] += t; v[6] += t2; v[7] += t2 * t; v[8] += t2 * t2;
-        v[9] += c; v[10] += c * t; v[11] += c * t2;
-        v[12] += dc; v[13] += dc * t; v[14] += dc * t2;
+    // every thread sums its own rows in ascending order (the bits of the polynomial depend on it); the loop runs per warp
+    // so that the warp can append its records together
+    for (int w0 = blockIdx.x * PP_TPB + (threadIdx.x & ~31); w0 < n; w0 += gridDim.x * PP_TPB) {
+        const int i = w0 + lane;
+        GroundPt g;
+        g.ground = false;
+        if (i < n) {
+            const float *r = a.pts + (beg + i) * 5;
+            const float row[4] = {__ldcs(r), __ldcs(r + 1), __ldcs(r + 2), __ldcs(r + 3)};
+            g = ground_point(a, cp, row);
+        }
+        int bx = -1;
+        if (g.ground) {
+            const double dd = g.d - 30.0, yy = g.norm_i - 50.0;              // shifted sums (conditioning)
+            v[0] += 1.0; v[1] += dd; v[2] += yy; v[3] += dd * dd; v[4] += dd * yy;
+            vmax = fmax(vmax, g.norm_i);
+            const double t = (g.d - 40.0) / 30.0, t2 = t * t;
+            const double c = g.cosang, dc = g.d * g.cosang;
+            v[5] += t; v[6] += t2; v[7] += t2 * t; v[8] += t2 * t2;
+            v[9] += c; v[10] += c * t; v[11] += c * t2;
+            v[12] += dc; v[13] += dc * t; v[14] += dc * t2;
+            if (g.norm_i >= 5.0) bx = edge_bin(g.d, 10.0, 70.0, HIST_NX);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, bx >= 0);
+        if (m) {
+            int k0 = 0;
+            if (lane == 0) k0 = atomicAdd(&a.rec_cnt[b], __popc(m));
+            k0 = __shfl_sync(0xffffffffu, k0, 0);
+            if (bx >= 0) {
+                const int64_t k = beg + k0 + __popc(m & ((1u << lane) - 1u));
+                a.rec_norm[k] = g.norm_i;
+                a.rec_bin[k] = (unsigned char)bx;
+            }
+        }
     }
 #pragma unroll
     for (int s = 16; s > 0; s >>= 1) vmax = fmax(vmax, __shfl_down_sync(0xffffffffu, vmax, s));
@@ -465,79 +507,89 @@ __device__ __forceinline__ void warp_reduce_partials(const double *partial, int 
     if (vmax) *vmax = m;
 }
 
-__global__ void k_ground_stats_final(PreArgs a, int n_blocks)
+// ---- 6. the 50 x 2555 histogram, one slab of range bins per CTA in shared memory; first least-populated intensity bins ------
+// grid (slabs, cloud).  Every CTA reduces the ground pass's partials itself (the same fixed-order code, so the same bits) to
+// learn n_ground and ymax; the CTA of slab 0 stores the reduction in CloudPre.  Each CTA reads the cloud's range-bin records
+// (1 B each) and the I/cos of the records of its own slab.  The slab width trades shared memory per CTA (the kernel runs
+// next to the scan kernel) against re-reads of the record list.
+#ifndef LSS_HIST_SLAB
+#define LSS_HIST_SLAB 5
+#endif
+constexpr int HIST_SLAB = LSS_HIST_SLAB, HIST_SLABS = (HIST_NX + HIST_SLAB - 1) / HIST_SLAB, HIST_TPB = 512;
+
+__global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_blocks)
 {
-    const int b = blockIdx.x;
-    double v[15], vmax;
-    warp_reduce_partials<15>(a.partial + (size_t)b * a.max_blocks * 16, n_blocks, v, &vmax);
-    if (threadIdx.x != 0) return;
-    CloudPre &cp = a.cp[b];
-    cp.n_ground = (int)v[0];
-    cp.mom[0] = v[0];
-    for (int k = 0; k < 10; k++) cp.mom[1 + k] = v[5 + k];
-    cp.ymax = fabs(vmax);
-    if (v[0] >= 3.0) {
-        const double n = v[0], mx_ = v[1] / n, my_ = v[2] / n;
-        const double sxx = v[3] - n * mx_ * mx_, sxy = v[4] - n * mx_ * my_;
-        const double slope = sxy / sxx;                                   // scipy.stats.linregress
-        cp.lin[0] = slope;
-        cp.lin[1] = (my_ + 50.0) - slope * (mx_ + 30.0);
-    } else {
-        cp.lin[0] = cp.lin[1] = 0.0;
-        if (a.raise_few) atomicMax(a.status, LSS_ERR_TOO_FEW_GROUND);
+    extern __shared__ unsigned hist[];         // [HIST_SLAB * HIST_NY]
+    __shared__ double stat[2];                 // n_ground, ymax
+    const int b = blockIdx.y, bx0 = blockIdx.x * HIST_SLAB;
+    const int nbx = min(HIST_SLAB, HIST_NX - bx0);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (warp == 0) {
+        double v[15], vmax;
+        warp_reduce_partials<15>(a.partial + (size_t)b * a.max_blocks * 16, n_blocks, v, &vmax);
+        if (lane == 0) {
+            stat[0] = v[0];
+            stat[1] = fabs(vmax);
+            if (blockIdx.x == 0) {
+                CloudPre &cp = a.cp[b];
+                cp.n_ground = (int)v[0];
+                cp.mom[0] = v[0];
+                for (int k = 0; k < 10; k++) cp.mom[1 + k] = v[5 + k];
+                cp.ymax = fabs(vmax);
+                if (v[0] >= 3.0) {
+                    const double n = v[0], mx_ = v[1] / n, my_ = v[2] / n;
+                    const double sxx = v[3] - n * mx_ * mx_, sxy = v[4] - n * mx_ * my_;
+                    const double slope = sxy / sxx;                                   // scipy.stats.linregress
+                    cp.lin[0] = slope;
+                    cp.lin[1] = (my_ + 50.0) - slope * (mx_ + 30.0);
+                } else {
+                    cp.lin[0] = cp.lin[1] = 0.0;
+                    if (a.raise_few) atomicMax(a.status, LSS_ERR_TOO_FEW_GROUND);
+                }
+            }
+        }
     }
-}
-
-// ---- 6. 50 x 2555 histogram of (range, I/cos) over the ground points (augmentation.py:232-233) --------------------------------
-__device__ __forceinline__ int edge_bin(double v, double lo, double hi, int nb)
-{
-    // np.histogramdd: searchsorted(edges, v, 'right') - 1 with edges = linspace(lo, hi, nb + 1); the last bin is closed
-    if (!(v >= lo) || !(v <= hi)) return -1;
-    const double step = (hi - lo) / nb;
-    int k = (int)((v - lo) / step);
-    k = k < 0 ? 0 : (k > nb ? nb : k);
-    // fix up against the edges as linspace produces them (k * step + lo; the last edge is exactly hi)
-    while (k > 0 && v < ((k == nb) ? hi : (k * step + lo))) k--;
-    while (k < nb && v >= ((k + 1 == nb) ? hi : ((k + 1) * step + lo))) k++;
-    if (k >= nb) k = nb - 1;            // v == hi belongs to the last bin
-    return k;
-}
-
-__global__ void __launch_bounds__(PP_TPB) k_ground_hist(PreArgs a)
-{
-    const int b = blockIdx.y;
-    const CloudPre cp = a.cp[b];
-    if (cp.n_ground < 3) return;
+    __syncthreads();
+    const int n_ground = (int)stat[0];
+    const double ymax = stat[1];
+    if (n_ground < 3) return;
+    int32_t *ymins = a.ymins + b * HIST_NX + bx0;
+    if (a.ymins_in) {                           // parity replay: the reference host's own picks, no histogram needed
+        for (int k = threadIdx.x; k < nbx; k += HIST_TPB) {
+            const int inj = a.ymins_in[b * HIST_NX + bx0 + k];
+            ymins[k] = inj < 0 ? 0 : (inj >= HIST_NY ? HIST_NY - 1 : inj);
+        }
+        return;
+    }
+    for (int k = threadIdx.x; k < nbx * HIST_NY; k += HIST_TPB) hist[k] = 0;
+    __syncthreads();
     const int64_t beg = a.cloud_off[b];
-    const int n = (a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - beg));
-    unsigned *hist = a.hist + (size_t)b * HIST_NX * HIST_NY;
-    for (int i = blockIdx.x * PP_TPB + threadIdx.x; i < n; i += gridDim.x * PP_TPB) {
-        const GroundPt g = ground_point(a, cp, a.pts + (beg + i) * 5);
-        if (!g.ground) continue;
-        const int bx = edge_bin(g.d, 10.0, 70.0, HIST_NX);
-        const int by = edge_bin(g.norm_i, 5.0, cp.ymax, HIST_NY);
-        if (bx >= 0 && by >= 0) atomicAdd(&hist[bx * HIST_NY + by], 1u);
+    const int n_rec = a.rec_cnt[b];
+    const unsigned char *bins = a.rec_bin + beg;
+    const double *norms = a.rec_norm + beg;
+    constexpr int U = 4;                        // records in flight per thread
+    for (int k0 = threadIdx.x; k0 < n_rec; k0 += U * HIST_TPB) {
+        int rel[U];
+#pragma unroll
+        for (int u = 0; u < U; u++) {
+            const int k = k0 + u * HIST_TPB;
+            rel[u] = k < n_rec ? (int)bins[k] - bx0 : -1;
+        }
+#pragma unroll
+        for (int u = 0; u < U; u++)
+            if ((unsigned)rel[u] < (unsigned)nbx) {
+                const int by = edge_bin(norms[k0 + u * HIST_TPB], 5.0, ymax, HIST_NY);
+                if (by >= 0) atomicAdd(&hist[rel[u] * HIST_NY + by], 1u);
+            }
     }
-}
-
-// ---- 7. per range bin: first least-populated non-empty intensity bin; second regression ------------------------------------
-__global__ void __launch_bounds__(1024) k_hist_minima(PreArgs a)
-{
-    __shared__ double xs[HIST_NX], ys[HIST_NX];
-    __shared__ int okf[HIST_NX];
-    const int b = blockIdx.x;
-    CloudPre &cp = a.cp[b];
-    if (cp.n_ground < 3) return;
-    const int lane = threadIdx.x & 31;
-    const unsigned *hist = a.hist + (size_t)b * HIST_NX * HIST_NY;
-    const double ystep = (cp.ymax - 5.0) / HIST_NY;
-    for (int warp = threadIdx.x >> 5; warp < HIST_NX; warp += 32) {
+    __syncthreads();
+    for (int w = warp; w < nbx; w += HIST_TPB / 32) {
         // empty bins count as len(pointcloud_planes) (augmentation.py:234-235); argmin keeps the first minimum
         unsigned best = 0xffffffffu;
         int bidx = 0x7fffffff;
         for (int k = lane; k < HIST_NY; k += 32) {
-            unsigned c = hist[warp * HIST_NY + k];
-            if (c == 0) c = (unsigned)cp.n_ground;
+            unsigned c = hist[w * HIST_NY + k];
+            if (c == 0) c = (unsigned)n_ground;
             if (c < best) { best = c; bidx = k; }           // ascending k per lane: first occurrence per lane
         }
         for (int s = 16; s > 0; s >>= 1) {
@@ -545,30 +597,43 @@ __global__ void __launch_bounds__(1024) k_hist_minima(PreArgs a)
             const int oi = __shfl_down_sync(0xffffffffu, bidx, s);
             if (ob < best || (ob == best && oi < bidx)) { best = ob; bidx = oi; }
         }
-        if (a.ymins_in) {                       // parity replay: the reference host's own pick for this range bin
-            const int inj = a.ymins_in[b * HIST_NX + warp];
-            bidx = inj < 0 ? 0 : (inj >= HIST_NY ? HIST_NY - 1 : inj);
-        }
-        if (lane == 0) {
-            a.ymins[b * HIST_NX + warp] = bidx;
-            // yedges[ymins] with yedges = np.linspace(5, ymax, 2556): arange * step + start, last edge = stop
-            const double mv = (bidx == HIST_NY) ? cp.ymax : __dadd_rn(__dmul_rn((double)bidx, ystep), 5.0);
-            okf[warp] = mv > 5.0;                                                       // augmentation.py:238
-            ys[warp] = mv;
-            const double e0 = warp * (60.0 / HIST_NX) + 10.0;
-            const double e1 = (warp + 1 == HIST_NX) ? 70.0 : ((warp + 1) * (60.0 / HIST_NX) + 10.0);
-            xs[warp] = (e0 + e1) / 2;                                                   // augmentation.py:240-241
-        }
+        if (lane == 0) ymins[w] = bidx;
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
+}
+
+// ---- 7. second regression over the minima; quadratic fit of noise*cos over range (simulation.py:462-467) ------------------
+// The point of range bin k: its centre and the lower edge of its picked intensity bin, yedges[ymins] with
+// yedges = np.linspace(5, ymax, 2556) (arange * step + start, last edge = stop); used when that edge is above 5
+// (augmentation.py:238-241).
+__device__ __forceinline__ bool minima_point(int k, int bidx, double ymax, double ystep, double &x, double &y)
+{
+    y = (bidx == HIST_NY) ? ymax : __dadd_rn(__dmul_rn((double)bidx, ystep), 5.0);
+    const double e0 = k * (60.0 / HIST_NX) + 10.0;
+    const double e1 = (k + 1 == HIST_NX) ? 70.0 : ((k + 1) * (60.0 / HIST_NX) + 10.0);
+    x = (e0 + e1) / 2;
+    return y > 5.0;
+}
+
+// np.polyfit(d, noise * cos, 2) over the ground points with noise = noise_floor * (pmin0 * d + pmin1) (augmentation.py:252):
+// the right-hand sides S y t^k = noise_floor * (pmin0 * S d cos t^k + pmin1 * S cos t^k) come from the moment sums of the
+// ground pass, so the fit needs no pass of its own.
+__global__ void k_poly_solve(PreArgs a, double *poly_out /* [B*3] or null */, double *plane_out /* [B*4] or null */,
+                             double *fit_out /* [B*8] or null */, int32_t *ymins_out /* [B*50] or null */)
+{
+    const int b = blockIdx.x;
+    CloudPre &cp = a.cp[b];
+    if (threadIdx.x != 0) return;
+    if (cp.n_ground >= 3) {
+        const int32_t *ymins = a.ymins + b * HIST_NX;
+        const double ystep = (cp.ymax - 5.0) / HIST_NY;
         int m = 0;
-        double sx = 0, sy = 0;
-        for (int k = 0; k < HIST_NX; k++) if (okf[k]) { m++; sx += xs[k]; sy += ys[k]; }
+        double sx = 0, sy = 0, x, y;
+        for (int k = 0; k < HIST_NX; k++) if (minima_point(k, ymins[k], cp.ymax, ystep, x, y)) { m++; sx += x; sy += y; }
         if (m > 3) {                                                                     // augmentation.py:248-251
             const double mx_ = sx / m, my_ = sy / m;
             double sxx = 0, sxy = 0;
-            for (int k = 0; k < HIST_NX; k++) if (okf[k]) { sxx += (xs[k] - mx_) * (xs[k] - mx_); sxy += (xs[k] - mx_) * (ys[k] - my_); }
+            for (int k = 0; k < HIST_NX; k++)
+                if (minima_point(k, ymins[k], cp.ymax, ystep, x, y)) { sxx += (x - mx_) * (x - mx_); sxy += (x - mx_) * (y - my_); }
             cp.pmin[0] = sxy / sxx;
             cp.pmin[1] = my_ - cp.pmin[0] * mx_;
         } else {
@@ -576,19 +641,6 @@ __global__ void __launch_bounds__(1024) k_hist_minima(PreArgs a)
             cp.pmin[1] = cp.lin[1];
         }
     }
-}
-
-// ---- 8. quadratic fit of noise*cos over range (simulation.py:462-467) ---------------------------------------------------------
-// np.polyfit(d, noise * cos, 2) over the ground points with noise = noise_floor * (pmin0 * d + pmin1) (augmentation.py:252):
-// the right-hand sides S y t^k = noise_floor * (pmin0 * S d cos t^k + pmin1 * S cos t^k) come from the moment sums of the
-// first ground pass, so the fit needs no pass of its own.
-__global__ void k_poly_solve(PreArgs a, int n_blocks, double *poly_out /* [B*3] or null */, double *plane_out /* [B*4] or null */,
-                             double *fit_out /* [B*8] or null */, int32_t *ymins_out /* [B*50] or null */)
-{
-    const int b = blockIdx.x;
-    CloudPre &cp = a.cp[b];
-    if (threadIdx.x != 0) return;
-    (void)n_blocks;
     double s[8];
     s[0] = cp.mom[0]; s[1] = cp.mom[1]; s[2] = cp.mom[2]; s[3] = cp.mom[3]; s[4] = cp.mom[4];
     for (int k = 0; k < 3; k++) s[5 + k] = a.noise_floor * (cp.pmin[0] * cp.mom[8 + k] + cp.pmin[1] * cp.mom[5 + k]);
@@ -627,7 +679,7 @@ __global__ void k_poly_solve(PreArgs a, int n_blocks, double *poly_out /* [B*3] 
 
 }  // namespace
 
-struct PrepassLayout { int64_t cp, win, stage, tile_cnt, tile_base, hist, trial, partial, plane_in, ymins, ymins_in, total; int max_blocks; };
+struct PrepassLayout { int64_t cp, rec_cnt, win, stage, tile_cnt, tile_base, trial, partial, plane_in, ymins, ymins_in, total; int max_blocks; };
 
 static PrepassLayout prepass_layout(int64_t n_total, int n_clouds)
 {
@@ -635,11 +687,11 @@ static PrepassLayout prepass_layout(int64_t n_total, int n_clouds)
     L.max_blocks = 64;
     int64_t o = 0;
     L.cp = o;       o = align_up(o + (int64_t)sizeof(CloudPre) * n_clouds, 256);
+    L.rec_cnt = o;  o = align_up(o + (int64_t)n_clouds * 4, 256);
     L.win = o;      o = align_up(o + n_total * 3 * 4, 256);
-    L.stage = o;    o = align_up(o + n_total * 3 * 4, 256);
+    L.stage = o;    o = align_up(o + n_total * 3 * 4, 256);    // then the histogram records: 8 + 1 B per row
     L.tile_cnt = o; o = align_up(o + (n_total / 32 + n_clouds + 2) * 4, 256);
     L.tile_base = o; o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
-    L.hist = o;     o = align_up(o + (int64_t)n_clouds * HIST_NX * HIST_NY * 4, 256);
     L.trial = o;    o = align_up(o + (int64_t)n_clouds * RANSAC_T * 8 * 8, 256);
     L.partial = o;  o = align_up(o + (int64_t)n_clouds * L.max_blocks * 16 * 8, 256);
     L.plane_in = o; o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
@@ -682,7 +734,9 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     a.stage = (float *)(ws + L.stage);
     a.tile_cnt = (int *)(ws + L.tile_cnt);
     a.tile_base = (const int32_t *)(ws + L.tile_base);
-    a.hist = (unsigned *)(ws + L.hist);
+    a.rec_norm = (double *)(ws + L.stage);
+    a.rec_bin = (unsigned char *)(ws + L.stage + N * 8);
+    a.rec_cnt = (int *)(ws + L.rec_cnt);
     a.trial = (double *)(ws + L.trial);
     a.partial = (double *)(ws + L.partial);
     a.max_blocks = L.max_blocks;
@@ -700,8 +754,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
 
     {
         ZeroRegions z;
-        z.add(a.cp, sizeof(CloudPre) * B);
-        z.add(a.hist, (size_t)B * HIST_NX * HIST_NY * 4);
+        z.add(a.cp, (size_t)(L.rec_cnt - L.cp) + sizeof(int) * B);     // CloudPre records and record cursors
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
     }
     {
@@ -713,19 +766,20 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
         } else {
             const int max_tiles = (int)std::max<int64_t>(1, (max_n + WTILE - 1) / WTILE);
             LSS_CUDA_CHECK(e, lss_launch(e, k_window_tiles, dim3(max_tiles, B), WTILE, 0, stream, a));
-            const size_t gather_smem = sizeof(int) * ((size_t)max_tiles * (WTILE / 32) + 2);
+            const size_t gather_smem = sizeof(int) * ((size_t)(max_n + 31) / 32 + 2);
             if (gather_smem > 48 * 1024)
-                LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_window_gather, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)gather_smem));
-            LSS_CUDA_CHECK(e, lss_launch(e, k_window_gather, B, 1024, gather_smem, stream, a));
-            LSS_CUDA_CHECK(e, lss_launch(e, k_window_mad, B, 1024, 0, stream, a));
+                LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_window_gather_mad, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       (int)gather_smem));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_window_gather_mad, B, 1024, gather_smem, stream, a));
             LSS_CUDA_CHECK(e, lss_launch(e, k_ransac_trials, dim3(RANSAC_T, B), PP_TPB, 0, stream, a));
             LSS_CUDA_CHECK(e, lss_launch(e, k_ransac_refit, B, PP_TPB, 0, stream, a));
         }
         LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats, dim3(nblk, B), PP_TPB, 0, stream, a));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats_final, B, 32, 0, stream, a, nblk));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_hist, dim3(nblk, B), PP_TPB, 0, stream, a));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_hist_minima, B, 1024, 0, stream, a));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_poly_solve, B, 32, 0, stream, a, nblk, d_poly_out, d_plane_out, io.d_fit_out,
+        const size_t hist_smem = sizeof(unsigned) * HIST_SLAB * HIST_NY;
+        if (hist_smem > 48 * 1024)
+            LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_ground_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_smem));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_hist, dim3(HIST_SLABS, B), HIST_TPB, hist_smem, stream, a, nblk));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_poly_solve, B, 32, 0, stream, a, d_poly_out, d_plane_out, io.d_fit_out,
                                      io.d_ymins_out));
     }
     return LSS_OK;
