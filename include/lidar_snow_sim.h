@@ -431,6 +431,13 @@ LSS_API const char *lss_kernel_name(int kernel);
 /* test hook: the beam azimuth the kernels compute when no d_theta is supplied, (float)atan2((double)y, (double)x)
  * (simulation.py:91), element-wise on device arrays of n float32 values                                              */
 LSS_API lss_status lss_debug_azimuth(lss_engine *e, const float *d_y, const float *d_x, int64_t n, float *d_out, void *stream);
+/* diagnostic hook: where the solve kernel's time goes, in a library built with -DLSS_SOLVE_PHASE_CLOCKS (otherwise
+ * LSS_ERR_INVALID_ARG, and lss_last_error says so).  Synchronises the device, copies the counters summed over every
+ * solve launch since the last reset to h_out (NULL: no copy; else n >= LSS_DEBUG_SOLVE_PHASE_WORDS) and, if reset != 0,
+ * zeroes them.  h_out[0..7): warp cycles in tile fetch, fill, range sort + claiming, pulses, piece sweep, piece
+ * evaluation + argmax, stores + statistics; [7] tiles solved; [8] warps that ran; [9 + c] listed beams of work class c. */
+#define LSS_DEBUG_SOLVE_PHASE_WORDS 137
+LSS_API lss_status lss_debug_solve_phases(lss_engine *e, int reset, uint64_t *h_out, int n);
 /* test hook: the engine's range grid R = np.round(np.linspace(0, 120 + c*tau_h, 1230), 2) (simulation.py:111-116),
  * 1230 doubles written to h_out.  Host only, needs no GPU.                                                          */
 LSS_API lss_status lss_debug_range_grid(double *h_out);

@@ -80,6 +80,7 @@ SIGNATURES = [
     ('lss_launch_count', _c.c_int64, [_P]),
     ('lss_debug_range_grid', _c.c_int, [_P]),
     ('lss_debug_azimuth', _c.c_int, [_P, _P, _P, _c.c_int64, _P, _P]),
+    ('lss_debug_solve_phases', _c.c_int, [_P, _c.c_int, _P, _c.c_int]),
     ('lss_noise_threshold_poly', _c.c_int, [_P, _P, _P, _c.c_int, _c.c_double, _P, _P, _P, _P, _P, _P, _P, _c.c_int64,
                                             _P]),
     ('lss_prepass_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),

@@ -19,7 +19,9 @@
 //     (occluders + 1 per beam) with a warp scan of the counts the scan kernel delivered;
 //   * the hits are loaded COOPERATIVELY: arena slot s is filled by lane s mod 32, whatever beam it belongs to (owner by
 //     a shuffle binary search over the offsets, the slot's particle = the r-th hit index the scan stored for the owner),
-//     so the index -> record loads of all beams are in flight together; the owner then orders its few slots by range;
+//     in passes (all index loads of a round, then all record loads, by cp.async), so the loads of all beams are in flight
+//     together; the owner then orders its few slots by range;
+//   * a warp claims its next tile when it starts one and loads that tile's chunk id and items while it solves this one;
 //   * nearest-first claiming runs in place in the arena: the union list lives in the slots of the already processed
 //     hits, pulses (range, ratio) are compacted to the front;
 //   * waveform: sin(pi (R_k - r) / (c tau)) = sin(pi a_k) cos(pi b) - cos(pi a_k) sin(pi b) with a_k = R_k / (c tau) from a
@@ -39,7 +41,7 @@ namespace {
 constexpr int SOLVE_TPB = 128;
 constexpr int SOLVE_WARPS = SOLVE_TPB / 32;
 #ifndef LSS_SOLVE_CTAS
-#define LSS_SOLVE_CTAS 6
+#define LSS_SOLVE_CTAS 5         // 96 registers: six CTAs would hold the pipelined tile to 80 and spill
 #endif
 #ifndef LSS_SOLVE_ARENA
 #define LSS_SOLVE_ARENA 160
@@ -368,6 +370,66 @@ __device__ __forceinline__ void pulse_phase(double r, double &sb, double &cb)
     cb = fma(-corr, s, c);
 }
 
+// cp.async of 4 / 8 bytes global -> shared (the fill of k_solve: loads in flight without registers); a lane's copies
+// are complete after cp_async_wait_all(), and visible to the other lanes of the warp after a __syncwarp() that follows
+__device__ __forceinline__ void cp_async4(void *dst, const void *src)
+{
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async8(void *dst, const void *src)
+{
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;\n" ::: "memory"); }
+
+// Phase clocks of k_solve, a diagnostic build only (-DLSS_SOLVE_PHASE_CLOCKS in LSS_NVCC_FLAGS; tools/solve_phases.py):
+// lane 0 of every warp sums, in shared memory, the clock64() cycles its warp spends in each phase of its tiles, and adds
+// the sums to g_solve_phase when the warp runs out of tiles; lss_debug_solve_phases reads them back.  Every stamp is
+// taken where the warp is converged; claiming and pulses run in one lane-divergent block, so the lanes stamp the end of
+// their claiming and the warp's last one splits the block.  Without the flag every macro below is empty.
+#ifdef LSS_SOLVE_PHASE_CLOCKS
+enum { PH_FETCH, PH_FILL, PH_CLAIM, PH_PULSES, PH_SWEEP, PH_EVAL, PH_STORE, PH_N };
+static_assert(PH_N + 2 + LIST_CLASSES == LSS_DEBUG_SOLVE_PHASE_WORDS, "layout of lss_debug_solve_phases");
+__device__ unsigned long long g_solve_phase[LSS_DEBUG_SOLVE_PHASE_WORDS];   // phases, tiles, warps, beams per class
+#define PHASE_INIT()                                                                                                  \
+    __shared__ unsigned long long s_ph[SOLVE_WARPS][PH_N + 1];                                                        \
+    if (lane <= PH_N) s_ph[wid][lane] = 0ull;                                                                         \
+    unsigned ph_t = (unsigned)clock64();                 /* 32-bit deltas: a phase is far below 2^32 cycles */        \
+    unsigned ph_split = 0u
+#define PHASE(k)                                                                                                      \
+    do {                                                                                                              \
+        const unsigned ph_n = (unsigned)clock64();                                                                    \
+        if (lane == 0) s_ph[wid][k] += ph_n - ph_t;                                                                   \
+        ph_t = ph_n;                                                                                                  \
+    } while (0)
+#define PHASE_MARK() (ph_split = (unsigned)clock64() - ph_t)
+#define PHASE_SPLIT(k0, k1)                                                                                           \
+    do {                                                                                                              \
+        const unsigned ph_n = (unsigned)clock64();                                                                    \
+        const unsigned sp = __reduce_max_sync(FULL, ph_split);                                                        \
+        if (lane == 0) { s_ph[wid][k0] += sp; s_ph[wid][k1] += ph_n - ph_t - sp; }                                   \
+        ph_t = ph_n;                                                                                                  \
+        ph_split = 0u;                                                                                                \
+    } while (0)
+#define PHASE_TILE(cls, active)                                                                                       \
+    do {                                                                                                              \
+        const unsigned nb = __popc(__ballot_sync(FULL, active));                                                      \
+        if (lane == 0) { s_ph[wid][PH_N]++; atomicAdd(&g_solve_phase[PH_N + 2 + (cls)], (unsigned long long)nb); }    \
+    } while (0)
+#define PHASE_FLUSH()                                                                                                 \
+    do {                                                                                                              \
+        if (lane <= PH_N) atomicAdd(&g_solve_phase[lane], s_ph[wid][lane]);                                           \
+        if (lane == 0) atomicAdd(&g_solve_phase[PH_N + 1], 1ull);                                                     \
+    } while (0)
+#else
+#define PHASE_INIT()
+#define PHASE(k)
+#define PHASE_MARK()
+#define PHASE_SPLIT(k0, k1)
+#define PHASE_TILE(cls, active)
+#define PHASE_FLUSH()
+#endif
+
 __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs a, int *tile_cursor)
 {
     __shared__ double s_arena[SOLVE_WARPS][4][ARENA];
@@ -383,13 +445,15 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
     unsigned long long *W = reinterpret_cast<unsigned long long *>(A2);
 
     // tiles in class order, costliest class first; a tile holds beams of one class only.  s_tile0[c] = first tile of
-    // class c, s_tile0[LIST_CLASSES] = number of tiles.
+    // class c, s_tile0[LIST_CLASSES] = number of tiles; s_cnt[c] = listed beams of class c.
     __shared__ int s_tile0[LIST_CLASSES + 1];
-    const int *cls_cnt = a.hdr + LIST_CLASSES;
+    __shared__ int s_cnt[LIST_CLASSES];
     if (wid == 0) {
         int run = 0;
         for (int c0 = 0; c0 < LIST_CLASSES; c0 += 32) {
-            const int v = (cls_cnt[c0 + lane] + 31) >> 5;
+            const int n = a.hdr[LIST_CLASSES + c0 + lane];
+            s_cnt[c0 + lane] = n;
+            const int v = (n + 31) >> 5;
             int incl = v;
 #pragma unroll
             for (int sft = 1; sft < 32; sft <<= 1) {
@@ -405,24 +469,52 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
     const int n_tiles = s_tile0[LIST_CLASSES];
     const double ctau = 299792458.0 * 1e-8;
     const double inv_step = (double)(LSS_M_EXT - 1) / (120 + ctau);
+    PHASE_INIT();
 
-    for (;;) {
-        int tile = 0;
-        if (lane == 0) tile = atomicAdd(tile_cursor, 1);
-        tile = __shfl_sync(FULL, tile, 0);
-        if (tile >= n_tiles) break;
-        int cls = 0;                                        // the tile's class: last c with s_tile0[c] <= tile
+    // A tile's loads are a chain: tile number -> class and beam number (shared memory) -> chunk id -> item.  Each warp
+    // claims its next tile when it starts one and runs the chain for it while this one is solved: the chunk id is
+    // requested after the fill, the items after claiming, so they arrive by the time the next tile starts.  A warp
+    // whose claim is past the last tile stops after the tile it has.
+    const auto beam_of = [&](int t, int &c, int &j) {       // this lane's beam of tile t: number j in class c, if any
+        c = 0;                                              // (the last c with s_tile0[c] <= t)
 #pragma unroll
         for (int step = LIST_CLASSES / 2; step; step >>= 1)
-            if (s_tile0[cls + step] <= tile) cls += step;
-        const int j = (tile - s_tile0[cls]) * 32 + lane;    // number of this lane's beam in its class
-        const bool active = j < cls_cnt[cls];
-        SolveItem it;
-        it.key = 0ull; it.hit_off = 0; it.L = 0; it.th32 = 0.0f; it.px = 0.0f; it.py = 0.0f; it.pz = 0.0f;
-        if (active) {
-            const int chunk = a.chunk_tab[(int64_t)cls * a.chunks_per_class + j / LIST_CHUNK];
-            it = a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK];
-        }
+            if (s_tile0[c + step] <= t) c += step;
+        j = (t - s_tile0[c]) * 32 + lane;
+        return t < n_tiles && j < s_cnt[c];
+    };
+    const auto chunk_of = [&](int c, int j) { return a.chunk_tab[(int64_t)c * a.chunks_per_class + j / LIST_CHUNK]; };
+    const auto item_of = [&](int chunk, int j) { return a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK]; };
+    const auto empty_item = [] {
+        SolveItem e;
+        e.key = 0ull; e.hit_off = 0; e.L = 0; e.th32 = 0.0f; e.px = 0.0f; e.py = 0.0f; e.pz = 0.0f;
+        return e;
+    };
+    int tile = 0;
+    if (lane == 0) tile = atomicAdd(tile_cursor, 1);
+    tile = __shfl_sync(FULL, tile, 0);
+    SolveItem it = empty_item();
+    {
+        int c, j;
+        if (beam_of(tile, c, j)) it = item_of(chunk_of(c, j), j);
+    }
+
+    while (tile < n_tiles) {
+        int cls, jn;
+        const bool active = beam_of(tile, cls, jn);
+        int nxt = 0;
+        if (lane == 0) nxt = atomicAdd(tile_cursor, 1);
+        int nchunk = 0;                                     // chunk of this lane's beam of the next tile, 0: none
+        bool fetched = false;
+        SolveItem nx = empty_item();
+        const auto next_chunk = [&] {                       // after the fill
+            nxt = __shfl_sync(FULL, nxt, 0);
+            if (beam_of(nxt, cls, jn)) nchunk = chunk_of(cls, jn);
+        };
+        const auto next_item = [&] {                        // after claiming
+            if (nchunk > 0) nx = item_of(nchunk, jn);
+            fetched = true;
+        };
         // the item holds all the solve needs of the input row (the intensity only matters if the waveform is solved,
         // and then it is replaced)
         const int b = (int)((it.key >> 32) & 0xffffu);
@@ -447,6 +539,8 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         // and occluder count stay as the scan wrote them)
         if (L > SOLVE_LCAP) raise_status(a.status, LSS_ERR_OCCLUDER_OVERFLOW);
         const int need = (L > 0 && L <= SOLVE_LCAP) ? L + 1 : 0;
+        PHASE_TILE(cls, active);
+        PHASE(PH_FETCH);
 
         // ---- rounds: as many beams of the tile as fit into the arena (normally all of them) ---------------------------
         unsigned remaining = __ballot_sync(FULL, need > 0);
@@ -469,6 +563,12 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
             int kbest = 0;
 
             // ---- cooperative fill: arena slot s <- the r-th hit of its owner beam, (a1, a2, range) --------------------
+            // Three passes, so that two round trips of dependent loads are exposed per round of the arena instead of
+            // two per 32 slots, and no register holds a load in flight (cp.async into shared memory):
+            //   1. the particle index of every slot (PK[s], -1: nothing to load) and its owner lane (PK[ARENA + s]);
+            //   2. the record and the tangents of every slot into A0 .. A3 and PD (all unused until claiming);
+            //   3. each slot's exact test and (a1, a2, range), in place.
+            // (Slot L of a beam is its hard target, filled later; a beam without stored hits is filled after the passes.)
 #pragma unroll 1
             for (int s0 = 0; s0 < total; s0 += 32) {
                 const int s = s0 + lane;
@@ -483,20 +583,44 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 const int Lj = __shfl_sync(FULL, L, j);
                 const int hoj = __shfl_sync(FULL, it.hit_off, j);
                 const int inr = __shfl_sync(FULL, (int)in_round, j);
+                if (s < total) {
+                    PK[ARENA + s] = j;
+                    if (inr && r < Lj && hoj >= 0) cp_async4(&PK[s], &a.hit_idx[hoj + r]);
+                    else PK[s] = -1;
+                }
+            }
+            cp_async_wait_all();
+            __syncwarp();
+#pragma unroll 1
+            for (int s = lane; s < total; s += 32) {
+                const int pi = PK[s];
+                if (pi >= 0) {
+                    cp_async8(&A0[s], &a.rec[pi].phi);
+                    cp_async8(&A1[s], &a.rec[pi].rho);
+                    cp_async8(&A2[s], &a.rec[pi].alpha);
+                    cp_async8(&A3[s], &a.tan[pi].t_right);
+                    cp_async8(&PD[s], &a.tan[pi].t_left);
+                }
+            }
+            cp_async_wait_all();
+            __syncwarp();
+#pragma unroll 1
+            for (int s0 = 0; s0 < total; s0 += 32) {
+                const int s = s0 + lane;
+                const int j = s < total ? PK[ARENA + s] : 0;
                 Beam bj;
                 bj.d = shfl_f64(bm.d, j);
                 bj.right = shfl_f64(bm.right, j);
                 bj.left = shfl_f64(bm.left, j);
                 bj.straddle = bj.right > bj.left;
-                // (slot L of a beam is its hard target: filled later; a beam without stored hits is filled below)
-                if (s < total && inr && r < Lj && hoj >= 0) {
-                    const int pi = a.hit_idx[hoj + r];
-                    const ParticleTan tn = a.tan[pi];               // (both records requested before either is used)
+                if (s < total && PK[s] >= 0) {
+                    ParticleRec rc;
+                    rc.phi = A0[s]; rc.rho = A1[s]; rc.alpha = A2[s];
                     double rho;
                     bool rh, lh;
-                    exact_hit(a.rec + pi, bj, rho, rh, lh);
-                    A0[s] = rh ? bj.right : tn.t_right;             // geometry.py:26-27: a limit ray the disk crosses clips
-                    A1[s] = lh ? bj.left : tn.t_left;
+                    exact_hit(&rc, bj, rho, rh, lh);
+                    A0[s] = rh ? bj.right : A3[s];                  // geometry.py:26-27: a limit ray the disk crosses clips
+                    A1[s] = lh ? bj.left : __longlong_as_double((long long)PD[s]);
                     A2[s] = rho;
                 }
             }
@@ -513,6 +637,8 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 });
             }
             __syncwarp();
+            if (!fetched) next_chunk();
+            PHASE(PH_FILL);
 
             if (in_round) {
                 // order by range (np.argsort, simulation.py:416); the prefix is sorted by the float32 range already, so this
@@ -581,6 +707,7 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 n_claim = P;
                 double ratio_hard = ((ep_max - ep_min) - claimed_total) / a.div_rad;
                 ratio_hard = ratio_hard < 0 ? 0 : (ratio_hard > 1 ? 1 : ratio_hard);
+                PHASE_MARK();
 
                 if (P > 0) {
                     // ---- pulses of the waveform (simulation.py:137-149) --------------------------------------------------
@@ -620,6 +747,8 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                     else n_pulses = P + 1;
                 }
             }
+            PHASE_SPLIT(PH_CLAIM, PH_PULSES);
+            if (!fetched) next_item();
 
             // ---- argmax of the summed waveform (simulation.py:148-153) -----------------------------------------------------
             // Only samples inside some pulse window are non-zero.  Pulse ranges ascend, so first and end samples of the
@@ -689,6 +818,7 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
             const int pex = pincl - np_mine;
             const int ptotal = __shfl_sync(FULL, pincl, 31);
             __syncwarp();
+            PHASE(PH_SWEEP);
             {
                 const float step = (float)((120 + ctau) / (double)(LSS_M_EXT - 1));
                 const float ctau_f = (float)ctau;
@@ -753,6 +883,7 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 if (v > best) { best = v; kbest = PK[2 * off + r]; }
             }
             __syncwarp();
+            PHASE(PH_EVAL);
 
             if (n_pulses > 0) {
                 // ---- new range / intensity / label (simulation.py:151-188) -------------------------------------------------
@@ -779,7 +910,9 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 out_i = (float)ci;
             }
             __syncwarp();
+            PHASE(PH_STORE);
         }
+        if (!fetched) { next_chunk(); next_item(); }        // (no beam of the tile needed a round)
 
         // ---- np.round of the intensity column (simulation.py:516), store, label-1 statistics (simulation.py:170) ----------
         if (active) {
@@ -803,7 +936,11 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
             const unsigned sum = __reduce_add_sync(mb, on ? (unsigned)att_new_i : 0u);
             if (on && lane == __ffs(mb) - 1) atomicAdd(&a.att_sum[b], (unsigned long long)sum);
         }
+        PHASE(PH_STORE);
+        tile = nxt;
+        it = nx;
     }
+    PHASE_FLUSH();
 }
 
 }  // namespace
@@ -824,6 +961,24 @@ extern "C" lss_status lss_debug_azimuth(lss_engine *e, const float *d_y, const f
     LSS_CUDA_CHECK(e, lss_launch(e, k_debug_azimuth, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, d_y, d_x,
                                  d_out, n));
     return LSS_OK;
+}
+
+extern "C" lss_status lss_debug_solve_phases(lss_engine *e, int reset, uint64_t *h_out, int n)
+{
+    if (!e || (h_out && n < LSS_DEBUG_SOLVE_PHASE_WORDS)) return LSS_ERR_INVALID_ARG;
+#ifdef LSS_SOLVE_PHASE_CLOCKS
+    DeviceGuard g(e->device);
+    LSS_CUDA_CHECK(e, cudaDeviceSynchronize());
+    if (h_out) LSS_CUDA_CHECK(e, cudaMemcpyFromSymbol(h_out, g_solve_phase, sizeof(g_solve_phase)));
+    if (reset) {
+        static const unsigned long long zero[LSS_DEBUG_SOLVE_PHASE_WORDS] = {};
+        LSS_CUDA_CHECK(e, cudaMemcpyToSymbol(g_solve_phase, zero, sizeof(zero)));
+    }
+    return LSS_OK;
+#else
+    (void)reset;
+    return lss_fail(e, LSS_ERR_INVALID_ARG, "lss_debug_solve_phases: the library was built without -DLSS_SOLVE_PHASE_CLOCKS");
+#endif
 }
 
 cudaError_t lss_launch_scan(lss_engine *e, const DevArgs &a, cudaStream_t stream)
