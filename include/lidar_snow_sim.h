@@ -309,6 +309,36 @@ LSS_API lss_status lss_lisa_batch(lss_engine *e, const double *d_points, int n_f
                                   int mode, double alpha, double r_min, double r_max, double beam_divergence,
                                   double min_diameter, double range_accuracy, int signal_last,
                                   const double *d_draw_table, int table_len, uint64_t seed, double *d_out, void *stream);
+/* The dataset's whole LISA block (dense_dataset.py:713-746) on a batch of device-resident float32 clouds, a rain rate per
+ * cloud, e.g. the slot-compacted output of lss_dror_batch or lss_fog_batch_params.  For each valid row of an applied cloud b:
+ *   LISA input    x, y, z widened to float64, intensity (double)(I / 255.0f) (NumPy divides the float32 column in float32)
+ *   experiment    exactly lss_lisa_batch's, with cloud b's rain rate, alpha and seed
+ *   output row    x, y, z and round(i_new * 255) (half to even) rounded to float32, the label (1 not scattered,
+ *                 2 scattered) in column 4, columns >= 5 copied; rows with label 0 (lost) are dropped
+ * A cloud's rows are bit-identical to lss_lisa_batch on its float64 conversion followed by those host steps.
+ *   d_points        float32[n_total * n_features], n_features >= 5 (x, y, z, intensity in [0, 255], channel, ...).  The
+ *                   dataset block's n_features = 4 branch (a new float64 array) is not reproduced: LSS_ERR_INVALID_ARG.
+ *                   As in the reference, column 4 holds LISA's label afterwards, not the channel.
+ *   h_cloud_offsets int64[n_clouds + 1] host; d_cloud_counts int32[n_clouds] device or NULL: valid rows per cloud slot
+ *   h_rain_rate, h_alpha   float64[n_clouds] host: Rr [mm/h] (> 0 on every applied cloud) and LISA.alpha(LISA.Nd(D, Rr))
+ *   h_seed          uint64[n_clouds] host: key of the counter-based generator (with the row index inside the cloud, so a
+ *                   cloud's draws do not depend on its place in the batch); may be NULL with a draw table
+ *   h_apply         uint8[n_clouds] host or NULL (= every cloud): clouds with 0 are copied through whole (the dataset's
+ *                   per-sample coin flip), their rain rate is not read
+ *   mode, r_min, r_max, beam_divergence, min_diameter, range_accuracy, signal_last, d_draw_table, table_len   as
+ *                   lss_lisa_batch (one draw table for every cloud; LSS_ERR_WORKSPACE, asynchronous, if it is too short)
+ *   d_out_points    float32[n_total * n_features]: each cloud's kept rows in input order at the front of its slot; rows
+ *                   behind them unspecified.  Must not alias d_points.
+ *   d_out_counts    int32[n_clouds] kept rows;  d_out_n_lost  int32[n_clouds] rows with label 0 (0 for clouds not applied)
+ *   d_workspace     lss_lisa_cloud_batch_workspace_bytes(n_total, n_clouds) bytes.  No allocation, no synchronisation. */
+LSS_API lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                        const int32_t *d_cloud_counts, int n_clouds, const double *h_rain_rate,
+                                        const double *h_alpha, const uint64_t *h_seed, const uint8_t *h_apply, int mode,
+                                        double r_min, double r_max, double beam_divergence, double min_diameter,
+                                        double range_accuracy, int signal_last, const double *d_draw_table, int table_len,
+                                        float *d_out_points, int32_t *d_out_counts, int32_t *d_out_n_lost,
+                                        void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_lisa_cloud_batch_workspace_bytes(int64_t n_total, int n_clouds);
 
 /* ---- point-range mask + voxelisation ("next" row, SURVEY.md 8f-4) ---------------------------------------------------------
  * The detector-input stage of the reference's data path on device-resident clouds, e.g. the slot-compacted output of

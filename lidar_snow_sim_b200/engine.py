@@ -517,6 +517,46 @@ class SnowfallEngine:
                 out['work'] = self._ws_dror[:32].view(torch.int64).clone()
         return out
 
+    def lisa_cloud_batch(self, points, cloud_offsets, rain_rate, alpha, seed, mode, r_min=0.9, r_max=120.0,
+                         beam_divergence=3e-3, min_diameter=0.05, range_accuracy=0.09, signal_last=False, counts=None,
+                         apply=None, draw_table=None):
+        """
+        The dataset's LISA block (dense_dataset.py:732-746) on a batch of device-resident clouds (lss_lisa_cloud_batch,
+        current stream, no synchronisation).  points: CUDA float32 (N, F), F >= 5, intensity in [0, 255]; rain_rate,
+        alpha, seed: length-B host sequences (seed may be None with a draw table); mode 0 'rain', 1 'gunn', 2 'sekhon';
+        counts: optional CUDA int32 (B,) valid rows per slot; apply: optional length-B booleans (clouds with False are
+        copied through); draw_table: CUDA float64 fixed-seed draw sequence or None.  Returns dict(points (N, F) float32:
+        each cloud's kept rows at the front of its slot, label in column 4; counts (B,) int32; n_lost (B,) int32).
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        N = int(off[-1])
+        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
+        assert points.dim() == 2
+        F = int(points.shape[1])
+        if counts is not None:
+            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        if draw_table is not None:
+            assert draw_table.is_cuda and draw_table.dtype == torch.float64 and draw_table.is_contiguous()
+        rr, al = [np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (B,))) for v in (rain_rate, alpha)]
+        sd = None if seed is None else np.ascontiguousarray(np.broadcast_to(np.asarray(seed, dtype=np.uint64), (B,)))
+        ap = None if apply is None else np.ascontiguousarray(np.asarray(apply, dtype=bool).reshape(B), dtype=np.uint8)
+        with torch.cuda.device(self.device):
+            out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device),
+                       counts=torch.empty((B,), dtype=torch.int32, device=self.device),
+                       n_lost=torch.empty((B,), dtype=torch.int32, device=self.device))
+            need = self.lib.lss_lisa_cloud_batch_workspace_bytes(N, B)
+            if getattr(self, '_ws_lisa', None) is None or self._ws_lisa.numel() < need:
+                self._ws_lisa = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_lisa_cloud_batch(
+                self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, _ptr(rr), _ptr(al), _ptr(sd), _ptr(ap), int(mode),
+                float(r_min), float(r_max), float(beam_divergence), float(min_diameter), float(range_accuracy),
+                1 if signal_last else 0, _ptr(draw_table), 0 if draw_table is None else int(draw_table.numel()),
+                _ptr(out['points']), _ptr(out['counts']), _ptr(out['n_lost']), _ptr(self._ws_lisa),
+                int(self._ws_lisa.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out
+
     def gather_push(self, points, counts, d_cloud_offsets, n_rows, world, rank, peer_points, peer_counts, mc_points=0,
                     mc_counts=0, blocks=0):
         """lss_gather_push on the current stream: write the kept rows of this rank's slot-compacted batch (+ counts) into

@@ -126,6 +126,75 @@ class OnTheFlyWeather:
         return points
 
 
+_LISA_CHANCES = {'8in9': [1, 1, 1, 1, 1, 1, 1, 1, 0], '1in10': [1, 0, 0, 0, 0, 0, 0, 0, 0, 0]}   # dense_dataset.py:717-722
+
+
+def _lisa_draws(method, rainfall_rates):
+    """The block's draws from NumPy's global generator for one sample: the coin flip, then the rain rate under 'uniform'
+    (dense_dataset.py:717-730).  Returns (applied, rain rate)."""
+    choices = [0]
+    for key, c in _LISA_CHANCES.items():
+        if key in method:
+            choices = c
+            break
+    if not np.random.choice(choices):
+        return False, 0
+    rainfall_rate = 0
+    if 'uniform' in method:
+        rainfall_rate = np.random.choice(rainfall_rates)
+    return True, rainfall_rate
+
+
+def lisa_block(points, dataset_cfg, lisa, rainfall_rates, training=True):
+    """The LISA block of `DenseDataset.__getitem__` (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:713-746) on one
+    NumPy cloud, over `lisa.augment` (a LISA): same config key (`LISA: '<...>_<uniform>_<8in9 | 1in10>'`), same draws
+    from NumPy's global generator, same host conversions (intensity / 255 in float32, round(i * 255) half to even, the
+    cast back into `points`, label-0 rows dropped).  As in the reference, column 4 holds LISA's label afterwards, and
+    without 'uniform' the rain rate is 0, which LISA rejects.  The caller's array is not modified."""
+    if not (training and 'LISA' in dataset_cfg):
+        return points
+    applied, rainfall_rate = _lisa_draws(dataset_cfg['LISA'], rainfall_rates)
+    if not applied:
+        return points
+    before_lisa = np.zeros((points.shape[0], 4))
+    before_lisa[:, :3] = points[:, :3]
+    before_lisa[:, 3] = points[:, 3] / 255
+    after_lisa = lisa.augment(pc=before_lisa, Rr=rainfall_rate)
+    after_lisa[:, 3] = np.round(after_lisa[:, 3] * 255)
+    if points.shape[1] < 5:
+        points = np.zeros((points.shape[0], points.shape[1] + 1))
+    else:
+        points = points.copy()
+    points[:, :5] = after_lisa[:, :5]
+    return points[np.where(points[:, 4] != 0)]
+
+
+def lisa_block_batch(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, counts=None, training=True):
+    """`lisa_block` for a batch of device-resident clouds in one LISA.augment_batch call: points CUDA float32 (N, F),
+    F >= 5; cloud b = rows cloud_offsets[b]:cloud_offsets[b+1] (the first counts[b] with `counts`).  The draws are taken
+    sample by sample in batch order -- coin flip, rain rate, and for an applied sample the generator key augment would
+    draw -- so every cloud's rows and NumPy's global state afterwards equal B lisa_block calls in turn.  Returns
+    dict(points (N, F) float32, each cloud's rows at the front of its slot; counts (B,) int32; n_lost (B,) int32)."""
+    import torch
+    off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+    B = off.shape[0] - 1
+    if points.dim() != 2 or points.shape[1] < 5:
+        raise ValueError('lisa_block_batch needs (N, >= 5) float32 rows (the F = 4 branch builds a float64 array)')
+    apply = np.zeros(B, dtype=bool)
+    rates = np.zeros(B)
+    seeds = np.zeros(B, dtype=np.uint64)
+    if training and 'LISA' in dataset_cfg:
+        for b in range(B):
+            apply[b], rates[b] = _lisa_draws(dataset_cfg['LISA'], rainfall_rates)
+            if apply[b]:
+                seeds[b] = lisa.draw_seed()
+    if not apply.any():
+        slot = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
+        return dict(points=points, counts=slot if counts is None else counts,
+                    n_lost=torch.zeros(B, dtype=torch.int32, device=points.device))
+    return lisa.augment_batch(points, off, rates, counts=counts, apply=apply, seeds=seeds)
+
+
 def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None, lut=None):
     """The 'CVL' branch of `DenseDataset.foggify` (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:988-1009): fog
     simulation with attenuation `alpha` (a string like '0.060' in the reference's curriculum; '0.000' = clear) and the

@@ -102,6 +102,17 @@ class LISA:
             self._tables[key] = t
         return t
 
+    @staticmethod
+    def draw_seed():
+        """The generator key of one augment call, drawn from NumPy's global generator (two randint calls)."""
+        return int(np.random.randint(0, 2 ** 31 - 1)) | (int(np.random.randint(0, 2 ** 31 - 1)) << 31)
+
+    def _draws_bound(self, Rr, r_far):
+        """Upper bound on the draws of one return: 1 + ranges + diameters + the Gaussian's rejection pairs."""
+        half = 1e-3 * (1e3 * np.tan(self.beam_divergence) * self.r_max) / 2
+        n_max = self.density(Rr, self.min_diameter) * (np.pi / 3) * max(r_far, 1.0) * (half * max(r_far, 1.0) / self.r_max) ** 2
+        return int(2 * (n_max + 2) + 128)
+
     def augment(self, pc: np.ndarray, Rr, fixed_seed: bool = False) -> np.ndarray:
         """LISA.monte_carlo_augment (lisa.py:293-341)."""
         engine = self.engine or default_engine()
@@ -116,12 +127,9 @@ class LISA:
         out = torch.empty((n, F + 2), dtype=torch.float64, device=engine.device)
         seed = 0
         if not fixed_seed:
-            seed = int(np.random.randint(0, 2 ** 31 - 1)) | (int(np.random.randint(0, 2 ** 31 - 1)) << 31)
-        # upper bound on the draws of one return: 1 + ranges + diameters + the Gaussian's rejection pairs
-        half = 1e-3 * (1e3 * np.tan(self.beam_divergence) * self.r_max) / 2
+            seed = self.draw_seed()
         r_far = float(np.sqrt((pc[:, :3] ** 2).sum(axis=1).max())) if n else 0.0
-        n_max = self.density(Rr, self.min_diameter) * (np.pi / 3) * max(r_far, 1.0) * (half * max(r_far, 1.0) / self.r_max) ** 2
-        need = int(2 * (n_max + 2) + 128)
+        need = self._draws_bound(Rr, r_far)
         while True:
             table = self._draw_table(engine, need) if fixed_seed else None
             with torch.cuda.device(engine.device):
@@ -138,3 +146,49 @@ class LISA:
                     raise
                 need *= 4                                              # the draw table was too short for some return
         return out.cpu().numpy()
+
+    def augment_batch(self, points, cloud_offsets, Rr, counts=None, apply=None, fixed_seed=False, seeds=None):
+        """The dataset's LISA block (dense_dataset.py:732-746) on a batch of device-resident clouds, one call.
+
+        points: CUDA float32 (N, F), F >= 5, intensity in [0, 255]; cloud b = rows cloud_offsets[b]:cloud_offsets[b+1]
+        (the first counts[b] of them with `counts`, a CUDA int32 (B,)); Rr: rain rate per cloud (or one for all);
+        apply: per cloud, False = copy the cloud through (the dataset's coin flip; its Rr is not used).
+        Cloud b's rows equal augment() on the dataset's float64 conversion of the cloud, then round(i * 255), the float32
+        cast and the removal of label-0 rows.  Without fixed_seed the applied clouds draw their keys in batch order with
+        augment's two np.random.randint calls (`seeds` passes keys drawn elsewhere instead, one per cloud), so each
+        sees the NumPy state a loop of augment calls would give it.  Runs on the current stream without synchronising,
+        except with fixed_seed, which checks (and grows) the draw table like augment.
+        Returns dict(points (N, F) float32: kept rows at the front of each slot; counts (B,) int32; n_lost (B,) int32)."""
+        engine = self.engine or default_engine()
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        rr = np.broadcast_to(np.asarray(Rr, dtype=np.float64), (B,))
+        ap = np.ones(B, dtype=bool) if apply is None else np.asarray(apply, dtype=bool).reshape(B)
+        alpha = np.zeros(B)
+        for b in np.flatnonzero(ap):
+            if not rr[b] > 0:
+                raise ValueError(f'bad LISA parameters: rain rate {rr[b]} of cloud {b}')
+            alpha[b] = float(self.alpha(self.Nd(self.D, float(rr[b]))))
+        mode = _MODES[self.atm_model][0]
+        kw = dict(r_min=float(self.r_min), r_max=float(self.r_max), beam_divergence=float(self.beam_divergence),
+                  min_diameter=float(self.min_diameter), range_accuracy=float(self.range_accuracy),
+                  signal_last=self.signal == 'last', counts=counts, apply=ap)
+        if not fixed_seed:
+            if seeds is None:
+                seeds = np.zeros(B, dtype=np.uint64)
+                for b in np.flatnonzero(ap):
+                    seeds[b] = self.draw_seed()
+            return engine.lisa_cloud_batch(points, off, rr, alpha, seeds, mode, **kw)
+        # the largest bound over the batch: the densest applied rain rate at the farthest return
+        r_far = float(torch.linalg.vector_norm(points[:, :3], dim=1).max()) if points.shape[0] else 0.0
+        need = max([self._draws_bound(float(rr[b]), r_far) for b in np.flatnonzero(ap)], default=1)
+        while True:
+            table = self._draw_table(engine, need)
+            out = engine.lisa_cloud_batch(points, off, rr, alpha, None, mode, draw_table=table, **kw)
+            try:
+                engine.check()
+                return out
+            except RuntimeError:
+                if need > (1 << 26):
+                    raise
+                need *= 4                                              # the draw table was too short for some return
