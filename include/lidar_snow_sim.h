@@ -287,6 +287,32 @@ LSS_API lss_status lss_fog_integral_tables(lss_engine *e, const lss_fog_table_pa
                                            double *d_out, void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_fog_integral_tables_workspace_bytes(int n, int n_tables);
 
+/* ---- Mie efficiency tables for LISA --------------------------------------------------------------------------------------
+ * The extinction and backscattering efficiencies LISA reads from mie_<n>_lambda_<wl>.npz (lib/LISA/python/lisa.py:446-465:
+ * PyMieScatt.MieQ_withDiameterRange, logD grid of 2000 diameters from 1 nm to 1 cm), generated on the device for any real
+ * refractive index and wavelength instead of the four shipped files.  Per (table, diameter), x = (pi * d_nm) / wavelength_nm:
+ *   x <= 0.05   Rayleigh: L = (m^2 - 1) / (m^2 + 2), qsca = 8 L^2 x^4 / 3, qext = qsca, qback = 1.5 qsca
+ *   x >  0.05   Bohren & Huffman series in float64 to n_stop = round(2 + x + 4 x^(1/3)) (half to even): the logarithmic
+ *               derivative D_n(m x) by downward recurrence from 0 at n_mx = round(max(n_stop, |m x|) + 16), psi_n and chi_n
+ *               by upward recurrence from sin x and cos x, qext = (2 / x^2) sum (2n + 1) Re(a_n + b_n),
+ *               qback = |sum (2n + 1) (-1)^n (a_n - b_n)|^2 / x^2
+ * PyMieScatt takes psi_n / chi_n from Bessel functions: the shipped tables agree to 2e-12 (qext) and 5e-8 (qback) relative.
+ *   h_refractive_index, h_wavelength_nm   float64[n_tables] host: table t's real refractive index m and wavelength [nm]
+ *   h_diameter_nm   float64[n_diameters] host: the diameter grid [nm] shared by every table (the npz files store
+ *                   D = d_nm * 1e-6 [mm])
+ *   d_out           float64[n_tables * n_diameters * 2] device: table t, diameter j = (qext, qback)
+ *   d_workspace     lss_mie_tables_workspace_bytes(...) bytes, which depend on the inputs (D_1 .. D_nstop of every series
+ *                   row: 40 MB for the shipped 905 nm water grid).  No allocation, no synchronisation.
+ * Invalid arguments fail with LSS_ERR_INVALID_ARG: a non-finite or non-positive m, wavelength or diameter, zero tables or
+ * diameters, or a row whose n_mx exceeds LSS_MIE_MAX_ORDER (x of about 1.9e5 at m = 1.33, e.g. a 5 cm drop at 905 nm).
+ * The workspace query returns -1 for them.                                                                             */
+#define LSS_MIE_MAX_ORDER 262144
+LSS_API lss_status lss_mie_tables(lss_engine *e, const double *h_refractive_index, const double *h_wavelength_nm,
+                                  int n_tables, const double *h_diameter_nm, int n_diameters, double *d_out,
+                                  void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_mie_tables_workspace_bytes(const double *h_refractive_index, const double *h_wavelength_nm,
+                                               int n_tables, const double *h_diameter_nm, int n_diameters);
+
 /* ---- LISA Monte-Carlo rain / snow augmenter ("next" row, SURVEY.md 8f-3) ----------------------------------------------
  * LISA.monte_carlo_augment (lib/LISA/python/lisa.py:293-341) with the per-return experiment monte_carlo_lisa (:34-190) on
  * device-resident returns; caller: DenseDataset.__getitem__ (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:713-746).

@@ -95,6 +95,8 @@ SIGNATURES = [
     ('lss_fog_batch_params_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_fog_integral_tables', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int64, _P]),
     ('lss_fog_integral_tables_workspace_bytes', _c.c_int64, [_c.c_int, _c.c_int]),
+    ('lss_mie_tables', _c.c_int, [_P, _P, _P, _c.c_int, _P, _c.c_int, _P, _P, _c.c_int64, _P]),
+    ('lss_mie_tables_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int, _P, _c.c_int]),
     ('lss_lisa_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int64, _c.c_double, _c.c_int, _c.c_double, _c.c_double, _c.c_double,
                                   _c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _c.c_int, _c.c_uint64, _P, _P]),
     ('lss_lisa_cloud_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _P, _c.c_int, _c.c_double,

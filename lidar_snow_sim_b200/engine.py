@@ -442,6 +442,30 @@ class SnowfallEngine:
         _lib.check(st, self.h)
         return out
 
+    def mie_tables(self, refractive_indices, wavelengths_nm, diameters_nm=None):
+        """
+        LISA's Mie efficiency tables generated on the device (lss_mie_tables, current stream, no synchronisation): for
+        each (real refractive index, wavelength [nm]) pair, (qext, qback) at every diameter of `diameters_nm` [nm], as
+        PyMieScatt.MieQ_withDiameterRange computes them for lisa.py:446-465.  diameters_nm defaults to its logD grid of
+        2000 diameters from 1 nm to 1 cm.  Returns a CUDA float64 tensor (T, n_diameters, 2).
+        """
+        m = np.ascontiguousarray(np.atleast_1d(np.asarray(refractive_indices, dtype=np.float64)))
+        wl = np.ascontiguousarray(np.atleast_1d(np.asarray(wavelengths_nm, dtype=np.float64)))
+        if m.ndim != 1 or m.shape != wl.shape:
+            raise ValueError('need one wavelength per refractive index')
+        if diameters_nm is None:
+            diameters_nm = np.logspace(0, 7, 2000)
+        d = np.ascontiguousarray(np.asarray(diameters_nm, dtype=np.float64).reshape(-1))
+        T, nd = int(m.shape[0]), int(d.shape[0])
+        need = int(self.lib.lss_mie_tables_workspace_bytes(_ptr(m), _ptr(wl), T, _ptr(d), nd))
+        with torch.cuda.device(self.device):
+            out = torch.empty((T, nd, 2), dtype=torch.float64, device=self.device)
+            ws = torch.empty(max(need, 0) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_mie_tables(self.h, _ptr(m), _ptr(wl), T, _ptr(d), nd, _ptr(out), _ptr(ws), int(ws.numel()),
+                                         self._stream())
+        _lib.check(st, self.h)
+        return out
+
     def voxelize_batch(self, points, cloud_offsets, point_cloud_range, voxel_size, max_points_per_voxel, max_voxels,
                        counts=None, mask_xy_range=True):
         """

@@ -1,1 +1,1 @@
-from .simulation import LISA  # noqa: F401
+from .simulation import LISA, generate_mie_tables, mie_table  # noqa: F401

@@ -9,8 +9,10 @@ DenseDataset.__getitem__, lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:71
 
 Same constructor arguments and defaults, same `augment(pc, Rr, fixed_seed=False)` call and return layout.  The
 extinction coefficient alpha(Rr) is integrated on the host from the tabulated Mie efficiencies exactly like LISA.alpha
-(:468-482); the table is the reference's data file `mie_<refractive index>_λ_<wavelength>.npz` (arrays D, qext; pass its
-path / directory as `mie_table`, or the arrays themselves) -- generating it needs PyMieScatt and is offline tooling.
+(:468-482).  By default the table is the reference's data file `mie_<refractive index>_λ_<wavelength>.npz` (arrays D,
+qext; pass its path / directory as `mie_table`, or the arrays themselves).  `mie_table='device'` generates it on the GPU
+instead (`mie_table()`, the PyMieScatt computation of lisa.py:446-465), for any wavelength; `generate_mie_tables()`
+writes such tables as files the reference's LISA loads too.
 
 Randomness: with `fixed_seed=True` (every return re-seeds NumPy's generator with 666, lisa.py:54-55) the device replays
 NumPy's own draw sequence and reproduces the reference up to libm rounding.  Without it the reference is not
@@ -20,6 +22,7 @@ generator seeded from NumPy's global state (so np.random.seed() still controls i
 The fog / haze / spray modes of the reference (`average_augment`, `goodin_augment`) are not part of this path.
 """
 import os
+import weakref
 from pathlib import Path
 
 import numpy as np
@@ -30,6 +33,44 @@ from ..engine import default_engine, _ptr
 
 _MODES = {'rain': (0, 1.328), 'gunn': (1, 1.3031), 'sekhon': (2, 1.3031)}
 _SEED = 666                                         # lisa.py:55
+_DEVICE_MIE = weakref.WeakKeyDictionary()           # engine -> {(m, wavelength, nd, diameter_range): (D, qext, qback)}
+
+
+def _device_table(engine, refractive_index, wavelength, nd=2000, diameter_range=(1, 1e7)):
+    """(D, qext, qback) of one table, generated once per engine and arguments (the cached arrays: do not modify)."""
+    engine = engine or default_engine()
+    key = (float(refractive_index), float(wavelength), int(nd), tuple(float(v) for v in diameter_range))
+    cache = _DEVICE_MIE.setdefault(engine, {})
+    if key not in cache:
+        d = np.logspace(np.log10(diameter_range[0]), np.log10(diameter_range[1]), int(nd))
+        q = engine.mie_tables([key[0]], [key[1]], d)[0].cpu().numpy()
+        cache[key] = (d * 1e-6, np.ascontiguousarray(q[:, 0]), np.ascontiguousarray(q[:, 1]))
+    return cache[key]
+
+
+def mie_table(refractive_index, wavelength, nd=2000, diameter_range=(1, 1e7), engine=None):
+    """The Mie efficiency table LISA.calc_Mie_params computes with PyMieScatt (lisa.py:446-465), generated on the device:
+    (D [mm], qext, qback) as float64 NumPy arrays over nd log-spaced diameters d_nm in diameter_range [nm], with
+    D = d_nm * 1e-6.  wavelength in nm; refractive_index real.  Cached per engine and arguments."""
+    return tuple(a.copy() for a in _device_table(engine, refractive_index, wavelength, nd, diameter_range))
+
+
+def generate_mie_tables(pairs, save_path, engine=None):
+    """Write the table of each (refractive_index, wavelength) pair as save_path/mie_<refractive_index>_λ_<wavelength>.npz
+    with the keys D, qext, qback: the file name and format lisa.py:463 writes, which both LISA here and the reference's
+    LISA load.  The values are formatted as given (905, not 905.0, for the reference's default).  Returns the paths."""
+    engine = engine or default_engine()
+    save_path = Path(save_path)
+    save_path.mkdir(parents=True, exist_ok=True)
+    pairs = list(pairs)
+    d = np.logspace(0, 7, 2000)
+    q = engine.mie_tables([float(m) for m, _ in pairs], [float(w) for _, w in pairs], d).cpu().numpy()
+    paths = []
+    for (m, w), t in zip(pairs, q):
+        path = save_path / f'mie_{m}_λ_{w}.npz'
+        np.savez(str(path), D=d * 1e-6, qext=t[:, 0], qback=t[:, 1])
+        paths.append(path)
+    return paths
 
 
 def _size_law(mode, Rr):
@@ -59,6 +100,9 @@ class LISA:
         self._tables = {}
 
     def _load_mie(self, mie_table):
+        if isinstance(mie_table, str) and mie_table == 'device':
+            D, qext, _ = _device_table(self.engine, self.refractive_index, self.wavelength)
+            return D.copy(), qext.copy()
         if isinstance(mie_table, (tuple, list)):
             return np.asarray(mie_table[0], dtype=np.float64), np.asarray(mie_table[1], dtype=np.float64)
         name = f'mie_{self.refractive_index}_λ_{self.wavelength}.npz'
@@ -72,8 +116,9 @@ class LISA:
             if c.is_file():
                 dat = np.load(str(c))
                 return np.asarray(dat['D'], dtype=np.float64), np.asarray(dat['qext'], dtype=np.float64)
-        raise FileNotFoundError(f"Mie coefficient table '{name}' not found (pass mie_table=<path | directory | (D, qext)> or "
-                                f"set LSS_LISA_MIE_DIR; the reference ships it in lib/LISA/python/)")
+        raise FileNotFoundError(f"Mie coefficient table '{name}' not found (pass mie_table=<path | directory | (D, qext)>, "
+                                f"set LSS_LISA_MIE_DIR, or generate it with mie_table='device'; the reference ships "
+                                f"it in lib/LISA/python/)")
 
     # ---- the reference's helpers the callers use (pointcloud_viewer.py:2794-2796) ------------------------------------
     def Nd(self, D, Rr):
