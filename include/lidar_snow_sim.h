@@ -426,6 +426,58 @@ LSS_API lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_fe
                                   void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_dror_workspace_bytes(int64_t n_total, int n_clouds);
 
+/* ---- row selection between fog and LISA: STRONGEST_LAST_FILTER and FOV_POINTS_ONLY ----------------------------------
+ * The two keys of DenseDataset.__getitem__ (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:677-711) on batches of
+ * device-resident clouds.  Both keep whole rows (every column), stably, at the front of each output slot.
+ *
+ * lss_strongest_last_batch: compare_points (dense_dataset.py:519-562) cloud by cloud, then pc_master[mask].  With n_l,
+ * n_s the valid rows of cloud b's last and strongest echo clouds: master = strongest if n_s > n_l, else last (ties
+ * too); slave = the other, len_s its rows, diff = |n_s - n_l|.  Master row i is kept iff
+ *     i < len_s and an exactly equal slave row (float32 x, y, z; -0 == +0, NaN equals nothing) lies in
+ *     [max(0, i - diff), i], or, when i - diff < 0, in [max(0, len_s + i - diff), len_s - 1]
+ *     (the reference's j loop with Python's negative indices, ended by its IndexError), and
+ *     sqrtf((x*x + y*y) + z*z) > (float)min_dist in float32 (np.linalg.norm against the Python float).
+ * The cost per row does not depend on diff (a sort of the slave rows by a hash of their xyz, then a binary search).
+ *   d_last, d_strongest   float32[rows * n_features], n_features >= 3, the same for both; cloud b of each starts at row
+ *                   h_*_offsets[b] (int64[n_clouds + 1], host); d_*_counts int32[n_clouds] device or NULL: valid rows per slot
+ *   min_dist        the reference's 3.0 by default (not NaN)
+ *   output slots    cloud b's slot has max(slot of b in d_last, slot of b in d_strongest) rows; slots are consecutive
+ *   d_out_points    float32[sum of the output slots * n_features]: cloud b's kept master rows in order at the front of
+ *                   its slot, rows behind them unspecified.  Must not alias d_last or d_strongest.
+ *   d_out_counts    int32[n_clouds] kept rows;  d_out_master_is_strongest  uint8[n_clouds] 1 if the master is strongest
+ *   d_out_mask      uint8[sum of the output slots] or NULL: compare_points' mask, 1 / 0 for the first n_master rows of
+ *                   each slot (n_master = max(n_l, n_s)), rows behind them untouched
+ *   d_workspace     lss_strongest_last_batch_workspace_bytes(h_last_offsets, h_strongest_offsets, n_clouds) bytes; that
+ *                   query needs a CUDA device (radix sort scratch) and returns -1 without one or for bad offsets
+ * Exact: comparisons and integer counts only.  3 staging copies and 6 launches (the sort counted as one); no
+ * allocation, no synchronisation.                                                                                        */
+LSS_API lss_status lss_strongest_last_batch(lss_engine *e, const float *d_last, const int64_t *h_last_offsets,
+                                            const int32_t *d_last_counts, const float *d_strongest,
+                                            const int64_t *h_strongest_offsets, const int32_t *d_strongest_counts,
+                                            int n_features, int n_clouds, double min_dist, float *d_out_points,
+                                            int32_t *d_out_counts, uint8_t *d_out_master_is_strongest,
+                                            uint8_t *d_out_mask, void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_strongest_last_batch_workspace_bytes(const int64_t *h_last_offsets, const int64_t *h_strongest_offsets,
+                                                         int n_clouds);
+/* lss_camera_fov_batch: FOV_POINTS_ONLY, pts_rect = calib.lidar_to_rect(points[:, 0:3]) then get_fov_flag(pts_rect,
+ * img_shape, calib) (dense_dataset.py:36-44,689-711), with the camera of lss_set_camera: float32, u = img[0] / rect_z and
+ * v = img[1] / rect_z in [0, img_w) x [0, img_h), depth >= 0.  The projection is the one lss_snowfall_batch's
+ * LSS_FLAG_CAMERA_FOV uses, so both filters keep the same rows.  A cloud with no row left gets count 0 (the dataset then
+ * draws another sample; that is the caller's).
+ *   d_points        float32[n_total * n_features], n_features >= 3; h_cloud_offsets int64[n_clouds + 1] host;
+ *                   d_cloud_counts int32[n_clouds] device or NULL: valid rows per slot
+ *   h_img_shape     int32[n_clouds * 2] host (img_h, img_w) per cloud, the sample's info['image']['image_shape'], or
+ *                   NULL: the shape given to lss_set_camera
+ *   d_out_points    float32[n_total * n_features]: kept rows in order at the front of each slot.  Must not alias d_points.
+ *   d_out_counts    int32[n_clouds];  d_out_mask  uint8[n_total] or NULL: the flag of every valid row
+ *   d_workspace     lss_camera_fov_batch_workspace_bytes(n_total, n_clouds) bytes
+ * LSS_ERR_NO_SENSOR without a camera.  3 staging copies and 3 kernels; no allocation, no synchronisation.              */
+LSS_API lss_status lss_camera_fov_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                        const int32_t *d_cloud_counts, int n_clouds, const int32_t *h_img_shape,
+                                        float *d_out_points, int32_t *d_out_counts, uint8_t *d_out_mask,
+                                        void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_camera_fov_batch_workspace_bytes(int64_t n_total, int n_clouds);
+
 /* ---- exchange step of the sharded batch (SURVEY.md 8e, BASELINE.json configs[3]) ------------------------------------------
  * The reference has no multi-GPU augmentation; its collectives are OpenPCDet's result merging
  * (lib/OpenPCDet/pcdet/utils/commu_utils.py:77,90: all_gather of pickled, variable-size objects).  The sharded engine

@@ -109,6 +109,11 @@ SIGNATURES = [
     ('lss_dror_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_int, _c.c_double,
                                   _c.c_uint32, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_dror_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_strongest_last_batch', _c.c_int, [_P, _P, _P, _P, _P, _P, _P, _c.c_int, _c.c_int, _c.c_double, _P, _P, _P, _P,
+                                            _P, _c.c_int64, _P]),
+    ('lss_strongest_last_batch_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int]),
+    ('lss_camera_fov_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_camera_fov_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_gather_push', _c.c_int, [_P, _P, _P, _P, _c.c_int, _c.c_int64, _c.c_int, _c.c_int, _P, _P, _P, _P, _c.c_int, _P]),
     ('lss_dart_throwing', _c.c_int, [_c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _P, _c.c_int64,
                                      _c.POINTER(_c.c_int64)]),

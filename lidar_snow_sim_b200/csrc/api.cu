@@ -338,7 +338,8 @@ lss_status lss_set_profiling(lss_engine *e, int enable)
 }
 
 static const char *kernel_names[LSS_K_COUNT] = {"channel_sort", "prepass", "snowfall", "compact", "keep", "wet_ground", "fog",
-                                                "snowfall_scan", "snowfall_solve", "voxelize", "dror", "lisa", "fog_lut", "mie"};
+                                                "snowfall_scan", "snowfall_solve", "voxelize", "dror", "lisa", "fog_lut", "mie",
+                                                "select"};
 
 const char *lss_kernel_name(int kernel) { return (kernel >= 0 && kernel < LSS_K_COUNT) ? kernel_names[kernel] : ""; }
 

@@ -78,6 +78,26 @@ struct CameraConst {
     int img_h, img_w;
 };
 
+// Camera field-of-view test of one lidar point: calib.lidar_to_rect then get_fov_flag (calibration_kitti.py:65-84,
+// dense_dataset.py:36-44), float32 with the BLAS dot products' fused multiply-adds in their order.  The one definition
+// of the projection: k_keep (snowfall.cu) and k_fov (select.cu) both call it, so the two filters agree row for row.
+// The image shape is read through pointers, only when the bounds test gets to it.
+__device__ __forceinline__ bool lss_camera_fov(const CameraConst *cam, float out_x, float out_y, float out_z,
+                                               const int *img_h, const int *img_w)
+{
+    const float *M = cam->M, *P2 = cam->P2;
+    float rx = fmaf(out_z, M[6], fmaf(out_y, M[3], out_x * M[0])) + M[9];
+    float ry = fmaf(out_z, M[7], fmaf(out_y, M[4], out_x * M[1])) + M[10];
+    float rz = fmaf(out_z, M[8], fmaf(out_y, M[5], out_x * M[2])) + M[11];
+    float u = fmaf(rz, P2[2], fmaf(ry, P2[1], rx * P2[0])) + P2[3];
+    float v = fmaf(rz, P2[6], fmaf(ry, P2[5], rx * P2[4])) + P2[7];
+    float wd = fmaf(rz, P2[10], fmaf(ry, P2[9], rx * P2[8])) + P2[11];
+    u = u / rz;
+    v = v / rz;
+    const float depth = wd - P2[11];
+    return (u >= 0.0f) && (u < (float)*img_w) && (v >= 0.0f) && (v < (float)*img_h) && (depth >= 0.0f);
+}
+
 struct lss_host_pipe;
 struct lss_engine {
     int device = 0;
@@ -211,7 +231,7 @@ inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStrea
 
 enum { LSS_K_SORT = 0, LSS_K_PREPASS = 1, LSS_K_SNOWFALL = 2, LSS_K_COMPACT = 3, LSS_K_FINALIZE = 4, LSS_K_WET = 5,
        LSS_K_FOG = 6, LSS_K_SCAN = 7, LSS_K_SOLVE = 8, LSS_K_VOXEL = 9, LSS_K_DROR = 10, LSS_K_LISA = 11,
-       LSS_K_FOG_LUT = 12, LSS_K_MIE = 13, LSS_K_COUNT = 14 };   // 7, 8: inside the LSS_K_SNOWFALL bracket
+       LSS_K_FOG_LUT = 12, LSS_K_MIE = 13, LSS_K_SELECT = 14, LSS_K_COUNT = 15 };   // 7, 8: inside the LSS_K_SNOWFALL bracket
 
 struct KernelTimer {        // RAII: records begin/end events around the launches of its scope when profiling is on
     lss_engine *e; cudaStream_t s; int idx = -1;

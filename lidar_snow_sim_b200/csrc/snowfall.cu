@@ -169,19 +169,7 @@ __global__ void __launch_bounds__(KEEP_TPB) k_keep(DevArgs a)
             att = keep && label == 1 && ch < LSS_N_CHANNELS;  // num_attenuated is counted BEFORE the FOV filter (:525)
             if (keep && (a.flags & LSS_FLAG_CAMERA_FOV)) {
                 const float *row = a.aug + (beg + i) * 5;
-                const float out_x = row[0], out_y = row[1], out_z = row[2];
-                const float *M = a.camera->M, *P2 = a.camera->P2;
-                float rx = fmaf(out_z, M[6], fmaf(out_y, M[3], out_x * M[0])) + M[9];
-                float ry = fmaf(out_z, M[7], fmaf(out_y, M[4], out_x * M[1])) + M[10];
-                float rz = fmaf(out_z, M[8], fmaf(out_y, M[5], out_x * M[2])) + M[11];
-                float u = fmaf(rz, P2[2], fmaf(ry, P2[1], rx * P2[0])) + P2[3];
-                float v = fmaf(rz, P2[6], fmaf(ry, P2[5], rx * P2[4])) + P2[7];
-                float wd = fmaf(rz, P2[10], fmaf(ry, P2[9], rx * P2[8])) + P2[11];
-                u = u / rz;
-                v = v / rz;
-                const float depth = wd - P2[11];
-                keep = (u >= 0.0f) && (u < (float)a.camera->img_w) && (v >= 0.0f) && (v < (float)a.camera->img_h) &&
-                       (depth >= 0.0f);
+                keep = lss_camera_fov(a.camera, row[0], row[1], row[2], &a.camera->img_h, &a.camera->img_w);
             }
             a.code_keep[beg + i] = keep ? (uint8_t)ch : (uint8_t)255;
             if (a.code_all) a.code_all[beg + i] = (uint8_t)ch;

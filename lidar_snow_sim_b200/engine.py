@@ -541,6 +541,85 @@ class SnowfallEngine:
                 out['work'] = self._ws_dror[:32].view(torch.int64).clone()
         return out
 
+    def strongest_last_batch(self, last, last_offsets, strongest, strongest_offsets, min_dist=3.0, last_counts=None,
+                             strongest_counts=None, want_mask=False):
+        """
+        The dataset's STRONGEST_LAST_FILTER (compare_points, dense_dataset.py:519-562, then pc_master[mask]) on a batch
+        of device-resident echo pairs (lss_strongest_last_batch, current stream, no synchronisation).  last / strongest:
+        CUDA float32 (N_l, F) / (N_s, F), F >= 3, cloud b at rows *_offsets[b]:*_offsets[b+1] (the first *_counts[b] with
+        counts).  Cloud b's output slot has max(slot_l, slot_s) rows.  Returns dict(points (N_out, F) float32, each
+        cloud's kept master rows at the front of its slot; offsets int64 host array (B + 1) of those slots; counts (B,)
+        int32; master_is_strongest (B,) uint8 [, mask (N_out,) uint8: compare_points' mask on each slot's master rows]).
+        """
+        off_l = np.ascontiguousarray(last_offsets, dtype=np.int64)
+        off_s = np.ascontiguousarray(strongest_offsets, dtype=np.int64)
+        B = off_l.shape[0] - 1
+        if off_s.shape != off_l.shape:
+            raise ValueError('last and strongest need the same number of clouds')
+        for pts, off in ((last, off_l), (strongest, off_s)):
+            if off[0] != 0 or (np.diff(off) < 0).any():              # (the workspace query cannot say why it fails)
+                raise ValueError('cloud_offsets must start at 0 and be non-decreasing')
+            assert pts.is_cuda and pts.dtype == torch.float32 and pts.is_contiguous() and pts.dim() == 2
+            assert pts.shape[0] == int(off[-1])
+        if last.shape[1] != strongest.shape[1]:
+            raise ValueError('last and strongest need the same number of columns')
+        F = int(last.shape[1])
+        for c in (last_counts, strongest_counts):
+            if c is not None:
+                assert c.is_cuda and c.dtype == torch.int32 and c.shape == (B,)
+        off_o = np.concatenate([[0], np.cumsum(np.maximum(np.diff(off_l), np.diff(off_s)))]).astype(np.int64)
+        N = int(off_o[-1])
+        with torch.cuda.device(self.device):
+            out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device), offsets=off_o,
+                       counts=torch.empty((B,), dtype=torch.int32, device=self.device),
+                       master_is_strongest=torch.empty((B,), dtype=torch.uint8, device=self.device))
+            if want_mask:
+                out['mask'] = torch.zeros((N,), dtype=torch.uint8, device=self.device)
+            need = self.lib.lss_strongest_last_batch_workspace_bytes(_ptr(off_l), _ptr(off_s), B)
+            if need < 0:
+                raise RuntimeError('lss_strongest_last_batch_workspace_bytes failed (bad offsets or no CUDA device?)')
+            if getattr(self, '_ws_sel', None) is None or self._ws_sel.numel() < need:
+                self._ws_sel = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_strongest_last_batch(
+                self.h, _ptr(last), _ptr(off_l), _ptr(last_counts), _ptr(strongest), _ptr(off_s), _ptr(strongest_counts),
+                F, B, float(min_dist), _ptr(out['points']), _ptr(out['counts']), _ptr(out['master_is_strongest']),
+                _ptr(out.get('mask')), _ptr(self._ws_sel), int(self._ws_sel.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out
+
+    def camera_fov_batch(self, points, cloud_offsets, counts=None, img_shapes=None, want_mask=False):
+        """
+        The dataset's FOV_POINTS_ONLY (calib.lidar_to_rect + get_fov_flag, dense_dataset.py:36-44,689-711) on a batch of
+        device-resident clouds with this engine's camera (set_camera; lss_camera_fov_batch, current stream, no
+        synchronisation).  points: CUDA float32 (N, F), F >= 3; counts: optional CUDA int32 (B,) valid rows per slot;
+        img_shapes: optional (B, 2) host (img_h, img_w) per cloud, default the camera's.  Returns dict(points (N, F)
+        float32, each cloud's rows inside the image at the front of its slot; counts (B,) int32 -- 0 where the dataset
+        would draw another sample [, mask (N,) uint8 flag of every valid row]).
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        N = int(off[-1])
+        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
+        assert points.dim() == 2
+        F = int(points.shape[1])
+        if counts is not None:
+            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        shp = None if img_shapes is None else np.ascontiguousarray(
+            np.broadcast_to(np.asarray(img_shapes, dtype=np.int32).reshape(-1, 2), (B, 2)))
+        with torch.cuda.device(self.device):
+            out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device),
+                       counts=torch.empty((B,), dtype=torch.int32, device=self.device))
+            if want_mask:
+                out['mask'] = torch.zeros((N,), dtype=torch.uint8, device=self.device)
+            need = self.lib.lss_camera_fov_batch_workspace_bytes(N, B)
+            if getattr(self, '_ws_fov', None) is None or self._ws_fov.numel() < need:
+                self._ws_fov = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_camera_fov_batch(self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, _ptr(shp),
+                                               _ptr(out['points']), _ptr(out['counts']), _ptr(out.get('mask')),
+                                               _ptr(self._ws_fov), int(self._ws_fov.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out
+
     def lisa_cloud_batch(self, points, cloud_offsets, rain_rate, alpha, seed, mode, r_min=0.9, r_max=120.0,
                          beam_divergence=3e-3, min_diameter=0.05, range_accuracy=0.09, signal_last=False, counts=None,
                          apply=None, draw_table=None):

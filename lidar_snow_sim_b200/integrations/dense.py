@@ -238,3 +238,61 @@ def dror_filter(points, dataset_cfg, split, engine=None):
         keep_indices[snow] = False
         points = points[keep_indices]
     return points
+
+
+def compare_points(path_last, path_strongest, min_dist=3., engine=None):
+    """`DenseDataset.compare_points` (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:519-562) with the reference's
+    signature and return value, computed by the engine (lss_strongest_last_batch): reads the two float32 (N, 5) .bin
+    files and returns (pc_master, mask, num_last, num_strongest, diff), pc_master the longer cloud (the last one on a
+    tie) and mask a bool array, so `pc_master[mask]` is the dataset's STRONGEST_LAST_FILTER."""
+    import torch
+    engine = engine or default_engine()
+    pc_l = np.fromfile(path_last, dtype=np.float32).reshape((-1, 5))
+    pc_s = np.fromfile(path_strongest, dtype=np.float32).reshape((-1, 5))
+    num_last, num_strongest = len(pc_l), len(pc_s)
+    pc_master = pc_s if num_strongest > num_last else pc_l
+    res = engine.strongest_last_batch(torch.from_numpy(pc_l).to(engine.device), np.array([0, num_last]),
+                                      torch.from_numpy(pc_s).to(engine.device), np.array([0, num_strongest]),
+                                      min_dist=min_dist, want_mask=True)
+    mask = res['mask'][:len(pc_master)].cpu().numpy().astype(bool)
+    return pc_master, mask, num_last, num_strongest, abs(num_strongest - num_last)
+
+
+def point_selection_batch(points, cloud_offsets, dataset_cfg, img_shapes=None, last=None, counts=None, sensor=None,
+                          engine=None):
+    """The STRONGEST_LAST_FILTER and FOV_POINTS_ONLY keys of `DenseDataset.__getitem__` (dense_dataset.py:677-711), in
+    that order, on a batch of device-resident clouds: points CUDA float32 (N, F), F >= 3, cloud b at rows
+    cloud_offsets[b]:cloud_offsets[b+1] (the first counts[b] with `counts`).
+      STRONGEST_LAST_FILTER   `points` are the strongest-echo clouds and `last` = (points, offsets[, counts]) the
+                              last-echo clouds of the same samples; each sample becomes pc_master[mask] of compare_points.
+                              As in the reference, the key excludes FOG_AUGMENTATION.
+      FOV_POINTS_ONLY         the rows inside the camera image, img_shapes (B, 2) (h, w) per sample (info['image']
+                              ['image_shape']) or None for the camera's; sensor 'hdl64' / 'vlp32' first sets the engine's
+                              camera to that calibration (get_calib(sensor_type)), None keeps the engine's camera.  A
+                              sample with no row left gets count 0: drawing another index is the caller's, as in the
+                              dataset.
+    Returns dict(points, offsets (B + 1) int64 host array of the result's slots, counts (B,) int32 CUDA tensor)."""
+    off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+    if dataset_cfg.get('STRONGEST_LAST_FILTER', False) or dataset_cfg.get('FOV_POINTS_ONLY', False):
+        engine = engine or default_engine()
+    res = dict(points=points, offsets=off, counts=counts)
+    if dataset_cfg.get('STRONGEST_LAST_FILTER', False):
+        assert not dataset_cfg.get('FOG_AUGMENTATION', False), \
+            'strongest == last filter is mutually exlusive with fog augmentation'
+        if last is None:
+            raise ValueError('STRONGEST_LAST_FILTER needs the last-echo clouds (last=(points, offsets[, counts]))')
+        last_points, last_offsets = last[0], last[1]
+        last_counts = last[2] if len(last) > 2 else None
+        r = engine.strongest_last_batch(last_points, last_offsets, points, off, last_counts=last_counts,
+                                        strongest_counts=counts)
+        res = dict(points=r['points'], offsets=r['offsets'], counts=r['counts'])
+    if dataset_cfg.get('FOV_POINTS_ONLY', False):
+        if sensor is not None:
+            from ..calib.dense_camera import DENSE_CAMERAS
+            engine.set_camera(DENSE_CAMERAS[sensor])
+        r = engine.camera_fov_batch(res['points'], res['offsets'], counts=res['counts'], img_shapes=img_shapes)
+        res = dict(points=r['points'], offsets=res['offsets'], counts=r['counts'])
+    if res['counts'] is None:
+        import torch
+        res['counts'] = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
+    return res
