@@ -4,13 +4,13 @@
 #include "common.cuh"
 
 // One beam of the solve list, written by the scan kernel (32 bytes).  The scan has already walked the beam's whole
-// bucket prefix and tested every candidate exactly, so it hands over WHICH particles hit (their indices, in prefix
-// order, in the hit array), the azimuth it used and the beam's point and channel: the solve kernel never reads the
-// input row.
+// bucket prefix and tested every candidate exactly, so it hands over its hits as the solve claims them (the hit
+// records, in prefix order, in the hit arrays), the azimuth it used and the beam's point and channel: the solve kernel
+// never reads the input row, a particle record or a tangent.
 struct __align__(16) SolveItem {
     unsigned long long key;       // channel << 56 | work class << 48 | cloud << 32 | row
-    int hit_off;                  // first of the beam's L entries of hit_idx[]; -1: the hit array was full, the solve
-                                  // kernel walks the bucket prefix again
+    int hit_off;                  // first of the beam's L slots of hit_a1[] / hit_a2[] / hit_rho[]; -1: the hit arrays
+                                  // were full, the solve kernel walks the bucket prefix again
     int L;                        // occluders
     float th32;                   // beam azimuth in [0, 2 pi) as the scan used it
     float px, py, pz;             // the input point
@@ -65,8 +65,12 @@ struct DevArgs {
     SolveItem *items;
     int *chunk_tab;
     int chunks_per_class;
-    int *hdr;                    // [0] chunks allocated, [1] tile cursor, [2] hit positions used, class counts
-    int *hit_idx;                // particle indices of the hits of the listed beams
+    int *hdr;                    // [0] chunks allocated, [1] tile cursor, [2] hit slots allocated, class counts
+    // hit records of the listed beams, structure of arrays, hit_cap slots each: what the solve's claiming starts from,
+    // a1 = right limit if the disk crosses it, else t_right; a2 = left limit if crossed, else t_left; the planar range
+    double *hit_a1;
+    double *hit_a2;
+    double *hit_rho;
     int hit_cap;
     // plane-major schedule of the scan kernel: warp tile s of the launch is (cloud, first row) = sched[s] (cloud << 32 | row;
     // bits 48.. hold the sort key), warp tiles of the whole batch sorted by plane
@@ -80,7 +84,7 @@ constexpr int SNOW_TPB = 128;
 constexpr int SNOW_WARPS = SNOW_TPB / 32;
 constexpr int TILE = 1024;                          // rows per scatter tile
 constexpr int NBINS = LSS_N_CHANNELS + 1;           // + "not a valid channel" (sorted last)
-constexpr int LIST_HDR_BYTES = 1024;  // ints: [0] chunks allocated, [1] tile cursor, [2] hit positions, [C..2C) class counts
+constexpr int LIST_HDR_BYTES = 1024;  // ints: [0] chunks allocated, [1] tile cursor, [2] hit slots, [C..2C) class counts
 constexpr int LIST_CLASSES = 128;     // solve list bucketed by work class (occluder count), costliest class first
 constexpr int LIST_CHUNK = 1024;      // solve items per chunk of a class (a multiple of 32: a solve tile is in one chunk)
 // scan schedule: warp tiles counting-sorted by the plane (mod SCHED_PLANES) of their first row's channel; rows without a

@@ -61,7 +61,9 @@ __global__ void __launch_bounds__(SCHED_KEY_TPB) k_sched_key(const float *__rest
 // counting sort of the schedule entries by bin (k_sched_key's histogram, then the bin cursors in hist[SCHED_BINS ..]):
 // block-local ranks in shared memory, one global cursor update per bin and block.  Order inside a bin is arbitrary.
 // ---------------------------------------------------------------------------------------------------------------------
-constexpr int HIT_POS_PER_BEAM = 6;                 // capacity of the hit-position array per beam of the batch
+// hit slots per beam of the batch (one per survivor of the scan's broad phase; 24 B each).  Measured on 32 synthetic
+// 64 x 2048 clouds: 0.72 per beam at 2.5 mm/h (the bench), 2.19 at 10 mm/h and 0.2 m/s (the densest of tools/sweep.py)
+constexpr int HIT_SLOTS_PER_BEAM = 3;
 constexpr int SCHED_PER_THREAD = 2;
 __global__ void __launch_bounds__(256) k_sched_sort(const unsigned long long *__restrict__ in, unsigned long long *out,
                                                     int *hist, int n)
@@ -328,6 +330,8 @@ struct WsLayout {
         order, thresh, counters, counters_bytes, list, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
 };
 
+int64_t hit_cap(int64_t n_total) { return std::min<int64_t>(n_total * HIT_SLOTS_PER_BEAM + 4096, 0x7fffffff); }
+
 WsLayout ws_layout(int64_t n_total, int n_clouds)
 {
     WsLayout w;
@@ -351,12 +355,11 @@ WsLayout ws_layout(int64_t n_total, int n_clouds)
     w.counters_bytes = align_up((int64_t)n_clouds * 2 * 4, 8) + (int64_t)n_clouds * LSS_N_CHANNELS * 4 + (int64_t)n_clouds * 8;
     w.counters = o;   o = align_up(o + w.counters_bytes, 256);
     // list header | solve list chunks (every beam may have occluders; each class leaves at most one chunk partly filled)
-    //   | hit particle indices (int32; HIT_POS_PER_BEAM per beam of the batch on average: the surveyed densities give 1-5 occluders
-    //   on a third of the beams)
+    //   | hit records a1 | a2 | range (float64 each, HIT_SLOTS_PER_BEAM slots per beam of the batch + 4096)
     w.chunks_per_class = (n_total + LIST_CHUNK - 1) / LIST_CHUNK;
     w.list = o;       o = align_up(o + LIST_HDR_BYTES +
                                    (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK * (int64_t)sizeof(SolveItem) +
-                                   (n_total * HIT_POS_PER_BEAM + 4096) * 4, 256);
+                                   hit_cap(n_total) * 3 * 8, 256);
     // chunk table of the solve list: LIST_CLASSES x chunks_per_class ids
     w.chunk_tab = o;  o = align_up(o + (int64_t)LIST_CLASSES * w.chunks_per_class * 4, 256);
     // scan schedule: bin counts and cursors | warp-tile entries, unsorted + sorted
@@ -479,7 +482,10 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.att_sum = d_att_sum;
     a.status = e->d_status;
     SolveItem *d_solve_list = (SolveItem *)(ws + w.list + LIST_HDR_BYTES);   // (chunks_per_class + LIST_CLASSES) chunks
-    a.hit_idx = (int *)(d_solve_list + (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK);
+    a.hit_cap = (int)hit_cap(N);
+    a.hit_a1 = (double *)(d_solve_list + (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK);
+    a.hit_a2 = a.hit_a1 + a.hit_cap;
+    a.hit_rho = a.hit_a2 + a.hit_cap;
     // Device pre-pass: plane + laser parameters + threshold polynomial (simulation.py:449-467), on the cloud as given.
     // Only k_keep needs its result, so it runs on one of the engine's high-priority side streams next to the beam kernels (a
     // chain of small latency-bound kernels).  It is forked before the scan, whose CTAs retire continuously: the persistent
@@ -506,7 +512,6 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             return ps != LSS_OK ? ps : lss_fail(e, LSS_ERR_CUDA, "event record failed");
         }
     }
-    a.hit_cap = (int)std::min<int64_t>(N * HIT_POS_PER_BEAM + 4096, 0x7fffffff);
     cudaError_t ce;                                 // (checked after the join: never leave the side stream dangling)
     {
         KernelTimer kt(e, LSS_K_SNOWFALL, stream);

@@ -4,8 +4,8 @@
 //            of snowfall.cu, k_sched_key), rows read and written at their input positions: float32 range / azimuth, walk of the
 //            beam's azimuth bucket of its channel's snowflake plane (float32 broad phase, exact float64 disk / wedge test)
 //            over the WHOLE prefix of entries nearer than the target.  Beams without occluder (~2/3) are finished here;
-//            the others are pushed to the solve list together with what the walk found: the particle indices of the
-//            hits (in prefix order) and the azimuth.                         (tools/snowfall/simulation.py:80-101, 329-390)
+//            the others are pushed to the solve list together with what the walk found: the hit records (a1, a2, range
+//            of each hit, in prefix order) and the azimuth.                  (tools/snowfall/simulation.py:80-101, 329-390)
 //   k_solve  the listed beams, class by class: tangent angles of the hits, nearest-first claiming of the beam's
 //            angular sub-intervals, summed sin^2 waveform + argmax, relabel / move the point, label-1 statistics.
 //                                                                              (simulation.py:118-188, 231-295, 391-424)
@@ -18,9 +18,9 @@
 //   * NO local memory: the beams of a warp share a shared-memory arena of ARENA slots, allocated exactly
 //     (occluders + 1 per beam) with a warp scan of the counts the scan kernel delivered;
 //   * the hits are loaded COOPERATIVELY: arena slot s is filled by lane s mod 32, whatever beam it belongs to (owner by
-//     a shuffle binary search over the offsets, the slot's particle = the r-th hit index the scan stored for the owner),
-//     in passes (all index loads of a round, then all record loads, by cp.async), so the loads of all beams are in flight
-//     together; the owner then orders its few slots by range;
+//     a shuffle binary search over the offsets, the slot's hit = the r-th hit record the scan stored for the owner), all
+//     copies of a round by cp.async, so the loads of all beams are in flight together; the owner then orders its few
+//     slots by range;
 //   * a warp claims its next tile when it starts one and loads that tile's chunk id and items while it solves this one;
 //   * nearest-first claiming runs in place in the arena: the union list lives in the slots of the already processed
 //     hits, pulses (range, ratio) are compacted to the front;
@@ -33,7 +33,7 @@
 //     all 32 beams are handled one per lane, with uniform code.
 //
 // A beam takes up to SOLVE_LCAP = 128 occluders, the engine's hard cap: more raise LSS_ERR_OCCLUDER_OVERFLOW.  A beam
-// whose hit indices the scan could not store (hit array full) has its bucket prefix walked again by its own lane.
+// whose hits the scan could not store (hit arrays full) has its bucket prefix walked again by its own lane.
 #include "beam.cuh"
 
 namespace {
@@ -70,18 +70,19 @@ __device__ __forceinline__ void beam_limits(float th32, double half_div, Beam &b
 }
 
 // simulation.py:345-385 for one particle: planar range strictly below the target range, centre inside the beam or
-// disk crossing one of the two limit rays
+// disk crossing one of the two limit rays.  No early exit on the range: the three fields of the record are needed
+// together, so their loads are issued together (with an exit, phi and alpha would be loaded after the range test, a
+// second round trip)
 __device__ __forceinline__ bool exact_hit(const ParticleRec *rp, const Beam &bm, double &rho, bool &right_hit, bool &left_hit)
 {
     rho = rp->rho;
-    if (!(rho < bm.d)) return false;
     const double phi = rp->phi, alpha = rp->alpha;
-    bool inside = (bm.right <= phi) && (phi <= bm.left);
-    if (bm.straddle) inside = inside || ((bm.right - LSS_TWO_PI <= phi) && (phi <= bm.left)) ||
-                              ((bm.right <= phi) && (phi <= bm.left + LSS_TWO_PI));
+    bool inside = (bm.right <= phi) & (phi <= bm.left);
+    if (bm.straddle) inside = inside | ((bm.right - LSS_TWO_PI <= phi) & (phi <= bm.left)) |
+                              ((bm.right <= phi) & (phi <= bm.left + LSS_TWO_PI));
     right_hit = within(bm.right - phi, alpha);
     left_hit = within(bm.left - phi, alpha);
-    return inside || right_hit || left_hit;
+    return (rho < bm.d) & (inside | right_hit | left_hit);
 }
 
 // the beam's azimuth bucket of its channel's plane: entries e0 .. e1 of the index (sorted by range), the azimuth
@@ -135,17 +136,11 @@ __device__ __forceinline__ int for_each_hit(const DevArgs &a, const Bucket &k, c
 //   A  each lane walks its beam's bucket prefix with the float32 broad phase only -- a streaming read of 8-byte
 //      entries, four loads in flight -- and notes the particle indices of the survivors (shared memory, SURV_CAP per lane);
 //   B  the survivors of all 32 beams are tested exactly by ALL lanes, one survivor per lane and round (owner by a
-//      shuffle binary search), so the record loads of the whole warp are in flight together; hits are flagged in a
-//      per-beam bit mask.
+//      shuffle binary search), so the record and tangent loads of the whole warp are in flight together; hits are
+//      flagged in a per-beam bit mask, and each hit's record (a1, a2, range) is stored at its rank among its beam's
+//      hits, in a region of one slot per survivor that the warp allocates before the tests.
 // Lanes with more than SURV_CAP survivors (extreme densities) fall back to the serial walk.
 constexpr int SURV_CAP = 20;
-
-__device__ __forceinline__ double shfl_f64(double v, int src)
-{
-    const long long b = __double_as_longlong(v);
-    const int lo = __shfl_sync(FULL, (int)(unsigned)b, src), hi = __shfl_sync(FULL, (int)(b >> 32), src);
-    return __longlong_as_double(((long long)hi << 32) | (unsigned)lo);
-}
 
 #ifndef LSS_SCAN_CTAS
 #define LSS_SCAN_CTAS 10
@@ -167,7 +162,9 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     const int i = w0 + lane;
     const bool active = i < n;
     const int nf_w = min(32, n - w0) * 5;                           // floats of this warp's rows
-    float px = 0, py = 0, pz = 0, pint = 0, pch = 0;
+    // the row stays in s_rows until the rows go back: px, py, pz and the intensity are read from there again where they
+    // are needed, so that no register holds them through the phases
+    float px = 0, py = 0, pz = 0, pch = 0;
     {   // coalesced load of the warp's 32 rows (160 floats)
         const float *src = a.pts + (beg + w0) * 5;
 #pragma unroll
@@ -178,7 +175,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
         __syncwarp();
         if (active) {
             const float *row = &s_rows[wid][5 * lane];
-            px = row[0]; py = row[1]; pz = row[2]; pint = row[3]; pch = row[4];
+            px = row[0]; py = row[1]; pz = row[2]; pch = row[4];
         }
     }
     // np.linalg.norm([x, y, z], axis=0) in float32: sqrt((x*x + y*y) + z*z), no FMA   (simulation.py:89)
@@ -190,13 +187,10 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     bkt.e0 = bkt.e1 = 0; bkt.th_rel = 0.0f; bkt.pbase = 0;
     bool slow = false;
     float th32 = 0.0f;
-    Beam bm;
-    bm.d = (double)d32; bm.right = bm.left = 0.0; bm.straddle = false;
     if (active && ch < LSS_N_CHANNELS) {
         out_l = 0.0f;
         th32 = a.theta ? a.theta[beg + i] : azimuth32(py, px);
         if (th32 < 0.0f) th32 = __fadd_rn(th32, 6.2831855f);
-        beam_limits(th32, a.half_div, bm);
         const int plane = a.order[b * LSS_N_CHANNELS + ch];
         if (plane >= 0 && plane < a.n_planes && th32 == th32) {
             bkt = beam_bucket(a, plane, th32);
@@ -233,6 +227,11 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     }
     const int off = incl - mine;
     const int total = __shfl_sync(FULL, incl, 31);
+    // hit slots of the warp, one per survivor: beam j owns [hbase + off_j, hbase + incl_j) and keeps its hits compacted
+    // at the front of it, in prefix order, as the solve kernel's fill takes them (a region that ends past hit_cap is not
+    // stored: the solve kernel walks that beam's prefix again)
+    int hbase = 0;
+    if (lane == 0 && total > 0) hbase = atomicAdd(a.hdr + 2, total);
     __syncwarp();
 #pragma unroll 1
     for (int s0 = 0; s0 < total; s0 += 32) {
@@ -244,83 +243,90 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
             const int oc = __shfl_sync(FULL, off, c & 31);
             if (c < 32 && oc <= s) j = c;
         }
-        const int r = s - __shfl_sync(FULL, off, j);
+        const int off_j = __shfl_sync(FULL, off, j);
+        const int r = s - off_j;
         const long long pbj = __shfl_sync(FULL, bkt.pbase, j);
-        Beam bj;
-        bj.d = shfl_f64(bm.d, j);
-        bj.right = shfl_f64(bm.right, j);
-        bj.left = shfl_f64(bm.left, j);
-        bj.straddle = bj.right > bj.left;
+        Beam bj;                                                // the owner's limits, from its range and azimuth
+        bj.d = (double)__shfl_sync(FULL, d32, j);
+        beam_limits(__shfl_sync(FULL, th32, j), a.half_div, bj);
+        bool hit = false;
+        double rho = 0.0, a1 = 0.0, a2 = 0.0;
         if (s < total) {
-            double rho;
+            const long long pi = pbj + s_idx[wid][j][r];
+            const ParticleTan tn = a.tan[pi];                   // issued with the record: one round trip for both
             bool rh, lh;
-            if (exact_hit(a.rec + pbj + s_idx[wid][j][r], bj, rho, rh, lh)) atomicOr(&s_hit[wid][j], 1u << r);
+            hit = exact_hit(a.rec + pi, bj, rho, rh, lh);
+            a1 = rh ? bj.right : tn.t_right;                    // geometry.py:26-27: a limit ray the disk crosses clips
+            a2 = lh ? bj.left : tn.t_left;
+            if (hit) atomicOr(&s_hit[wid][j], 1u << r);
+        }
+        const int region = __shfl_sync(FULL, hbase, 0) + off_j;
+        const bool stored = region + (__shfl_sync(FULL, incl, j) - off_j) <= a.hit_cap;
+        __syncwarp();
+        // every survivor of beam j before r has been tested by now (this round or an earlier one): the hits among them
+        // are this hit's rank
+        if (hit && stored) {
+            const int k = region + __popc(s_hit[wid][j] & ((1u << r) - 1u));
+            a.hit_a1[k] = a1;
+            a.hit_a2[k] = a2;
+            a.hit_rho[k] = rho;
         }
     }
     __syncwarp();
-    unsigned hits = s_hit[wid][lane];
-    int L = __popc(hits);
+    hbase = __shfl_sync(FULL, hbase, 0);
+    int L = __popc(s_hit[wid][lane]);
+    Beam bm;                                                    // this lane's limits, for the serial walk
+    bm.d = (double)d32;
+    beam_limits(th32, a.half_div, bm);
     if (slow) L = for_each_hit(a, bkt, bm, d32, [](int, double, bool, bool) {});   // serial fallback: count the hits
-    // ---- beams with occluders: warp-aggregated push to the solve list, hit positions to the position array -------------------
+    // ---- beams with occluders: warp-aggregated push to the solve list -----------------------------------------------------
     {
         const bool push = L > 0;
         const unsigned pm = __ballot_sync(FULL, push);
-        int lincl = push ? L : 0;
-#pragma unroll
-        for (int sft = 1; sft < 32; sft <<= 1) {
-            const int t = __shfl_up_sync(FULL, lincl, sft);
-            if (lane >= sft) lincl += t;
-        }
-        const int ltotal = __shfl_sync(FULL, lincl, 31);
-        if (pm) {
-            int hbase = 0;
-            const int leader = __ffs(pm) - 1;
-            if (lane == leader) hbase = atomicAdd(a.hdr + 2, ltotal);
-            hbase = __shfl_sync(FULL, hbase, leader);
-            if (push) {
-                // work class = number of occluders (then far / near target): what a beam costs the solve kernel -- claiming,
-                // pulses, the sweep over the window ends -- is per-beam serial work proportional to it, and a warp runs as long as
-                // its slowest lane, so the 32 beams of a tile should have the same count.  The costliest class comes first so
-                // that the kernel's tail is cheap tiles; beams with 64 .. 128 occluders (rare) share the costliest class.
-                const int cls = LIST_CLASSES - 1 - min(LIST_CLASSES - 1, 2 * min(L, 63) + (d32 > 40.0f ? 1 : 0));
-                // append to the class's bucket: number j in the class, warp-aggregated per class
-                const unsigned cm = __match_any_sync(pm, cls);
-                const int cl = __ffs(cm) - 1;
-                int j = 0;
-                if (lane == cl) j = atomicAdd(a.hdr + LIST_CLASSES + cls, __popc(cm));
-                j = __shfl_sync(cm, j, cl) + __popc(cm & ((1u << lane) - 1u));
-                // the beam that takes the first number of a chunk allocates it; the others wait for its id.  Every
-                // lane of the warp stores its allocations before any lane waits, and a warp allocates right after
-                // its numbers were handed out, so every awaited store is already on its way.
-                int *ct = a.chunk_tab + (int64_t)cls * a.chunks_per_class + j / LIST_CHUNK;
-                if (j % LIST_CHUNK == 0) atomicExch(ct, atomicAdd(a.hdr, 1) + 1);
-                __syncwarp(pm);
-                int chunk;
-                while ((chunk = *(volatile int *)ct) == 0) {}
-                const int hoff = hbase + lincl - L;
-                const bool fits = hoff + L <= a.hit_cap;        // position array full: the solve kernel walks the prefix
-                {
-                    SolveItem it;           // (only beams with a valid channel walk a bucket: ch < 64)
-                    it.key = ((unsigned long long)ch << 56) | ((unsigned long long)cls << 48) |
-                             ((unsigned long long)b << 32) | (unsigned)i;
-                    it.hit_off = fits ? hoff : -1;
-                    it.L = L;
-                    it.th32 = th32;
-                    it.px = px;
-                    it.py = py;
-                    it.pz = pz;
-                    a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK] = it;
-                }
-                if (fits) {
-                    int *hp = a.hit_idx + hoff;                 // particle indices of the hits, in prefix (~ range) order
-                    if (!slow) {
-                        const int *pos = s_idx[wid][lane];
-#pragma unroll 1
-                        for (int k = 0; hits; hits &= hits - 1) hp[k++] = (int)bkt.pbase + pos[__ffs(hits) - 1];
-                    } else {
-                        for_each_hit(a, bkt, bm, d32, [&](int pi, double, bool, bool) { *hp++ = pi; });
-                    }
-                }
+        if (push) {
+            // work class = number of occluders (then far / near target): what a beam costs the solve kernel -- claiming,
+            // pulses, the sweep over the window ends -- is per-beam serial work proportional to it, and a warp runs as long as
+            // its slowest lane, so the 32 beams of a tile should have the same count.  The costliest class comes first so
+            // that the kernel's tail is cheap tiles; beams with 64 .. 128 occluders (rare) share the costliest class.
+            const int cls = LIST_CLASSES - 1 - min(LIST_CLASSES - 1, 2 * min(L, 63) + (d32 > 40.0f ? 1 : 0));
+            // append to the class's bucket: number j in the class, warp-aggregated per class
+            const unsigned cm = __match_any_sync(pm, cls);
+            const int cl = __ffs(cm) - 1;
+            int j = 0;
+            if (lane == cl) j = atomicAdd(a.hdr + LIST_CLASSES + cls, __popc(cm));
+            j = __shfl_sync(cm, j, cl) + __popc(cm & ((1u << lane) - 1u));
+            // the beam that takes the first number of a chunk allocates it; the others wait for its id.  Every
+            // lane of the warp stores its allocations before any lane waits, and a warp allocates right after
+            // its numbers were handed out, so every awaited store is already on its way.
+            int *ct = a.chunk_tab + (int64_t)cls * a.chunks_per_class + j / LIST_CHUNK;
+            if (j % LIST_CHUNK == 0) atomicExch(ct, atomicAdd(a.hdr, 1) + 1);
+            __syncwarp(pm);
+            int chunk;
+            while ((chunk = *(volatile int *)ct) == 0) {}
+            // a beam with more than SURV_CAP survivors (rare) has no region in the warp's slots: it takes L slots of its
+            // own and stores its hits in the serial walk
+            const int hoff = slow ? atomicAdd(a.hdr + 2, L) : hbase + off;
+            const bool fits = hoff + (slow ? L : mine) <= a.hit_cap;   // hit arrays full: the solve kernel walks the prefix
+            {
+                SolveItem it;           // (only beams with a valid channel walk a bucket: ch < 64)
+                it.key = ((unsigned long long)ch << 56) | ((unsigned long long)cls << 48) |
+                         ((unsigned long long)b << 32) | (unsigned)i;
+                it.hit_off = fits ? hoff : -1;
+                it.L = L;
+                it.th32 = th32;
+                it.px = s_rows[wid][5 * lane];
+                it.py = s_rows[wid][5 * lane + 1];
+                it.pz = s_rows[wid][5 * lane + 2];
+                a.items[(int64_t)(chunk - 1) * LIST_CHUNK + j % LIST_CHUNK] = it;
+            }
+            if (fits && slow) {
+                int k = hoff;
+                for_each_hit(a, bkt, bm, d32, [&](int pi, double rho, bool rh, bool lh) {
+                    a.hit_a1[k] = rh ? bm.right : a.tan[pi].t_right;
+                    a.hit_a2[k] = lh ? bm.left : a.tan[pi].t_left;
+                    a.hit_rho[k] = rho;
+                    k++;
+                });
             }
         }
     }
@@ -329,7 +335,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     __syncwarp();
     if (active) {
         float *row = &s_rows[wid][5 * lane];
-        const float out_i = rintf(pint);                            // np.round of the intensity column (simulation.py:516)
+        const float out_i = rintf(row[3]);                          // np.round of the intensity column (simulation.py:516)
         row[3] = out_i;
         row[4] = out_l;
         if (a.nocc) a.nocc[beg + i] = 0;
@@ -370,12 +376,8 @@ __device__ __forceinline__ void pulse_phase(double r, double &sb, double &cb)
     cb = fma(-corr, s, c);
 }
 
-// cp.async of 4 / 8 bytes global -> shared (the fill of k_solve: loads in flight without registers); a lane's copies
-// are complete after cp_async_wait_all(), and visible to the other lanes of the warp after a __syncwarp() that follows
-__device__ __forceinline__ void cp_async4(void *dst, const void *src)
-{
-    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
-}
+// cp.async of 8 bytes global -> shared (the fill of k_solve: loads in flight without registers); a lane's copies are
+// complete after cp_async_wait_all(), and visible to the other lanes of the warp after a __syncwarp() that follows
 __device__ __forceinline__ void cp_async8(void *dst, const void *src)
 {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;\n" ::"r"((unsigned)__cvta_generic_to_shared(dst)), "l"(src) : "memory");
@@ -529,7 +531,7 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
         long long att_new_i = -1;
         int n_claim = 0;
 
-        // what the scan kernel found on this beam's bucket prefix: L hits, their particle indices in hit_idx[hit_off ..]
+        // what the scan kernel found on this beam's bucket prefix: L hits, their records in hit_a1 / a2 / rho[hit_off ..]
         const int L = active ? it.L : 0;
         Beam bm;
         bm.d = (double)d32;
@@ -562,13 +564,10 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
             double best = 0.0;
             int kbest = 0;
 
-            // ---- cooperative fill: arena slot s <- the r-th hit of its owner beam, (a1, a2, range) --------------------
-            // Three passes, so that two round trips of dependent loads are exposed per round of the arena instead of
-            // two per 32 slots, and no register holds a load in flight (cp.async into shared memory):
-            //   1. the particle index of every slot (PK[s], -1: nothing to load) and its owner lane (PK[ARENA + s]);
-            //   2. the record and the tangents of every slot into A0 .. A3 and PD (all unused until claiming);
-            //   3. each slot's exact test and (a1, a2, range), in place.
-            // (Slot L of a beam is its hard target, filled later; a beam without stored hits is filled after the passes.)
+            // ---- cooperative fill: arena slot s <- the r-th hit record of its owner beam, (a1, a2, range) -------------
+            // The scan stored the records contiguously per beam, so a round of the arena is one pass of cp.async copies
+            // (no register holds a load in flight) and one round trip.  (Slot L of a beam is its hard target, filled
+            // later; a beam without stored hits is filled after the pass.)
 #pragma unroll 1
             for (int s0 = 0; s0 < total; s0 += 32) {
                 const int s = s0 + lane;
@@ -583,47 +582,14 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
                 const int Lj = __shfl_sync(FULL, L, j);
                 const int hoj = __shfl_sync(FULL, it.hit_off, j);
                 const int inr = __shfl_sync(FULL, (int)in_round, j);
-                if (s < total) {
-                    PK[ARENA + s] = j;
-                    if (inr && r < Lj && hoj >= 0) cp_async4(&PK[s], &a.hit_idx[hoj + r]);
-                    else PK[s] = -1;
+                if (s < total && inr && r < Lj && hoj >= 0) {
+                    cp_async8(&A0[s], &a.hit_a1[hoj + r]);
+                    cp_async8(&A1[s], &a.hit_a2[hoj + r]);
+                    cp_async8(&A2[s], &a.hit_rho[hoj + r]);
                 }
             }
             cp_async_wait_all();
             __syncwarp();
-#pragma unroll 1
-            for (int s = lane; s < total; s += 32) {
-                const int pi = PK[s];
-                if (pi >= 0) {
-                    cp_async8(&A0[s], &a.rec[pi].phi);
-                    cp_async8(&A1[s], &a.rec[pi].rho);
-                    cp_async8(&A2[s], &a.rec[pi].alpha);
-                    cp_async8(&A3[s], &a.tan[pi].t_right);
-                    cp_async8(&PD[s], &a.tan[pi].t_left);
-                }
-            }
-            cp_async_wait_all();
-            __syncwarp();
-#pragma unroll 1
-            for (int s0 = 0; s0 < total; s0 += 32) {
-                const int s = s0 + lane;
-                const int j = s < total ? PK[ARENA + s] : 0;
-                Beam bj;
-                bj.d = shfl_f64(bm.d, j);
-                bj.right = shfl_f64(bm.right, j);
-                bj.left = shfl_f64(bm.left, j);
-                bj.straddle = bj.right > bj.left;
-                if (s < total && PK[s] >= 0) {
-                    ParticleRec rc;
-                    rc.phi = A0[s]; rc.rho = A1[s]; rc.alpha = A2[s];
-                    double rho;
-                    bool rh, lh;
-                    exact_hit(&rc, bj, rho, rh, lh);
-                    A0[s] = rh ? bj.right : A3[s];                  // geometry.py:26-27: a limit ray the disk crosses clips
-                    A1[s] = lh ? bj.left : __longlong_as_double((long long)PD[s]);
-                    A2[s] = rho;
-                }
-            }
             if (in_round && it.hit_off < 0) {
                 // the scan could not store this beam's hits (hit array full, rare): its lane walks the bucket prefix
                 // again and fills its slots in prefix order, the order the scan would have stored them in
