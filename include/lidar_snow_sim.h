@@ -184,7 +184,11 @@ LSS_API int64_t lss_launch_count(const lss_engine *e);
  *   d_fit_out    float64[n_clouds*8] or NULL, device: linregress slope, intercept of I/cos over range
  *                (augmentation.py:216-219); slope, intercept of the per-bin minima fit (:249); ymax (:233); n_ground;
  *                points in the mounting window (planes.py:21-27); 1 if the flat-earth fallback was taken (:29-32)
- *   d_ymins_out  int32[n_clouds*50] or NULL, device: the picks used (-1: fewer than 3 ground points)                    */
+ *   d_ymins_out  int32[n_clouds*50] or NULL, device: the picks used (-1: fewer than 3 ground points)
+ * Cloud size: the plane fit gathers each cloud's mounting window with one shared-memory count per 32 rows, so without
+ * h_plane_in a cloud may have at most ((opt-in shared memory per block - 2.2 KB) / 4 - 2) * 32 rows (H100: about
+ * 1.84 M).  A larger one is refused with LSS_ERR_INVALID_ARG before anything is enqueued; the same holds for
+ * lss_snowfall_batch[_host] with LSS_FLAG_DEVICE_PREPASS and lss_wet_ground_batch.                                    */
 LSS_API lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
                                     int n_clouds, double noise_floor, const double *h_plane_in,
                                     const int32_t *h_ymins_in, double *d_poly_out, double *d_plane_out,

@@ -294,6 +294,7 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
     BatchGeometry geo;
     if (lss_status rc = lss_batch_geometry(e, h_cloud_offsets, n_clouds, 0, geo)) return rc;
     DeviceGuard g(e->device);
+    if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, n_clouds, h_plane_in != nullptr)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     const int64_t off_bytes = align_up((int64_t)(n_clouds + 1) * 8, 256);
     if (workspace_bytes < off_bytes + lss_prepass_ws_bytes(geo.n, n_clouds))

@@ -374,6 +374,11 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
                            const int64_t *h_cloud_off, int n_clouds, double delta, double noise_floor, int flat_earth,
                            int range64, int raise_few_ground, const PrepassIO &io, void *d_ws, int64_t ws_bytes,
                            void **cloudpre_out, cudaStream_t stream);
+// LSS_ERR_INVALID_ARG when the pre-pass cannot fit the plane of the batch's largest cloud: the mounting-window gather keeps
+// one count per 32-row tile in shared memory, so a cloud is limited by the device's opt-in shared memory per block (H100:
+// about 1.84 M rows).  Enqueues nothing; always LSS_OK when the plane is given.  lss_prepass_run checks it first, and the
+// entry points call it before their own first enqueue.
+lss_status lss_prepass_check(lss_engine *e, const int64_t *h_cloud_off, int n_clouds, bool plane_given);
 int64_t lss_snowfall_ws_bytes(int64_t n_total, int n_clouds);
 // byte offset, inside the snowfall workspace, of the device copy of the cloud offsets (int64[n_clouds + 1]) a call uploads
 int64_t lss_snowfall_ws_cloud_off(int64_t n_total, int n_clouds);

@@ -176,6 +176,8 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
     auto it = e->tables.find(table_id);
     if (it == e->tables.end()) return lss_fail(e, LSS_ERR_NO_TABLE, "unknown table id");
     DeviceGuard g(e->device);
+    if ((flags & LSS_FLAG_THRESHOLD_FILTER) && (flags & LSS_FLAG_DEVICE_PREPASS) && !h_thresh_poly)
+        if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, B, false)) return rc;
 
     n_chunks = std::max(1, std::min(n_chunks <= 0 ? 4 : n_chunks, B));
     std::vector<int> bounds(n_chunks + 1);

@@ -703,6 +703,43 @@ static PrepassLayout prepass_layout(int64_t n_total, int n_clouds)
 
 int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds) { return prepass_layout(n_total, n_clouds).total; }
 
+// dynamic shared memory of k_window_gather_mad: the prefix of the tile counts of the largest cloud
+static size_t gather_dyn_smem(int64_t max_n) { return sizeof(int) * ((size_t)(max_n + 31) / 32 + 2); }
+
+static int64_t largest_cloud(const int64_t *h_cloud_off, int n_clouds)
+{
+    int64_t max_n = 0;
+    for (int b = 0; b < n_clouds; b++) max_n = std::max<int64_t>(max_n, h_cloud_off[b + 1] - h_cloud_off[b]);
+    return max_n;
+}
+
+// static shared memory of k_window_gather_mad and the device's opt-in limit of a block's shared memory
+static lss_status gather_smem_limits(lss_engine *e, size_t &static_bytes, size_t &optin_bytes)
+{
+    cudaFuncAttributes fa;
+    int optin = 0;
+    LSS_CUDA_CHECK(e, cudaFuncGetAttributes(&fa, k_window_gather_mad));
+    LSS_CUDA_CHECK(e, cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, e->device));
+    static_bytes = fa.sharedSizeBytes;
+    optin_bytes = (size_t)optin;
+    return LSS_OK;
+}
+
+lss_status lss_prepass_check(lss_engine *e, const int64_t *h_cloud_off, int n_clouds, bool plane_given)
+{
+    if (plane_given || n_clouds <= 0) return LSS_OK;
+    const int64_t max_n = largest_cloud(h_cloud_off, n_clouds);
+    size_t static_bytes = 0, optin_bytes = 0;
+    if (lss_status rc = gather_smem_limits(e, static_bytes, optin_bytes)) return rc;
+    if (static_bytes + gather_dyn_smem(max_n) <= optin_bytes) return LSS_OK;
+    const int64_t limit = ((int64_t)((optin_bytes - static_bytes) / sizeof(int)) - 2) * 32;
+    char msg[256];
+    snprintf(msg, sizeof(msg), "pre-pass: a cloud of %lld rows is larger than the %lld rows whose mounting window this "
+             "device can gather (shared memory); give its plane or split it", (long long)max_n, (long long)limit);
+    e->last_error = msg;
+    return LSS_ERR_INVALID_ARG;
+}
+
 // Runs the whole pre-pass for a batch.  d_poly_out / d_plane_out: device [B*3] / [B*4] (either may be null).
 // h_plane_in: optional host [B*4] (w0, w1, w2, h) to use instead of the RANSAC estimate.
 // d_cloudpre_out: optional device pointer receiving the address of the per-cloud CloudPre records (for wet ground).
@@ -716,6 +753,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     const int B = n_clouds;
     const int64_t N = h_cloud_off[B];
     const PrepassLayout L = prepass_layout(N, B);
+    if (lss_status rc = lss_prepass_check(e, h_cloud_off, B, h_plane_in != nullptr)) return rc;
     if (ws_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "pre-pass workspace too small");
     char *ws = (char *)d_ws;
     PreArgs a;
@@ -748,8 +786,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
         a.ymins_in = (const int32_t *)(ws + L.ymins_in);
     }
     if (cloudpre_out) *cloudpre_out = a.cp;
-    int64_t max_n = 0;
-    for (int b = 0; b < B; b++) max_n = std::max<int64_t>(max_n, h_cloud_off[b + 1] - h_cloud_off[b]);
+    const int64_t max_n = largest_cloud(h_cloud_off, B);
     int nblk = (int)std::min<int64_t>(L.max_blocks, std::max<int64_t>(1, (max_n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
 
     {
@@ -766,8 +803,11 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
         } else {
             const int max_tiles = (int)std::max<int64_t>(1, (max_n + WTILE - 1) / WTILE);
             LSS_CUDA_CHECK(e, lss_launch(e, k_window_tiles, dim3(max_tiles, B), WTILE, 0, stream, a));
-            const size_t gather_smem = sizeof(int) * ((size_t)(max_n + 31) / 32 + 2);
-            if (gather_smem > 48 * 1024)
+            // a block gets 48 KB of shared memory without opting in, static and dynamic together
+            const size_t gather_smem = gather_dyn_smem(max_n);
+            size_t static_bytes = 0, optin_bytes = 0;
+            if (lss_status rc = gather_smem_limits(e, static_bytes, optin_bytes)) return rc;
+            if (static_bytes + gather_smem > 48 * 1024)
                 LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_window_gather_mad, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                        (int)gather_smem));
             LSS_CUDA_CHECK(e, lss_launch(e, k_window_gather_mad, B, 1024, gather_smem, stream, a));

@@ -404,6 +404,10 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     const int n_wtiles = wg.tile_base[B];
     if ((s.d_out_perm || s.d_out_nocc) && !s.d_out_full)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "d_out_perm / d_out_nocc need d_out_full");
+    const bool device_prepass = (s.flags & LSS_FLAG_THRESHOLD_FILTER) && (s.flags & LSS_FLAG_DEVICE_PREPASS) &&
+                                !s.h_thresh_poly;
+    if (device_prepass)
+        if (lss_status rc = lss_prepass_check(e, s.h_cloud_offsets, B, s.h_plane_in != nullptr)) return rc;
 
     char *ws = (char *)s.d_workspace;
     float *d_aug = (float *)(ws + w.aug);
@@ -491,8 +495,6 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     // chain of small latency-bound kernels).  It is forked before the scan, whose CTAs retire continuously: the persistent
     // solve kernel holds every SM's registers until its last tile, so a chain forked after the scan would find no room for
     // its 1024-thread CTAs and become the critical path.
-    const bool device_prepass = (s.flags & LSS_FLAG_THRESHOLD_FILTER) && (s.flags & LSS_FLAG_DEVICE_PREPASS) &&
-                                !s.h_thresh_poly;
     cudaEvent_t ev_join = nullptr;
     if (device_prepass) {
         cudaStream_t side = nullptr;

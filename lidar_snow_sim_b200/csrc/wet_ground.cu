@@ -175,6 +175,7 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
     if (!d_points) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
     const WetLayout L = wet_layout(N, B);
     if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, B, h_plane_in != nullptr)) return rc;
     char *ws = (char *)d_workspace;
     WetArgs a;
     a.seg = seg_tiles(ws + L.seg, B);

@@ -229,15 +229,20 @@ def snow_cloud(pc_sorted, tables, order, sensor, beam_divergence_deg, theta=None
 # ----------------------------------------------------------------------------------------------------------------------
 # cloud-level pre / post (NumPy / SciPy / scikit-learn, same calls as the reference)
 # ----------------------------------------------------------------------------------------------------------------------
+def mounting_window(pointcloud):
+    """valid_loc of tools/wet_ground/planes.py:21-27: the rows calculate_plane fits its plane to."""
+    return (pointcloud[:, 2] < -1.55) & \
+           (pointcloud[:, 2] > -1.86 - 0.01 * pointcloud[:, 0]) & \
+           (pointcloud[:, 0] > 10) & \
+           (pointcloud[:, 0] < 70) & \
+           (pointcloud[:, 1] > -3) & \
+           (pointcloud[:, 1] < 3)
+
+
 def calculate_plane(pointcloud, standart_height=-1.55):
     """tools/wet_ground/planes.py:12-50 with loss='squared_error' (the sklearn>=1.2 spelling of 'squared_loss')."""
     from sklearn.linear_model import RANSACRegressor
-    valid_loc = (pointcloud[:, 2] < -1.55) & \
-                (pointcloud[:, 2] > -1.86 - 0.01 * pointcloud[:, 0]) & \
-                (pointcloud[:, 0] > 10) & \
-                (pointcloud[:, 0] < 70) & \
-                (pointcloud[:, 1] > -3) & \
-                (pointcloud[:, 1] < 3)
+    valid_loc = mounting_window(pointcloud)
     pc_rect = pointcloud[valid_loc]
     if pc_rect.shape[0] <= pc_rect.shape[1]:
         w = [0, 0, 1]
