@@ -523,11 +523,16 @@ LSS_API lss_status lss_dart_throwing_planes(int n_planes, double occupancy_ratio
  * device memory (feed lss_upload_particles_device).  The acceptance rule and the stop criterion are the reference's;
  * the random stream is a counter-based generator keyed by (seed, plane, dart) instead of NumPy's PCG64, so parity with
  * the reference's tables is statistical (use lss_dart_throwing for stream-exact tables).
- *   n_candidates       darts thrown per plane (must be enough to reach the occupancy: LSS_ERR_WORKSPACE otherwise)
+ *   n_candidates       darts thrown per plane (must be enough to reach the occupancy: LSS_ERR_WORKSPACE otherwise).
+ *                      Dart i of plane p is the same for every n_candidates > i, so a larger value extends the stream
+ *                      and leaves a table that was complete unchanged
  *   d_xyr_out          float64[n_planes * capacity_per_plane * 3]: plane p at offset p * capacity_per_plane rows
  *   d_counts           int32[n_planes] accepted rows per plane
  *   d_candidates_out   float64[n_planes * n_candidates * 3] or NULL: every dart in throw order (test hook)
- * Synchronises the stream.                                                                                              */
+ * LSS_ERR_WORKSPACE has exactly three causes, each named by lss_last_error: workspace_bytes below
+ * lss_sample_particles_workspace_bytes, the occupancy not reached with n_candidates darts, or more accepted darts than
+ * capacity_per_plane (capacity_per_plane >= n_candidates always suffices).  There is no limit on how many earlier
+ * darts may overlap a dart.  Synchronises the stream.                                                                  */
 LSS_API lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ratio, double precipitation_rate,
                                 double R_0, int distribution, uint64_t seed, int64_t n_candidates, double *d_xyr_out,
                                 int64_t capacity_per_plane, int32_t *d_counts, double *d_candidates_out,

@@ -9,15 +9,15 @@
 //   k_darts      candidate i of plane p from hash(seed, p, i, draw): centre uniform in the disk, diameter ~ Exp truncated at
 //                20 mm, random slice height -> (x, y, r); candidates covering the origin are invalid      (:145-167)
 //                and every valid candidate is pushed into a per-plane spatial hash (cell 0.25 m >> 2 r_max)
-//   k_conflicts  every candidate looks for overlapping candidates with a SMALLER index in the 3x3 neighbourhood (:170)
-//   k_resolve    greedy acceptance in index order restricted to the (very few) candidates that have such conflicts
+//   k_conflicts  every candidate looks for an overlapping candidate with a SMALLER index in the 3x3 neighbourhood (:170)
+//                and, if it finds one, is marked undecided
+//   k_resolve    greedy acceptance in index order restricted to the undecided candidates, each checked against the
+//                accepted darts of its 3x3 neighbourhood
 //   k_cut        inclusive scan of the accepted areas in index order, cut at the first index where the target area is
 //                reached (:142,181-182), stable compaction of the accepted darts before the cut
 #include "common.cuh"
 
 namespace {
-
-constexpr int MAX_CONF = 6;           // earlier overlapping candidates remembered per dart (occupancy ~1e-5: ~0)
 
 struct SampArgs {
     int n_planes;
@@ -26,17 +26,14 @@ struct SampArgs {
     unsigned long long seed;
     double *cand;             // [P*M*3]
     unsigned char *state;     // [P*M] 0 invalid/rejected, 1 accepted, 2 undecided
-    int *conf;                // [P*M*MAX_CONF] earlier overlapping candidates (-1 = none)
     unsigned long long *hkey; // [P*H] cell keys of the hash table (~0 = empty)
-    int *hhead;               // [P*H] head of the cell's list
+    int *hhead;               // [P*H] head of the cell's list (valid candidates only)
     int *next;                // [P*M]
-    int H;                    // table size per plane (power of two)
-    int *undecided;           // [P*(1+U)] count + list
-    int U;
+    int H;                    // table size per plane (power of two, >= 2M: an insertion always finds a free slot)
     double *out;              // [P*cap*3]
     long long cap;
     int *counts;              // [P]
-    int *flags;               // [P] 1 = target not reached with M candidates, 2 = capacity / conflict overflow
+    int *flags;               // [P] 1 = target not reached with M candidates, 2 = more accepted darts than cap
 };
 
 __device__ __forceinline__ unsigned long long mix64(unsigned long long x)
@@ -96,22 +93,20 @@ __global__ void k_darts(SampArgs a)
     c[0] = x; c[1] = y; c[2] = r;
     const bool valid = (r > 0.0) && !(x * x + y * y <= r * r);                           // :166
     a.state[(size_t)p * a.M + i] = valid ? 1 : 0;
-    for (int k = 0; k < MAX_CONF; k++) a.conf[((size_t)p * a.M + i) * MAX_CONF + k] = -1;
     if (valid) {
-        const int s = slot_of(a, p, cell_key(x, y, a.R0), true);
-        if (s < 0) { a.flags[p] = 2; return; }
+        const int s = slot_of(a, p, cell_key(x, y, a.R0), true);          // >= 0: at most M keys in >= 2M slots
         a.next[(size_t)p * a.M + i] = atomicExch(&a.hhead[(size_t)p * a.H + s], i);
     }
 }
 
-__global__ void k_conflicts(SampArgs a)
+// does a dart thrown before dart j (i < j) overlap it (sampling.py:170)?  The hash holds valid darts only; with
+// ACCEPTED only those whose state is 1 count.
+template <bool ACCEPTED>
+__device__ bool earlier_overlap(const SampArgs &a, int p, int j)
 {
-    const int p = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
-    if (j >= a.M || !a.state[(size_t)p * a.M + j]) return;
     const double *c = a.cand + ((size_t)p * a.M + j) * 3;
     const double x = c[0], y = c[1], r = c[2];
     const int cx = (int)floor((x + a.R0) * 4.0), cy = (int)floor((y + a.R0) * 4.0);
-    int nc = 0;
     for (int dy = -1; dy <= 1; dy++)
         for (int dx = -1; dx <= 1; dx++) {
             if (cx + dx < 0 || cy + dy < 0) continue;
@@ -120,44 +115,34 @@ __global__ void k_conflicts(SampArgs a)
             if (s < 0) continue;
             for (int i = a.hhead[(size_t)p * a.H + s]; i >= 0; i = a.next[(size_t)p * a.M + i]) {
                 if (i >= j) continue;                                         // only darts thrown earlier matter
+                if (ACCEPTED && a.state[(size_t)p * a.M + i] != 1) continue;
                 const double *o = a.cand + ((size_t)p * a.M + i) * 3;
                 const double ddx = o[0] - x, ddy = o[1] - y, rr = o[2] + r;
-                if (ddx * ddx + ddy * ddy <= rr * rr) {                       // sampling.py:170
-                    if (nc < MAX_CONF) a.conf[((size_t)p * a.M + j) * MAX_CONF + nc] = i;
-                    else a.flags[p] = 2;
-                    nc++;
-                }
+                if (ddx * ddx + ddy * ddy <= rr * rr) return true;
             }
         }
-    if (nc > 0) {
-        a.state[(size_t)p * a.M + j] = 2;
-        const int pos = atomicAdd(&a.undecided[(size_t)p * (1 + a.U)], 1);
-        if (pos < a.U) a.undecided[(size_t)p * (1 + a.U) + 1 + pos] = j;
-        else a.flags[p] = 2;
-    }
+    return false;
 }
 
-// one thread per plane: the undecided darts in index order (a handful): accepted iff no accepted earlier dart overlaps
+__global__ void k_conflicts(SampArgs a)
+{
+    const int p = blockIdx.y, j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= a.M || !a.state[(size_t)p * a.M + j]) return;
+    if (earlier_overlap<false>(a, p, j)) a.state[(size_t)p * a.M + j] = 2;
+}
+
+// one warp per plane: the undecided darts in index order, each accepted iff no accepted earlier dart overlaps it.
+// Lane 0 decides them all, so every state it reads (i < j) is final: written by itself or left by k_conflicts.
 __global__ void k_resolve(SampArgs a)
 {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    const int p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (p >= a.n_planes) return;
-    int *list = a.undecided + (size_t)p * (1 + a.U);
-    const int n = min(list[0], a.U);
-    for (int s = 1; s < n; s++) {                       // insertion sort by dart index
-        const int key = list[1 + s];
-        int t = s - 1;
-        while (t >= 0 && list[1 + t] > key) { list[2 + t] = list[1 + t]; t--; }
-        list[2 + t] = key;
-    }
-    for (int s = 0; s < n; s++) {
-        const int j = list[1 + s];
-        bool ok = true;
-        for (int k = 0; k < MAX_CONF; k++) {
-            const int i = a.conf[((size_t)p * a.M + j) * MAX_CONF + k];
-            if (i >= 0 && a.state[(size_t)p * a.M + i] == 1) ok = false;      // i < j: already decided
+    unsigned char *state = a.state + (size_t)p * a.M;
+    for (int j0 = 0; j0 < a.M; j0 += 32) {
+        for (unsigned m = __ballot_sync(0xffffffffu, j0 + lane < a.M && state[j0 + lane] == 2); m; m &= m - 1) {
+            const int j = j0 + __ffs(m) - 1;
+            if (lane == 0) state[j] = earlier_overlap<true>(a, p, j) ? 0 : 1;
         }
-        a.state[(size_t)p * a.M + j] = ok ? 1 : 0;
     }
 }
 
@@ -255,7 +240,7 @@ __global__ void __launch_bounds__(1024) k_count(SampArgs a)
     if (tid == 0) a.counts[p] = run_cnt;
 }
 
-struct SampLayout { int64_t cand, state, conf, hkey, hhead, next, undecided, flags, total; int H, U; };
+struct SampLayout { int64_t cand, state, hkey, hhead, next, flags, total; int H; };
 
 SampLayout samp_layout(int n_planes, int64_t M)
 {
@@ -263,15 +248,12 @@ SampLayout samp_layout(int n_planes, int64_t M)
     int H = 1;
     while (H < 2 * M) H <<= 1;
     L.H = H;
-    L.U = 4096;
     int64_t o = 0;
     L.cand = o;      o = align_up(o + (int64_t)n_planes * M * 3 * 8, 256);
     L.state = o;     o = align_up(o + (int64_t)n_planes * M, 256);
-    L.conf = o;      o = align_up(o + (int64_t)n_planes * M * MAX_CONF * 4, 256);
     L.hkey = o;      o = align_up(o + (int64_t)n_planes * H * 8, 256);
     L.hhead = o;     o = align_up(o + (int64_t)n_planes * H * 4, 256);
     L.next = o;      o = align_up(o + (int64_t)n_planes * M * 4, 256);
-    L.undecided = o; o = align_up(o + (int64_t)n_planes * (1 + L.U) * 4, 256);
     L.flags = o;     o = align_up(o + (int64_t)n_planes * 4, 256);
     L.total = o;
     return L;
@@ -317,13 +299,10 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
     a.seed = seed;
     a.cand = (double *)(ws + L.cand);
     a.state = (unsigned char *)(ws + L.state);
-    a.conf = (int *)(ws + L.conf);
     a.hkey = (unsigned long long *)(ws + L.hkey);
     a.hhead = (int *)(ws + L.hhead);
     a.next = (int *)(ws + L.next);
     a.H = L.H;
-    a.undecided = (int *)(ws + L.undecided);
-    a.U = L.U;
     a.out = d_xyr_out;
     a.cap = capacity_per_plane;
     a.counts = d_counts;
@@ -332,7 +311,6 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
     do {
         if (cudaMemsetAsync(a.hkey, 0xff, (size_t)n_planes * L.H * 8, st) != cudaSuccess ||
             cudaMemsetAsync(a.hhead, 0xff, (size_t)n_planes * L.H * 4, st) != cudaSuccess ||
-            cudaMemsetAsync(a.undecided, 0, (size_t)n_planes * (1 + L.U) * 4, st) != cudaSuccess ||
             cudaMemsetAsync(a.flags, 0, (size_t)n_planes * 4, st) != cudaSuccess) {
             rc = lss_fail(e, LSS_ERR_CUDA, "sampler memset failed");
             break;
@@ -340,7 +318,7 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
         const dim3 grid((unsigned)((n_candidates + 255) / 256), n_planes);
         if (lss_launch(e, k_darts, grid, 256, 0, st, a) != cudaSuccess ||
             lss_launch(e, k_conflicts, grid, 256, 0, st, a) != cudaSuccess ||
-            lss_launch(e, k_resolve, (n_planes + 63) / 64, 64, 0, st, a) != cudaSuccess ||
+            lss_launch(e, k_resolve, (n_planes + 3) / 4, 128, 0, st, a) != cudaSuccess ||
             lss_launch(e, k_cut, n_planes, 1024, 0, st, a) != cudaSuccess ||
             lss_launch(e, k_count, n_planes, 1024, 0, st, a) != cudaSuccess) {
             rc = lss_fail(e, LSS_ERR_CUDA, "sampler launch failed");
@@ -357,7 +335,7 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
         }
         for (int p = 0; p < n_planes; p++) {
             if (flags[p] == 1) { rc = lss_fail(e, LSS_ERR_WORKSPACE, "n_candidates too small to reach the occupancy"); break; }
-            if (flags[p] == 2) { rc = lss_fail(e, LSS_ERR_WORKSPACE, "sampler capacity exceeded"); break; }
+            if (flags[p] == 2) { rc = lss_fail(e, LSS_ERR_WORKSPACE, "capacity_per_plane too small for the accepted darts"); break; }
         }
     } while (0);
     if (dev_prev != e->device && dev_prev >= 0) cudaSetDevice(dev_prev);

@@ -14,6 +14,9 @@ from . import _lib
 from .calib.hdl64e_s3 import sensor_arrays
 
 DEFAULT_MAX_DIVERGENCE_RAD = 3e-3          # callers pass beam_divergence = degrees(3e-3) (precompute.py:104)
+# sample_tables_device calls the sampler at most this often: the darts per plane start at 1.5x the expected table size
+# (+4096) and double after each call that ends short of the occupancy; the last call's failure is raised
+SAMPLER_ATTEMPTS = 4
 
 
 def _ptr(t):
@@ -111,23 +114,23 @@ class SnowfallEngine:
             raise NotImplementedError('Distribution model unknown.')
         occ = compute_occupancy(float(snowfall_rate), float(terminal_velocity))
         rr = float(snowfall_rate_to_rainfall_rate(float(snowfall_rate), float(terminal_velocity)))
-        cap = _expected_capacity(occ, rr, R_0, mode)
+        M = _expected_capacity(occ, rr, R_0, mode)
         with torch.cuda.device(self.device):
-            while True:
-                M = cap
+            for attempt in range(SAMPLER_ATTEMPTS):
+                # the output holds M rows per plane, as many as there are darts, so only a target not reached with M
+                # darts (the stream is keyed per dart: more darts extend it, they do not change it) can fail here
                 need = self.lib.lss_sample_particles_workspace_bytes(n_planes, M)
                 ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
-                out = torch.empty((n_planes, cap, 3), dtype=torch.float64, device=self.device)
+                out = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device)
                 counts = torch.empty((n_planes,), dtype=torch.int32, device=self.device)
                 cand = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device) if return_candidates else None
                 st = self.lib.lss_sample_particles(self.h, n_planes, occ, rr, float(R_0), _DIST[mode], int(seed), M,
-                                                   _ptr(out), cap, _ptr(counts), _ptr(cand), _ptr(ws), int(ws.numel()),
+                                                   _ptr(out), M, _ptr(counts), _ptr(cand), _ptr(ws), int(ws.numel()),
                                                    self._stream())
-                if st == _lib.LSS_ERR_WORKSPACE:
-                    cap *= 2
-                    continue
-                _lib.check(st, self.h)
-                break
+                if st != _lib.LSS_ERR_WORKSPACE or attempt == SAMPLER_ATTEMPTS - 1:
+                    break
+                M *= 2
+            _lib.check(st, self.h)
             cnt = counts.cpu().numpy().astype(np.int64)
             off = np.concatenate([[0], np.cumsum(cnt)])
             xyr = torch.cat([out[p, :cnt[p]] for p in range(n_planes)], dim=0).contiguous()

@@ -2,37 +2,13 @@
 import numpy as np
 import pytest
 import torch
-from scipy.spatial import cKDTree
 
+import sampler_stream as SS
 from helpers import DIV
 from lidar_snow_sim_b200.snowfall import sampling as S
 from lidar_snow_sim_b200.synthetic import synthetic_cloud
 
 pytestmark = pytest.mark.gpu
-
-
-def greedy_reference(cand, target_area):
-    """The reference's sequential rule applied to a given dart sequence (sampling.py:142-183)."""
-    x, y, r = cand.T
-    valid = (r > 0) & ~(x * x + y * y <= r * r)
-    pairs = cKDTree(cand[:, :2]).query_pairs(0.0201, output_type='ndarray')
-    earlier = {}
-    for i, j in pairs:
-        lo, hi = (i, j) if i < j else (j, i)
-        if (x[lo] - x[hi]) ** 2 + (y[lo] - y[hi]) ** 2 <= (r[lo] + r[hi]) ** 2:
-            earlier.setdefault(hi, []).append(lo)
-    acc = valid.copy()
-    for j in sorted(earlier):
-        if acc[j] and any(acc[i] for i in earlier[j]):
-            acc[j] = False
-    area = 0.0
-    keep = []
-    for i in np.nonzero(acc)[0]:
-        if not area < target_area:
-            break
-        keep.append(i)
-        area += np.pi * r[i] ** 2
-    return np.array(keep), area
 
 
 @pytest.mark.parametrize('mode,rate,vel', [('gunn', 2.5, 1.6), ('sekhon', 1.0, 0.6)])
@@ -42,7 +18,8 @@ def test_device_sampler_is_the_greedy_rule(engine, mode, rate, vel):
     occ = S.compute_occupancy(rate, vel)
     target = occ * np.pi * 80.0 ** 2
     for p in range(3):
-        keep, area = greedy_reference(cand[p], target)
+        x, y, r = cand[p].T
+        keep, area, _ = SS.greedy(cand[p], (r > 0) & ~(x * x + y * y <= r * r), target)
         got = xyr[off[p]:off[p + 1]]
         assert np.array_equal(got, cand[p][keep]), f'plane {p}'
         assert area >= target > area - np.pi * got[-1, 2] ** 2
