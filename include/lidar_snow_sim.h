@@ -42,8 +42,13 @@ typedef enum {
     LSS_ERR_OCCLUDER_OVERFLOW = 6,   /* more than 128 occluders on one beam */
     LSS_ERR_WORKSPACE = 7,        /* caller-supplied workspace too small */
     LSS_ERR_NO_SENSOR = 8,        /* AssertionError analogue: sensor constants missing (simulation.py:35,474-480) */
-    LSS_ERR_TOO_FEW_GROUND = 9    /* TypeError analogue: fewer than 3 ground points, estimate_laser_parameters returns
+    LSS_ERR_TOO_FEW_GROUND = 9,   /* TypeError analogue: fewer than 3 ground points, estimate_laser_parameters returns
                                      None (tools/wet_ground/augmentation.py:213-214) and simulation.py:462 fails */
+    LSS_ERR_INTENSITY_RANGE = 10  /* ValueError analogue: a cloud's I/cos maximum over its ground points is NaN, infinite
+                                     or below 5, so np.histogram2d(..., range=(..., (5, ymax))) raises
+                                     (tools/wet_ground/augmentation.py:232-233).  Latched for a cloud with >= 3 ground
+                                     points (lss_noise_threshold_poly, LSS_FLAG_DEVICE_PREPASS) or >= 1000
+                                     (lss_wet_ground_batch, which returns that cloud unchanged) */
 } lss_status;
 
 /* flags for lss_snowfall_batch */
@@ -184,7 +189,9 @@ LSS_API int64_t lss_launch_count(const lss_engine *e);
  *   d_fit_out    float64[n_clouds*8] or NULL, device: linregress slope, intercept of I/cos over range
  *                (augmentation.py:216-219); slope, intercept of the per-bin minima fit (:249); ymax (:233); n_ground;
  *                points in the mounting window (planes.py:21-27); 1 if the flat-earth fallback was taken (:29-32)
- *   d_ymins_out  int32[n_clouds*50] or NULL, device: the picks used (-1: fewer than 3 ground points)
+ *   d_ymins_out  int32[n_clouds*50] or NULL, device: the picks used (-1: fewer than 3 ground points, or an I/cos range
+ *                that LSS_ERR_INTENSITY_RANGE describes; the minima fit is then the first regression).  An I/cos maximum of
+ *                exactly 5 bins over NumPy's widened range (4.5, 5.5).
  * Cloud size: the plane fit gathers each cloud's mounting window with one shared-memory count per 32 rows, so without
  * h_plane_in a cloud may have at most ((opt-in shared memory per block - 2.2 KB) / 4 - 2) * 32 rows (H100: about
  * 1.84 M).  A larger one is refused with LSS_ERR_INVALID_ARG before anything is enqueued; the same holds for
@@ -209,14 +216,20 @@ LSS_API int64_t lss_prepass_workspace_bytes(int64_t n_total, int n_clouds);
  *                     compacted to the front of the cloud's slot
  *   d_out_intensity64 float64[n_total] or NULL: column 3 of the output rows in the reference's float64
  *   d_out_counts      int32[n_clouds]
- *   d_out_passthrough int32[n_clouds] or NULL: 1 where the cloud had < 1000 ground points and is returned unchanged (:51-52)
- *   d_out_plane       float64[n_clouds*4] or NULL                                                                       */
+ *   d_out_passthrough int32[n_clouds] or NULL: 0 where the cloud was augmented; 1 where it had < 1000 ground points and
+ *                     is returned unchanged (:51-52); 2 where its I/cos range is degenerate (LSS_ERR_INTENSITY_RANGE,
+ *                     latched for lss_check_async): the reference raises ValueError there, the cloud is returned
+ *                     unchanged and the other clouds of the batch are augmented as usual
+ *   d_out_plane       float64[n_clouds*4] or NULL
+ *   d_out_fit         float64[n_clouds*8] or NULL, d_out_ymins int32[n_clouds*50] or NULL: the fits and picks of the
+ *                     ground band, float64 ranges, laid out as in lss_noise_threshold_poly                            */
 LSS_API lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
                                 const int32_t *d_cloud_counts, int n_clouds, double water_height, double pavement_depth,
                                 double noise_floor, double power_factor, int flat_earth, double delta, int replace,
                                 const double *h_plane_in, const int32_t *h_ymins_in, float *d_out_points,
                                 double *d_out_intensity64, int32_t *d_out_counts, int32_t *d_out_passthrough,
-                                double *d_out_plane, void *d_workspace, int64_t workspace_bytes, void *stream);
+                                double *d_out_plane, double *d_out_fit, int32_t *d_out_ymins, void *d_workspace,
+                                int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_wet_ground_workspace_bytes(int64_t n_total, int n_clouds);
 
 /* ---- fog simulation ("next" row, SURVEY.md 8f-3) -----------------------------------------------------------------------

@@ -20,6 +20,7 @@ LSS_ERR_OCCLUDER_OVERFLOW = 6
 LSS_ERR_WORKSPACE = 7
 LSS_ERR_NO_SENSOR = 8
 LSS_ERR_TOO_FEW_GROUND = 9
+LSS_ERR_INTENSITY_RANGE = 10
 
 FLAG_THRESHOLD_FILTER = 0x1
 FLAG_CAMERA_FOV = 0x2
@@ -48,6 +49,7 @@ _EXC = {
     LSS_ERR_WORKSPACE: RuntimeError,
     LSS_ERR_NO_SENSOR: AssertionError,           # simulation.py:35
     LSS_ERR_TOO_FEW_GROUND: TypeError,           # estimate_laser_parameters -> None, simulation.py:457-462
+    LSS_ERR_INTENSITY_RANGE: ValueError,         # np.histogram2d's range (5, max(I/cos)), augmentation.py:232-233
 }
 
 # every symbol include/lidar_snow_sim.h declares: (name, restype, argtypes)
@@ -85,7 +87,8 @@ SIGNATURES = [
                                             _P]),
     ('lss_prepass_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_wet_ground_batch', _c.c_int, [_P, _P, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _c.c_double,
-                                        _c.c_int, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+                                        _c.c_int, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                        _c.c_int64, _P]),
     ('lss_wet_ground_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_fog_batch', _c.c_int, [_P, _P, _c.c_int, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _P, _c.c_uint32,
                                  _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),

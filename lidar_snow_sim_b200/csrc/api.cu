@@ -51,6 +51,8 @@ const char *lss_status_string(lss_status s)
         case LSS_ERR_WORKSPACE: return "workspace too small";
         case LSS_ERR_NO_SENSOR: return "sensor / camera constants not set";
         case LSS_ERR_TOO_FEW_GROUND: return "fewer than 3 ground points: laser parameters cannot be estimated";
+        case LSS_ERR_INTENSITY_RANGE:
+            return "intensity histogram range (5, max(I/cos)) of the ground points is not finite or max is below 5";
     }
     return "unknown status";
 }

@@ -352,6 +352,8 @@ struct CloudPre {            // per-cloud scratch / results, float64
     // polynomial needs no further pass over the cloud once that fit is known)
     double mom[11];
 };
+// np.histogram2d(..., range=(..., (5, ymax))) (augmentation.py:232-233) raises ValueError unless ymax is finite and >= 5
+__device__ __forceinline__ bool lss_intensity_range_ok(double ymax) { return ymax >= 5.0 && !isinf(ymax); }
 // p . w exactly as written, without FMA contraction, so that every kernel classifies a point identically
 __device__ __forceinline__ double lss_plane_dot(double x, double y, double z, const double *w)
 {
@@ -368,7 +370,11 @@ struct PrepassIO {
     double *d_plane_out = nullptr;          // device [B*4]
     double *d_fit_out = nullptr;            // device [B*8]: lin slope, lin intercept, pmin slope, pmin intercept, ymax,
                                             //               n_ground, n_window, flat-earth fallback taken
-    int32_t *d_ymins_out = nullptr;         // device [B*50] the picks used (-1: fewer than 3 ground points)
+    int32_t *d_ymins_out = nullptr;         // device [B*50] the picks used (-1: fewer than 3 ground points or a
+                                            //               degenerate intensity range)
+    // a cloud with at least this many ground points latches LSS_ERR_INTENSITY_RANGE when its I/cos range is degenerate
+    // (the snowfall path fits from 3 ground points on; wet ground returns below 1000 first, augmentation.py:51-52)
+    int range_min_ground = 3;
 };
 lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_cloud_off, const int32_t *d_cloud_cnt,
                            const int64_t *h_cloud_off, int n_clouds, double delta, double noise_floor, int flat_earth,

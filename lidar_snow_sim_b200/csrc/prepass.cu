@@ -31,6 +31,7 @@ struct PreArgs {
     const int64_t *cloud_off;  // [B+1]: cloud b starts at row cloud_off[b]
     const int32_t *cloud_cnt;  // optional [B]: number of valid rows of cloud b (slot-compacted input); null: off[b+1]-off[b]
     int raise_few;             // latch LSS_ERR_TOO_FEW_GROUND when a cloud has < 3 ground points (snowfall path)
+    int range_min_ground;      // latch LSS_ERR_INTENSITY_RANGE from this many ground points on (PrepassIO)
     int range64;               // ranges in float64 (wet ground: the reference's ground array is float64) or float32
     int n_clouds;
     double delta;            // ground band half width: 0.5 in simulation.py:450, `delta` in augmentation.py:46
@@ -421,10 +422,22 @@ __device__ __forceinline__ int edge_bin(double v, double lo, double hi, int nb)
     return k;
 }
 
+// The intensity axis of the histogram: (5, ymax), except that NumPy widens an empty range (5, 5) to (4.5, 5.5)
+// (np.histogramdd's _get_outer_edges).  Only meaningful when lss_intensity_range_ok(ymax).
+__device__ __forceinline__ void intensity_edges(double ymax, double &lo, double &hi)
+{
+    lo = ymax == 5.0 ? 4.5 : 5.0;
+    hi = ymax == 5.0 ? 5.5 : ymax;
+}
+
+// np.max: a NaN anywhere makes the maximum NaN (fmax would drop it)
+__device__ __forceinline__ double nan_max(double a, double b) { return (a != a || a > b) ? a : b; }
+
 // ---- 5. the ground pass: count, max(I/cos), regression and moment sums; histogram records; grid (blocks, cloud) --------------
-// A ground point goes into the 50 x 2555 histogram when its range bin exists (10 <= d <= 70) and 5 <= I/cos <= ymax.
-// ymax is the maximum of I/cos over the ground points, so I/cos <= ymax holds for all of them once I/cos >= 5: the
-// record needs only the range bin and I/cos, and the intensity bin is taken once ymax is known (k_ground_hist).
+// A ground point goes into the 50 x 2555 histogram when its range bin exists (10 <= d <= 70) and lo <= I/cos <= hi,
+// (lo, hi) = intensity_edges(ymax).  ymax is the maximum of I/cos over the ground points, so I/cos <= hi holds for all of
+// them: the record needs only the range bin and I/cos (kept from 4.5 on, the lowest lo), and the intensity bin is taken
+// once ymax is known (k_ground_hist).
 __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
 {
     __shared__ double red[15 * (PP_TPB / 32)];
@@ -452,13 +465,13 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
         if (g.ground) {
             const double dd = g.d - 30.0, yy = g.norm_i - 50.0;              // shifted sums (conditioning)
             v[0] += 1.0; v[1] += dd; v[2] += yy; v[3] += dd * dd; v[4] += dd * yy;
-            vmax = fmax(vmax, g.norm_i);
+            vmax = nan_max(vmax, g.norm_i);
             const double t = (g.d - 40.0) / 30.0, t2 = t * t;
             const double c = g.cosang, dc = g.d * g.cosang;
             v[5] += t; v[6] += t2; v[7] += t2 * t; v[8] += t2 * t2;
             v[9] += c; v[10] += c * t; v[11] += c * t2;
             v[12] += dc; v[13] += dc * t; v[14] += dc * t2;
-            if (g.norm_i >= 5.0) bx = edge_bin(g.d, 10.0, 70.0, HIST_NX);
+            if (g.norm_i >= 4.5) bx = edge_bin(g.d, 10.0, 70.0, HIST_NX);
         }
         const unsigned m = __ballot_sync(0xffffffffu, bx >= 0);
         if (m) {
@@ -473,11 +486,11 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
         }
     }
 #pragma unroll
-    for (int s = 16; s > 0; s >>= 1) vmax = fmax(vmax, __shfl_down_sync(0xffffffffu, vmax, s));
+    for (int s = 16; s > 0; s >>= 1) vmax = nan_max(vmax, __shfl_down_sync(0xffffffffu, vmax, s));
     if ((threadIdx.x & 31) == 0) mx[threadIdx.x >> 5] = vmax;
     block_sum<15>(v, red);
     if (threadIdx.x == 0) {
-        for (int q = 0; q < PP_TPB / 32; q++) vmax = fmax(vmax, mx[q]);
+        for (int q = 0; q < PP_TPB / 32; q++) vmax = nan_max(vmax, mx[q]);
         double *p = a.partial + ((size_t)b * a.max_blocks + blockIdx.x) * 16;
         for (int k = 0; k < 15; k++) p[k] = v[k];
         p[15] = vmax;
@@ -496,13 +509,13 @@ __device__ __forceinline__ void warp_reduce_partials(const double *partial, int 
         const double *p = partial + (size_t)q * 16;
 #pragma unroll
         for (int k = 0; k < NV; k++) v[k] += p[k];
-        if (vmax) m = fmax(m, p[NV]);
+        if (vmax) m = nan_max(m, p[NV]);
     }
 #pragma unroll
     for (int s = 16; s > 0; s >>= 1) {
 #pragma unroll
         for (int k = 0; k < NV; k++) v[k] += __shfl_xor_sync(0xffffffffu, v[k], s);
-        m = fmax(m, __shfl_xor_sync(0xffffffffu, m, s));
+        m = nan_max(m, __shfl_xor_sync(0xffffffffu, m, s));
     }
     if (vmax) *vmax = m;
 }
@@ -546,13 +559,17 @@ __global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_block
                     cp.lin[0] = cp.lin[1] = 0.0;
                     if (a.raise_few) atomicMax(a.status, LSS_ERR_TOO_FEW_GROUND);
                 }
+                if (v[0] >= (double)a.range_min_ground && !lss_intensity_range_ok(cp.ymax))
+                    atomicMax(a.status, LSS_ERR_INTENSITY_RANGE);
             }
         }
     }
     __syncthreads();
     const int n_ground = (int)stat[0];
     const double ymax = stat[1];
-    if (n_ground < 3) return;
+    if (n_ground < 3 || !lss_intensity_range_ok(ymax)) return;     // no picks (k_poly_solve)
+    double ylo, yhi;
+    intensity_edges(ymax, ylo, yhi);
     int32_t *ymins = a.ymins + b * HIST_NX + bx0;
     if (a.ymins_in) {                           // parity replay: the reference host's own picks, no histogram needed
         for (int k = threadIdx.x; k < nbx; k += HIST_TPB) {
@@ -578,7 +595,7 @@ __global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_block
 #pragma unroll
         for (int u = 0; u < U; u++)
             if ((unsigned)rel[u] < (unsigned)nbx) {
-                const int by = edge_bin(norms[k0 + u * HIST_TPB], 5.0, ymax, HIST_NY);
+                const int by = edge_bin(norms[k0 + u * HIST_TPB], ylo, yhi, HIST_NY);
                 if (by >= 0) atomicAdd(&hist[rel[u] * HIST_NY + by], 1u);
             }
     }
@@ -603,11 +620,11 @@ __global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_block
 
 // ---- 7. second regression over the minima; quadratic fit of noise*cos over range (simulation.py:462-467) ------------------
 // The point of range bin k: its centre and the lower edge of its picked intensity bin, yedges[ymins] with
-// yedges = np.linspace(5, ymax, 2556) (arange * step + start, last edge = stop); used when that edge is above 5
-// (augmentation.py:238-241).
-__device__ __forceinline__ bool minima_point(int k, int bidx, double ymax, double ystep, double &x, double &y)
+// yedges = np.linspace(ylo, yhi, 2556) (arange * step + start, last edge = stop; intensity_edges); used when that edge is
+// above 5 (augmentation.py:238-241).
+__device__ __forceinline__ bool minima_point(int k, int bidx, double ylo, double yhi, double ystep, double &x, double &y)
 {
-    y = (bidx == HIST_NY) ? ymax : __dadd_rn(__dmul_rn((double)bidx, ystep), 5.0);
+    y = (bidx == HIST_NY) ? yhi : __dadd_rn(__dmul_rn((double)bidx, ystep), ylo);
     const double e0 = k * (60.0 / HIST_NX) + 10.0;
     const double e1 = (k + 1 == HIST_NX) ? 70.0 : ((k + 1) * (60.0 / HIST_NX) + 10.0);
     x = (e0 + e1) / 2;
@@ -623,17 +640,23 @@ __global__ void k_poly_solve(PreArgs a, double *poly_out /* [B*3] or null */, do
     const int b = blockIdx.x;
     CloudPre &cp = a.cp[b];
     if (threadIdx.x != 0) return;
+    // a degenerate intensity range has no histogram and no picks: the reference raises there (LSS_ERR_INTENSITY_RANGE)
+    // or, wet ground below 1000 ground points, never bins; the fits fall back to the first regression
+    const bool picked = cp.n_ground >= 3 && lss_intensity_range_ok(cp.ymax);
     if (cp.n_ground >= 3) {
         const int32_t *ymins = a.ymins + b * HIST_NX;
-        const double ystep = (cp.ymax - 5.0) / HIST_NY;
+        double ylo, yhi;
+        intensity_edges(cp.ymax, ylo, yhi);
+        const double ystep = (yhi - ylo) / HIST_NY;
         int m = 0;
         double sx = 0, sy = 0, x, y;
-        for (int k = 0; k < HIST_NX; k++) if (minima_point(k, ymins[k], cp.ymax, ystep, x, y)) { m++; sx += x; sy += y; }
+        for (int k = 0; k < HIST_NX && picked; k++)
+            if (minima_point(k, ymins[k], ylo, yhi, ystep, x, y)) { m++; sx += x; sy += y; }
         if (m > 3) {                                                                     // augmentation.py:248-251
             const double mx_ = sx / m, my_ = sy / m;
             double sxx = 0, sxy = 0;
             for (int k = 0; k < HIST_NX; k++)
-                if (minima_point(k, ymins[k], cp.ymax, ystep, x, y)) { sxx += (x - mx_) * (x - mx_); sxy += (x - mx_) * (y - my_); }
+                if (minima_point(k, ymins[k], ylo, yhi, ystep, x, y)) { sxx += (x - mx_) * (x - mx_); sxy += (x - mx_) * (y - my_); }
             cp.pmin[0] = sxy / sxx;
             cp.pmin[1] = my_ - cp.pmin[0] * mx_;
         } else {
@@ -674,7 +697,7 @@ __global__ void k_poly_solve(PreArgs a, double *poly_out /* [B*3] or null */, do
         f[0] = cp.lin[0]; f[1] = cp.lin[1]; f[2] = cp.pmin[0]; f[3] = cp.pmin[1]; f[4] = cp.ymax;
         f[5] = (double)cp.n_ground; f[6] = (double)cp.n_window; f[7] = (double)cp.flat;
     }
-    if (ymins_out) for (int k = 0; k < HIST_NX; k++) ymins_out[b * HIST_NX + k] = cp.n_ground >= 3 ? a.ymins[b * HIST_NX + k] : -1;
+    if (ymins_out) for (int k = 0; k < HIST_NX; k++) ymins_out[b * HIST_NX + k] = picked ? a.ymins[b * HIST_NX + k] : -1;
 }
 
 }  // namespace
@@ -762,6 +785,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     a.cloud_cnt = d_cloud_cnt;
     a.range64 = range64;
     a.raise_few = raise_few_ground;
+    a.range_min_ground = io.range_min_ground;
     a.n_clouds = B;
     a.delta = delta;
     a.noise_floor = noise_floor;

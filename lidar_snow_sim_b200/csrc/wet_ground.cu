@@ -8,7 +8,9 @@
 //                           (augmentation.py:150-159), column 4 rewritten; stable, tile parallel (segments.cuh)
 //
 // All per-point physics in float64, as the reference (its ground array is float64, augmentation.py:50).
-// A cloud with fewer than 1000 ground points is passed through unchanged (augmentation.py:51-52).
+// A cloud with fewer than 1000 ground points is passed through unchanged (augmentation.py:51-52).  So is one whose
+// I/cos range is degenerate, where the reference raises ValueError (augmentation.py:232-233): the pre-pass latches
+// LSS_ERR_INTENSITY_RANGE and the other clouds of the batch are augmented as usual.
 #include "segments.cuh"
 
 namespace {
@@ -28,9 +30,16 @@ struct WetArgs {
     float *out;                   // [N*5] slot-compacted rows
     double *out_i64;              // optional [N] float64 intensity of the output rows
     int32_t *out_counts;          // [B]
-    int32_t *out_passthrough;     // [B] 1 = cloud returned unchanged
+    int32_t *out_passthrough;     // [B] 0 = augmented, 1 = < 1000 ground points, 2 = degenerate I/cos range; 1, 2: unchanged
     SegTiles seg;                 // tiles of WET_TILE rows; class 0 = not ground, 1 = ground kept
 };
+
+// 0: augmented; 1: fewer than 1000 ground points (augmentation.py:51-52); 2: the reference raises ValueError at :232-233
+__device__ __forceinline__ int wet_passthrough(const CloudPre &cp)
+{
+    if (cp.n_ground < 1000) return 1;
+    return lss_intensity_range_ok(cp.ymax) ? 0 : 2;
+}
 
 struct Fresnel { double rs, ts, rp, tp, aout; };
 
@@ -61,7 +70,7 @@ __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
     const CloudPre cp = a.cp[b];
     const int64_t beg = a.cloud_off[b];
     const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
-    const bool pass = cp.n_ground < 1000;                                  // augmentation.py:51-52
+    const bool pass = wet_passthrough(cp) != 0;
     for (int i = blockIdx.x * WET_TPB + threadIdx.x; i < n; i += gridDim.x * WET_TPB) {
         const float *r = a.pts + (beg + i) * 5;
         const double x = r[0], y = r[1], z = r[2], inten = r[3];
@@ -100,10 +109,11 @@ __global__ void __launch_bounds__(WET_TILE) k_wet_scatter(WetArgs a)
 {
     const int b = blockIdx.y, tile = blockIdx.x;
     const CloudPre &cp = a.cp[b];
-    const bool pass = cp.n_ground < 1000;
+    const int pass_code = wet_passthrough(cp);
+    const bool pass = pass_code != 0;
     if (tile == 0 && threadIdx.x == 0) {
         a.out_counts[b] = a.seg.total[0][b] + a.seg.total[1][b];
-        if (a.out_passthrough) a.out_passthrough[b] = pass ? 1 : 0;
+        if (a.out_passthrough) a.out_passthrough[b] = pass_code;
     }
     const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
     if (tile * WET_TILE >= n) return;
@@ -156,7 +166,8 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
                                 double noise_floor, double power_factor, int flat_earth, double delta, int replace,
                                 const double *h_plane_in, const int32_t *h_ymins_in, float *d_out_points,
                                 double *d_out_intensity64, int32_t *d_out_counts, int32_t *d_out_passthrough,
-                                double *d_out_plane, void *d_workspace, int64_t workspace_bytes, void *stream)
+                                double *d_out_plane, double *d_out_fit, int32_t *d_out_ymins, void *d_workspace,
+                                int64_t workspace_bytes, void *stream)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
     BatchGeometry g;
@@ -189,6 +200,9 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
     io.h_plane_in = h_plane_in;
     io.h_ymins_in = h_ymins_in;
     io.d_plane_out = d_out_plane;
+    io.d_fit_out = d_out_fit;
+    io.d_ymins_out = d_out_ymins;
+    io.range_min_ground = 1000;                                               // augmentation.py:51-52 returns first
     if (lss_status rc = lss_prepass_run(e, d_points, d_off, d_cloud_counts, h_cloud_offsets, B, delta, noise_floor,
                                         flat_earth, 1, 0, io, ws + L.prepass, L.prepass_bytes, &cp_ptr, st))
         return rc;

@@ -309,11 +309,13 @@ class SnowfallEngine:
 
     def wet_ground_batch(self, points, cloud_offsets, counts=None, water_height=0.001, pavement_depth=0.0012,
                          noise_floor=0.7, power_factor=15, flat_earth=False, delta=0.5, replace=True, plane=None,
-                         want_intensity64=False, ymins=None, out=None):
+                         want_intensity64=False, ymins=None, out=None, want_fits=False):
         """
         Batched ground_water_augmentation() on device-resident clouds (current stream, no synchronisation).
         counts: optional CUDA int32 (B,) valid rows per cloud slot (fused snow -> wet path).
-        Returns dict(points (N,5) float32 slot-compacted, counts (B,), passthrough (B,), plane (B,4) [, intensity64]).
+        Returns dict(points (N,5) float32 slot-compacted, counts (B,), passthrough (B,), plane (B,4) [, intensity64]
+        [, fits (B,8) float64, picks (B,50) int32 with want_fits, laid out as in noise_threshold_poly]).
+        passthrough: 0 augmented, 1 fewer than 1000 ground points, 2 degenerate I/cos range (check() raises ValueError).
         """
         off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
         B = off.shape[0] - 1
@@ -331,6 +333,9 @@ class SnowfallEngine:
                            plane=torch.empty((B, 4), dtype=torch.float64, device=self.device))
             if want_intensity64 and 'intensity64' not in out:
                 out['intensity64'] = torch.empty((N,), dtype=torch.float64, device=self.device)
+            if want_fits and 'fits' not in out:
+                out.update(fits=torch.empty((B, 8), dtype=torch.float64, device=self.device),
+                           picks=torch.empty((B, 50), dtype=torch.int32, device=self.device))
             need = self.lib.lss_wet_ground_workspace_bytes(N, B)
             if getattr(self, '_ws_wet', None) is None or self._ws_wet.numel() < need:
                 self._ws_wet = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
@@ -339,7 +344,8 @@ class SnowfallEngine:
                 float(noise_floor), float(power_factor), 1 if flat_earth else 0, float(delta), 1 if replace else 0,
                 _ptr(pl), _ptr(ym), _ptr(out['points']), _ptr(out.get('intensity64')) if want_intensity64 else None,
                 _ptr(out['counts']),
-                _ptr(out['passthrough']), _ptr(out['plane']), _ptr(self._ws_wet), int(self._ws_wet.numel()),
+                _ptr(out['passthrough']), _ptr(out['plane']), _ptr(out.get('fits')) if want_fits else None,
+                _ptr(out.get('picks')) if want_fits else None, _ptr(self._ws_wet), int(self._ws_wet.numel()),
                 self._stream())
         _lib.check(st, self.h)
         return out

@@ -12,6 +12,7 @@ import pytest
 import torch
 
 from lidar_snow_sim_b200.synthetic import synthetic_cloud
+from wet_model import range32, restate as restate_model
 
 pytestmark = pytest.mark.gpu
 
@@ -19,29 +20,9 @@ H = -6.0                        # plane (0, 0, -1), h = -6: ground is -6.5 < z <
 PLANE = np.array([[0.0, 0.0, -1.0, H]])
 
 
-def range32(p):
-    x, y, z = (p[:, k].astype(np.float32) for k in range(3))
-    return np.sqrt((x * x + y * y) + z * z).astype(np.float64)
-
-
 def restate(pc, plane=PLANE[0]):
-    """The device's ground mask, range, I/cos and histogram picks in NumPy (snowfall path: float32 range)."""
-    x, y, z = (pc[:, k].astype(np.float64) for k in range(3))
-    pw = (x * plane[0] + y * plane[1]) + z * plane[2]
-    hgt = pw + plane[3]
-    ground = (hgt < 0.5) & (hgt > -0.5)
-    d = range32(pc)[ground]
-    with np.errstate(divide='ignore', invalid='ignore'):
-        c = pw[ground] / (d * np.sqrt(plane[0] ** 2 + plane[1] ** 2 + plane[2] ** 2))
-        c = np.where((c >= -1) & (c <= 1), c, np.nan)
-        norm = pc[ground, 3].astype(np.float64) / c
-    n_ground = int(ground.sum())
-    ymax = abs(np.nanmax(norm)) if n_ground else 0.0
-    if n_ground < 3:
-        return n_ground, ymax, np.full(50, -1, np.int32), d, norm
-    hist = np.histogram2d(d, norm, bins=[np.linspace(10, 70, 51), np.linspace(5, ymax, 2556)])[0]
-    hist[hist == 0] = n_ground
-    return n_ground, ymax, hist.argmin(axis=1).astype(np.int32), d, norm
+    """The device's ground mask, range, I/cos and histogram picks (snowfall path: float32 range, delta 0.5)."""
+    return restate_model(pc, plane, delta=0.5, range64_=False, flat_earth=False)
 
 
 def exact_row(dist, intensity=None, norm=None):
