@@ -552,6 +552,43 @@ LSS_API lss_status lss_sample_particles(lss_engine *e, int n_planes, double occu
                                 void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_sample_particles_workspace_bytes(int n_planes, int64_t n_candidates);
 
+/* PA-AUG (lib/pa_aug/part_aware_augmentation.py; DenseDataset's PA_AUG_STRING block) on a batch of device-resident
+ * clouds, in two calls around the host planner (lidar_snow_sim_b200/pa_aug/plan.py), which replays the reference's
+ * random draws on the member counts the first call produces.  Both calls take the same workspace, which carries the
+ * partition from the first call to the second.
+ *   d_points        float32 (N, n_features), n_features >= 3 (== 4 to apply); cloud b at rows h_cloud_offsets[b].. (the first
+ *                   d_cloud_counts[b] rows, or the slot, when d_cloud_counts is NULL)
+ *   d_planes        float64 [boxes][9][6][4]: per box its six face planes then its parts' (n0, n1, n2, d), in the
+ *                   boxes' dtype (float32 values are exact in float64); boxes_f64 != 0 tests in float64, else float32
+ *   d_nparts        int32 [boxes]: 8 or 4 parts;  h_box_offsets: int64 [B + 1], at most 256 boxes per cloud
+ *   d_class_totals  int32 [8 * boxes + B] out: rows of every (box, part), cloud b's classes at 8 * h_box_offsets[b] + b,
+ *                   class 8 * j + k for part k of box j, class 8 * M_b for the rows in no box
+ * lss_pa_apply_batch: d_class_start int64 [8 * boxes + B], the exclusive scan of the totals over the batch (n_members
+ * their sum).  Segment tables int64 [.][6] (kind 0 members of class ref / 1 FPS-selected rows from row ref / 2 noise
+ * rows from row ref, rows, first destination row ascending, first step, steps); steps float64 [.][12] (op 1 sub, 2 add,
+ * 3 mul, 4 div by params[0..2], 5 rotate out_k = (p0 m[0][k] + p1 m[1][k]) + p2 m[2][k], 6 add the normals rows from
+ * params[0], all four columns; compute in float64 != 0; store in float64 != 0; 9 params).  d_fps_segs fill the
+ * n_fps_rows rows the FPS jobs (int64 [.][5]: first row, rows, K, start, first output row) read; d_segs fill d_out,
+ * n_out rows of (x, y, z, intensity), float64 if out_f64 else float32.                                               */
+LSS_API int64_t lss_pa_partition_workspace_bytes(const int64_t *h_cloud_offsets, const int64_t *h_box_offsets,
+                                                 int n_clouds);
+LSS_API lss_status lss_pa_partition_batch(lss_engine *e, const float *d_points, int n_features,
+                                          const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts, int n_clouds,
+                                          const double *d_planes, const int32_t *d_nparts, const int64_t *h_box_offsets,
+                                          int boxes_f64, int32_t *d_class_totals, void *d_workspace,
+                                          int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_pa_apply_workspace_bytes(const int64_t *h_cloud_offsets, const int64_t *h_box_offsets, int n_clouds,
+                                             int64_t n_members, int64_t n_fps_rows, int64_t n_fps_out);
+LSS_API lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int n_features,
+                                      const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts, int n_clouds,
+                                      const double *d_planes, const int32_t *d_nparts, const int64_t *h_box_offsets,
+                                      int boxes_f64, const int64_t *d_class_start, int64_t n_members,
+                                      const int64_t *d_fps_segs, int n_fps_segs, int64_t n_fps_rows,
+                                      const int64_t *d_fps_jobs, int n_fps_jobs, int64_t n_fps_out,
+                                      const int64_t *d_segs, int n_segs, const double *d_steps, const double *d_noise,
+                                      const double *d_normals, int64_t n_out, void *d_out, int out_f64,
+                                      void *d_workspace, int64_t workspace_bytes, void *stream);
+
 /* Optional per-kernel timing for bench.py's roofline: when enabled every kernel launch is bracketed by CUDA events
  * on the launching stream.  lss_kernel_times() (call after synchronising) accumulates and returns, per kernel id
  * 0..n-1 (names via lss_kernel_name), total milliseconds and number of launches; reset != 0 clears the totals.     */

@@ -117,6 +117,12 @@ SIGNATURES = [
     ('lss_strongest_last_batch_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int]),
     ('lss_camera_fov_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_camera_fov_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_pa_partition_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int]),
+    ('lss_pa_partition_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _c.c_int, _P, _P, _c.c_int64, _P]),
+    ('lss_pa_apply_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int, _c.c_int64, _c.c_int64, _c.c_int64]),
+    ('lss_pa_apply_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _c.c_int, _P, _c.c_int64, _P,
+                                      _c.c_int, _c.c_int64, _P, _c.c_int, _c.c_int64, _P, _c.c_int, _P, _P, _P,
+                                      _c.c_int64, _P, _c.c_int, _P, _c.c_int64, _P]),
     ('lss_gather_push', _c.c_int, [_P, _P, _P, _P, _c.c_int, _c.c_int64, _c.c_int, _c.c_int, _P, _P, _P, _P, _c.c_int, _P]),
     ('lss_dart_throwing', _c.c_int, [_c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _P, _c.c_int64,
                                      _c.POINTER(_c.c_int64)]),

@@ -231,7 +231,7 @@ inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStrea
 
 enum { LSS_K_SORT = 0, LSS_K_PREPASS = 1, LSS_K_SNOWFALL = 2, LSS_K_COMPACT = 3, LSS_K_FINALIZE = 4, LSS_K_WET = 5,
        LSS_K_FOG = 6, LSS_K_SCAN = 7, LSS_K_SOLVE = 8, LSS_K_VOXEL = 9, LSS_K_DROR = 10, LSS_K_LISA = 11,
-       LSS_K_FOG_LUT = 12, LSS_K_MIE = 13, LSS_K_SELECT = 14, LSS_K_COUNT = 15 };   // 7, 8: inside the LSS_K_SNOWFALL bracket
+       LSS_K_FOG_LUT = 12, LSS_K_MIE = 13, LSS_K_SELECT = 14, LSS_K_PA = 15, LSS_K_COUNT = 16 };   // 7, 8: inside the LSS_K_SNOWFALL bracket
 
 struct KernelTimer {        // RAII: records begin/end events around the launches of its scope when profiling is on
     lss_engine *e; cudaStream_t s; int idx = -1;

@@ -669,6 +669,74 @@ class SnowfallEngine:
         _lib.check(st, self.h)
         return out
 
+    def pa_partition_batch(self, points, cloud_offsets, planes, nparts, box_offsets, boxes_f64, counts=None):
+        """
+        PA-AUG's partition (lss_pa_partition_batch, current stream, no synchronisation): which rows of every cloud lie
+        in which (box, part).  points: CUDA float32 (N, F), F >= 3; planes: CUDA float64 (M, 9, 6, 4) and nparts CUDA
+        int32 (M,) from pa_aug.plan.box_planes; box_offsets: (B + 1) host int64.  Returns the CUDA int32
+        (8 * M + B,) class totals (cloud b's classes at 8 * box_offsets[b] + b: 8 per box, then its background).
+        The partition stays in this engine's PA-AUG workspace for pa_apply_batch.
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        boff = np.ascontiguousarray(box_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.dim() == 2
+        assert points.shape[0] == int(off[-1]) and boff.shape == off.shape
+        M = int(boff[-1])
+        assert planes.is_cuda and planes.dtype == torch.float64 and planes.shape[0] == M and nparts.shape == (M,)
+        if counts is not None:
+            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        need = self.lib.lss_pa_partition_workspace_bytes(_ptr(off), _ptr(boff), B)
+        if need < 0:
+            raise ValueError('bad cloud_offsets / box_offsets (at most 256 boxes per cloud)')
+        with torch.cuda.device(self.device):
+            totals = torch.empty((8 * M + B,), dtype=torch.int32, device=self.device)
+            if getattr(self, '_ws_pa', None) is None or self._ws_pa.numel() < need:
+                self._ws_pa = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            self._pa_part_bytes = int(need)
+            st = self.lib.lss_pa_partition_batch(self.h, _ptr(points), int(points.shape[1]), _ptr(off), _ptr(counts), B,
+                                                 _ptr(planes), _ptr(nparts), _ptr(boff), 1 if boxes_f64 else 0,
+                                                 _ptr(totals), _ptr(self._ws_pa), int(self._ws_pa.numel()),
+                                                 self._stream())
+        _lib.check(st, self.h)
+        return totals
+
+    def pa_apply_batch(self, points, cloud_offsets, planes, nparts, box_offsets, boxes_f64, class_start, n_members,
+                       fps_segs, n_fps_rows, fps_jobs, n_fps_out, segs, steps, noise, normals, n_out, out_dtype,
+                       counts=None):
+        """
+        PA-AUG's row work after the plan (lss_pa_apply_batch, current stream, no synchronisation), on the partition the
+        last pa_partition_batch of this engine left: member lists, the FPS of the thinned parts, the output rows.
+        Plan tables: CUDA tensors as include/lidar_snow_sim.h describes them.  Returns CUDA (n_out, 4) out_dtype
+        (torch.float32 or torch.float64).
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        boff = np.ascontiguousarray(box_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        assert out_dtype in (torch.float32, torch.float64)
+        for t in (class_start, fps_segs, fps_jobs, segs):
+            assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
+        for t in (steps, noise, normals):
+            assert t.is_cuda and t.dtype == torch.float64 and t.is_contiguous()
+        need = self.lib.lss_pa_apply_workspace_bytes(_ptr(off), _ptr(boff), B, int(n_members), int(n_fps_rows),
+                                                     int(n_fps_out))
+        if need < 0:
+            raise ValueError('bad PA-AUG plan sizes')
+        with torch.cuda.device(self.device):
+            if self._ws_pa.numel() < need:                        # keep the partition: it lives at the front
+                ws = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+                ws[:self._pa_part_bytes].copy_(self._ws_pa[:self._pa_part_bytes])
+                self._ws_pa = ws
+            out = torch.empty((int(n_out), 4), dtype=out_dtype, device=self.device)
+            st = self.lib.lss_pa_apply_batch(
+                self.h, _ptr(points), int(points.shape[1]), _ptr(off), _ptr(counts), B, _ptr(planes), _ptr(nparts),
+                _ptr(boff), 1 if boxes_f64 else 0, _ptr(class_start), int(n_members), _ptr(fps_segs),
+                int(fps_segs.shape[0]), int(n_fps_rows), _ptr(fps_jobs), int(fps_jobs.shape[0]), int(n_fps_out),
+                _ptr(segs), int(segs.shape[0]), _ptr(steps), _ptr(noise), _ptr(normals), int(n_out), _ptr(out),
+                1 if out_dtype == torch.float64 else 0, _ptr(self._ws_pa), int(self._ws_pa.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out
+
     def gather_push(self, points, counts, d_cloud_offsets, n_rows, world, rank, peer_points, peer_counts, mc_points=0,
                     mc_counts=0, blocks=0):
         """lss_gather_push on the current stream: write the kept rows of this rank's slot-compacted batch (+ counts) into

@@ -296,3 +296,34 @@ def point_selection_batch(points, cloud_offsets, dataset_cfg, img_shapes=None, l
         import torch
         res['counts'] = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
     return res
+
+
+def pa_aug_block(data_dict, dataset_cfg, training=True, engine=None):
+    """DenseDataset.__getitem__'s PA_AUG_STRING block (dense_dataset.py:938-949) on the engine, literally: class names
+    ['Car', 'Pedestrian', 'Cyclist'], gt_names from the boxes' last column, the rows replaced by the float64 result and
+    gt_boxes filtered by the mask.  It runs after prepare_data, so its rows never reach the voxels (INTEGRATION.md)."""
+    from ..pa_aug import CLASS_NAMES, PartAwareAugmentation
+    if training and 'PA_AUG_STRING' in dataset_cfg:
+        gt_names = np.asarray([CLASS_NAMES[int(c) - 1] for c in data_dict['gt_boxes'][:, -1]])
+        pa_aug = PartAwareAugmentation(data_dict['points'], data_dict['gt_boxes'], gt_names, CLASS_NAMES,
+                                       engine=engine)
+        data_dict['points'], gt_boxes_mask = pa_aug.augment(pa_aug_param=dataset_cfg['PA_AUG_STRING'])
+        data_dict['gt_boxes'] = data_dict['gt_boxes'][gt_boxes_mask]
+    return data_dict
+
+
+def pa_aug_block_batch(points, cloud_offsets, gt_boxes, box_offsets, dataset_cfg, training=True, counts=None,
+                       out_dtype=None, engine=None):
+    """pa_aug_block on B device-resident clouds (pa_aug_batch), in batch order.  Returns dict(points, offsets, counts,
+    gt_boxes: the kept boxes of every cloud, box_offsets), or None when the block does not run (not training, or no
+    PA_AUG_STRING)."""
+    import torch
+    from ..pa_aug import pa_aug_batch
+    if not (training and 'PA_AUG_STRING' in dataset_cfg):
+        return None
+    r = pa_aug_batch(points, cloud_offsets, gt_boxes, box_offsets, dataset_cfg['PA_AUG_STRING'], counts=counts,
+                     out_dtype=out_dtype or torch.float32, engine=engine)
+    keep = np.concatenate([np.asarray(m, bool).reshape(-1) for m in r['gt_boxes_mask']] + [np.zeros(0, bool)])
+    r['gt_boxes'] = gt_boxes[torch.from_numpy(keep).to(gt_boxes.device) if isinstance(gt_boxes, torch.Tensor) else keep]
+    r['box_offsets'] = np.concatenate([[0], np.cumsum([int(np.sum(m)) for m in r['gt_boxes_mask']])]).astype(np.int64)
+    return r
