@@ -137,6 +137,22 @@ LSS_API lss_status lss_snowfall_batch(lss_engine *e, int table_id, const float *
                               double noise_floor, uint32_t flags, float *d_out_points,
                               int32_t *d_out_counts, double *d_out_stats, float *d_out_full, int32_t *d_out_perm,
                               int32_t *d_out_nocc, void *d_workspace, int64_t workspace_bytes, void *stream);
+/* lss_snowfall_batch on slot-compacted input (the output of lss_camera_fov_batch, lss_lisa_cloud_batch, lss_dror_batch,
+ * ...): the same arguments plus
+ *   d_cloud_counts   int32[n_clouds] device or NULL: cloud b is rows h_cloud_offsets[b] .. h_cloud_offsets[b] + count[b];
+ *                                         NULL: the whole slot (= lss_snowfall_batch, which forwards here)
+ * Rows past a cloud's count are absent: the pre-pass, the beam kernels, the keep decision, the channel sort, the
+ * outputs and the stats ignore them, and they may hold anything (NaN included).  A count of 0 is an empty cloud.  The
+ * output layout is unchanged: each cloud's kept rows go to the front of its own slot.  d_theta and the debug views
+ * stay in input order; what they hold for rows past the count is unspecified.                                       */
+LSS_API lss_status lss_snowfall_batch_slots(lss_engine *e, int table_id, const float *d_points,
+                                            const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts, int n_clouds,
+                                            const int32_t *h_order, double beam_divergence_deg, const float *d_theta,
+                                            const double *h_thresh_poly, const double *h_plane_in,
+                                            const int32_t *h_ymins_in, double noise_floor, uint32_t flags,
+                                            float *d_out_points, int32_t *d_out_counts, double *d_out_stats,
+                                            float *d_out_full, int32_t *d_out_perm, int32_t *d_out_nocc,
+                                            void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_snowfall_workspace_bytes(int64_t n_total, int n_clouds);
 /* Host-to-host batched augment(): the reference's call shape (numpy cloud in -> numpy cloud out,
  * simulation.py:427-544) for a batch.  h_points / h_out_* are HOST buffers (page-locked memory gives full PCIe speed;
@@ -230,6 +246,21 @@ LSS_API lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, co
                                 double *d_out_intensity64, int32_t *d_out_counts, int32_t *d_out_passthrough,
                                 double *d_out_plane, double *d_out_fit, int32_t *d_out_ymins, void *d_workspace,
                                 int64_t workspace_bytes, void *stream);
+/* lss_wet_ground_batch with one water height per cloud (the dataset draws one per sample):
+ *   h_water_height    float64[n_clouds] host, replacing the scalar water_height; f = clip(h / pavement_depth, 0, 1) per
+ *                     cloud, in lss_wet_ground_batch's expression (which forwards here with its height for every cloud)
+ * Everything else as lss_wet_ground_batch, with one difference: a cloud with a degenerate I/cos range is reported in
+ * d_out_passthrough as 2 and returned unchanged, and NO error is latched (the dataset swallows that ValueError per
+ * sample, dense_dataset.py:834-837; latched, it would surface at the caller's next unrelated lss_check_async).      */
+LSS_API lss_status lss_wet_ground_batch_params(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
+                                               const int32_t *d_cloud_counts, int n_clouds,
+                                               const double *h_water_height, double pavement_depth,
+                                               double noise_floor, double power_factor, int flat_earth, double delta,
+                                               int replace, const double *h_plane_in, const int32_t *h_ymins_in,
+                                               float *d_out_points, double *d_out_intensity64, int32_t *d_out_counts,
+                                               int32_t *d_out_passthrough, double *d_out_plane, double *d_out_fit,
+                                               int32_t *d_out_ymins, void *d_workspace, int64_t workspace_bytes,
+                                               void *stream);
 LSS_API int64_t lss_wet_ground_workspace_bytes(int64_t n_total, int n_clouds);
 
 /* ---- fog simulation ("next" row, SURVEY.md 8f-3) -----------------------------------------------------------------------

@@ -71,6 +71,8 @@ SIGNATURES = [
                                   _c.POINTER(_c.c_int64)]),
     ('lss_snowfall_batch', _c.c_int, [_P, _c.c_int, _P, _P, _c.c_int, _P, _c.c_double, _P, _P, _P, _P, _c.c_double,
                                       _c.c_uint32, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_snowfall_batch_slots', _c.c_int, [_P, _c.c_int, _P, _P, _P, _c.c_int, _P, _c.c_double, _P, _P, _P, _P,
+                                            _c.c_double, _c.c_uint32, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_snowfall_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_host_pipe_trace', _c.c_int, [_P, _P, _c.c_int]),
     ('lss_snowfall_batch_host', _c.c_int, [_P, _c.c_int, _P, _P, _c.c_int, _P, _c.c_double, _P, _c.c_double, _c.c_uint32,
@@ -89,6 +91,9 @@ SIGNATURES = [
     ('lss_wet_ground_batch', _c.c_int, [_P, _P, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _c.c_double,
                                         _c.c_int, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                         _c.c_int64, _P]),
+    ('lss_wet_ground_batch_params', _c.c_int, [_P, _P, _P, _P, _c.c_int, _P, _c.c_double, _c.c_double, _c.c_double,
+                                               _c.c_int, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                               _P, _c.c_int64, _P]),
     ('lss_wet_ground_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_fog_batch', _c.c_int, [_P, _P, _c.c_int, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _P, _c.c_uint32,
                                  _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),

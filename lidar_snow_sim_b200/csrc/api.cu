@@ -248,6 +248,20 @@ lss_status lss_snowfall_batch(lss_engine *e, int table_id, const float *d_points
                               int32_t *d_out_counts, double *d_out_stats, float *d_out_full, int32_t *d_out_perm,
                               int32_t *d_out_nocc, void *d_workspace, int64_t workspace_bytes, void *stream)
 {
+    return lss_snowfall_batch_slots(e, table_id, d_points, h_cloud_offsets, nullptr, n_clouds, h_order,
+                                    beam_divergence_deg, d_theta, h_thresh_poly, h_plane_in, h_ymins_in, noise_floor,
+                                    flags, d_out_points, d_out_counts, d_out_stats, d_out_full, d_out_perm, d_out_nocc,
+                                    d_workspace, workspace_bytes, stream);
+}
+
+lss_status lss_snowfall_batch_slots(lss_engine *e, int table_id, const float *d_points, const int64_t *h_cloud_offsets,
+                                    const int32_t *d_cloud_counts, int n_clouds, const int32_t *h_order,
+                                    double beam_divergence_deg, const float *d_theta, const double *h_thresh_poly,
+                                    const double *h_plane_in, const int32_t *h_ymins_in, double noise_floor,
+                                    uint32_t flags, float *d_out_points, int32_t *d_out_counts, double *d_out_stats,
+                                    float *d_out_full, int32_t *d_out_perm, int32_t *d_out_nocc, void *d_workspace,
+                                    int64_t workspace_bytes, void *stream)
+{
     if (!e) return LSS_ERR_INVALID_ARG;
     if (!h_cloud_offsets || !h_order || n_clouds < 0 || !d_out_points || !d_out_counts || !d_out_stats)
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
@@ -260,6 +274,7 @@ lss_status lss_snowfall_batch(lss_engine *e, int table_id, const float *d_points
     a.ts = &it->second;
     a.d_points = d_points;
     a.h_cloud_offsets = h_cloud_offsets;
+    a.d_cloud_counts = d_cloud_counts;
     a.n_clouds = n_clouds;
     a.h_order = h_order;
     a.beam_divergence_deg = beam_divergence_deg;

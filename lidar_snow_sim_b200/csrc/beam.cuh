@@ -1,7 +1,7 @@
 // beam.cuh -- argument block, constants and small device helpers shared by the per-beam kernels
 // (snowfall.cu: schedule / keep / scatter; solve.cu: the scan and solve kernels).
 #pragma once
-#include "common.cuh"
+#include "segments.cuh"
 
 // One beam of the solve list, written by the scan kernel (32 bytes).  The scan has already walked the beam's whole
 // bucket prefix and tested every candidate exactly, so it hands over its hits as the solve claims them (the hit
@@ -32,6 +32,7 @@ struct DevArgs {
     const float *pts;            // rows in input order
     const float *theta;          // optional, input order
     const int64_t *cloud_off;    // [B+1] device
+    const int32_t *cloud_cnt;    // [B] device valid rows per slot (seg_rows), or null: the whole slot
     const int32_t *order;        // [B*64] device
     const double *thresh;        // [B*3] device or null
     const SensorConst *sensor;
@@ -88,8 +89,13 @@ constexpr int LIST_HDR_BYTES = 1024;  // ints: [0] chunks allocated, [1] tile cu
 constexpr int LIST_CLASSES = 128;     // solve list bucketed by work class (occluder count), costliest class first
 constexpr int LIST_CHUNK = 1024;      // solve items per chunk of a class (a multiple of 32: a solve tile is in one chunk)
 // scan schedule: warp tiles counting-sorted by the plane (mod SCHED_PLANES) of their first row's channel; rows without a
-// valid channel get the last bin.  Only locality depends on the bins, never a result.
-constexpr int SCHED_PLANES = 64;
+// valid channel get the last bin.  Only locality depends on the bins, never a result.  A stack of S table sets (plane
+// 64 s + p is plane p of set s) shares the 64 bins; -DLSS_SCHED_PLANES=64*S keys them by the stacked plane instead
+// (DESIGN.md §7.7 measured both).
+#ifndef LSS_SCHED_PLANES
+#define LSS_SCHED_PLANES 64
+#endif
+constexpr int SCHED_PLANES = LSS_SCHED_PLANES;
 constexpr int SCHED_BINS = SCHED_PLANES + 1;
 
 __device__ __forceinline__ void raise_status(int *status, int code) { atomicMax(status, code); }

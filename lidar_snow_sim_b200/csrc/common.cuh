@@ -315,6 +315,7 @@ struct SnowfallArgs {
     const TableSet *ts;
     const float *d_points;
     const int64_t *h_cloud_offsets;
+    const int32_t *d_cloud_counts = nullptr;    // device [B] valid rows per slot, or null: the whole slot
     int n_clouds;
     const int32_t *h_order;
     double beam_divergence_deg;

@@ -438,6 +438,13 @@ __device__ __forceinline__ double nan_max(double a, double b) { return (a != a |
 // (lo, hi) = intensity_edges(ymax).  ymax is the maximum of I/cos over the ground points, so I/cos <= hi holds for all of
 // them: the record needs only the range bin and I/cos (kept from 4.5 on, the lowest lo), and the intensity bin is taken
 // once ymax is known (k_ground_hist).
+// CTAs of a cloud's ground pass: a function of its own row count only, so that the cloud's sums -- and every bit
+// downstream of them -- do not depend on the other clouds of the batch (launched with enough for the largest)
+__device__ __forceinline__ int ground_blocks(int n, int launched)
+{
+    return min(launched, max(1, (n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
+}
+
 __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
 {
     __shared__ double red[15 * (PP_TPB / 32)];
@@ -446,13 +453,15 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
     const CloudPre cp = a.cp[b];
     const int64_t beg = a.cloud_off[b];
     const int n = (a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - beg));
+    const int nb = ground_blocks(n, gridDim.x);
+    if ((int)blockIdx.x >= nb) return;
     const int lane = threadIdx.x & 31;
     // 0 n, 1-4 first regression (shifted), 5-8 S t .. S t^4, 9-11 S cos t^k, 12-14 S d cos t^k
     double v[15] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
     double vmax = -1e300;
     // every thread sums its own rows in ascending order (the bits of the polynomial depend on it); the loop runs per warp
     // so that the warp can append its records together
-    for (int w0 = blockIdx.x * PP_TPB + (threadIdx.x & ~31); w0 < n; w0 += gridDim.x * PP_TPB) {
+    for (int w0 = blockIdx.x * PP_TPB + (threadIdx.x & ~31); w0 < n; w0 += nb * PP_TPB) {
         const int i = w0 + lane;
         GroundPt g;
         g.ground = false;
@@ -539,7 +548,8 @@ __global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_block
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (warp == 0) {
         double v[15], vmax;
-        warp_reduce_partials<15>(a.partial + (size_t)b * a.max_blocks * 16, n_blocks, v, &vmax);
+        const int n = a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - a.cloud_off[b]);
+        warp_reduce_partials<15>(a.partial + (size_t)b * a.max_blocks * 16, ground_blocks(n, n_blocks), v, &vmax);
         if (lane == 0) {
             stat[0] = v[0];
             stat[1] = fabs(vmax);

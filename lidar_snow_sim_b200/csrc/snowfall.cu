@@ -37,19 +37,22 @@ namespace {
 // ---------------------------------------------------------------------------------------------------------------------
 constexpr int SCHED_KEY_TPB = 128;
 
+// Every warp tile of the slot gets an entry (the schedule has one per slot tile); a tile past the cloud's count has no
+// rows for the scan and takes the last bin.
 __global__ void __launch_bounds__(SCHED_KEY_TPB) k_sched_key(const float *__restrict__ pts, const int64_t *__restrict__ cloud_off,
+                                                            const int32_t *__restrict__ cloud_cnt,
                                                             const int32_t *__restrict__ order, const int32_t *__restrict__ wtile_base,
                                                             unsigned long long *ent, int *hist)
 {
     const int b = blockIdx.y, t = blockIdx.x * SCHED_KEY_TPB + threadIdx.x;
     const int64_t beg = cloud_off[b];
-    const int n = (int)(cloud_off[b + 1] - beg);
-    if (blockIdx.x * SCHED_KEY_TPB * 32 >= n) return;
+    const int n_slot = (int)(cloud_off[b + 1] - beg);
+    if (blockIdx.x * SCHED_KEY_TPB * 32 >= n_slot) return;
     const int w0 = 32 * t;
-    const bool on = w0 < n;
+    const bool on = w0 < n_slot;
     int bin = -1;
     if (on) {
-        const int ch = channel_bin(pts[(beg + w0) * 5 + 4]);
+        const int ch = w0 < seg_rows(cloud_off, cloud_cnt, b) ? channel_bin(pts[(beg + w0) * 5 + 4]) : LSS_N_CHANNELS;
         bin = ch < LSS_N_CHANNELS ? order[b * LSS_N_CHANNELS + ch] % SCHED_PLANES : SCHED_PLANES;
         ent[wtile_base[b] + t] = ((unsigned long long)bin << 48) | ((unsigned long long)b << 32) | (unsigned)w0;
     }
@@ -131,8 +134,9 @@ __global__ void __launch_bounds__(KEEP_TPB) k_keep(DevArgs a)
     __shared__ int s_cnt[2];
     const int b = blockIdx.y, tile = blockIdx.x;
     const int64_t beg = a.cloud_off[b];
-    const int n = (int)(a.cloud_off[b + 1] - beg);
-    if (tile * TILE >= n) return;
+    // every tile of the slot writes its histogram rows (k_tile_scan reads them all); rows past the count are absent
+    if (tile * TILE >= (int)(a.cloud_off[b + 1] - beg)) return;
+    const int n_tile = seg_rows(a.cloud_off, a.cloud_cnt, b) - tile * TILE;     // valid rows from the tile's first on
     if (threadIdx.x < NBINS) { h_keep[threadIdx.x] = 0; h_all[threadIdx.x] = 0; }
     if (threadIdx.x < 2) s_cnt[threadIdx.x] = 0;
     const bool thr_on = a.flags & LSS_FLAG_THRESHOLD_FILTER;
@@ -142,7 +146,7 @@ __global__ void __launch_bounds__(KEEP_TPB) k_keep(DevArgs a)
     for (int k = 0; k < KEEP_ROWS; k++) {
         const int i = tile * TILE + k * KEEP_TPB + threadIdx.x;
         tags[k] = 0; d32s[k] = 0.0f; out_is[k] = 0.0f;
-        if (i < n) {
+        if (k * KEEP_TPB + (int)threadIdx.x < n_tile) {
             tags[k] = __ldcs(a.keep_tag + beg + i);
             if (thr_on) { d32s[k] = __ldcs(a.keep_d + beg + i); out_is[k] = __ldcs(a.keep_i + beg + i); }
         }
@@ -154,7 +158,7 @@ __global__ void __launch_bounds__(KEEP_TPB) k_keep(DevArgs a)
 #pragma unroll
     for (int k = 0; k < KEEP_ROWS; k++) {
         const int i = tile * TILE + k * KEEP_TPB + threadIdx.x;
-        const bool active = i < n;
+        const bool active = k * KEEP_TPB + (int)threadIdx.x < n_tile;
         bool keep = false, att = false;
         int ch = -1;
         if (active) {
@@ -287,6 +291,7 @@ __global__ void __launch_bounds__(1024) k_tile_scan(unsigned *hist, const int32_
 __global__ void __launch_bounds__(TILE) k_scatter(const float *__restrict__ aug, const uint8_t *__restrict__ code,
                                                    const unsigned *__restrict__ tile_off,
                                                    const int64_t *__restrict__ cloud_off,
+                                                   const int32_t *__restrict__ cloud_cnt,
                                                    const int32_t *__restrict__ tile_base,
                                                    float *__restrict__ out, const int32_t *__restrict__ nocc_in,
                                                    int32_t *__restrict__ nocc_out, int32_t *__restrict__ perm_out)
@@ -294,7 +299,7 @@ __global__ void __launch_bounds__(TILE) k_scatter(const float *__restrict__ aug,
     __shared__ unsigned warp_cnt[TILE / 32][NBINS];
     const int b = blockIdx.y, tile = blockIdx.x;
     const int64_t beg = cloud_off[b];
-    const int n = (int)(cloud_off[b + 1] - beg);
+    const int n = seg_rows(cloud_off, cloud_cnt, b);
     const int i = tile * TILE + threadIdx.x;
     if (tile * TILE >= n) return;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -461,6 +466,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.pts = s.d_points;
     a.theta = s.d_theta;
     a.cloud_off = d_off;
+    a.cloud_cnt = s.d_cloud_counts;
     a.order = d_order;
     a.thresh = d_thresh;
     a.sensor = e->d_sensor;
@@ -506,7 +512,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
         io.h_plane_in = s.h_plane_in;
         io.h_ymins_in = s.h_ymins_in;
         io.d_poly_out = d_thresh;
-        lss_status ps = lss_prepass_run(e, s.d_points, d_off, nullptr, s.h_cloud_offsets, B, 0.5, s.noise_floor, 0, 0, 1,
+        lss_status ps = lss_prepass_run(e, s.d_points, d_off, s.d_cloud_counts, s.h_cloud_offsets, B, 0.5, s.noise_floor, 0, 0, 1,
                                 io, ws + w.prepass, w.prepass_bytes, nullptr, side);
         const cudaError_t je = cudaEventRecord(ev_join, side);
         if (ps != LSS_OK || je != cudaSuccess) {
@@ -528,7 +534,8 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             unsigned long long *d_sched = d_ent + w.sched_tiles;
             const int max_wtiles = (int)((max_n + 31) / 32);
             ce = lss_launch(e, k_sched_key, dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B),
-                            SCHED_KEY_TPB, 0, stream, s.d_points, d_off, d_order, d_tile_base + B + 1, d_ent, d_sched_hist);
+                            SCHED_KEY_TPB, 0, stream, s.d_points, d_off, s.d_cloud_counts, d_order, d_tile_base + B + 1,
+                            d_ent, d_sched_hist);
             if (ce == cudaSuccess)
                 ce = lss_launch(e, k_sched_sort, (unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)),
                                 256, 0, stream, d_ent, d_sched, d_sched_hist, n_wtiles);
@@ -559,14 +566,14 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     {
         KernelTimer kt(e, LSS_K_COMPACT, stream);
         LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, d_aug, d_code_keep, d_hist_keep, d_off,
-                                     d_tile_base, s.d_out_points, nullptr, nullptr, nullptr));
+                                     s.d_cloud_counts, d_tile_base, s.d_out_points, nullptr, nullptr, nullptr));
     }
     if (want_all) {     // un-filtered, channel-sorted debug views (tests): full rows, original index, occluder counts
         KernelTimer kt(e, LSS_K_COMPACT, stream);
         LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, d_hist_all, d_tile_base, nullptr, nullptr, nullptr,
                                      nullptr, nullptr, nullptr));
         LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, d_aug, d_code_all, d_hist_all, d_off,
-                                     d_tile_base, s.d_out_full, d_nocc_tmp, s.d_out_nocc, s.d_out_perm));
+                                     s.d_cloud_counts, d_tile_base, s.d_out_full, d_nocc_tmp, s.d_out_nocc, s.d_out_perm));
     }
     return LSS_OK;
 }

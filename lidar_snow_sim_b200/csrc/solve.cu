@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     const unsigned long long se = a.sched[st];
     const int b = (int)((se >> 32) & 0xffffu), w0 = (int)(unsigned)se;  // cloud, first row of this warp
     const int64_t beg = a.cloud_off[b];
-    const int n = (int)(a.cloud_off[b + 1] - beg);
+    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);            // a tile past the count: no lane active, nothing moved
     const int i = w0 + lane;
     const bool active = i < n;
     const int nf_w = min(32, n - w0) * 5;                           // floats of this warp's rows

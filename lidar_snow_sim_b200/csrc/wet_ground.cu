@@ -7,10 +7,15 @@
 //                           output order of the reference: all non-ground rows first, then the kept ground rows
 //                           (augmentation.py:150-159), column 4 rewritten; stable, tile parallel (segments.cuh)
 //
-// All per-point physics in float64, as the reference (its ground array is float64, augmentation.py:50).
+// All per-point physics in float64, as the reference (its ground array is float64, augmentation.py:50).  The wet fraction
+// f = clip(water_height / pavement_depth, 0, 1) is one value per cloud (lss_wet_ground_batch_params).
 // A cloud with fewer than 1000 ground points is passed through unchanged (augmentation.py:51-52).  So is one whose
-// I/cos range is degenerate, where the reference raises ValueError (augmentation.py:232-233): the pre-pass latches
-// LSS_ERR_INTENSITY_RANGE and the other clouds of the batch are augmented as usual.
+// I/cos range is degenerate, where the reference raises ValueError (augmentation.py:232-233): lss_wet_ground_batch
+// latches LSS_ERR_INTENSITY_RANGE for it, lss_wet_ground_batch_params only reports it; the other clouds of the batch
+// are augmented as usual.
+#include <climits>
+#include <vector>
+
 #include "segments.cuh"
 
 namespace {
@@ -23,7 +28,8 @@ struct WetArgs {
     const int64_t *cloud_off;
     const int32_t *cloud_cnt;     // optional (slot-compacted input)
     const CloudPre *cp;
-    double delta, noise_floor, power_factor, f_wet;   // f = clip(water_height / pavement_depth, 0, 1)
+    double delta, noise_floor, power_factor;
+    const double *f_wet;          // [B] f = clip(water_height / pavement_depth, 0, 1) per cloud
     int flat_earth, replace;
     uint8_t *cls;                 // [N] 0 = not ground, 1 = ground kept, 2 = ground dropped
     double *new_i;                // [N] new intensity of ground points (float64)
@@ -71,6 +77,7 @@ __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
     const int64_t beg = a.cloud_off[b];
     const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
     const bool pass = wet_passthrough(cp) != 0;
+    const double f_wet = a.f_wet[b];
     for (int i = blockIdx.x * WET_TPB + threadIdx.x; i < n; i += gridDim.x * WET_TPB) {
         const float *r = a.pts + (beg + i) * 5;
         const double x = r[0], y = r[1], z = r[2], inten = r[3];
@@ -91,7 +98,7 @@ __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
             const double ts = f1.ts * rho * f2.ts / (1 - rho * f2.rs);                          // :86
             const double tp = f1.tp * rho * f2.tp / (1 - rho * f2.rp);                          // :89
             const double t = fmax(tp, ts);                                                      // augmentation.py:119
-            const double tw = (1 - a.f_wet) * refl + a.f_wet * t / ang;                         // :123
+            const double tw = (1 - f_wet) * refl + f_wet * t / ang;                             // :123
             double ni = rel_out * ca * tw;                                                      // :126
             ni = ni < 0 ? 0 : (ni > inten ? inten : ni);
             const double thr = noise * ca;
@@ -134,13 +141,14 @@ __global__ void __launch_bounds__(WET_TILE) k_wet_scatter(WetArgs a)
     }
 }
 
-struct WetLayout { int64_t off, cls, new_i, seg, seg_total, prepass, prepass_bytes, total; };
+struct WetLayout { int64_t off, f_wet, cls, new_i, seg, seg_total, prepass, prepass_bytes, total; };
 
 WetLayout wet_layout(int64_t n_total, int n_clouds)
 {
     WetLayout L;
     int64_t o = 0;
     L.off = o;      o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
+    L.f_wet = o;    o = align_up(o + (int64_t)n_clouds * 8, 256);
     L.cls = o;      o = align_up(o + n_total, 256);
     L.new_i = o;    o = align_up(o + n_total * 8, 256);
     L.seg = o;      o += seg_ws_bytes(n_total, n_clouds, WET_TILE, 2);
@@ -151,23 +159,14 @@ WetLayout wet_layout(int64_t n_total, int n_clouds)
     return L;
 }
 
-}  // namespace
-
-extern "C" {
-
-int64_t lss_wet_ground_workspace_bytes(int64_t n_total, int n_clouds)
-{
-    if (n_total < 0 || n_clouds < 0) return -1;
-    return wet_layout(n_total, n_clouds).total;
-}
-
-lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
-                                const int32_t *d_cloud_counts, int n_clouds, double water_height, double pavement_depth,
-                                double noise_floor, double power_factor, int flat_earth, double delta, int replace,
-                                const double *h_plane_in, const int32_t *h_ymins_in, float *d_out_points,
-                                double *d_out_intensity64, int32_t *d_out_counts, int32_t *d_out_passthrough,
-                                double *d_out_plane, double *d_out_fit, int32_t *d_out_ymins, void *d_workspace,
-                                int64_t workspace_bytes, void *stream)
+// latch_range: latch LSS_ERR_INTENSITY_RANGE for a cloud of >= 1000 ground points with a degenerate I/cos range
+lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
+                          const int32_t *d_cloud_counts, int n_clouds, const double *h_water_height,
+                          double pavement_depth, double noise_floor, double power_factor, int flat_earth, double delta,
+                          int replace, const double *h_plane_in, const int32_t *h_ymins_in, float *d_out_points,
+                          double *d_out_intensity64, int32_t *d_out_counts, int32_t *d_out_passthrough,
+                          double *d_out_plane, double *d_out_fit, int32_t *d_out_ymins, void *d_workspace,
+                          int64_t workspace_bytes, void *stream, bool latch_range)
 {
     if (!e) return LSS_ERR_INVALID_ARG;
     BatchGeometry g;
@@ -202,7 +201,7 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
     io.d_plane_out = d_out_plane;
     io.d_fit_out = d_out_fit;
     io.d_ymins_out = d_out_ymins;
-    io.range_min_ground = 1000;                                               // augmentation.py:51-52 returns first
+    io.range_min_ground = latch_range ? 1000 : INT_MAX;                       // augmentation.py:51-52 returns first
     if (lss_status rc = lss_prepass_run(e, d_points, d_off, d_cloud_counts, h_cloud_offsets, B, delta, noise_floor,
                                         flat_earth, 1, 0, io, ws + L.prepass, L.prepass_bytes, &cp_ptr, st))
         return rc;
@@ -213,8 +212,15 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
     a.delta = delta;
     a.noise_floor = noise_floor;
     a.power_factor = power_factor;
-    double f = water_height / pavement_depth;                                 // augmentation.py:122
-    a.f_wet = f < 0 ? 0 : (f > 1 ? 1 : f);
+    {
+        std::vector<double> f_wet(B);
+        for (int b = 0; b < B; b++) {
+            const double f = h_water_height[b] / pavement_depth;                // augmentation.py:122
+            f_wet[b] = f < 0 ? 0 : (f > 1 ? 1 : f);
+        }
+        LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.f_wet, f_wet.data(), sizeof(double) * B, st));
+        a.f_wet = (const double *)(ws + L.f_wet);
+    }
     a.flat_earth = flat_earth;
     a.replace = replace;
     a.cls = (uint8_t *)(ws + L.cls);
@@ -235,6 +241,47 @@ lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int6
     LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.seg));
     LSS_CUDA_CHECK(e, lss_launch(e, k_wet_scatter, dim3(max_tiles, B), WET_TILE, 0, st, a));
     return LSS_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int64_t lss_wet_ground_workspace_bytes(int64_t n_total, int n_clouds)
+{
+    if (n_total < 0 || n_clouds < 0) return -1;
+    return wet_layout(n_total, n_clouds).total;
+}
+
+lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
+                                const int32_t *d_cloud_counts, int n_clouds, double water_height, double pavement_depth,
+                                double noise_floor, double power_factor, int flat_earth, double delta, int replace,
+                                const double *h_plane_in, const int32_t *h_ymins_in, float *d_out_points,
+                                double *d_out_intensity64, int32_t *d_out_counts, int32_t *d_out_passthrough,
+                                double *d_out_plane, double *d_out_fit, int32_t *d_out_ymins, void *d_workspace,
+                                int64_t workspace_bytes, void *stream)
+{
+    const std::vector<double> heights((size_t)std::max(n_clouds, 0), water_height);
+    return wet_ground_run(e, d_points, h_cloud_offsets, d_cloud_counts, n_clouds, heights.data(), pavement_depth,
+                          noise_floor, power_factor, flat_earth, delta, replace, h_plane_in, h_ymins_in, d_out_points,
+                          d_out_intensity64, d_out_counts, d_out_passthrough, d_out_plane, d_out_fit, d_out_ymins,
+                          d_workspace, workspace_bytes, stream, true);
+}
+
+lss_status lss_wet_ground_batch_params(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
+                                       const int32_t *d_cloud_counts, int n_clouds, const double *h_water_height,
+                                       double pavement_depth, double noise_floor, double power_factor, int flat_earth,
+                                       double delta, int replace, const double *h_plane_in, const int32_t *h_ymins_in,
+                                       float *d_out_points, double *d_out_intensity64, int32_t *d_out_counts,
+                                       int32_t *d_out_passthrough, double *d_out_plane, double *d_out_fit,
+                                       int32_t *d_out_ymins, void *d_workspace, int64_t workspace_bytes, void *stream)
+{
+    if (!e) return LSS_ERR_INVALID_ARG;
+    if (!h_water_height && n_clouds > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null water heights");
+    return wet_ground_run(e, d_points, h_cloud_offsets, d_cloud_counts, n_clouds, h_water_height, pavement_depth,
+                          noise_floor, power_factor, flat_earth, delta, replace, h_plane_in, h_ymins_in, d_out_points,
+                          d_out_intensity64, d_out_counts, d_out_passthrough, d_out_plane, d_out_fit, d_out_ymins,
+                          d_workspace, workspace_bytes, stream, false);
 }
 
 }  // extern "C"

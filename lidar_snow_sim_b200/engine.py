@@ -158,11 +158,13 @@ class SnowfallEngine:
     def snowfall_batch(self, table_id, points, cloud_offsets, order, beam_divergence_deg, theta=None,
                        thresh_poly=None, plane=None, ymins=None, noise_floor=0.7, threshold_filter=True, camera_fov=False,
                        device_prepass=False, assume_sorted=False, want_full=False, want_perm=False, want_nocc=False,
-                       out=None, workspace=None):
+                       out=None, workspace=None, counts=None):
         """
         Batched augment() on device-resident clouds (enqueued on torch's current stream, no synchronisation).
 
         points: CUDA float32 (N, 5); cloud_offsets: int64 host array (B + 1); order: int32 host (B, 64).
+        counts: optional CUDA int32 (B,) valid rows per slot (slot-compacted input, lss_snowfall_batch_slots): cloud b
+        is rows cloud_offsets[b] .. cloud_offsets[b] + counts[b], and the rows behind them are ignored.
         plane (B,4) / ymins (B,50): optional host arrays replayed by the device pre-pass (lss_noise_threshold_poly).
         Returns dict(points=(N,5) slot-compacted rows, counts=(B,), stats=(B,4) [, full, perm, nocc]).
         Call `check()` (synchronises) to surface asynchronous device errors.
@@ -188,6 +190,8 @@ class SnowfallEngine:
             tp = np.ascontiguousarray(thresh_poly, dtype=np.float64).reshape(B, 3)
         if theta is not None:
             assert theta.is_cuda and theta.dtype == torch.float32 and theta.shape[0] == N
+        if counts is not None:
+            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,) and counts.is_contiguous()
         pl = None if plane is None else np.ascontiguousarray(plane, dtype=np.float64).reshape(B, 4)
         ym = None if ymins is None else np.ascontiguousarray(ymins, dtype=np.int32).reshape(B, 50)
         with torch.cuda.device(self.device):
@@ -208,8 +212,8 @@ class SnowfallEngine:
             else:
                 ws = workspace
                 assert ws.numel() >= self.lib.lss_snowfall_workspace_bytes(N, B)
-            st = self.lib.lss_snowfall_batch(
-                self.h, int(table_id), _ptr(points), _ptr(off), B, _ptr(order), float(beam_divergence_deg),
+            st = self.lib.lss_snowfall_batch_slots(
+                self.h, int(table_id), _ptr(points), _ptr(off), _ptr(counts), B, _ptr(order), float(beam_divergence_deg),
                 _ptr(theta), _ptr(tp), _ptr(pl), _ptr(ym), float(noise_floor), flags, _ptr(out['points']),
                 _ptr(out['counts']),
                 _ptr(out['stats']), _ptr(out.get('full')) if want_full else None,
@@ -313,6 +317,8 @@ class SnowfallEngine:
         """
         Batched ground_water_augmentation() on device-resident clouds (current stream, no synchronisation).
         counts: optional CUDA int32 (B,) valid rows per cloud slot (fused snow -> wet path).
+        water_height: a number, or a (B,) array of one height per cloud (lss_wet_ground_batch_params; a degenerate I/cos
+        range is then only reported as passthrough 2, and check() does not raise for it).
         Returns dict(points (N,5) float32 slot-compacted, counts (B,), passthrough (B,), plane (B,4) [, intensity64]
         [, fits (B,8) float64, picks (B,50) int32 with want_fits, laid out as in noise_threshold_poly]).
         passthrough: 0 augmented, 1 fewer than 1000 ground points, 2 degenerate I/cos range (check() raises ValueError).
@@ -339,8 +345,15 @@ class SnowfallEngine:
             need = self.lib.lss_wet_ground_workspace_bytes(N, B)
             if getattr(self, '_ws_wet', None) is None or self._ws_wet.numel() < need:
                 self._ws_wet = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_wet_ground_batch(
-                self.h, _ptr(points), _ptr(off), _ptr(counts), B, float(water_height), float(pavement_depth),
+            per_cloud = np.ndim(water_height) > 0
+            if per_cloud:
+                heights = np.ascontiguousarray(water_height, dtype=np.float64).reshape(-1)
+                if heights.shape[0] != B:
+                    raise ValueError(f'water_height: {heights.shape[0]} heights for {B} clouds')
+            call = self.lib.lss_wet_ground_batch_params if per_cloud else self.lib.lss_wet_ground_batch
+            st = call(
+                self.h, _ptr(points), _ptr(off), _ptr(counts), B, _ptr(heights) if per_cloud else float(water_height),
+                float(pavement_depth),
                 float(noise_floor), float(power_factor), 1 if flat_earth else 0, float(delta), 1 if replace else 0,
                 _ptr(pl), _ptr(ym), _ptr(out['points']), _ptr(out.get('intensity64')) if want_intensity64 else None,
                 _ptr(out['counts']),

@@ -15,6 +15,8 @@ on the device once per (mode, pair) and cached.
     aug = OnTheFlyWeather(dataset_cfg, rainfall_rates=[...])        # in DenseDataset.__init__
     points = aug(points, training=self.training)                    # replaces dense_dataset.py:749-837
 """
+import random
+
 import numpy as np
 
 from ..engine import default_engine
@@ -63,6 +65,7 @@ class OnTheFlyWeather:
                               for rs, tv in zip(DATASET_SNOWFALL_RATES, DATASET_TERMINAL_VELOCITIES)]
         self.rainfall_rates = list(rainfall_rates)
         self._tables = {}
+        self._stacks = {}
 
     def _engine(self):
         if self.engine is None:
@@ -73,30 +76,34 @@ class OnTheFlyWeather:
         key = (mode, rainfall_rate)
         if key not in self._tables:
             if rainfall_rate not in self.pairs:
-                raise FileNotFoundError(f'no (snowfall_rate, terminal_velocity) pair with rain rate {rainfall_rate}')
+                raise FileNotFoundError(_no_pair_message(rainfall_rate))
             rs, tv = self.pairs[rainfall_rate]
             self._tables[key] = self._engine().sample_tables_device(mode, rs, tv, seed=self.table_seed)
         return self._tables[key]
 
-    def __call__(self, points, training=True):
+    def _draws(self):
+        """The block's draws for one sample, in the order __call__ takes them (dense_dataset.py:750-832): the SNOW coin
+        flip and rain rate (NumPy's global generator), the channel order of an applied snow sample (random.shuffle on
+        Python's global generator, as augment takes it, simulation.py:485-486), then the WET_SURFACE coin flip or
+        COUPLED and the water height.  A rain rate without a (snowfall_rate, terminal_velocity) pair prints the
+        reference's message and is not applied (dense_dataset.py:784-786).  Returns dict(snow, mode, rainfall_rate,
+        order, wet, water_height)."""
         cfg = self.cfg
-        snowfall_augmentation_applied = False
-        if training and 'SNOW' in cfg:
+        d = dict(snow=False, mode=None, rainfall_rate=0, order=None, wet=False, water_height=None)
+        if 'SNOW' in cfg:
             sampling, mode, chance = cfg['SNOW'].split('_')[:3]
             choices = _CHANCES.get(chance, [0])
             if np.random.choice(choices):
                 rainfall_rate = 0
                 if sampling == 'uniform':
                     rainfall_rate = int(np.random.choice(self.rainfall_rates))
-                try:
-                    tid = self._table(mode, rainfall_rate)
-                    pc = np.ascontiguousarray(points[:, :5], dtype=np.float32)
-                    pc = pc[get_fov_flag(pc[:, 0:3])]                                  # precompute.py:96-99
-                    _, points = augment(pc, '', float(np.degrees(3e-3)), engine=self._engine(), tables=tid)
-                    snowfall_augmentation_applied = True
-                except FileNotFoundError as exc:                                       # dense_dataset.py:784-786
-                    print(f'\n{exc}')
-        if training and 'WET_SURFACE' in cfg:
+                if rainfall_rate in self.pairs:
+                    order = list(range(64))
+                    random.shuffle(order)
+                    d.update(snow=True, mode=mode, rainfall_rate=rainfall_rate, order=order)
+                else:
+                    print(f'\n{_no_pair_message(rainfall_rate)}')
+        if 'WET_SURFACE' in cfg:
             method = cfg['WET_SURFACE']
             choices = [0]
             if '1in2' in method:
@@ -105,7 +112,7 @@ class OnTheFlyWeather:
                 choices = [0, 0, 0, 1]
             elif '1in10' in method:
                 choices = [0, 0, 0, 0, 0, 0, 0, 0, 0, 1]
-            apply_coupled = 'COUPLED' in cfg and snowfall_augmentation_applied
+            apply_coupled = 'COUPLED' in cfg and d['snow']
             if 'COUPLED' in cfg:
                 choices = [0]
             if np.random.choice(choices) or apply_coupled:
@@ -118,12 +125,111 @@ class OnTheFlyWeather:
                     probabilities = 5 * np.ones_like(elements)
                     probabilities[0], probabilities[1], probabilities[2] = 15, 25, 15
                     water_height = np.random.choice(elements, 1, p=probabilities / 100)
-                try:
-                    points = ground_water_augmentation(points, water_height=float(np.asarray(water_height).reshape(-1)[0]),
-                                                       debug=False, engine=self._engine())
-                except (TypeError, ValueError):                                        # dense_dataset.py:834-837
-                    pass
+                d.update(wet=True, water_height=float(np.asarray(water_height).reshape(-1)[0]))
+        return d
+
+    def __call__(self, points, training=True):
+        if not training:
+            return points
+        d = self._draws()
+        if d['snow']:
+            tid = self._table(d['mode'], d['rainfall_rate'])
+            pc = np.ascontiguousarray(points[:, :5], dtype=np.float32)
+            pc = pc[get_fov_flag(pc[:, 0:3])]                                  # precompute.py:96-99
+            _, points = augment(pc, '', float(np.degrees(3e-3)), engine=self._engine(), tables=tid, order=d['order'])
+        if d['wet']:
+            try:
+                points = ground_water_augmentation(points, water_height=d['water_height'], debug=False,
+                                                   engine=self._engine())
+            except (TypeError, ValueError):                                        # dense_dataset.py:834-837
+                pass
         return points
+
+    def _stack(self, mode):
+        """One table of 64 S planes for mode: set s (planes 64 s .. 64 s + 63) is the table _table(mode, rate) would
+        upload for the s-th rain rate with a pair, drawn with the same seed.  Returns (table id, {rain rate: s})."""
+        if mode not in self._stacks:
+            rates = sorted({int(r) for r in self.rainfall_rates} & set(self.pairs))
+            eng = self._engine()
+            xyrs, offs, base = [], [np.zeros(1, np.int64)], 0
+            for rate in rates:
+                rs, tv = self.pairs[rate]
+                xyr, off = eng.sample_tables_device(mode, rs, tv, seed=self.table_seed, upload=False)
+                xyrs.append(xyr)
+                offs.append(off[1:] + base)
+                base += int(off[-1])
+            import torch
+            tid = eng.upload_tables_device(torch.cat(xyrs, dim=0).contiguous(), np.concatenate(offs))
+            self._stacks[mode] = (tid, {rate: s for s, rate in enumerate(rates)})
+        return self._stacks[mode]
+
+    def batch(self, points, cloud_offsets, counts=None, training=True):
+        """__call__ on a batch of device-resident clouds in the slot layout: points CUDA float32 (N, 5), cloud b at rows
+        cloud_offsets[b] .. cloud_offsets[b] + counts[b] (CUDA int32 (B,); None: whole slots).  The draws are
+        _draws() sample by sample in batch order, so decisions, rates, orders, heights and both global generators end
+        as after B __call__s.  The snow clouds are gathered, FOV-filtered (camera_fov_batch), augmented in one
+        snowfall_batch on a stack of the rain rates' table sets and scattered back; then the wet clouds, with one
+        water height each.  The counts stay on the device.
+        Returns dict(points (N, 5) float32 in the input slots, counts (B,) int32 CUDA, intensity64 (N,) float64 CUDA:
+        column 3 as the per-sample result holds it (the new intensity of wet rows, the float32 value elsewhere),
+        snow, wet: (B,) host bool).  Differences from __call__: an error of the snowfall pre-pass surfaces at
+        engine.check(), after every sample's draws; a degenerate I/cos range in a wet cloud leaves it unchanged
+        without raising (INTEGRATION.md)."""
+        import torch
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        if not (isinstance(points, torch.Tensor) and points.is_cuda and points.dtype == torch.float32 and
+                points.dim() == 2 and points.shape[1] == 5 and points.shape[0] == int(off[-1])):
+            raise ValueError('OnTheFlyWeather.batch needs CUDA float32 (N, 5) rows in the slots of cloud_offsets')
+        dev = points.device
+        slot = np.diff(off)
+        if counts is None:
+            counts = torch.from_numpy(slot.astype(np.int32)).to(dev)
+        snow = np.zeros(B, dtype=bool)
+        wet = np.zeros(B, dtype=bool)
+        draws = []
+        if training and ('SNOW' in self.cfg or 'WET_SURFACE' in self.cfg):
+            draws = [self._draws() for _ in range(B)]
+            snow[:] = [d['snow'] for d in draws]
+            wet[:] = [d['wet'] for d in draws]
+        if not (snow.any() or wet.any()):
+            return dict(points=points, counts=counts, intensity64=points[:, 3].double(), snow=snow, wet=wet)
+        eng = self._engine()
+        points, counts = points.clone(), counts.clone()
+
+        def gather(sel):                            # row indexes of the selected slots, their offsets, the cloud indexes
+            b = np.flatnonzero(sel)
+            sub = np.concatenate([[0], np.cumsum(slot[b])]).astype(np.int64)
+            shift = torch.from_numpy(off[b] - sub[:-1]).to(dev)
+            rows = torch.arange(int(sub[-1]), device=dev) + torch.repeat_interleave(
+                shift, torch.from_numpy(slot[b]).to(dev), output_size=int(sub[-1]))
+            return rows, sub, torch.from_numpy(b).to(dev)
+
+        if snow.any():
+            mode = draws[int(np.flatnonzero(snow)[0])]['mode']
+            tid, sets = self._stack(mode)
+            rows, sub, b_dev = gather(snow)
+            fov = eng.camera_fov_batch(points[rows], sub, counts=counts[b_dev])          # precompute.py:96-99
+            order = np.stack([np.asarray(draws[k]['order'], np.int32) + 64 * sets[draws[k]['rainfall_rate']]
+                              for k in np.flatnonzero(snow)])
+            res = eng.snowfall_batch(tid, fov['points'], sub, order, float(np.degrees(3e-3)), counts=fov['counts'],
+                                     threshold_filter=True, camera_fov=True, device_prepass=True)
+            points[rows] = res['points']
+            counts[b_dev] = res['counts']
+        intensity64 = points[:, 3].double()
+        if wet.any():
+            rows, sub, b_dev = gather(wet)
+            heights = np.array([draws[k]['water_height'] for k in np.flatnonzero(wet)])
+            res = eng.wet_ground_batch(points[rows], sub, counts=counts[b_dev], water_height=heights,
+                                       want_intensity64=True)
+            points[rows] = res['points']
+            counts[b_dev] = res['counts']
+            intensity64[rows] = res['intensity64']
+        return dict(points=points, counts=counts, intensity64=intensity64, snow=snow, wet=wet)
+
+
+def _no_pair_message(rainfall_rate):
+    return f'no (snowfall_rate, terminal_velocity) pair with rain rate {rainfall_rate}'
 
 
 _LISA_CHANCES = {'8in9': [1, 1, 1, 1, 1, 1, 1, 1, 0], '1in10': [1, 0, 0, 0, 0, 0, 0, 0, 0, 0]}   # dense_dataset.py:717-722

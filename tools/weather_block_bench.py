@@ -1,0 +1,155 @@
+"""
+The dataset's SNOW / WET_SURFACE block on 32 x 131 072-row bench.make_workload clouds (SNOW: uniform_gunn_8in9,
+WET_SURFACE: 1in2, with and without COUPLED), median of --iters synchronised calls of each:
+
+  block         OnTheFlyWeather.batch on the device-resident batch
+  sequential    32 OnTheFlyWeather.__call__s on host clouds, host conversions included
+  dense/slots   snowfall_batch on the camera-FOV clouds repacked dense, against the same clouds in their slots with
+                counts (lss_snowfall_batch_slots)
+  stack         snowfall_batch on the stacked table of the dataset's eight rain rates, every cloud on a random set
+
+    python tools/weather_block_bench.py [--iters 10] [--only-stack]
+
+The scan schedule's bins are a compile-time choice (LSS_SCHED_PLANES): build once with the default and once with
+LSS_NVCC_FLAGS=-DLSS_SCHED_PLANES=512 and run --only-stack on the second build.  Prints one JSON line with the card
+and its power limit.
+"""
+import argparse
+import json
+import os
+import random
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def card():
+    try:
+        return subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
+                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+    except Exception:                                              # noqa: BLE001
+        return 'unknown'
+
+
+def median_ms(fn, iters, sync):
+    fn(0)
+    sync()
+    t = []
+    for i in range(iters):
+        t0 = time.perf_counter()
+        fn(i)
+        sync()
+        t.append(time.perf_counter() - t0)
+    return float(np.median(t) * 1e3)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--clouds', type=int, default=32)
+    ap.add_argument('--iters', type=int, default=10)
+    ap.add_argument('--only-stack', action='store_true')
+    a = ap.parse_args()
+    import torch
+    from bench import make_workload
+    from lidar_snow_sim_b200.engine import SnowfallEngine
+    from lidar_snow_sim_b200.integrations.dense import OnTheFlyWeather
+    eng = SnowfallEngine(0)
+    sync = torch.cuda.synchronize
+    clouds, _ = make_workload(0, a.clouds)
+    off = np.concatenate([[0], np.cumsum([c.shape[0] for c in clouds])]).astype(np.int64)
+    pts = torch.from_numpy(np.concatenate(clouds)).cuda()
+    div = float(np.degrees(3e-3))
+    res = dict(clouds=a.clouds, rows_per_cloud=int(clouds[0].shape[0]), iters=a.iters, card=card(),
+               build_flags=os.environ.get('LSS_NVCC_FLAGS', ''))
+
+    base = OnTheFlyWeather({'SNOW': 'uniform_gunn_8in9'}, engine=eng)
+    tid, sets = base._stack('gunn')
+    res['stack_table_bytes'] = eng.table_info(tid)['bytes']
+    res['stack_rain_rates'] = sorted(sets)
+    res['set_table_bytes'] = {}
+    for rate in sorted(sets):
+        t = base._table('gunn', rate)
+        res['set_table_bytes'][rate] = eng.table_info(t)['bytes']
+        eng.free_tables(t)
+    base._tables.clear()
+
+    rng = np.random.default_rng(0)
+    orders = np.stack([rng.permutation(64) for _ in range(a.clouds)]).astype(np.int32)
+    stack_orders = orders + 64 * rng.integers(0, len(sets), a.clouds, dtype=np.int32)[:, None]
+    kw = dict(threshold_filter=True, camera_fov=True, device_prepass=True)
+    res['stack_ms'] = median_ms(lambda i: eng.snowfall_batch(tid, pts, off, stack_orders, div, **kw), a.iters, sync)
+    eng.check()
+    if a.only_stack:
+        print(json.dumps(res))
+        return
+
+    # dense against slots: the camera-FOV clouds in their slots, and repacked dense
+    fov = eng.camera_fov_batch(pts, off)
+    cnt = fov['counts'].cpu().numpy()
+    host = fov['points'].cpu().numpy()
+    dense = torch.from_numpy(np.concatenate([host[off[b]:off[b] + cnt[b]] for b in range(a.clouds)])).cuda()
+    off_d = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int64)
+    one = base.pairs[34]
+    t34 = eng.sample_tables_device('gunn', one[0], one[1], seed=base.table_seed)
+    res['fov_rows'] = int(cnt.sum())
+    res['dense_ms'] = median_ms(lambda i: eng.snowfall_batch(t34, dense, off_d, orders, div, **kw), a.iters, sync)
+    res['slots_ms'] = median_ms(lambda i: eng.snowfall_batch(t34, fov['points'], off, orders, div,
+                                                            counts=fov['counts'], **kw), a.iters, sync)
+    eng.check()
+    eng.free_tables(t34)
+
+    def gather_scatter(i):                      # what one sub-batch of all 32 clouds costs the block in torch index ops
+        slot = np.diff(off)
+        shift = torch.from_numpy(off[:-1] - off[:-1]).cuda()
+        rows = torch.arange(int(off[-1]), device='cuda') + torch.repeat_interleave(
+            shift, torch.from_numpy(slot).cuda(), output_size=int(off[-1]))
+        sub = pts[rows]
+        out = pts.clone()
+        out[rows] = sub
+
+    res['gather_scatter_ms'] = median_ms(gather_scatter, a.iters, sync)
+
+    for name, cfg in (('uncoupled', {'SNOW': 'uniform_gunn_8in9', 'WET_SURFACE': '1in2'}),
+                      ('coupled', {'SNOW': 'uniform_gunn_8in9', 'WET_SURFACE': '1in2', 'COUPLED': True})):
+        aug = OnTheFlyWeather(cfg, engine=eng)
+        aug._stacks['gunn'] = (tid, sets)
+
+        def seeded(i):
+            np.random.seed(1000 + i)
+            random.seed(1000 + i)
+
+        def block(i):
+            seeded(i)
+            aug.batch(pts, off)
+
+        def sequential(i):
+            seeded(i)
+            for c in clouds:
+                aug(c)
+
+        ms_block = median_ms(block, a.iters, sync)
+        eng.check()
+        eng.set_profiling(True)                     # the engine's kernels inside the block; the rest is torch + host
+        eng.kernel_times(reset=True)
+        for i in range(a.iters):
+            block(i)
+        sync()
+        kernel_ms = {k: v[0] / a.iters for k, v in eng.kernel_times(reset=True).items() if v[1]}   # (timers nest)
+        eng.set_profiling(False)
+        ms_seq = median_ms(sequential, a.iters, sync)
+        seeded(0)
+        r = aug.batch(pts, off)
+        res[name] = dict(block_ms=ms_block, block_kernel_ms=kernel_ms, sequential_ms=ms_seq, snow=int(r['snow'].sum()),
+                         wet=int(r['wet'].sum()))
+        for t in aug._tables.values():
+            eng.free_tables(t)
+    print(json.dumps(res))
+
+
+if __name__ == '__main__':
+    main()
