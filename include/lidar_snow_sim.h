@@ -620,6 +620,43 @@ LSS_API lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int 
                                       const double *d_normals, int64_t n_out, void *d_out, int out_f64,
                                       void *d_workspace, int64_t workspace_bytes, void *stream);
 
+/* OpenPCDet's DATA_AUGMENTOR point path (gt_sampling, random_world_flip / rotation / scaling) on a batch of device-
+ * resident clouds, in two calls around the host planner (lidar_snow_sim_b200/augmentor/plan.py), which replays the
+ * reference's random draws and does the box-level work.
+ * lss_gt_collide_batch: whether iou_bev(candidate, box) != 0 (iou3d_cpu.cpp) for every sampled candidate against every
+ * box of its cloud, then which candidates are valid (DataBaseSampler.__call__).
+ *   d_boxes          float32 [boxes][11]: x, y, z, dx, dy, dz, heading, cosf(h), sinf(h), cosf(-h), sinf(-h) (the C
+ *                    library's cosf / sinf); cloud b's boxes from d_box_offsets[b]: d_n_gt[b] gt boxes, then the candidates
+ *                    grouped by class, class c of cloud b at candidates d_class_offsets[b * 9 + c] .. [b * 9 + c + 1]
+ *   d_bits_offsets   int64 [B]: pair (i, j) of cloud b (candidate i, box j) at d_bits[d_bits_offsets[b] + i * boxes_b + j];
+ *                    max_pairs = the largest candidates_b * boxes_b
+ *   d_valid          uint8 [boxes] out: 1 for a valid candidate, 0 for the rest and for gt boxes
+ * lss_gt_paste_batch: drops the scene rows inside the enlarged valid boxes (check_pt_in_box3d_cpu), writes each cloud's
+ * object rows then its kept scene rows through the cloud's ops, and the counts.
+ *   d_points         float32 (N, n_features >= 3); cloud b at h_cloud_offsets[b] (its first d_cloud_counts[b] rows, or
+ *                    the slot when d_cloud_counts is NULL)
+ *   d_rm_boxes       float32 [.][9]: x, y, z, dx, dy, dz, cosf(-h), sinf(-h), 0; cloud b's from d_rm_offsets[b] (int64
+ *                    [B + 1]), at most max_rm_boxes per cloud
+ *   d_ops            float32 [B][max_ops][3]: (code, p0, p1) in order, 0 none, 1 flip x (y = -y), 2 flip y (x = -x),
+ *                    3 rotate by (cos, sin) = (p0, p1), 4 scale x, y, z by p0
+ *   d_db             float32 [db rows][n_features]; d_objects int64 [n_objects][4]: first db row, first output row,
+ *                    cloud, first object row of the batch (ascending); d_object_shift float64 [n_objects][4]: the box
+ *                    centre added in double, then mv_height subtracted from z in double
+ *   d_out_offsets    int64 [B + 1] output slots; d_object_rows int32 [B] object rows at the front of each slot
+ *   d_out            float32 (d_out_offsets[B], n_features) out; d_counts int32 [B] out: rows of each slot            */
+LSS_API lss_status lss_gt_collide_batch(lss_engine *e, int n_clouds, int n_classes, const float *d_boxes,
+                                        const int64_t *d_box_offsets, const int32_t *d_n_gt,
+                                        const int32_t *d_class_offsets, const int64_t *d_bits_offsets,
+                                        int64_t max_pairs, uint8_t *d_bits, uint8_t *d_valid, void *stream);
+LSS_API int64_t lss_gt_paste_workspace_bytes(const int64_t *h_cloud_offsets, int n_clouds);
+LSS_API lss_status lss_gt_paste_batch(lss_engine *e, const float *d_points, int n_features,
+                                      const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts, int n_clouds,
+                                      const float *d_rm_boxes, const int64_t *d_rm_offsets, int max_rm_boxes,
+                                      const float *d_ops, int max_ops, const float *d_db, const int64_t *d_objects,
+                                      const double *d_object_shift, int n_objects, int64_t n_object_rows,
+                                      const int64_t *d_out_offsets, const int32_t *d_object_rows, float *d_out,
+                                      int32_t *d_counts, void *d_workspace, int64_t workspace_bytes, void *stream);
+
 /* Optional per-kernel timing for bench.py's roofline: when enabled every kernel launch is bracketed by CUDA events
  * on the launching stream.  lss_kernel_times() (call after synchronising) accumulates and returns, per kernel id
  * 0..n-1 (names via lss_kernel_name), total milliseconds and number of launches; reset != 0 clears the totals.     */

@@ -128,6 +128,10 @@ SIGNATURES = [
     ('lss_pa_apply_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _c.c_int, _P, _c.c_int64, _P,
                                       _c.c_int, _c.c_int64, _P, _c.c_int, _c.c_int64, _P, _c.c_int, _P, _P, _P,
                                       _c.c_int64, _P, _c.c_int, _P, _c.c_int64, _P]),
+    ('lss_gt_collide_batch', _c.c_int, [_P, _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _c.c_int64, _P, _P, _P]),
+    ('lss_gt_paste_workspace_bytes', _c.c_int64, [_P, _c.c_int]),
+    ('lss_gt_paste_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _P, _c.c_int, _P, _P, _P,
+                                      _c.c_int, _c.c_int64, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_gather_push', _c.c_int, [_P, _P, _P, _P, _c.c_int, _c.c_int64, _c.c_int, _c.c_int, _P, _P, _P, _P, _c.c_int, _P]),
     ('lss_dart_throwing', _c.c_int, [_c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _P, _c.c_int64,
                                      _c.POINTER(_c.c_int64)]),

@@ -750,6 +750,56 @@ class SnowfallEngine:
         _lib.check(st, self.h)
         return out
 
+    def gt_collide_batch(self, boxes, box_offsets, n_gt, class_offsets, bits_offsets, max_pairs, n_pairs, n_classes):
+        """
+        GT sampling's collision test (lss_gt_collide_batch, current stream, no synchronisation).  boxes: CUDA float32
+        (M, 11); box_offsets (B + 1,) / bits_offsets (B,) CUDA int64; n_gt (B,) / class_offsets (B, 9) CUDA int32.
+        Returns (valid, bits): CUDA uint8 (M,) and (n_pairs,).
+        """
+        B = int(n_gt.shape[0])
+        assert boxes.is_cuda and boxes.dtype == torch.float32 and boxes.is_contiguous() and boxes.shape[1] == 11
+        for t, dt in ((box_offsets, torch.int64), (bits_offsets, torch.int64), (n_gt, torch.int32),
+                      (class_offsets, torch.int32)):
+            assert t.is_cuda and t.dtype == dt and t.is_contiguous()
+        with torch.cuda.device(self.device):
+            valid = torch.empty((boxes.shape[0],), dtype=torch.uint8, device=self.device)
+            bits = torch.empty((max(int(n_pairs), 1),), dtype=torch.uint8, device=self.device)
+            st = self.lib.lss_gt_collide_batch(self.h, B, int(n_classes), _ptr(boxes), _ptr(box_offsets), _ptr(n_gt),
+                                               _ptr(class_offsets), _ptr(bits_offsets), int(max_pairs), _ptr(bits),
+                                               _ptr(valid), self._stream())
+        _lib.check(st, self.h)
+        return valid, bits[:int(n_pairs)]
+
+    def gt_paste_batch(self, points, cloud_offsets, rm_boxes, rm_offsets, max_rm, ops, db, objects, object_shift,
+                       n_object_rows, out_offsets, object_rows, n_out, counts=None):
+        """
+        GT sampling's row work, with the world flip / rotation / scaling (lss_gt_paste_batch, current stream, no
+        synchronisation).  points: CUDA float32 (N, F); cloud_offsets (B + 1) host int64; the tables are CUDA tensors
+        laid out as include/lidar_snow_sim.h describes them.  Returns (rows, counts): CUDA float32 (n_out, F) in the
+        slots out_offsets, and CUDA int32 (B,).
+        """
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        B = off.shape[0] - 1
+        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.dim() == 2
+        assert points.shape[0] == int(off[-1]) and db.shape[1] == points.shape[1]
+        if counts is not None:
+            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        need = self.lib.lss_gt_paste_workspace_bytes(_ptr(off), B)
+        if need < 0:
+            raise ValueError('bad cloud_offsets')
+        with torch.cuda.device(self.device):
+            if getattr(self, '_ws_gt', None) is None or self._ws_gt.numel() < need:
+                self._ws_gt = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            out = torch.empty((int(n_out), points.shape[1]), dtype=torch.float32, device=self.device)
+            out_counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+            st = self.lib.lss_gt_paste_batch(
+                self.h, _ptr(points), int(points.shape[1]), _ptr(off), _ptr(counts), B, _ptr(rm_boxes),
+                _ptr(rm_offsets), int(max_rm), _ptr(ops), int(ops.shape[1]), _ptr(db), _ptr(objects),
+                _ptr(object_shift), int(objects.shape[0]), int(n_object_rows), _ptr(out_offsets), _ptr(object_rows),
+                _ptr(out), _ptr(out_counts), _ptr(self._ws_gt), int(self._ws_gt.numel()), self._stream())
+        _lib.check(st, self.h)
+        return out, out_counts
+
     def gather_push(self, points, counts, d_cloud_offsets, n_rows, world, rank, peer_points, peer_counts, mc_points=0,
                     mc_counts=0, blocks=0):
         """lss_gather_push on the current stream: write the kept rows of this rank's slot-compacted batch (+ counts) into

@@ -433,3 +433,25 @@ def pa_aug_block_batch(points, cloud_offsets, gt_boxes, box_offsets, dataset_cfg
     r['gt_boxes'] = gt_boxes[torch.from_numpy(keep).to(gt_boxes.device) if isinstance(gt_boxes, torch.Tensor) else keep]
     r['box_offsets'] = np.concatenate([[0], np.cumsum([int(np.sum(m)) for m in r['gt_boxes_mask']])]).astype(np.int64)
     return r
+
+
+def data_augmentor_batch(augmentor, points, cloud_offsets, gt_boxes, box_offsets, gt_names, dataset_cfg, mor=None,
+                         counts=None, road_planes=None, calib=None, gt_boxes_mask=None, training=True, engine=None):
+    """
+    prepare_data's DataAugmentor.forward (pcdet/datasets/dataset.py:138-148) for B clouds, in __getitem__ order after
+    the weather block: points are the CUDA rows OnTheFlyWeather.batch returns (slots + counts), gt_boxes / gt_names the
+    host boxes after the dataset's COMPENSATE.  gt_boxes_mask defaults to prepare_data's (names in class_names); mor
+    (per cloud) rides along in the reference's data_dict and changes nothing here.  A COMPENSATE that is not all zeros
+    would move the float64 rows off the float32 grid the device holds, so it raises NotImplementedError.
+    Returns augmentor.forward_batch's result, or None when not training (the dataset skips the augmentor then).
+    """
+    if not training:
+        return None
+    comp = dataset_cfg.get('COMPENSATE', None) if hasattr(dataset_cfg, 'get') else None
+    if comp and any(float(c) != 0.0 for c in comp):
+        raise NotImplementedError('data_augmentor_batch: COMPENSATE other than [0, 0, 0]')
+    if comp and not any(n == 'random_world_rotation' for n, _ in augmentor.queue):
+        # the reference's rows are float64 after COMPENSATE; only the rotation's float32 cast makes them float32
+        raise NotImplementedError('data_augmentor_batch: COMPENSATE without random_world_rotation')
+    return augmentor.forward_batch(points, cloud_offsets, gt_boxes, box_offsets, gt_names, counts=counts,
+                                   road_planes=road_planes, calib=calib, gt_boxes_mask=gt_boxes_mask, engine=engine)
