@@ -4,6 +4,9 @@ SnowfallEngine -- thin host-side owner of one C-ABI engine (one GPU).  PyTorch i
 
 One process per GPU: create one engine per rank; clouds are independent, so a batch shards across ranks with no
 data-path collective (see lidar_snow_sim_b200/distributed.py for the gather of the augmented batch).
+
+Every public method checks all of its arguments (ValueError, like the library's LSS_ERR_INVALID_ARG) before it
+allocates, touches the device or calls the library: a pointer reaches a kernel only from a tensor that was checked.
 """
 import ctypes
 
@@ -17,6 +20,7 @@ DEFAULT_MAX_DIVERGENCE_RAD = 3e-3          # callers pass beam_divergence = degr
 # sample_tables_device calls the sampler at most this often: the darts per plane start at 1.5x the expected table size
 # (+4096) and double after each call that ends short of the occupancy; the last call's failure is raised
 SAMPLER_ATTEMPTS = 4
+_CPU = torch.device('cpu')
 
 
 def _ptr(t):
@@ -27,6 +31,59 @@ def _ptr(t):
     if isinstance(t, np.ndarray):
         return ctypes.c_void_p(t.ctypes.data)
     raise TypeError(type(t))
+
+
+def _cloud_offsets(offsets, name='cloud_offsets'):
+    """(off, B, N): host row offsets as a contiguous int64 array of B + 1 entries, the number of clouds and of rows.
+    That they start at 0 and never decrease is checked by the library, which names the argument."""
+    off = np.ascontiguousarray(offsets, dtype=np.int64)
+    if off.ndim != 1 or off.shape[0] == 0:
+        raise ValueError(f'{name}: expected a 1-D array of B + 1 row offsets, got shape {off.shape}')
+    return off, off.shape[0] - 1, int(off[-1])
+
+
+def _check_tensor(name, t, device, dtype, shape=None, min_cols=0, optional=False):
+    """
+    Raise ValueError unless `t` is a contiguous tensor of `dtype` on `device` (None: on any CUDA device, for mappings of
+    another rank's buffers) of shape `shape`, where None matches any size and dimension 1 has at least min_cols entries.
+    None passes for an optional argument.
+    """
+    if t is None and optional:
+        return
+    if (isinstance(t, torch.Tensor) and (t.is_cuda if device is None else t.device == device) and t.dtype == dtype
+            and t.is_contiguous()
+            and (shape is None or t.shape == shape
+                 or (t.dim() == len(shape) and all(w is None or s == w for s, w in zip(t.shape, shape))))
+            and (not min_cols or t.shape[1] >= min_cols)):
+        return
+    dims = [] if shape is None else ['*' if w is None else str(w) for w in shape]
+    if min_cols:
+        dims[1] = f'n_features >= {min_cols}'
+    want = (f'a contiguous {dtype} tensor on {device or "a CUDA device"}'
+            + ('' if shape is None else f' of shape ({", ".join(dims)}{"," if len(dims) == 1 else ""})'))
+    got = (f'a {"" if t.is_contiguous() else "non-contiguous "}{t.dtype} tensor of shape {tuple(t.shape)} on {t.device}'
+           if isinstance(t, torch.Tensor) else type(t).__name__)
+    raise ValueError(f'{name}: expected {want}, got {got}')
+
+
+def _outputs(out, device, **spec):
+    """`out` (None, or the dict a previous call returned, to reuse its buffers) with a buffer for every key of spec whose
+    value (shape, dtype) is not false: the buffers out has are checked, then the missing ones allocated (pinned on the
+    host)."""
+    out = {} if out is None else out
+    for k, v in spec.items():
+        if v and k in out:
+            _check_tensor(f"out['{k}']", out[k], device, v[1], v[0])
+    for k, v in spec.items():
+        if v and k not in out:
+            t = torch.empty(v[0], dtype=v[1], device=device)
+            out[k] = t.pin_memory() if device == _CPU else t
+    return out
+
+
+def _snowfall_flags(threshold_filter, camera_fov, device_prepass, assume_sorted=False):
+    return ((_lib.FLAG_THRESHOLD_FILTER if threshold_filter else 0) | (_lib.FLAG_CAMERA_FOV if camera_fov else 0)
+            | (_lib.FLAG_DEVICE_PREPASS if device_prepass else 0) | (_lib.FLAG_ASSUME_SORTED if assume_sorted else 0))
 
 
 class SnowfallEngine:
@@ -45,7 +102,8 @@ class SnowfallEngine:
             from .calib.dense_camera import STF_HDL64_CAMERA as camera
         self.set_camera(camera)
         self._tables = {}
-        self._ws = None
+        self._scratch_ws = {}                   # entry point -> its cached workspace (_scratch)
+        self._pa_part_bytes = None              # the partition pa_partition_batch left at the front of the 'pa' workspace
 
     # ------------------------------------------------------------------------------------------------------------------
     def close(self):
@@ -61,6 +119,27 @@ class SnowfallEngine:
 
     def _stream(self):
         return ctypes.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def _call(self, name, *args, check=True):
+        """
+        self.lib.<name>(handle, *args, current stream) on the engine's device.  Device tensors are passed as they are:
+        their pointers are taken here, after the caller's checks.  Host arrays go through _ptr.  Raises the status
+        through _lib.check unless check=False, and returns it.
+        """
+        with torch.cuda.device(self.device):
+            st = getattr(self.lib, name)(self.h, *[a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args],
+                                         self._stream())
+        if check:
+            _lib.check(st, self.h)
+        return st
+
+    def _scratch(self, name, need):
+        """The cached uint8 workspace of entry point `name`, reallocated at 1.25x + 256 bytes when it holds fewer than
+        `need`.  Calls of one entry point in flight on several streams would share it (snowfall_batch takes its own)."""
+        ws = self._scratch_ws.get(name)
+        if ws is None or ws.numel() < need:
+            ws = self._scratch_ws[name] = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+        return ws
 
     def set_camera(self, camera):
         P2 = np.ascontiguousarray(camera['P2'], dtype=np.float32).reshape(3, 4)
@@ -79,25 +158,23 @@ class SnowfallEngine:
                 raise ValueError('particle table must be (N, 3)')
             off[k + 1] = off[k] + t.shape[0]
         xyr = np.ascontiguousarray(np.concatenate([np.asarray(t, dtype=np.float64) for t in tables], axis=0))
-        tid = ctypes.c_int(0)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.lss_upload_particles(self.h, len(tables), _ptr(xyr), _ptr(off),
-                                                     float(max_beam_divergence_rad), int(n_buckets), self._stream(),
-                                                     ctypes.byref(tid)), self.h)
-        self._tables[tid.value] = dict(n_planes=len(tables), max_div=float(max_beam_divergence_rad))
-        return tid.value
+        return self._upload('lss_upload_particles', _ptr(xyr), off, max_beam_divergence_rad, n_buckets)
 
     def upload_tables_device(self, xyr, plane_offsets, max_beam_divergence_rad=DEFAULT_MAX_DIVERGENCE_RAD,
                              n_buckets=2048):
         """xyr: CUDA float64 tensor (sum Np, 3); plane_offsets: int64 host array (n_planes + 1)."""
-        off = np.ascontiguousarray(plane_offsets, dtype=np.int64)
-        assert xyr.is_cuda and xyr.dtype == torch.float64 and xyr.is_contiguous()
+        off, _, n_rows = _cloud_offsets(plane_offsets, 'plane_offsets')
+        _check_tensor('xyr', xyr, self.device, torch.float64, (n_rows, 3))
+        return self._upload('lss_upload_particles_device', xyr, off, max_beam_divergence_rad, n_buckets)
+
+    def _upload(self, name, xyr, off, max_div, n_buckets):
+        """lss_upload_particles[_device] of xyr (a host array's pointer or a checked device tensor)"""
         tid = ctypes.c_int(0)
         with torch.cuda.device(self.device):
-            _lib.check(self.lib.lss_upload_particles_device(self.h, len(off) - 1, _ptr(xyr), _ptr(off),
-                                                            float(max_beam_divergence_rad), int(n_buckets),
-                                                            self._stream(), ctypes.byref(tid)), self.h)
-        self._tables[tid.value] = dict(n_planes=len(off) - 1, max_div=float(max_beam_divergence_rad))
+            xyr = xyr.data_ptr() if isinstance(xyr, torch.Tensor) else xyr
+            _lib.check(getattr(self.lib, name)(self.h, len(off) - 1, xyr, _ptr(off), float(max_div), int(n_buckets),
+                                               self._stream(), ctypes.byref(tid)), self.h)
+        self._tables[tid.value] = dict(n_planes=len(off) - 1, max_div=float(max_div))
         return tid.value
 
     def sample_tables_device(self, mode, snowfall_rate, terminal_velocity, seed=1000, R_0=80.0, n_planes=64,
@@ -115,25 +192,23 @@ class SnowfallEngine:
         occ = compute_occupancy(float(snowfall_rate), float(terminal_velocity))
         rr = float(snowfall_rate_to_rainfall_rate(float(snowfall_rate), float(terminal_velocity)))
         M = _expected_capacity(occ, rr, R_0, mode)
-        with torch.cuda.device(self.device):
-            for attempt in range(SAMPLER_ATTEMPTS):
-                # the output holds M rows per plane, as many as there are darts, so only a target not reached with M
-                # darts (the stream is keyed per dart: more darts extend it, they do not change it) can fail here
-                need = self.lib.lss_sample_particles_workspace_bytes(n_planes, M)
-                ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
-                out = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device)
-                counts = torch.empty((n_planes,), dtype=torch.int32, device=self.device)
-                cand = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device) if return_candidates else None
-                st = self.lib.lss_sample_particles(self.h, n_planes, occ, rr, float(R_0), _DIST[mode], int(seed), M,
-                                                   _ptr(out), M, _ptr(counts), _ptr(cand), _ptr(ws), int(ws.numel()),
-                                                   self._stream())
-                if st != _lib.LSS_ERR_WORKSPACE or attempt == SAMPLER_ATTEMPTS - 1:
-                    break
-                M *= 2
-            _lib.check(st, self.h)
-            cnt = counts.cpu().numpy().astype(np.int64)
-            off = np.concatenate([[0], np.cumsum(cnt)])
-            xyr = torch.cat([out[p, :cnt[p]] for p in range(n_planes)], dim=0).contiguous()
+        for attempt in range(SAMPLER_ATTEMPTS):
+            # the output holds M rows per plane, as many as there are darts, so only a target not reached with M
+            # darts (the stream is keyed per dart: more darts extend it, they do not change it) can fail here
+            need = self.lib.lss_sample_particles_workspace_bytes(n_planes, M)
+            ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
+            out = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device)
+            counts = torch.empty((n_planes,), dtype=torch.int32, device=self.device)
+            cand = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device) if return_candidates else None
+            st = self._call('lss_sample_particles', n_planes, occ, rr, float(R_0), _DIST[mode], int(seed), M, out, M,
+                            counts, cand, ws, ws.numel(), check=False)
+            if st != _lib.LSS_ERR_WORKSPACE or attempt == SAMPLER_ATTEMPTS - 1:
+                break
+            M *= 2
+        _lib.check(st, self.h)
+        cnt = counts.cpu().numpy().astype(np.int64)
+        off = np.concatenate([[0], np.cumsum(cnt)])
+        xyr = torch.cat([out[p, :cnt[p]] for p in range(n_planes)], dim=0).contiguous()
         if not upload:
             return (xyr, off, cand) if return_candidates else (xyr, off)
         return self.upload_tables_device(xyr, off, max_beam_divergence_rad, n_buckets)
@@ -149,12 +224,6 @@ class SnowfallEngine:
         return dict(n_particles=a.value, n_entries=b.value, bytes=c.value)
 
     # ------------------------------------------------------------------------------------------------------------------
-    def _workspace(self, n_total, n_clouds):
-        need = self.lib.lss_snowfall_workspace_bytes(int(n_total), int(n_clouds))
-        if self._ws is None or self._ws.numel() < need:
-            self._ws = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-        return self._ws, need
-
     def snowfall_batch(self, table_id, points, cloud_offsets, order, beam_divergence_deg, theta=None,
                        thresh_poly=None, plane=None, ymins=None, noise_floor=0.7, threshold_filter=True, camera_fov=False,
                        device_prepass=False, assume_sorted=False, want_full=False, want_perm=False, want_nocc=False,
@@ -166,60 +235,33 @@ class SnowfallEngine:
         counts: optional CUDA int32 (B,) valid rows per slot (slot-compacted input, lss_snowfall_batch_slots): cloud b
         is rows cloud_offsets[b] .. cloud_offsets[b] + counts[b], and the rows behind them are ignored.
         plane (B,4) / ymins (B,50): optional host arrays replayed by the device pre-pass (lss_noise_threshold_poly).
+        workspace: optional CUDA uint8 tensor of at least lss_snowfall_workspace_bytes(N, B) bytes (default: the
+        engine's), for calls in flight on several streams.
         Returns dict(points=(N,5) slot-compacted rows, counts=(B,), stats=(B,4) [, full, perm, nocc]).
         Call `check()` (synchronises) to surface asynchronous device errors.
         """
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous()
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.shape[0] == N and points.shape[1] == 5
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, 5))
+        _check_tensor('theta', theta, self.device, torch.float32, (N,), optional=True)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        _check_tensor('workspace', workspace, self.device, torch.uint8, (None,), optional=True)
         order = np.ascontiguousarray(order, dtype=np.int32).reshape(B, 64)
-        flags = 0
-        if threshold_filter:
-            flags |= _lib.FLAG_THRESHOLD_FILTER
-        if camera_fov:
-            flags |= _lib.FLAG_CAMERA_FOV
-        if device_prepass:
-            flags |= _lib.FLAG_DEVICE_PREPASS
-        if assume_sorted:
-            flags |= _lib.FLAG_ASSUME_SORTED
-        want_full = want_full or want_perm or want_nocc      # the debug views are produced together
-        tp = None
-        if thresh_poly is not None:
-            tp = np.ascontiguousarray(thresh_poly, dtype=np.float64).reshape(B, 3)
-        if theta is not None:
-            assert theta.is_cuda and theta.dtype == torch.float32 and theta.shape[0] == N
-        if counts is not None:
-            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,) and counts.is_contiguous()
+        tp = None if thresh_poly is None else np.ascontiguousarray(thresh_poly, dtype=np.float64).reshape(B, 3)
         pl = None if plane is None else np.ascontiguousarray(plane, dtype=np.float64).reshape(B, 4)
         ym = None if ymins is None else np.ascontiguousarray(ymins, dtype=np.int32).reshape(B, 50)
-        with torch.cuda.device(self.device):
-            if out is None:
-                out = {}
-            if 'points' not in out:
-                out['points'] = torch.empty((N, 5), dtype=torch.float32, device=self.device)
-                out['counts'] = torch.empty((B,), dtype=torch.int32, device=self.device)
-                out['stats'] = torch.empty((B, 4), dtype=torch.float64, device=self.device)
-            if want_full and 'full' not in out:
-                out['full'] = torch.empty((N, 5), dtype=torch.float32, device=self.device)
-            if want_perm and 'perm' not in out:
-                out['perm'] = torch.empty((N,), dtype=torch.int32, device=self.device)
-            if want_nocc and 'nocc' not in out:
-                out['nocc'] = torch.empty((N,), dtype=torch.int32, device=self.device)
-            if workspace is None:
-                ws, need = self._workspace(N, B)
-            else:
-                ws = workspace
-                assert ws.numel() >= self.lib.lss_snowfall_workspace_bytes(N, B)
-            st = self.lib.lss_snowfall_batch_slots(
-                self.h, int(table_id), _ptr(points), _ptr(off), _ptr(counts), B, _ptr(order), float(beam_divergence_deg),
-                _ptr(theta), _ptr(tp), _ptr(pl), _ptr(ym), float(noise_floor), flags, _ptr(out['points']),
-                _ptr(out['counts']),
-                _ptr(out['stats']), _ptr(out.get('full')) if want_full else None,
-                _ptr(out.get('perm')) if want_perm else None, _ptr(out.get('nocc')) if want_nocc else None,
-                _ptr(ws), int(ws.numel()), self._stream())
-        _lib.check(st, self.h)
+        want_full = want_full or want_perm or want_nocc      # the debug views are produced together
+        out = _outputs(out, self.device, points=((N, 5), torch.float32), counts=((B,), torch.int32),
+                       stats=((B, 4), torch.float64), full=want_full and ((N, 5), torch.float32),
+                       perm=want_perm and ((N,), torch.int32), nocc=want_nocc and ((N,), torch.int32))
+        need = self.lib.lss_snowfall_workspace_bytes(N, B)
+        if workspace is not None and workspace.numel() < need:
+            raise ValueError(f'workspace: {workspace.numel()} bytes, the batch needs {need}')
+        ws = self._scratch('snowfall', need) if workspace is None else workspace
+        self._call('lss_snowfall_batch_slots', int(table_id), points, _ptr(off), counts, B, _ptr(order),
+                   float(beam_divergence_deg), theta, _ptr(tp), _ptr(pl), _ptr(ym), float(noise_floor),
+                   _snowfall_flags(threshold_filter, camera_fov, device_prepass, assume_sorted), out['points'],
+                   out['counts'], out['stats'], out.get('full') if want_full else None,
+                   out.get('perm') if want_perm else None, out.get('nocc') if want_nocc else None, ws, ws.numel())
         return out
 
     def snowfall_batch_host_submit(self, table_id, host_points, cloud_offsets, order, beam_divergence_deg,
@@ -233,36 +275,19 @@ class SnowfallEngine:
         2-3 in flight (a prefetching loader) batch k+1's copy-in, batch k's kernels and batch k-1's copy-out overlap.
         The input and `host_out` buffers must not be touched until the ticket has been waited for.
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
+        off, B, N = _cloud_offsets(cloud_offsets)
         if isinstance(host_points, np.ndarray):
             host_points = torch.from_numpy(np.ascontiguousarray(host_points, dtype=np.float32))
-        assert not host_points.is_cuda and host_points.dtype == torch.float32 and host_points.shape == (N, 5)
-        assert host_points.is_contiguous()
+        _check_tensor('host_points', host_points, _CPU, torch.float32, (N, 5))
         order = np.ascontiguousarray(order, dtype=np.int32).reshape(B, 64)
-        tp = None
-        if thresh_poly is not None:
-            tp = np.ascontiguousarray(thresh_poly, dtype=np.float64).reshape(B, 3)
-        flags = 0
-        if threshold_filter:
-            flags |= _lib.FLAG_THRESHOLD_FILTER
-        if camera_fov:
-            flags |= _lib.FLAG_CAMERA_FOV
-        if device_prepass:
-            flags |= _lib.FLAG_DEVICE_PREPASS
-        if host_out is None:
-            host_out = {}
-        if 'points' not in host_out:
-            host_out['points'] = torch.empty((N, 5), dtype=torch.float32).pin_memory()
-            host_out['counts'] = torch.empty((B,), dtype=torch.int32).pin_memory()
-            host_out['stats'] = torch.empty((B, 4), dtype=torch.float64).pin_memory()
-        assert host_out['points'].shape == (N, 5) and host_out['counts'].shape == (B,)
+        tp = None if thresh_poly is None else np.ascontiguousarray(thresh_poly, dtype=np.float64).reshape(B, 3)
+        host_out = _outputs(host_out, _CPU, points=((N, 5), torch.float32), counts=((B,), torch.int32),
+                            stats=((B, 4), torch.float64))
         ticket = ctypes.c_int(-1)
         st = self.lib.lss_snowfall_batch_host_submit(
             self.h, int(table_id), _ptr(host_points), _ptr(off), B, _ptr(order), float(beam_divergence_deg), _ptr(tp),
-            float(noise_floor), flags, int(n_chunks), _ptr(host_out['points']), _ptr(host_out['counts']),
-            _ptr(host_out['stats']), ctypes.byref(ticket))
+            float(noise_floor), _snowfall_flags(threshold_filter, camera_fov, device_prepass), int(n_chunks),
+            _ptr(host_out['points']), _ptr(host_out['counts']), _ptr(host_out['stats']), ctypes.byref(ticket))
         _lib.check(st, self.h)
         # the ticket keeps the buffers of the in-flight batch alive
         return dict(id=int(ticket.value), out=host_out, keep=(host_points, off, order, tp))
@@ -290,26 +315,17 @@ class SnowfallEngine:
         [, fits (B,8) float64, picks (B,50) int32 with want_fits].
         plane: optional host array (B,4) = (w0, w1, w2, h) to use instead of the RANSAC estimate;
         ymins: optional host int array (B,50), the reference host's np.argpartition picks (augmentation.py:236)."""
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape == (N, 5)
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, 5))
         pl = None if plane is None else np.ascontiguousarray(plane, dtype=np.float64).reshape(B, 4)
         ym = None if ymins is None else np.ascontiguousarray(ymins, dtype=np.int32).reshape(B, 50)
-        with torch.cuda.device(self.device):
-            need = self.lib.lss_prepass_workspace_bytes(N, B)
-            ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
-            poly = torch.empty((B, 3), dtype=torch.float64, device=self.device)
-            plane_out = torch.empty((B, 4), dtype=torch.float64, device=self.device)
-            fits = torch.empty((B, 8), dtype=torch.float64, device=self.device) if want_fits else None
-            picks = torch.empty((B, 50), dtype=torch.int32, device=self.device) if want_fits else None
-            st = self.lib.lss_noise_threshold_poly(self.h, _ptr(points), _ptr(off), B, float(noise_floor), _ptr(pl),
-                                                   _ptr(ym), _ptr(poly), _ptr(plane_out), _ptr(fits), _ptr(picks),
-                                                   _ptr(ws), int(ws.numel()), self._stream())
-        _lib.check(st, self.h)
-        if want_fits:
-            return poly, plane_out, fits, picks
-        return poly, plane_out
+        need = self.lib.lss_prepass_workspace_bytes(N, B)
+        ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
+        out = _outputs(None, self.device, poly=((B, 3), torch.float64), plane=((B, 4), torch.float64),
+                       fits=want_fits and ((B, 8), torch.float64), picks=want_fits and ((B, 50), torch.int32))
+        self._call('lss_noise_threshold_poly', points, _ptr(off), B, float(noise_floor), _ptr(pl), _ptr(ym), out['poly'],
+                   out['plane'], out.get('fits'), out.get('picks'), ws, ws.numel())
+        return tuple(out.values())                          # (poly, plane[, fits, picks])
 
     def wet_ground_batch(self, points, cloud_offsets, counts=None, water_height=0.001, pavement_depth=0.0012,
                          noise_floor=0.7, power_factor=15, flat_earth=False, delta=0.5, replace=True, plane=None,
@@ -323,44 +339,28 @@ class SnowfallEngine:
         [, fits (B,8) float64, picks (B,50) int32 with want_fits, laid out as in noise_threshold_poly]).
         passthrough: 0 augmented, 1 fewer than 1000 ground points, 2 degenerate I/cos range (check() raises ValueError).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape == (N, 5)
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, 5))
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
         pl = None if plane is None else np.ascontiguousarray(plane, dtype=np.float64).reshape(B, 4)
         ym = None if ymins is None else np.ascontiguousarray(ymins, dtype=np.int32).reshape(B, 50)
-        with torch.cuda.device(self.device):
-            if out is None:
-                out = {}
-            if 'points' not in out:                            # (pass the returned dict back in as `out` to reuse the buffers)
-                out.update(points=torch.empty((N, 5), dtype=torch.float32, device=self.device),
-                           counts=torch.empty((B,), dtype=torch.int32, device=self.device),
-                           passthrough=torch.empty((B,), dtype=torch.int32, device=self.device),
-                           plane=torch.empty((B, 4), dtype=torch.float64, device=self.device))
-            if want_intensity64 and 'intensity64' not in out:
-                out['intensity64'] = torch.empty((N,), dtype=torch.float64, device=self.device)
-            if want_fits and 'fits' not in out:
-                out.update(fits=torch.empty((B, 8), dtype=torch.float64, device=self.device),
-                           picks=torch.empty((B, 50), dtype=torch.int32, device=self.device))
-            need = self.lib.lss_wet_ground_workspace_bytes(N, B)
-            if getattr(self, '_ws_wet', None) is None or self._ws_wet.numel() < need:
-                self._ws_wet = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            per_cloud = np.ndim(water_height) > 0
-            if per_cloud:
-                heights = np.ascontiguousarray(water_height, dtype=np.float64).reshape(-1)
-                if heights.shape[0] != B:
-                    raise ValueError(f'water_height: {heights.shape[0]} heights for {B} clouds')
-            call = self.lib.lss_wet_ground_batch_params if per_cloud else self.lib.lss_wet_ground_batch
-            st = call(
-                self.h, _ptr(points), _ptr(off), _ptr(counts), B, _ptr(heights) if per_cloud else float(water_height),
-                float(pavement_depth),
-                float(noise_floor), float(power_factor), 1 if flat_earth else 0, float(delta), 1 if replace else 0,
-                _ptr(pl), _ptr(ym), _ptr(out['points']), _ptr(out.get('intensity64')) if want_intensity64 else None,
-                _ptr(out['counts']),
-                _ptr(out['passthrough']), _ptr(out['plane']), _ptr(out.get('fits')) if want_fits else None,
-                _ptr(out.get('picks')) if want_fits else None, _ptr(self._ws_wet), int(self._ws_wet.numel()),
-                self._stream())
-        _lib.check(st, self.h)
+        per_cloud = np.ndim(water_height) > 0
+        if per_cloud:
+            heights = np.ascontiguousarray(water_height, dtype=np.float64).reshape(-1)
+            if heights.shape[0] != B:
+                raise ValueError(f'water_height: {heights.shape[0]} heights for {B} clouds')
+        # (pass the returned dict back in as `out` to reuse the buffers)
+        out = _outputs(out, self.device, points=((N, 5), torch.float32), counts=((B,), torch.int32),
+                       passthrough=((B,), torch.int32), plane=((B, 4), torch.float64),
+                       intensity64=want_intensity64 and ((N,), torch.float64), fits=want_fits and ((B, 8), torch.float64),
+                       picks=want_fits and ((B, 50), torch.int32))
+        ws = self._scratch('wet', self.lib.lss_wet_ground_workspace_bytes(N, B))
+        self._call('lss_wet_ground_batch_params' if per_cloud else 'lss_wet_ground_batch', points, _ptr(off), counts, B,
+                   _ptr(heights) if per_cloud else float(water_height), float(pavement_depth), float(noise_floor),
+                   float(power_factor), 1 if flat_earth else 0, float(delta), 1 if replace else 0, _ptr(pl), _ptr(ym),
+                   out['points'], out.get('intensity64') if want_intensity64 else None, out['counts'],
+                   out['passthrough'], out['plane'], out.get('fits') if want_fits else None,
+                   out.get('picks') if want_fits else None, ws, ws.numel())
         return out
 
     def fog_batch(self, points, cloud_offsets, lut, alpha, beta, beta_0, hard=True, soft=True, gain=False, noise=0,
@@ -371,31 +371,10 @@ class SnowfallEngine:
         rng_states: host uint64 (B, 4) PCG64 states (variants 1-3) or ext_noise: CUDA float64 (N,) values by rank.
         Returns dict(points float64 (N, F), fog_mask uint8 (N,), info float64 (B, 3) [, rank int32 (N,)]).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
-        F = int(points.shape[1])
-        if lut is not None:
-            assert lut.is_cuda and lut.dtype == torch.float64 and lut.is_contiguous() and tuple(lut.shape) == (2001, 2)
-        rs = None if rng_states is None else np.ascontiguousarray(rng_states, dtype=np.uint64).reshape(B, 4)
-        if ext_noise is not None:
-            assert ext_noise.is_cuda and ext_noise.dtype == torch.float64 and ext_noise.numel() >= N
-        flags = (_lib.FOG_HARD if hard else 0) | (_lib.FOG_SOFT if soft else 0) | (_lib.FOG_GAIN if gain else 0)
-        with torch.cuda.device(self.device):
-            out = dict(points=torch.empty((N, F), dtype=torch.float64, device=self.device),
-                       fog_mask=torch.empty((N,), dtype=torch.uint8, device=self.device),
-                       info=torch.empty((B, 3), dtype=torch.float64, device=self.device))
-            if want_rank:
-                out['rank'] = torch.empty((N,), dtype=torch.int32, device=self.device)
-            need = self.lib.lss_fog_workspace_bytes(N, B)
-            ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_fog_batch(self.h, _ptr(points), F, _ptr(off), B, float(alpha), float(beta), float(beta_0),
-                                        _ptr(lut), flags, int(noise), int(noise_variant), _ptr(rs), _ptr(ext_noise),
-                                        _ptr(out['points']), _ptr(out['fog_mask']), _ptr(out.get('rank')),
-                                        _ptr(out['info']), _ptr(ws), int(ws.numel()), self._stream())
-        _lib.check(st, self.h)
-        return out
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('lut', lut, self.device, torch.float64, (2001, 2), optional=True)
+        return self._fog('lss_fog_batch', 'lss_fog_workspace_bytes', (float(alpha), float(beta), float(beta_0), lut),
+                         points, off, B, N, hard, soft, gain, noise, noise_variant, rng_states, ext_noise, want_rank)
 
     def fog_batch_params(self, points, cloud_offsets, luts, alpha, beta, beta_0, table_index=None, hard=True, soft=True,
                          gain=False, noise=0, noise_variant=1, rng_states=None, ext_noise=None, want_rank=False):
@@ -404,35 +383,29 @@ class SnowfallEngine:
         are length-B host sequences; luts: CUDA float64 (T, 2001, 2) stack of integral tables (e.g. fog_integral_tables);
         cloud b uses luts[table_index[b]].  A cloud's results are bit-identical to fog_batch with its own parameters.
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
-        F = int(points.shape[1])
-        T = 0
-        if luts is not None:
-            assert luts.is_cuda and luts.dtype == torch.float64 and luts.is_contiguous()
-            assert luts.dim() == 3 and tuple(luts.shape[1:]) == (2001, 2)
-            T = int(luts.shape[0])
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('luts', luts, self.device, torch.float64, (None, 2001, 2), optional=True)
         per = [np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (B,))) for v in (alpha, beta, beta_0)]
         ti = None if table_index is None else np.ascontiguousarray(table_index, dtype=np.int32).reshape(B)
+        params = (*[_ptr(v) for v in per], _ptr(ti), luts, 0 if luts is None else int(luts.shape[0]))
+        return self._fog('lss_fog_batch_params', 'lss_fog_batch_params_workspace_bytes', params, points, off, B, N, hard,
+                         soft, gain, noise, noise_variant, rng_states, ext_noise, want_rank)
+
+    def _fog(self, name, ws_name, params, points, off, B, N, hard, soft, gain, noise, noise_variant, rng_states,
+             ext_noise, want_rank):
+        """fog_batch and fog_batch_params, which differ in the entry point and its fog parameter block `params`"""
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=4)
+        _check_tensor('ext_noise', ext_noise, self.device, torch.float64, optional=True)
+        if ext_noise is not None and ext_noise.numel() < N:
+            raise ValueError(f'ext_noise: {ext_noise.numel()} values for {N} rows')
         rs = None if rng_states is None else np.ascontiguousarray(rng_states, dtype=np.uint64).reshape(B, 4)
-        if ext_noise is not None:
-            assert ext_noise.is_cuda and ext_noise.dtype == torch.float64 and ext_noise.numel() >= N
         flags = (_lib.FOG_HARD if hard else 0) | (_lib.FOG_SOFT if soft else 0) | (_lib.FOG_GAIN if gain else 0)
-        with torch.cuda.device(self.device):
-            out = dict(points=torch.empty((N, F), dtype=torch.float64, device=self.device),
-                       fog_mask=torch.empty((N,), dtype=torch.uint8, device=self.device),
-                       info=torch.empty((B, 3), dtype=torch.float64, device=self.device))
-            if want_rank:
-                out['rank'] = torch.empty((N,), dtype=torch.int32, device=self.device)
-            need = self.lib.lss_fog_batch_params_workspace_bytes(N, B)
-            ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_fog_batch_params(
-                self.h, _ptr(points), F, _ptr(off), B, *[_ptr(v) for v in per], _ptr(ti), _ptr(luts), T, flags,
-                int(noise), int(noise_variant), _ptr(rs), _ptr(ext_noise), _ptr(out['points']), _ptr(out['fog_mask']),
-                _ptr(out.get('rank')), _ptr(out['info']), _ptr(ws), int(ws.numel()), self._stream())
-        _lib.check(st, self.h)
+        F = points.shape[1]
+        out = _outputs(None, self.device, points=((N, F), torch.float64), fog_mask=((N,), torch.uint8),
+                       info=((B, 3), torch.float64), rank=want_rank and ((N,), torch.int32))
+        ws = torch.empty(int(getattr(self.lib, ws_name)(N, B)) + 256, dtype=torch.uint8, device=self.device)
+        self._call(name, points, F, _ptr(off), B, *params, flags, int(noise), int(noise_variant), _ptr(rs), ext_noise,
+                   out['points'], out['fog_mask'], out.get('rank'), out['info'], ws, ws.numel())
         return out
 
     def fog_integral_tables(self, params, shift=False, n=2000, r_range=200, r_0_max=200, granularity=None):
@@ -456,12 +429,10 @@ class SnowfallEngine:
             q.n, q.linear_xsi, q.shift = int(n), 1 if p.linear_xsi else 0, 1 if shift else 0
         steps = float(r_0_max) / float(granularity)
         rows = int(steps) + 1 if np.isfinite(steps) and 0 <= steps < 2 ** 24 else 0
-        with torch.cuda.device(self.device):
-            out = torch.empty((T, rows, 2), dtype=torch.float64, device=self.device)
-            need = self.lib.lss_fog_integral_tables_workspace_bytes(int(n), T)
-            ws = torch.empty(max(int(need), 0) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_fog_integral_tables(self.h, ctypes.cast(arr, ctypes.c_void_p), T, _ptr(out), _ptr(ws), int(ws.numel()), self._stream())
-        _lib.check(st, self.h)
+        out = torch.empty((T, rows, 2), dtype=torch.float64, device=self.device)
+        need = self.lib.lss_fog_integral_tables_workspace_bytes(int(n), T)
+        ws = torch.empty(max(int(need), 0) + 256, dtype=torch.uint8, device=self.device)
+        self._call('lss_fog_integral_tables', ctypes.cast(arr, ctypes.c_void_p), T, out, ws, ws.numel())
         return out
 
     def mie_tables(self, refractive_indices, wavelengths_nm, diameters_nm=None):
@@ -480,12 +451,9 @@ class SnowfallEngine:
         d = np.ascontiguousarray(np.asarray(diameters_nm, dtype=np.float64).reshape(-1))
         T, nd = int(m.shape[0]), int(d.shape[0])
         need = int(self.lib.lss_mie_tables_workspace_bytes(_ptr(m), _ptr(wl), T, _ptr(d), nd))
-        with torch.cuda.device(self.device):
-            out = torch.empty((T, nd, 2), dtype=torch.float64, device=self.device)
-            ws = torch.empty(max(need, 0) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_mie_tables(self.h, _ptr(m), _ptr(wl), T, _ptr(d), nd, _ptr(out), _ptr(ws), int(ws.numel()),
-                                         self._stream())
-        _lib.check(st, self.h)
+        out = torch.empty((T, nd, 2), dtype=torch.float64, device=self.device)
+        ws = torch.empty(max(need, 0) + 256, dtype=torch.uint8, device=self.device)
+        self._call('lss_mie_tables', _ptr(m), _ptr(wl), T, _ptr(d), nd, out, ws, ws.numel())
         return out
 
     def voxelize_batch(self, points, cloud_offsets, point_cloud_range, voxel_size, max_points_per_voxel, max_voxels,
@@ -497,27 +465,19 @@ class SnowfallEngine:
         int32 (B,) valid rows per cloud slot.  Returns dict(voxels (B, max_voxels, max_points, F) float32, coords
         (B, max_voxels, 4) int32 = (cloud, z, y, x), num_points (B, max_voxels) int32, n_voxels (B,) int32).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
-        F = int(points.shape[1])
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        F = points.shape[1]
         rng = np.ascontiguousarray(point_cloud_range, dtype=np.float32).reshape(6)
         vs = np.ascontiguousarray(voxel_size, dtype=np.float32).reshape(3)
         T, MV = int(max_points_per_voxel), int(max_voxels)
-        with torch.cuda.device(self.device):
-            out = dict(voxels=torch.empty((B, MV, T, F), dtype=torch.float32, device=self.device),
-                       coords=torch.empty((B, MV, 4), dtype=torch.int32, device=self.device),
-                       num_points=torch.empty((B, MV), dtype=torch.int32, device=self.device),
-                       n_voxels=torch.empty((B,), dtype=torch.int32, device=self.device))
-            need = self.lib.lss_voxelize_workspace_bytes(N, B, T, MV)
-            if getattr(self, '_ws_vox', None) is None or self._ws_vox.numel() < need:
-                self._ws_vox = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_voxelize_batch(self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, _ptr(rng), _ptr(vs), T, MV,
-                                             1 if mask_xy_range else 0, _ptr(out['voxels']), _ptr(out['coords']),
-                                             _ptr(out['num_points']), _ptr(out['n_voxels']), _ptr(self._ws_vox),
-                                             int(self._ws_vox.numel()), self._stream())
-        _lib.check(st, self.h)
+        out = _outputs(None, self.device, voxels=((B, MV, T, F), torch.float32), coords=((B, MV, 4), torch.int32),
+                       num_points=((B, MV), torch.int32), n_voxels=((B,), torch.int32))
+        ws = self._scratch('voxelize', self.lib.lss_voxelize_workspace_bytes(N, B, T, MV))
+        self._call('lss_voxelize_batch', points, F, _ptr(off), counts, B, _ptr(rng), _ptr(vs), T, MV,
+                   1 if mask_xy_range else 0, out['voxels'], out['coords'], out['num_points'], out['n_voxels'], ws,
+                   ws.numel())
         return out
 
     def dror_batch(self, points, cloud_offsets, alpha=0.16, beta=3.0, k_min=3, sr_min=0.04, counts=None, crop=False,
@@ -530,37 +490,22 @@ class SnowfallEngine:
         cube, counts int32 (B,) kept rows, n_snow int32 (B,) [, points (N, F) kept rows slot-compacted in input order]
         [, work: uint64 CUDA tensor (4,) = queries, cells visited, candidates tested, early exits]).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
-        assert points.dim() == 2
-        F = int(points.shape[1])
-        if counts is not None:
-            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        F = points.shape[1]
         flags = (_lib.DROR_CUBE if crop else 0) | (_lib.DROR_WORK_STATS if work_stats else 0)
-        with torch.cuda.device(self.device):
-            if out is None:
-                out = {}
-            if 'keep' not in out:
-                out.update(keep=torch.empty((N,), dtype=torch.uint8, device=self.device),
-                           counts=torch.empty((B,), dtype=torch.int32, device=self.device),
-                           n_snow=torch.empty((B,), dtype=torch.int32, device=self.device))
-            if want_points and 'points' not in out:
-                out['points'] = torch.empty((N, F), dtype=torch.float32, device=self.device)
-            need = self.lib.lss_dror_workspace_bytes(N, B)
-            if need < 0:
-                raise RuntimeError('lss_dror_workspace_bytes failed (no usable CUDA device?)')
-            if getattr(self, '_ws_dror', None) is None or self._ws_dror.numel() < need:
-                self._ws_dror = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_dror_batch(self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, float(alpha), float(beta),
-                                         int(k_min), float(sr_min), flags, _ptr(out['keep']),
-                                         _ptr(out['points']) if want_points else None, _ptr(out['counts']),
-                                         _ptr(out['n_snow']), _ptr(self._ws_dror), int(self._ws_dror.numel()),
-                                         self._stream())
-            _lib.check(st, self.h)
-            if work_stats:
-                out['work'] = self._ws_dror[:32].view(torch.int64).clone()
+        out = _outputs(out, self.device, keep=((N,), torch.uint8), counts=((B,), torch.int32),
+                       n_snow=((B,), torch.int32), points=want_points and ((N, F), torch.float32))
+        need = self.lib.lss_dror_workspace_bytes(N, B)
+        if need < 0:
+            raise RuntimeError('lss_dror_workspace_bytes failed (no usable CUDA device?)')
+        ws = self._scratch('dror', need)
+        self._call('lss_dror_batch', points, F, _ptr(off), counts, B, float(alpha), float(beta), int(k_min),
+                   float(sr_min), flags, out['keep'], out['points'] if want_points else None, out['counts'],
+                   out['n_snow'], ws, ws.numel())
+        if work_stats:
+            out['work'] = ws[:32].view(torch.int64).clone()
         return out
 
     def strongest_last_batch(self, last, last_offsets, strongest, strongest_offsets, min_dist=3.0, last_counts=None,
@@ -573,40 +518,34 @@ class SnowfallEngine:
         cloud's kept master rows at the front of its slot; offsets int64 host array (B + 1) of those slots; counts (B,)
         int32; master_is_strongest (B,) uint8 [, mask (N_out,) uint8: compare_points' mask on each slot's master rows]).
         """
-        off_l = np.ascontiguousarray(last_offsets, dtype=np.int64)
-        off_s = np.ascontiguousarray(strongest_offsets, dtype=np.int64)
-        B = off_l.shape[0] - 1
-        if off_s.shape != off_l.shape:
+        off_l, B, N_l = _cloud_offsets(last_offsets, 'last_offsets')
+        off_s, B_s, N_s = _cloud_offsets(strongest_offsets, 'strongest_offsets')
+        if B_s != B:
             raise ValueError('last and strongest need the same number of clouds')
-        for pts, off in ((last, off_l), (strongest, off_s)):
+        for off in (off_l, off_s):
             if off[0] != 0 or (np.diff(off) < 0).any():              # (the workspace query cannot say why it fails)
                 raise ValueError('cloud_offsets must start at 0 and be non-decreasing')
-            assert pts.is_cuda and pts.dtype == torch.float32 and pts.is_contiguous() and pts.dim() == 2
-            assert pts.shape[0] == int(off[-1])
+        _check_tensor('last', last, self.device, torch.float32, (N_l, None), min_cols=3)
+        _check_tensor('strongest', strongest, self.device, torch.float32, (N_s, None), min_cols=3)
         if last.shape[1] != strongest.shape[1]:
             raise ValueError('last and strongest need the same number of columns')
-        F = int(last.shape[1])
-        for c in (last_counts, strongest_counts):
-            if c is not None:
-                assert c.is_cuda and c.dtype == torch.int32 and c.shape == (B,)
+        _check_tensor('last_counts', last_counts, self.device, torch.int32, (B,), optional=True)
+        _check_tensor('strongest_counts', strongest_counts, self.device, torch.int32, (B,), optional=True)
+        F = last.shape[1]
         off_o = np.concatenate([[0], np.cumsum(np.maximum(np.diff(off_l), np.diff(off_s)))]).astype(np.int64)
         N = int(off_o[-1])
-        with torch.cuda.device(self.device):
-            out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device), offsets=off_o,
-                       counts=torch.empty((B,), dtype=torch.int32, device=self.device),
-                       master_is_strongest=torch.empty((B,), dtype=torch.uint8, device=self.device))
-            if want_mask:
-                out['mask'] = torch.zeros((N,), dtype=torch.uint8, device=self.device)
-            need = self.lib.lss_strongest_last_batch_workspace_bytes(_ptr(off_l), _ptr(off_s), B)
-            if need < 0:
-                raise RuntimeError('lss_strongest_last_batch_workspace_bytes failed (bad offsets or no CUDA device?)')
-            if getattr(self, '_ws_sel', None) is None or self._ws_sel.numel() < need:
-                self._ws_sel = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_strongest_last_batch(
-                self.h, _ptr(last), _ptr(off_l), _ptr(last_counts), _ptr(strongest), _ptr(off_s), _ptr(strongest_counts),
-                F, B, float(min_dist), _ptr(out['points']), _ptr(out['counts']), _ptr(out['master_is_strongest']),
-                _ptr(out.get('mask')), _ptr(self._ws_sel), int(self._ws_sel.numel()), self._stream())
-        _lib.check(st, self.h)
+        out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device), offsets=off_o,
+                   counts=torch.empty((B,), dtype=torch.int32, device=self.device),
+                   master_is_strongest=torch.empty((B,), dtype=torch.uint8, device=self.device))
+        if want_mask:
+            out['mask'] = torch.zeros((N,), dtype=torch.uint8, device=self.device)
+        need = self.lib.lss_strongest_last_batch_workspace_bytes(_ptr(off_l), _ptr(off_s), B)
+        if need < 0:
+            raise RuntimeError('lss_strongest_last_batch_workspace_bytes failed (bad offsets or no CUDA device?)')
+        ws = self._scratch('strongest_last', need)
+        self._call('lss_strongest_last_batch', last, _ptr(off_l), last_counts, strongest, _ptr(off_s), strongest_counts,
+                   F, B, float(min_dist), out['points'], out['counts'], out['master_is_strongest'], out.get('mask'), ws,
+                   ws.numel())
         return out
 
     def camera_fov_batch(self, points, cloud_offsets, counts=None, img_shapes=None, want_mask=False):
@@ -618,28 +557,18 @@ class SnowfallEngine:
         float32, each cloud's rows inside the image at the front of its slot; counts (B,) int32 -- 0 where the dataset
         would draw another sample [, mask (N,) uint8 flag of every valid row]).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
-        assert points.dim() == 2
-        F = int(points.shape[1])
-        if counts is not None:
-            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        F = points.shape[1]
         shp = None if img_shapes is None else np.ascontiguousarray(
             np.broadcast_to(np.asarray(img_shapes, dtype=np.int32).reshape(-1, 2), (B, 2)))
-        with torch.cuda.device(self.device):
-            out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device),
-                       counts=torch.empty((B,), dtype=torch.int32, device=self.device))
-            if want_mask:
-                out['mask'] = torch.zeros((N,), dtype=torch.uint8, device=self.device)
-            need = self.lib.lss_camera_fov_batch_workspace_bytes(N, B)
-            if getattr(self, '_ws_fov', None) is None or self._ws_fov.numel() < need:
-                self._ws_fov = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_camera_fov_batch(self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, _ptr(shp),
-                                               _ptr(out['points']), _ptr(out['counts']), _ptr(out.get('mask')),
-                                               _ptr(self._ws_fov), int(self._ws_fov.numel()), self._stream())
-        _lib.check(st, self.h)
+        out = _outputs(None, self.device, points=((N, F), torch.float32), counts=((B,), torch.int32))
+        if want_mask:
+            out['mask'] = torch.zeros((N,), dtype=torch.uint8, device=self.device)
+        ws = self._scratch('camera_fov', self.lib.lss_camera_fov_batch_workspace_bytes(N, B))
+        self._call('lss_camera_fov_batch', points, F, _ptr(off), counts, B, _ptr(shp), out['points'], out['counts'],
+                   out.get('mask'), ws, ws.numel())
         return out
 
     def lisa_cloud_batch(self, points, cloud_offsets, rain_rate, alpha, seed, mode, r_min=0.9, r_max=120.0,
@@ -653,34 +582,35 @@ class SnowfallEngine:
         copied through); draw_table: CUDA float64 fixed-seed draw sequence or None.  Returns dict(points (N, F) float32:
         each cloud's kept rows at the front of its slot, label in column 4; counts (B,) int32; n_lost (B,) int32).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        N = int(off[-1])
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.shape[0] == N
-        assert points.dim() == 2
-        F = int(points.shape[1])
-        if counts is not None:
-            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
-        if draw_table is not None:
-            assert draw_table.is_cuda and draw_table.dtype == torch.float64 and draw_table.is_contiguous()
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=5)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        _check_tensor('draw_table', draw_table, self.device, torch.float64, optional=True)
+        F = points.shape[1]
         rr, al = [np.ascontiguousarray(np.broadcast_to(np.asarray(v, dtype=np.float64), (B,))) for v in (rain_rate, alpha)]
         sd = None if seed is None else np.ascontiguousarray(np.broadcast_to(np.asarray(seed, dtype=np.uint64), (B,)))
         ap = None if apply is None else np.ascontiguousarray(np.asarray(apply, dtype=bool).reshape(B), dtype=np.uint8)
-        with torch.cuda.device(self.device):
-            out = dict(points=torch.empty((N, F), dtype=torch.float32, device=self.device),
-                       counts=torch.empty((B,), dtype=torch.int32, device=self.device),
-                       n_lost=torch.empty((B,), dtype=torch.int32, device=self.device))
-            need = self.lib.lss_lisa_cloud_batch_workspace_bytes(N, B)
-            if getattr(self, '_ws_lisa', None) is None or self._ws_lisa.numel() < need:
-                self._ws_lisa = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_lisa_cloud_batch(
-                self.h, _ptr(points), F, _ptr(off), _ptr(counts), B, _ptr(rr), _ptr(al), _ptr(sd), _ptr(ap), int(mode),
-                float(r_min), float(r_max), float(beam_divergence), float(min_diameter), float(range_accuracy),
-                1 if signal_last else 0, _ptr(draw_table), 0 if draw_table is None else int(draw_table.numel()),
-                _ptr(out['points']), _ptr(out['counts']), _ptr(out['n_lost']), _ptr(self._ws_lisa),
-                int(self._ws_lisa.numel()), self._stream())
-        _lib.check(st, self.h)
+        out = _outputs(None, self.device, points=((N, F), torch.float32), counts=((B,), torch.int32),
+                       n_lost=((B,), torch.int32))
+        ws = self._scratch('lisa', self.lib.lss_lisa_cloud_batch_workspace_bytes(N, B))
+        self._call('lss_lisa_cloud_batch', points, F, _ptr(off), counts, B, _ptr(rr), _ptr(al), _ptr(sd), _ptr(ap),
+                   int(mode), float(r_min), float(r_max), float(beam_divergence), float(min_diameter),
+                   float(range_accuracy), 1 if signal_last else 0, draw_table,
+                   0 if draw_table is None else draw_table.numel(), out['points'], out['counts'], out['n_lost'], ws,
+                   ws.numel())
         return out
+
+    def _pa_args(self, points, cloud_offsets, planes, nparts, box_offsets, counts):
+        """(off, B, boff, M) of the arguments pa_partition_batch and pa_apply_batch share, checked"""
+        off, B, N = _cloud_offsets(cloud_offsets)
+        boff, B_boxes, M = _cloud_offsets(box_offsets, 'box_offsets')
+        if B_boxes != B:
+            raise ValueError(f'box_offsets: {B_boxes + 1} entries for {B} clouds')
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=3)
+        _check_tensor('planes', planes, self.device, torch.float64, (M, 9, 6, 4))
+        _check_tensor('nparts', nparts, self.device, torch.int32, (M,))
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        return off, B, boff, M
 
     def pa_partition_batch(self, points, cloud_offsets, planes, nparts, box_offsets, boxes_f64, counts=None):
         """
@@ -690,28 +620,15 @@ class SnowfallEngine:
         (8 * M + B,) class totals (cloud b's classes at 8 * box_offsets[b] + b: 8 per box, then its background).
         The partition stays in this engine's PA-AUG workspace for pa_apply_batch.
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        boff = np.ascontiguousarray(box_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.dim() == 2
-        assert points.shape[0] == int(off[-1]) and boff.shape == off.shape
-        M = int(boff[-1])
-        assert planes.is_cuda and planes.dtype == torch.float64 and planes.shape[0] == M and nparts.shape == (M,)
-        if counts is not None:
-            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        off, B, boff, M = self._pa_args(points, cloud_offsets, planes, nparts, box_offsets, counts)
         need = self.lib.lss_pa_partition_workspace_bytes(_ptr(off), _ptr(boff), B)
         if need < 0:
             raise ValueError('bad cloud_offsets / box_offsets (at most 256 boxes per cloud)')
-        with torch.cuda.device(self.device):
-            totals = torch.empty((8 * M + B,), dtype=torch.int32, device=self.device)
-            if getattr(self, '_ws_pa', None) is None or self._ws_pa.numel() < need:
-                self._ws_pa = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            self._pa_part_bytes = int(need)
-            st = self.lib.lss_pa_partition_batch(self.h, _ptr(points), int(points.shape[1]), _ptr(off), _ptr(counts), B,
-                                                 _ptr(planes), _ptr(nparts), _ptr(boff), 1 if boxes_f64 else 0,
-                                                 _ptr(totals), _ptr(self._ws_pa), int(self._ws_pa.numel()),
-                                                 self._stream())
-        _lib.check(st, self.h)
+        totals = torch.empty((8 * M + B,), dtype=torch.int32, device=self.device)
+        ws = self._scratch('pa', need)
+        self._pa_part_bytes = int(need)
+        self._call('lss_pa_partition_batch', points, points.shape[1], _ptr(off), counts, B, planes, nparts, _ptr(boff),
+                   1 if boxes_f64 else 0, totals, ws, ws.numel())
         return totals
 
     def pa_apply_batch(self, points, cloud_offsets, planes, nparts, box_offsets, boxes_f64, class_start, n_members,
@@ -723,31 +640,30 @@ class SnowfallEngine:
         Plan tables: CUDA tensors as include/lidar_snow_sim.h describes them.  Returns CUDA (n_out, 4) out_dtype
         (torch.float32 or torch.float64).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        boff = np.ascontiguousarray(box_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        assert out_dtype in (torch.float32, torch.float64)
-        for t in (class_start, fps_segs, fps_jobs, segs):
-            assert t.is_cuda and t.dtype == torch.int64 and t.is_contiguous()
-        for t in (steps, noise, normals):
-            assert t.is_cuda and t.dtype == torch.float64 and t.is_contiguous()
+        off, B, boff, M = self._pa_args(points, cloud_offsets, planes, nparts, box_offsets, counts)
+        if out_dtype not in (torch.float32, torch.float64):
+            raise ValueError(f'out_dtype: expected torch.float32 or torch.float64, got {out_dtype}')
+        _check_tensor('class_start', class_start, self.device, torch.int64, (8 * M + B,))
+        for name, t, cols in (('fps_segs', fps_segs, 6), ('fps_jobs', fps_jobs, 5), ('segs', segs, 6)):
+            _check_tensor(name, t, self.device, torch.int64, (None, cols))
+        for name, t, cols in (('steps', steps, 12), ('noise', noise, 4), ('normals', normals, 4)):
+            _check_tensor(name, t, self.device, torch.float64, (None, cols))
+        if self._pa_part_bytes is None:
+            raise RuntimeError('pa_apply_batch needs the partition of a pa_partition_batch call on this engine first')
         need = self.lib.lss_pa_apply_workspace_bytes(_ptr(off), _ptr(boff), B, int(n_members), int(n_fps_rows),
                                                      int(n_fps_out))
         if need < 0:
             raise ValueError('bad PA-AUG plan sizes')
-        with torch.cuda.device(self.device):
-            if self._ws_pa.numel() < need:                        # keep the partition: it lives at the front
-                ws = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-                ws[:self._pa_part_bytes].copy_(self._ws_pa[:self._pa_part_bytes])
-                self._ws_pa = ws
-            out = torch.empty((int(n_out), 4), dtype=out_dtype, device=self.device)
-            st = self.lib.lss_pa_apply_batch(
-                self.h, _ptr(points), int(points.shape[1]), _ptr(off), _ptr(counts), B, _ptr(planes), _ptr(nparts),
-                _ptr(boff), 1 if boxes_f64 else 0, _ptr(class_start), int(n_members), _ptr(fps_segs),
-                int(fps_segs.shape[0]), int(n_fps_rows), _ptr(fps_jobs), int(fps_jobs.shape[0]), int(n_fps_out),
-                _ptr(segs), int(segs.shape[0]), _ptr(steps), _ptr(noise), _ptr(normals), int(n_out), _ptr(out),
-                1 if out_dtype == torch.float64 else 0, _ptr(self._ws_pa), int(self._ws_pa.numel()), self._stream())
-        _lib.check(st, self.h)
+        ws = self._scratch_ws['pa']
+        if ws.numel() < need:                                     # keep the partition: it lives at the front
+            ws = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            ws[:self._pa_part_bytes].copy_(self._scratch_ws['pa'][:self._pa_part_bytes])
+            self._scratch_ws['pa'] = ws
+        out = torch.empty((int(n_out), 4), dtype=out_dtype, device=self.device)
+        self._call('lss_pa_apply_batch', points, points.shape[1], _ptr(off), counts, B, planes, nparts, _ptr(boff),
+                   1 if boxes_f64 else 0, class_start, int(n_members), fps_segs, fps_segs.shape[0], int(n_fps_rows),
+                   fps_jobs, fps_jobs.shape[0], int(n_fps_out), segs, segs.shape[0], steps, noise, normals, int(n_out),
+                   out, 1 if out_dtype == torch.float64 else 0, ws, ws.numel())
         return out
 
     def gt_collide_batch(self, boxes, box_offsets, n_gt, class_offsets, bits_offsets, max_pairs, n_pairs, n_classes):
@@ -756,18 +672,16 @@ class SnowfallEngine:
         (M, 11); box_offsets (B + 1,) / bits_offsets (B,) CUDA int64; n_gt (B,) / class_offsets (B, 9) CUDA int32.
         Returns (valid, bits): CUDA uint8 (M,) and (n_pairs,).
         """
-        B = int(n_gt.shape[0])
-        assert boxes.is_cuda and boxes.dtype == torch.float32 and boxes.is_contiguous() and boxes.shape[1] == 11
-        for t, dt in ((box_offsets, torch.int64), (bits_offsets, torch.int64), (n_gt, torch.int32),
-                      (class_offsets, torch.int32)):
-            assert t.is_cuda and t.dtype == dt and t.is_contiguous()
-        with torch.cuda.device(self.device):
-            valid = torch.empty((boxes.shape[0],), dtype=torch.uint8, device=self.device)
-            bits = torch.empty((max(int(n_pairs), 1),), dtype=torch.uint8, device=self.device)
-            st = self.lib.lss_gt_collide_batch(self.h, B, int(n_classes), _ptr(boxes), _ptr(box_offsets), _ptr(n_gt),
-                                               _ptr(class_offsets), _ptr(bits_offsets), int(max_pairs), _ptr(bits),
-                                               _ptr(valid), self._stream())
-        _lib.check(st, self.h)
+        _check_tensor('n_gt', n_gt, self.device, torch.int32, (None,))
+        B = n_gt.shape[0]
+        _check_tensor('boxes', boxes, self.device, torch.float32, (None, 11))
+        _check_tensor('box_offsets', box_offsets, self.device, torch.int64, (B + 1,))
+        _check_tensor('class_offsets', class_offsets, self.device, torch.int32, (B, 9))
+        _check_tensor('bits_offsets', bits_offsets, self.device, torch.int64, (B,))
+        valid = torch.empty((boxes.shape[0],), dtype=torch.uint8, device=self.device)
+        bits = torch.empty((max(int(n_pairs), 1),), dtype=torch.uint8, device=self.device)
+        self._call('lss_gt_collide_batch', B, int(n_classes), boxes, box_offsets, n_gt, class_offsets, bits_offsets,
+                   int(max_pairs), bits, valid)
         return valid, bits[:int(n_pairs)]
 
     def gt_paste_batch(self, points, cloud_offsets, rm_boxes, rm_offsets, max_rm, ops, db, objects, object_shift,
@@ -778,26 +692,27 @@ class SnowfallEngine:
         laid out as include/lidar_snow_sim.h describes them.  Returns (rows, counts): CUDA float32 (n_out, F) in the
         slots out_offsets, and CUDA int32 (B,).
         """
-        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
-        B = off.shape[0] - 1
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous() and points.dim() == 2
-        assert points.shape[0] == int(off[-1]) and db.shape[1] == points.shape[1]
-        if counts is not None:
-            assert counts.is_cuda and counts.dtype == torch.int32 and counts.shape == (B,)
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=3)
+        F = points.shape[1]
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        _check_tensor('rm_boxes', rm_boxes, self.device, torch.float32)              # rows of 9, flat
+        _check_tensor('rm_offsets', rm_offsets, self.device, torch.int64, (B + 1,))
+        _check_tensor('ops', ops, self.device, torch.float32, (B, None, 3))
+        _check_tensor('db', db, self.device, torch.float32, (None, F))
+        _check_tensor('objects', objects, self.device, torch.int64, (None, 4))
+        _check_tensor('object_shift', object_shift, self.device, torch.float64, (objects.shape[0], 4))
+        _check_tensor('out_offsets', out_offsets, self.device, torch.int64, (B + 1,))
+        _check_tensor('object_rows', object_rows, self.device, torch.int32, (B,))
         need = self.lib.lss_gt_paste_workspace_bytes(_ptr(off), B)
         if need < 0:
             raise ValueError('bad cloud_offsets')
-        with torch.cuda.device(self.device):
-            if getattr(self, '_ws_gt', None) is None or self._ws_gt.numel() < need:
-                self._ws_gt = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            out = torch.empty((int(n_out), points.shape[1]), dtype=torch.float32, device=self.device)
-            out_counts = torch.empty((B,), dtype=torch.int32, device=self.device)
-            st = self.lib.lss_gt_paste_batch(
-                self.h, _ptr(points), int(points.shape[1]), _ptr(off), _ptr(counts), B, _ptr(rm_boxes),
-                _ptr(rm_offsets), int(max_rm), _ptr(ops), int(ops.shape[1]), _ptr(db), _ptr(objects),
-                _ptr(object_shift), int(objects.shape[0]), int(n_object_rows), _ptr(out_offsets), _ptr(object_rows),
-                _ptr(out), _ptr(out_counts), _ptr(self._ws_gt), int(self._ws_gt.numel()), self._stream())
-        _lib.check(st, self.h)
+        ws = self._scratch('gt_paste', need)
+        out = torch.empty((int(n_out), F), dtype=torch.float32, device=self.device)
+        out_counts = torch.empty((B,), dtype=torch.int32, device=self.device)
+        self._call('lss_gt_paste_batch', points, F, _ptr(off), counts, B, rm_boxes, rm_offsets, int(max_rm), ops,
+                   ops.shape[1], db, objects, object_shift, objects.shape[0], int(n_object_rows), out_offsets,
+                   object_rows, out, out_counts, ws, ws.numel())
         return out, out_counts
 
     def gather_push(self, points, counts, d_cloud_offsets, n_rows, world, rank, peer_points, peer_counts, mc_points=0,
@@ -806,21 +721,24 @@ class SnowfallEngine:
         every rank's gathered buffers (SURVEY.md 8e).  peer_points / peer_counts: per rank, a CUDA tensor mapping that
         rank's gathered buffer (world * n_rows, 5) float32 / (world * n_clouds,) int32 into this process (see
         distributed.BatchGather, which owns the symmetric allocations and the side stream)."""
-        B = int(d_cloud_offsets.shape[0]) - 1
-        assert points.is_cuda and points.dtype == torch.float32 and points.is_contiguous()
-        assert d_cloud_offsets.is_cuda and d_cloud_offsets.dtype == torch.int64
-        P = ctypes.c_void_p * int(world)
-        pp = P(*[t.data_ptr() for t in peer_points])
-        pc = P(*[t.data_ptr() for t in peer_counts])
-        with torch.cuda.device(self.device):
-            st = self.lib.lss_gather_push(self.h, _ptr(points), _ptr(counts), _ptr(d_cloud_offsets), B, int(n_rows), int(world),
-                                          int(rank), pp, pc, mc_points or None, mc_counts or None, int(blocks), self._stream())
-        _lib.check(st, self.h)
+        _check_tensor('d_cloud_offsets', d_cloud_offsets, self.device, torch.int64, (None,))
+        B = d_cloud_offsets.shape[0] - 1
+        _check_tensor('points', points, self.device, torch.float32, (None, 5))
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        peer_points, peer_counts, world = list(peer_points), list(peer_counts), int(world)
+        if len(peer_points) != world or len(peer_counts) != world:
+            raise ValueError(f'peer_points / peer_counts: {len(peer_points)} / {len(peer_counts)} buffers for {world} ranks')
+        for r in range(world):                  # mappings of the other ranks' buffers: any device
+            _check_tensor(f'peer_points[{r}]', peer_points[r], None, torch.float32, (world * int(n_rows), 5))
+            _check_tensor(f'peer_counts[{r}]', peer_counts[r], None, torch.int32, (world * B,))
+        P = ctypes.c_void_p * world
+        self._call('lss_gather_push', points, counts, d_cloud_offsets, B, int(n_rows), world, int(rank),
+                   P(*[t.data_ptr() for t in peer_points]), P(*[t.data_ptr() for t in peer_counts]), mc_points or None,
+                   mc_counts or None, int(blocks))
 
     def check(self):
         """Synchronise the current stream and raise the exception type the reference would have raised."""
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.lss_check_async(self.h, self._stream()), self.h)
+        self._call('lss_check_async')
 
     def launch_count(self):
         return int(self.lib.lss_launch_count(self.h))

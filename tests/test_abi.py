@@ -79,11 +79,32 @@ def test_focal_offset_matches_python():
         assert (1 - v * 100 / 13100) ** 2 == t * t          # simulation.py:76: pow(x, 2) == x*x for these values
 
 
-def _header_params(name):
+def _header_decl(name):
+    """(return type, [parameter declarations]) of `name` in include/lidar_snow_sim.h"""
     txt = open(os.path.join(ROOT, 'include', 'lidar_snow_sim.h')).read()
-    m = re.search(r'LSS_API[^;(]*?\b' + name + r'\s*\(([^;]*?)\)\s*;', txt, re.S)
+    m = re.search(r'LSS_API\s+([^;(]*?)\b' + name + r'\s*\(([^;]*?)\)\s*;', txt, re.S)
     assert m, name
-    return [p.strip() for p in m.group(1).split(',') if p.strip()]
+    return m.group(1).strip(), [p.strip() for p in m.group(2).split(',') if p.strip()]
+
+
+def _header_params(name):
+    return _header_decl(name)[1]
+
+
+_CTYPES = {'int': ctypes.c_int, 'int64_t': ctypes.c_int64, 'uint32_t': ctypes.c_uint32, 'uint64_t': ctypes.c_uint64,
+           'double': ctypes.c_double, 'lss_status': ctypes.c_int}
+
+
+def _binds(c_type, bound):
+    """whether the ctypes type `bound` is the binding of C type `c_type` (a declaration without its name)"""
+    words = c_type.replace('*', ' * ').replace('const', ' ').split()
+    if words == ['void']:
+        return bound is None
+    if words == ['char', '*']:
+        return bound is ctypes.c_char_p
+    if '*' in words:
+        return bound is ctypes.c_void_p or (isinstance(bound, type) and issubclass(bound, ctypes._Pointer))
+    return len(words) == 1 and bound is _CTYPES.get(words[0])
 
 
 def _call_args(text, call):
@@ -108,12 +129,17 @@ def _call_args(text, call):
 
 
 def test_signatures_and_documented_calls_have_the_header_arity():
-    """ctypes argtypes and the raw C-ABI examples of INTEGRATION.md follow the header's parameter lists."""
+    """ctypes restypes and argtypes and the raw C-ABI examples of INTEGRATION.md follow the header's declarations: the
+    same number of parameters, each bound as its C type (int c_int, int64_t c_int64, a pointer c_void_p or POINTER)."""
     from lidar_snow_sim_b200 import _lib
-    for name, _, argtypes in _lib.SIGNATURES:
-        params = _header_params(name)
-        n = 0 if params == ['void'] else len(params)
-        assert n == len(argtypes), f'{name}: header has {n} parameters, _lib.SIGNATURES {len(argtypes)}'
+    for name, restype, argtypes in _lib.SIGNATURES:
+        ret, params = _header_decl(name)
+        params = [] if params == ['void'] else params
+        assert len(params) == len(argtypes), f'{name}: header has {len(params)} parameters, _lib.SIGNATURES {len(argtypes)}'
+        assert _binds(ret, restype), f'{name}: returns {ret}, bound as {restype}'
+        for k, (p, a) in enumerate(zip(params, argtypes)):
+            c_type = re.sub(r'\b\w+$', '', p)                          # without the parameter's name
+            assert _binds(c_type, a), f'{name}: parameter {k} is {p!r}, bound as {a}'
     doc = open(os.path.join(ROOT, 'INTEGRATION.md')).read()
     for call, name in (('L.lss_snowfall_batch', 'lss_snowfall_batch'),
                        ('\nlss_snowfall_batch_host_submit', 'lss_snowfall_batch_host_submit')):
