@@ -442,6 +442,41 @@ LSS_API lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int 
                                       int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_voxelize_workspace_bytes(int64_t n_total, int n_clouds, int max_points_per_voxel, int max_voxels);
 
+/* ---- DATA_PROCESSOR: feature encoding, range mask, shuffle_points, voxels ----------------------------------------------
+ * prepare_data's tail (lib/OpenPCDet/pcdet/datasets/dataset.py:161-166) on a batch of device-resident clouds:
+ *   PointFeatureEncoder.absolute_coordinates_encoding   processor/point_feature_encoder.py:43-56: output column c is
+ *                                                       input column h_columns[c]; columns 0, 1, 2 are x, y, z
+ *   mask_points_and_boxes_outside_range (points)        data_processor.py:78-91 with mask_points != 0: x and y inside
+ *                                                       h_point_cloud_range, both ends inclusive, compared in double
+ *   shuffle_points                                      data_processor.py:93-103 with h_mt_state != NULL: cloud after
+ *                                                       cloud, exactly np.random.permutation(n_b) on the RandomState
+ *   transform_points_to_voxels                          lss_voxelize_batch on the result (mask_xy_range 0) when
+ *                                                       h_voxel_size != NULL
+ *   h_mt_state          uint32[625]: np.random.get_state()'s 624 key words, then pos (0 .. 624)
+ *   d_mt_state_out      uint32[625] device: key words and pos after the last draw (= h_mt_state when nothing is drawn)
+ *   h_point_cloud_range float64[6] (x0, y0, z0, x1, y1, z1); the voxel grid uses its float32 values
+ *   d_out_points        float32[n_total * n_features_out]: cloud b's rows at the front of its slot, d_out_counts[b] of them
+ *   d_out_voxels ...    as lss_voxelize_batch, with n_features_out features
+ * Asynchronous on `stream`; the counts stay on the device.  d_workspace: lss_processor_workspace_bytes(n_total, n_clouds,
+ * n_features_out, max_points_per_voxel, max_voxels) bytes (max_voxels 0 without voxels).                                 */
+LSS_API lss_status lss_processor_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                       const int32_t *d_cloud_counts, int n_clouds, const int32_t *h_columns,
+                                       int n_features_out, const double *h_point_cloud_range, int mask_points,
+                                       const uint32_t *h_mt_state, uint32_t *d_mt_state_out, const float *h_voxel_size,
+                                       int max_points_per_voxel, int max_voxels, float *d_out_points,
+                                       int32_t *d_out_counts, float *d_out_voxels, int32_t *d_out_coords,
+                                       int32_t *d_out_num_points, int32_t *d_out_n_voxels, void *d_workspace,
+                                       int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_processor_workspace_bytes(int64_t n_total, int n_clouds, int n_features_out, int max_points_per_voxel,
+                                              int max_voxels);
+/* The permutations themselves: d_out_perm[h_cloud_offsets[b] + r], r < n_b (d_cloud_counts[b], or the slot's length), is
+ * np.random.permutation(n_b)[r] for the clouds in turn on h_mt_state; d_mt_state_out as above.  d_workspace:
+ * lss_processor_workspace_bytes(n_total, n_clouds, 0, 0, 0) bytes.  Asynchronous on `stream`.                            */
+LSS_API lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts,
+                                            int n_clouds, const uint32_t *h_mt_state, int32_t *d_out_perm,
+                                            uint32_t *d_mt_state_out, void *d_workspace, int64_t workspace_bytes,
+                                            void *stream);
+
 /* ---- DROR snow removal ------------------------------------------------------------------------------------------------
  * Dynamic Radius Outlier Removal, dynamic_radius_outlier_filter (lib/cadc_devkit/other/dror.py:288-334), for every cloud of
  * a batch, as the dataset applies it under its DROR / DROR++ keys (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:588-616).

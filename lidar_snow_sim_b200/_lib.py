@@ -114,6 +114,10 @@ SIGNATURES = [
     ('lss_voxelize_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P,
                                       _P, _P, _c.c_int64, _P]),
     ('lss_voxelize_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int]),
+    ('lss_processor_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _c.c_int, _P, _c.c_int, _P, _P, _P,
+                                       _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_processor_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
+    ('lss_mt19937_permutations', _c.c_int, [_P, _P, _P, _c.c_int, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_dror_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_int, _c.c_double,
                                   _c.c_uint32, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_dror_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),

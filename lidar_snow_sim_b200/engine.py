@@ -81,6 +81,25 @@ def _outputs(out, device, **spec):
     return out
 
 
+def _mt_state():
+    """(words, state): NumPy's global RandomState as the 625 words the library reads (key, pos), and get_state()"""
+    st = np.random.get_state()
+    if st[0] != 'MT19937':
+        raise ValueError(f'NumPy\'s global generator is {st[0]}, not MT19937')
+    words = np.empty(625, np.uint32)
+    words[:624] = st[1]
+    words[624] = int(st[2])
+    return words, st
+
+
+def _set_mt_state(state, d_words):
+    """set NumPy's global RandomState to the device's final words (one synchronising 2.5 KB copy); the cached Gaussian
+    is untouched, as the permutations draw none"""
+    w = d_words.cpu().numpy().view(np.uint32)
+    _, _, _, has_gauss, gauss = state[1]
+    np.random.set_state(('MT19937', w[:624].copy(), int(w[624]), has_gauss, gauss))
+
+
 def _snowfall_flags(threshold_filter, camera_fov, device_prepass, assume_sorted=False):
     return ((_lib.FLAG_THRESHOLD_FILTER if threshold_filter else 0) | (_lib.FLAG_CAMERA_FOV if camera_fov else 0)
             | (_lib.FLAG_DEVICE_PREPASS if device_prepass else 0) | (_lib.FLAG_ASSUME_SORTED if assume_sorted else 0))
@@ -479,6 +498,60 @@ class SnowfallEngine:
                    1 if mask_xy_range else 0, out['voxels'], out['coords'], out['num_points'], out['n_voxels'], ws,
                    ws.numel())
         return out
+
+    def processor_batch(self, points, cloud_offsets, columns, point_cloud_range, counts=None, mask_points=True,
+                        shuffle=True, voxel_size=None, max_points_per_voxel=0, max_voxels=0):
+        """
+        The DataProcessor tail of prepare_data (lss_processor_batch, current stream): feature encoding through the
+        column map `columns` (x, y, z first), mask_points_by_range when mask_points, shuffle_points on NumPy's global
+        RandomState when shuffle (cloud after cloud, exactly np.random.permutation), and with voxel_size the voxels of
+        voxelize_batch.  points: CUDA float32 (N, F); counts: optional CUDA int32 (B,) valid rows per slot.  Returns
+        dict(points (N, len(columns)) float32 rows at the front of each slot, counts (B,) int32 CUDA [, voxels, coords,
+        num_points, n_voxels as voxelize_batch]).  With shuffle, the call synchronises once: it copies the generator's
+        final 625 words back and sets NumPy's state to them.
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        cols = np.ascontiguousarray(columns, dtype=np.int32).reshape(-1)
+        F, Fo = points.shape[1], cols.shape[0]
+        if not 3 <= Fo <= 16 or list(cols[:3]) != [0, 1, 2] or cols.min() < 0 or cols.max() >= F:
+            raise ValueError(f'columns: x, y, z (0, 1, 2) first, then at most 13 of the {F} input columns, got {cols}')
+        rng = np.ascontiguousarray(point_cloud_range, dtype=np.float64).reshape(6)
+        voxels = voxel_size is not None
+        T, MV = (int(max_points_per_voxel), int(max_voxels)) if voxels else (0, 0)
+        if voxels and (T <= 0 or MV <= 0):
+            raise ValueError('max_points_per_voxel > 0 and max_voxels > 0 required')
+        vs = np.ascontiguousarray(voxel_size, dtype=np.float32).reshape(3) if voxels else None
+        state = _mt_state() if shuffle else None
+        out = _outputs(None, self.device, points=((N, Fo), torch.float32), counts=((B,), torch.int32),
+                       state=shuffle and ((625,), torch.int32), voxels=voxels and ((B, MV, T, Fo), torch.float32),
+                       coords=voxels and ((B, MV, 4), torch.int32), num_points=voxels and ((B, MV), torch.int32),
+                       n_voxels=voxels and ((B,), torch.int32))
+        ws = self._scratch('processor', self.lib.lss_processor_workspace_bytes(N, B, Fo, T, MV))
+        self._call('lss_processor_batch', points, F, _ptr(off), counts, B, _ptr(cols), Fo, _ptr(rng),
+                   1 if mask_points else 0, None if state is None else _ptr(state[0]), out.get('state'), _ptr(vs), T,
+                   MV, out['points'], out['counts'], out.get('voxels'), out.get('coords'), out.get('num_points'),
+                   out.get('n_voxels'), ws, ws.numel())
+        if shuffle:
+            _set_mt_state(state, out.pop('state'))
+        return out
+
+    def mt19937_permutations(self, cloud_offsets, counts=None):
+        """
+        np.random.permutation(n_b) for the clouds in turn, drawn on the device from NumPy's global RandomState
+        (lss_mt19937_permutations), whose state is then set as B sequential calls leave it.  n_b = counts[b] (CUDA int32
+        (B,)) or the slot's length.  Returns a CUDA int32 (N,) tensor: cloud b's permutation at rows cloud_offsets[b]..
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        state = _mt_state()
+        out = _outputs(None, self.device, perm=((N,), torch.int32), state=((625,), torch.int32))
+        ws = self._scratch('processor', self.lib.lss_processor_workspace_bytes(N, B, 0, 0, 0))
+        self._call('lss_mt19937_permutations', _ptr(off), counts, B, _ptr(state[0]), out['perm'], out['state'], ws,
+                   ws.numel())
+        _set_mt_state(state, out['state'])
+        return out['perm']
 
     def dror_batch(self, points, cloud_offsets, alpha=0.16, beta=3.0, k_min=3, sr_min=0.04, counts=None, crop=False,
                    want_points=True, work_stats=False, out=None):

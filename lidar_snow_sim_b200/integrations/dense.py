@@ -455,3 +455,42 @@ def data_augmentor_batch(augmentor, points, cloud_offsets, gt_boxes, box_offsets
         raise NotImplementedError('data_augmentor_batch: COMPENSATE without random_world_rotation')
     return augmentor.forward_batch(points, cloud_offsets, gt_boxes, box_offsets, gt_names, counts=counts,
                                    road_planes=road_planes, calib=calib, gt_boxes_mask=gt_boxes_mask, engine=engine)
+
+
+def prepare_data_batch(points, cloud_offsets, gt_boxes, box_offsets, gt_names, class_names, encoder, processor,
+                       augmentor=None, dataset_cfg=None, counts=None, road_planes=None, calib=None, training=True,
+                       engine=None):
+    """
+    DatasetTemplate.prepare_data (pcdet/datasets/dataset.py:116-185) for B device-resident clouds, in batch order:
+    data_augmentor_batch when training, then per cloud keep_arrays_by_name and the class column, then the
+    PointFeatureEncoder (its column map) and the DataProcessor in one processor_batch call.  points / counts are the
+    CUDA rows in slots the blocks before return (cloud b at rows cloud_offsets[b]..); gt_boxes / gt_names host arrays,
+    cloud b's at box_offsets[b]...  Returns processor.forward_batch's dict plus gt_names (per cloud) and 'skipped': host
+    bool (B,), the clouds left without boxes in training.
+    Like the blocks before it, the batch takes NumPy's draws block by block: the B augmentor draws, then the B shuffles.
+    It equals B augmentor.forward calls followed by B (class column, encoder, DataProcessor.forward) calls, NumPy's state
+    included; the per-sample prepare_data interleaves the two (sample b's shuffle before sample b + 1's augmentor draws).
+    For a skipped cloud the reference draws np.random.randint(len(self)) and recurses into another sample; that draw is
+    not taken here, so exactness holds up to the first skipped cloud, and the caller replaces skipped clouds.
+    """
+    off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+    boff = np.ascontiguousarray(box_offsets, dtype=np.int64)
+    B = off.shape[0] - 1
+    names = np.asarray(gt_names)
+    if training:
+        r = data_augmentor_batch(augmentor, points, off, gt_boxes, boff, names, dataset_cfg, counts=counts,
+                                 road_planes=road_planes, calib=calib, engine=engine)
+        points, off, counts, boxes, names_b = r['points'], r['offsets'], r['counts'], r['gt_boxes'], r['gt_names']
+    else:
+        boxes = [gt_boxes[boff[b]:boff[b + 1]] for b in range(B)]
+        names_b = [names[boff[b]:boff[b + 1]] for b in range(B)]
+    for b in range(B):                                                   # dataset.py:150-156
+        selected = np.array([i for i, x in enumerate(names_b[b]) if x in class_names], dtype=np.int64)
+        boxes[b], names_b[b] = boxes[b][selected], names_b[b][selected]
+        classes = np.array([class_names.index(n) + 1 for n in names_b[b]], dtype=np.int32)
+        boxes[b] = np.concatenate((boxes[b], classes.reshape(-1, 1).astype(np.float32)), axis=1)
+    encoder._check_sweeps()
+    res = processor.forward_batch(points, off, counts=counts, gt_boxes=boxes, columns=encoder.columns(), engine=engine)
+    res['gt_names'] = names_b
+    res['skipped'] = np.array([training and len(x) == 0 for x in res['gt_boxes']], dtype=bool)
+    return res
