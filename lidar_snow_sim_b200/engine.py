@@ -20,6 +20,7 @@ DEFAULT_MAX_DIVERGENCE_RAD = 3e-3          # callers pass beam_divergence = degr
 # sample_tables_device calls the sampler at most this often: the darts per plane start at 1.5x the expected table size
 # (+4096) and double after each call that ends short of the occupancy; the last call's failure is raised
 SAMPLER_ATTEMPTS = 4
+MAX_CLOUDS = 65535                      # clouds per batch call: the kernels' grid y dimension (lss_batch_geometry)
 _CPU = torch.device('cpu')
 
 
@@ -33,13 +34,27 @@ def _ptr(t):
     raise TypeError(type(t))
 
 
-def _cloud_offsets(offsets, name='cloud_offsets'):
-    """(off, B, N): host row offsets as a contiguous int64 array of B + 1 entries, the number of clouds and of rows.
+def _check_n_clouds(B):
+    """Raise the library's ValueError for a batch of more than MAX_CLOUDS clouds here, before any workspace query: the
+    queries of some entry points can only answer -1 for it."""
+    if B > MAX_CLOUDS:
+        raise ValueError(f'at most {MAX_CLOUDS} clouds per call, got {B}')
+
+
+def _row_offsets(offsets, name):
+    """(off, B, N): host row offsets as a contiguous int64 array of B + 1 entries, the number of groups and of rows.
     That they start at 0 and never decrease is checked by the library, which names the argument."""
     off = np.ascontiguousarray(offsets, dtype=np.int64)
     if off.ndim != 1 or off.shape[0] == 0:
         raise ValueError(f'{name}: expected a 1-D array of B + 1 row offsets, got shape {off.shape}')
     return off, off.shape[0] - 1, int(off[-1])
+
+
+def _cloud_offsets(offsets, name='cloud_offsets'):
+    """_row_offsets of a batch of clouds: B is at most MAX_CLOUDS"""
+    off, B, N = _row_offsets(offsets, name)
+    _check_n_clouds(B)
+    return off, B, N
 
 
 def _check_tensor(name, t, device, dtype, shape=None, min_cols=0, optional=False):
@@ -182,7 +197,7 @@ class SnowfallEngine:
     def upload_tables_device(self, xyr, plane_offsets, max_beam_divergence_rad=DEFAULT_MAX_DIVERGENCE_RAD,
                              n_buckets=2048):
         """xyr: CUDA float64 tensor (sum Np, 3); plane_offsets: int64 host array (n_planes + 1)."""
-        off, _, n_rows = _cloud_offsets(plane_offsets, 'plane_offsets')
+        off, _, n_rows = _row_offsets(plane_offsets, 'plane_offsets')
         _check_tensor('xyr', xyr, self.device, torch.float64, (n_rows, 3))
         return self._upload('lss_upload_particles_device', xyr, off, max_beam_divergence_rad, n_buckets)
 
@@ -572,7 +587,7 @@ class SnowfallEngine:
                        n_snow=((B,), torch.int32), points=want_points and ((N, F), torch.float32))
         need = self.lib.lss_dror_workspace_bytes(N, B)
         if need < 0:
-            raise RuntimeError('lss_dror_workspace_bytes failed (no usable CUDA device?)')
+            raise RuntimeError('lss_dror_workspace_bytes failed (2^31 rows or more, or no usable CUDA device?)')
         ws = self._scratch('dror', need)
         self._call('lss_dror_batch', points, F, _ptr(off), counts, B, float(alpha), float(beta), int(k_min),
                    float(sr_min), flags, out['keep'], out['points'] if want_points else None, out['counts'],
@@ -747,6 +762,7 @@ class SnowfallEngine:
         """
         _check_tensor('n_gt', n_gt, self.device, torch.int32, (None,))
         B = n_gt.shape[0]
+        _check_n_clouds(B)
         _check_tensor('boxes', boxes, self.device, torch.float32, (None, 11))
         _check_tensor('box_offsets', box_offsets, self.device, torch.int64, (B + 1,))
         _check_tensor('class_offsets', class_offsets, self.device, torch.int32, (B, 9))
