@@ -17,7 +17,8 @@
 //     generates it (np.random.RandomState(666).random_sample) and the kernel indexes it -- results are the reference's up to
 //     libm rounding (pow, log, exp, tan), labels and choices exact;
 //   * otherwise the reference is not reproducible itself (a thread pool shares the global generator, :333-339); the kernel
-//     uses a counter-based generator (Philox-4x32-10) keyed by (seed, return index): parity is statistical.
+//     uses a counter-based generator (Philox-4x32-10) keyed by (seed, return index), restated in NumPy by
+//     tests/lisa_stream.py: tests/test_lisa_stream_gpu.py holds both kernels to the oracle replayed on that stream.
 #include "segments.cuh"
 #include <algorithm>
 #include <cmath>

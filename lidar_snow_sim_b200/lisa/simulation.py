@@ -173,7 +173,9 @@ class LISA:
         seed = 0
         if not fixed_seed:
             seed = self.draw_seed()
-        r_far = float(np.sqrt((pc[:, :3] ** 2).sum(axis=1).max())) if n else 0.0
+        r = np.sqrt((pc[:, :3] ** 2).sum(axis=1))
+        r = r[np.isfinite(r)]                                          # a NaN return draws no particles
+        r_far = float(r.max()) if r.size else 0.0
         need = self._draws_bound(Rr, r_far)
         while True:
             table = self._draw_table(engine, need) if fixed_seed else None
@@ -225,7 +227,9 @@ class LISA:
                     seeds[b] = self.draw_seed()
             return engine.lisa_cloud_batch(points, off, rr, alpha, seeds, mode, **kw)
         # the largest bound over the batch: the densest applied rain rate at the farthest return
-        r_far = float(torch.linalg.vector_norm(points[:, :3], dim=1).max()) if points.shape[0] else 0.0
+        r = torch.linalg.vector_norm(points[:, :3], dim=1)
+        r = r[torch.isfinite(r)]                                       # a NaN return draws no particles
+        r_far = float(r.max()) if r.numel() else 0.0
         need = max([self._draws_bound(float(rr[b]), r_far) for b in np.flatnonzero(ap)], default=1)
         while True:
             table = self._draw_table(engine, need)

@@ -14,7 +14,7 @@ return's draws do not depend on the others): tools/make_golden_lisa.py runs the 
 in-memory shims (PyMieScatt stub -- only needed when the Mie table file is missing, it is not --, scipy.integrate.trapz
 -> numpy.trapezoid for SciPy >= 1.14), return by return in one thread, and checks this restatement bit for bit.
 Without `fixed_seed` the reference itself is not reproducible (a ThreadPool over returns shares the global generator,
-lisa.py:333-339): parity is statistical there.
+lisa.py:333-339): the device's counter-based draws are served to this restatement by tests/lisa_stream.py instead.
 
 The random draws are taken from an explicit np.random.RandomState in the reference's order: rand() (probabilistic
 rounding of the particle count), rand(n) (ranges), rand(n') (diameters), normal(0, std) (range noise).

@@ -6,7 +6,9 @@ NumPy's MT19937 with 666, lisa.py:54-55).
 Bars: oracle == reference bit for bit (CPU); device: labels exact (lost / not scattered / scattered -- the particle counts,
 the argmax choices and the random stream position all enter them), coordinates / intensities within 1e-9 relative (device
 pow / log / exp vs NumPy's).  Without fixed_seed the reference is not reproducible itself (a thread pool shares the global
-generator): the device's counter-based generator is checked statistically against the oracle on NumPy's generator.
+generator): the device's counter-based draws are held to the oracle replayed on the restated stream in
+tests/test_lisa_stream_gpu.py (tests/lisa_stream.py); the statistical test here checks their law against the oracle on
+NumPy's generator.
 """
 import os
 
