@@ -477,6 +477,40 @@ LSS_API lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_clou
                                             uint32_t *d_mt_state_out, void *d_workspace, int64_t workspace_bytes,
                                             void *stream);
 
+/* ---- DENSE fog: haze_point_cloud -----------------------------------------------------------------------------------------
+ * haze_point_cloud (lib/LiDAR_fog_sim/SeeingThroughFog/tools/DatasetFoggification/lidar_foggification.py:61-149) with
+ * BetaRadomization.get_beta (beta_modification.py:116-147) for every cloud of a batch, every cloud drawing from the same
+ * MT19937 start state h_mt_state, as the dataset's per-sample BetaRadomization(seed=0) leaves NumPy's global RandomState
+ * (dense_dataset.py:977-985).  Per cloud: rows with d = sqrt(x*x + y*y + z*z) (float32) > dmin, in order; beta field
+ * beta_b + sum_k |ia sin(fa a + oa) / fa + ih sin(fa a + fh z + oh)|, a = tan(y / x) (x == 0 -> 0.0001) a correctly
+ * rounded float32; d_max = -log(n / (I + g)) / (2 beta) (float32 quotient and log); output rows [stable (d < d_max),
+ * intensity I exp(-beta d), label 0; cloud rows (d_max < d, ln 2 / beta < d, not lost), xyz * (ln 2 / beta) / d, label 1;
+ * random rows, the first int(fraction_random K') of permutation(K') of the candidates farther than dmin after their
+ * d_rand draw, xyz * d_rand / d, label 2].  h_beta[b] == 0 is the reference's tuple branch: every detectable row copied
+ * with label 0, after the N' lost draws; it needs n_features == 4 (the reference raises ValueError for more columns).
+ *   d_points        float32[n_total * n_features], n_features >= 4 (x, y, z, intensity, ...)
+ *   d_cloud_counts  int32[n_clouds] device or NULL: valid rows per slot
+ *   h_beta          float64[n_clouds] >= 0: BetaRadomization.beta of each cloud
+ *   h_fourier       float64[6 * n_components] (n_components <= 16): per component fa, fh, oa, oh, ih, ia, the offsets as
+ *                   propagate_in_time left them
+ *   noise_level, gain, dmin    the sensor's n, g (used as float32) and minimal distance
+ *   fraction_random in [0, 0.05]
+ *   h_mt_state      uint32[625]: np.random.get_state()'s key words and pos, the state every cloud starts from
+ *   d_angle         float32[n_total] device or NULL: the tangent of each row to use instead of the device's (replay of a
+ *                   host's float32 np.tan)
+ *   out_f64         != 0: d_out_points float64, else float32;  out_label != 0: n_features + 1 columns, else n_features
+ *   d_out_points    cloud b's rows at the front of its output slot, which starts at row sum_{c < b} (n_c + n_c / 20 + 1),
+ *                   n_c the slot lengths; d_out_counts[b] rows
+ *   d_mt_state_out  uint32[n_clouds * 625] device: each cloud's state after its draws (key, pos)
+ *   d_workspace     lss_haze_workspace_bytes(n_total, n_clouds) bytes.  Asynchronous on `stream`, no synchronisation.     */
+LSS_API lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                  const int32_t *d_cloud_counts, int n_clouds, const double *h_beta,
+                                  const double *h_fourier, int n_components, double noise_level, double gain, double dmin,
+                                  double fraction_random, const uint32_t *h_mt_state, const float *d_angle, int out_f64,
+                                  int out_label, void *d_out_points, int32_t *d_out_counts, uint32_t *d_mt_state_out,
+                                  void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_haze_workspace_bytes(int64_t n_total, int n_clouds);
+
 /* ---- DROR snow removal ------------------------------------------------------------------------------------------------
  * Dynamic Radius Outlier Removal, dynamic_radius_outlier_filter (lib/cadc_devkit/other/dror.py:288-334), for every cloud of
  * a batch, as the dataset applies it under its DROR / DROR++ keys (lib/OpenPCDet/pcdet/datasets/dense/dense_dataset.py:588-616).

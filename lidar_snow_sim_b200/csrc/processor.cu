@@ -9,27 +9,17 @@
 //
 // Kernels:
 //   k_enc_count / k_seg_scan / k_enc_write   encode + mask + stable compaction of every cloud slot (segments.cuh)
-//   k_mt_draw    ONE persistent CTA: MT19937 from the caller's get_state() words, twisted 624 words at a time in three
-//                dependent phases, and the rejection chain of random_interval (NumPy's legacy shuffle: for i = n-1 .. 1,
-//                j_i = the first tempered word w with (w & smear(i)) <= i) over every cloud in turn.  The rest of the
-//                current 624-word block is one chunk: when every step it can reach (i0 - C + 1 .. i0) shares one mask,
-//                a masked value v <= i0 - C is surely accepted, v > i0 surely rejected, and only the few v in
-//                (i0 - C, i0] need the exact count of accepts before them, resolved in order.  Other chunks (small i, a
-//                mask change, the end of a cloud) go to warp 0 in 32-word groups with the same rule, or word by word.
-//   k_shuffle    one CTA per cloud: the swaps (i, j_i) applied by deterministic reservations (Shun et al., SODA 2015):
-//                every round each step not yet done reserves positions i and j_i with priority i (later steps of the
-//                sequential loop lose); a step holding both swaps; equal to the sequential loop whatever the rounds
+//   k_mt_draw    ONE persistent CTA: MT19937 from the caller's get_state() words and the rejection chain of every cloud
+//                in turn (mt_chain, mt19937.cuh)
+//   k_shuffle    one CTA per cloud: the swaps (i, j_i) applied by deterministic reservations (mt19937.cuh)
 //   k_gather     rows into shuffled order in their slots
 // tests/shuffle_model.py restates the word generation, the chunk rule and the reservation shuffle in NumPy.
-#include "segments.cuh"
+#include "mt19937.cuh"
 
 namespace {
 
 constexpr int PTILE = 1024;
 constexpr int MAX_COLS = 16;
-constexpr int MT_N = 624, MT_M = 397;
-constexpr int MT_TPB = 640;                 // one thread per word of a block (20 warps)
-constexpr int SHUF_TPB = 1024;
 
 // ------------------------------------------------------------------------------------------------ encode + mask
 struct EncArgs {
@@ -81,216 +71,25 @@ struct DrawArgs {
     int n_clouds;
     int32_t *J;                             // [N]: J[off_b + i] = j_i, i = 1 .. n_b - 1
     uint32_t *state_out;                    // [625]: key, pos after the last draw
-};
 
-__device__ __forceinline__ uint32_t mt_temper(uint32_t y)
-{
-    y ^= y >> 11;
-    y ^= (y << 7) & 0x9d2c5680u;
-    y ^= (y << 15) & 0xefc60000u;
-    return y ^ (y >> 18);
-}
-
-__device__ __forceinline__ uint32_t mt_twist1(uint32_t cur, uint32_t nxt, uint32_t far)
-{
-    const uint32_t y = (cur & 0x80000000u) | (nxt & 0x7fffffffu);
-    return far ^ (y >> 1) ^ ((y & 1u) ? 0x9908b0dfu : 0u);
-}
-
-__device__ __forceinline__ int smear(int i)
-{
-    uint32_t m = (uint32_t)i;
-    m |= m >> 1; m |= m >> 2; m |= m >> 4; m |= m >> 8; m |= m >> 16;
-    return (int)m;
-}
-
-struct Chain { int b, i, pos, cur, done; };
-
-// the next cloud with at least two rows (fewer draw nothing), or done
-__device__ __forceinline__ void next_cloud(const DrawArgs &a, int &b, int &i, int &done)
-{
-    for (b = b + 1; b < a.n_clouds; b++) {
-        const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
-        if (n >= 2) { i = n - 1; return; }
+    // the next cloud with at least two rows (fewer draw nothing), or done
+    __device__ __forceinline__ void next(int &b, int &i, int &done) const
+    {
+        for (b = b + 1; b < n_clouds; b++) {
+            const int n = seg_rows(cloud_off, cloud_cnt, b);
+            if (n >= 2) { i = n - 1; return; }
+        }
+        done = 1;
     }
-    done = 1;
-}
+    __device__ __forceinline__ int64_t base(int b) const { return cloud_off[b]; }
+};
 
 __global__ void __launch_bounds__(MT_TPB, 1) k_mt_draw(MTState st, DrawArgs a)
 {
-    constexpr int NW = MT_TPB / 32;
-    __shared__ uint32_t key[2][MT_N];
-    __shared__ int warp_tot[NW];
-    __shared__ int amb_v[MT_N], amb_S[MT_N], cum[MT_N + 1];
-    __shared__ Chain s;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    for (int t = tid; t < MT_N; t += MT_TPB) key[0][t] = st.key[t];
-    if (tid == 0) {
-        s.b = -1; s.i = 0; s.pos = st.pos; s.cur = 0; s.done = 0;
-        next_cloud(a, s.b, s.i, s.done);
-    }
-    for (;;) {
-        __syncthreads();                                        // s is stable here
-        if (s.done) break;
-        if (s.pos == MT_N) {                                    // mt19937_gen, out of place
-            const uint32_t *o = key[s.cur];
-            uint32_t *nw = key[s.cur ^ 1];
-            if (tid < MT_N - MT_M) nw[tid] = mt_twist1(o[tid], o[tid + 1], o[tid + MT_M]);
-            __syncthreads();
-            if (tid < MT_N - MT_M) {
-                const int t = tid + (MT_N - MT_M);
-                nw[t] = mt_twist1(o[t], o[t + 1], nw[t - (MT_N - MT_M)]);
-            }
-            __syncthreads();
-            if (tid < MT_N - 2 * (MT_N - MT_M)) {
-                const int t = tid + 2 * (MT_N - MT_M);
-                nw[t] = mt_twist1(o[t], t + 1 < MT_N ? o[t + 1] : nw[0], nw[t - (MT_N - MT_M)]);
-            }
-            __syncthreads();
-            if (tid == 0) { s.cur ^= 1; s.pos = 0; }
-            continue;
-        }
-        const uint32_t *w = key[s.cur];
-        const int p = s.pos, i = s.i, C = MT_N - p;
-        const int mask = smear(i);
-        const int64_t base = a.cloud_off[s.b];
-        const int b0 = s.b;
-        __syncthreads();                                        // every thread has its copy before s changes
-        if (i - C + 1 >= (mask >> 1) + 1) {
-            // one mask for the chunk: sure accepts, sure rejects, and the ambiguous words in order
-            const bool in = tid >= p && tid < MT_N;
-            const int v = in ? (int)(mt_temper(w[tid]) & (uint32_t)mask) : 0;
-            const bool sure = in && v <= i - C, amb = in && !sure && v <= i;
-            const int x = (int)sure | ((int)amb << 16);         // both counts < 2^16: one scan
-            int incl = x;
-#pragma unroll
-            for (int d = 1; d < 32; d <<= 1) {
-                const int u = __shfl_up_sync(0xffffffffu, incl, d);
-                if (lane >= d) incl += u;
-            }
-            if (lane == 31) warp_tot[warp] = incl;
-            __syncthreads();
-            int pre = 0, tot = 0;
-#pragma unroll
-            for (int k = 0; k < NW; k++) {
-                const int c = warp_tot[k];
-                pre += k < warp ? c : 0;
-                tot += c;
-            }
-            const int excl = pre + incl - x;
-            const int S = excl & 0xffff, A = excl >> 16;
-            if (amb) { amb_v[A] = v; amb_S[A] = S; }
-            __syncthreads();
-            const int nA = tot >> 16, nS = tot & 0xffff;
-            if (tid == 0) {
-                int acc = 0;
-                cum[0] = 0;
-                for (int k = 0; k < nA; k++) {
-                    acc += amb_v[k] <= i - (amb_S[k] + acc);
-                    cum[k + 1] = acc;
-                }
-            }
-            __syncthreads();
-            if (sure || (amb && cum[A + 1] > cum[A])) a.J[base + i - (S + cum[A])] = v;
-            if (tid == 0) {
-                s.i = i - (nS + cum[nA]);
-                s.pos = MT_N;
-                if (s.i == 0) next_cloud(a, s.b, s.i, s.done);
-            }
-        } else if (warp == 0) {
-            // 32 words at a time: the same rule when one mask covers the group, else word by word
-            int q = p, ci = i, b = b0, done = 0;
-            int64_t cb = base;
-            while (q < MT_N) {
-                const int g = min(32, MT_N - q);
-                const uint32_t wd = lane < g ? mt_temper(w[q + lane]) : 0u;
-                const int m = smear(ci);
-                if (ci - g + 1 >= (m >> 1) + 1) {
-                    const int v = (int)(wd & (uint32_t)m);
-                    unsigned acc = __ballot_sync(0xffffffffu, lane < g && v <= ci - g);
-                    unsigned am = __ballot_sync(0xffffffffu, lane < g && v > ci - g && v <= ci);
-                    while (am) {
-                        const int k = __ffs(am) - 1;
-                        const int vk = __shfl_sync(0xffffffffu, v, k);
-                        if (vk <= ci - __popc(acc & ((1u << k) - 1u))) acc |= 1u << k;
-                        am &= am - 1u;
-                    }
-                    if ((acc >> lane) & 1u) a.J[cb + ci - __popc(acc & ((1u << lane) - 1u))] = v;
-                    ci -= __popc(acc);
-                    q += g;
-                    if (ci == 0) {
-                        next_cloud(a, b, ci, done);
-                        if (done) break;
-                        cb = a.cloud_off[b];
-                    }
-                } else {
-                    int k = 0;
-                    for (; k < g; k++) {
-                        const int v = (int)(__shfl_sync(0xffffffffu, wd, k) & (uint32_t)smear(ci));
-                        if (v > ci) continue;
-                        if (lane == 0) a.J[cb + ci] = v;
-                        if (--ci == 0) {
-                            next_cloud(a, b, ci, done);
-                            if (done) { k++; break; }
-                            cb = a.cloud_off[b];
-                        }
-                    }
-                    q += k;
-                    if (done) break;
-                }
-            }
-            if (lane == 0) { s.pos = q; s.i = ci; s.b = b; s.done = done; }
-        }
-    }
-    for (int t = tid; t < MT_N; t += MT_TPB) a.state_out[t] = key[s.cur][t];
-    if (tid == 0) a.state_out[MT_N] = (uint32_t)s.pos;
+    mt_chain(a, [&](int t) { return st.key[t]; }, st.pos, a.J, a.state_out);
 }
 
-// ------------------------------------------------------------------------------------------------ swaps + gather
-struct ShufArgs {
-    const int64_t *cloud_off;
-    const int32_t *cloud_cnt;
-    int32_t *J;                             // consumed: a done step's entry becomes -1
-    unsigned long long *R;                  // [N] reservations (round << 32 | step), zeroed here
-    int32_t *P;                             // [N] permutation of each cloud, indices inside the cloud
-};
-
-__global__ void __launch_bounds__(SHUF_TPB) k_shuffle(ShufArgs a)
-{
-    const int b = blockIdx.x;
-    const int n = seg_rows(a.cloud_off, a.cloud_cnt, b);
-    const int64_t base = a.cloud_off[b];
-    int32_t *J = a.J + base, *P = a.P + base;
-    unsigned long long *R = a.R + base;
-    for (int r = threadIdx.x; r < n; r += SHUF_TPB) { P[r] = r; R[r] = 0ull; }
-    if (n < 2) return;
-    __syncthreads();
-    for (unsigned long long round = 1;; round++) {
-        const unsigned long long hi = round << 32;
-        for (int i = 1 + threadIdx.x; i < n; i += SHUF_TPB) {
-            const int j = J[i];
-            if (j < 0) continue;
-            atomicMax(&R[i], hi | (unsigned)i);
-            atomicMax(&R[j], hi | (unsigned)i);
-        }
-        __syncthreads();
-        int left = 0;
-        for (int i = 1 + threadIdx.x; i < n; i += SHUF_TPB) {
-            const int j = J[i];
-            if (j < 0) continue;
-            if (R[i] == (hi | (unsigned)i) && R[j] == (hi | (unsigned)i)) {
-                const int t = P[i];
-                P[i] = P[j];
-                P[j] = t;
-                J[i] = -1;
-            } else {
-                left = 1;
-            }
-        }
-        if (!__syncthreads_or(left)) break;
-    }
-}
-
+// ------------------------------------------------------------------------------------------------ gather
 __global__ void __launch_bounds__(256) k_gather(const float *src, int F, const int64_t *cloud_off, const int32_t *cloud_cnt,
                                                 const int32_t *P, float *dst)
 {

@@ -568,6 +568,61 @@ class SnowfallEngine:
         _set_mt_state(state, out['state'])
         return out['perm']
 
+    def haze_batch(self, points, cloud_offsets, beta, fourier, noise_level=0.04, gain=0.45, dmin=2.0,
+                   fraction_random=0.05, counts=None, state=None, angle=None, out_dtype=torch.float32, label=False):
+        """
+        DENSE fog: haze_point_cloud with BetaRadomization's beta field (lss_haze_batch, current stream) for every cloud,
+        each drawing from the same MT19937 start state `state` (an np.random.get_state() tuple; None: NumPy's global
+        state), as the dataset's per-sample BetaRadomization(seed=0) makes them.  points: CUDA float32 (N, F), F >= 4;
+        counts: optional CUDA int32 (B,) valid rows per slot; beta: (B,) float64 >= 0, 0 = the reference's tuple
+        branch; fourier: (n_components, 6) float64 rows (fa, fh, oa, oh, ih, ia) after propagate_in_time; noise_level,
+        gain, dmin: the sensor's n, g, dmin; fraction_random in [0, 0.05]; angle: optional CUDA float32 (N,) tangent
+        per row to use instead of the device's correctly rounded one.  Returns dict(points (M, F + label) out_dtype with
+        cloud b's rows at offsets[b] (M = offsets[B], slots of n_b + n_b // 20 + 1 rows), offsets int64 numpy (B + 1,),
+        counts int32 CUDA (B,), states uint32 numpy (B, 625) each cloud's final key and pos).  The one synchronisation
+        is the copy of the states; NumPy's global state is then set to the last cloud's (the cached Gaussian as `state`
+        has it, as no Gaussian is drawn).
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=4)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        _check_tensor('angle', angle, self.device, torch.float32, (N,), optional=True)
+        if out_dtype not in (torch.float32, torch.float64):
+            raise ValueError(f'out_dtype: expected torch.float32 or torch.float64, got {out_dtype}')
+        betas = np.ascontiguousarray(beta, dtype=np.float64).reshape(-1)
+        if betas.shape[0] != B or not np.all(np.isfinite(betas) & (betas >= 0)):
+            raise ValueError(f'beta: expected {B} finite values >= 0, got {betas}')
+        four = np.ascontiguousarray(fourier, dtype=np.float64)
+        if four.ndim != 2 or four.shape[1] != 6 or four.shape[0] > 16:
+            raise ValueError(f'fourier: expected an (n_components <= 16, 6) array, got shape {four.shape}')
+        if not 0.0 <= fraction_random <= 0.05:
+            raise ValueError(f'fraction_random must be in [0, 0.05], got {fraction_random}')
+        if state is None:
+            words, state = _mt_state()
+        else:
+            if state[0] != 'MT19937' or not 0 <= int(state[2]) <= 624:
+                raise ValueError('state: expected an MT19937 np.random.get_state() tuple with pos in [0, 624]')
+            words = np.empty(625, np.uint32)
+            words[:624] = np.asarray(state[1], dtype=np.uint32)
+            words[624] = int(state[2])
+        F = points.shape[1]
+        Fo = F + (1 if label else 0)
+        n = np.diff(off)
+        out_off = np.zeros(B + 1, np.int64)
+        np.cumsum(n + n // 20 + 1, out=out_off[1:])
+        out = _outputs(None, self.device, points=((int(out_off[-1]), Fo), out_dtype), counts=((B,), torch.int32),
+                       states=((B, 625), torch.int32))
+        ws = self._scratch('haze', self.lib.lss_haze_workspace_bytes(N, B))
+        self._call('lss_haze_batch', points, F, _ptr(off), counts, B, _ptr(betas), _ptr(four), four.shape[0],
+                   float(noise_level), float(gain), float(dmin), float(fraction_random), _ptr(words), angle,
+                   1 if out_dtype == torch.float64 else 0, 1 if label else 0, out['points'], out['counts'],
+                   out['states'], ws, ws.numel())
+        states = out['states'].cpu().numpy().view(np.uint32)
+        if B > 0:
+            _, _, _, has_gauss, gauss = state
+            np.random.set_state(('MT19937', states[-1, :624].copy(), int(states[-1, 624]), has_gauss, gauss))
+        return {'points': out['points'], 'offsets': out_off, 'counts': out['counts'], 'states': states}
+
     def dror_batch(self, points, cloud_offsets, alpha=0.16, beta=3.0, k_min=3, sr_min=0.04, counts=None, crop=False,
                    want_points=True, work_stats=False, out=None):
         """

@@ -279,14 +279,8 @@ def simulate_fog_batch(ps, pcs, noise, gain=False, noise_variant='v1', hard=True
     simulate_fog(ps[b], pcs[b], noise, ..., rng=rngs[b], lut='device') called for b = 0, 1, ... in turn -- the generators
     are left where those calls leave them, also when clouds share one.
     """
-    variants = {'v1': 1, 'v2': 2, 'v3': 3, 'v4': 4}
-    if soft and noise > 0 and noise_variant not in variants:
-        raise NotImplementedError(f"noise variant '{noise_variant}' is not implemented (yet)")      # :264-266
     B = len(pcs)
-    ps = list(ps) if isinstance(ps, (list, tuple)) else [ps] * B
-    rngs = [RNG] * B if rngs is None else list(rngs)
-    if len(ps) != B or len(rngs) != B:
-        raise ValueError('ps, pcs and rngs must have one entry per cloud')
+    ps, rngs = _batch_args(ps, B, noise, noise_variant, soft, rngs)
     if B == 0:
         return []
     eng = engine or default_engine()
@@ -295,8 +289,56 @@ def simulate_fog_batch(ps, pcs, noise, gain=False, noise_variant='v1', hard=True
     if any(pc.ndim != 2 or pc.shape[1] != F for pc in pc32):
         raise ValueError('every cloud of a batch needs the same number of features')
     off = np.concatenate([[0], np.cumsum([pc.shape[0] for pc in pc32])]).astype(np.int64)
-    N = int(off[-1])
     d_pts = torch.from_numpy(np.concatenate(pc32)).to(eng.device)
+    res = simulate_fog_batch_device(ps, d_pts, off, noise, gain, noise_variant, hard, soft, engine=eng, rngs=rngs)
+    aug_all = res['points'].cpu().numpy()
+    info_all = res['info'].cpu().numpy()
+    mask_all = res['fog_mask'].cpu().numpy().astype(bool)
+    out = []
+    for b in range(B):
+        aug = aug_all[off[b]:off[b + 1]]
+        if not soft:
+            out.append((aug.astype(np.float32), None, None))
+            continue
+        info = info_all[b]
+        c = int(info[2])
+        fog_pc = aug[mask_all[off[b]:off[b + 1]]] if c > 0 else None
+        out.append((aug, fog_pc, {'min_fog_response': float(info[0]) if c else np.inf,
+                                  'max_fog_response': float(info[1]) if c else 0,
+                                  'num_fog_responses': c}))
+    return out
+
+
+_VARIANTS = {'v1': 1, 'v2': 2, 'v3': 3, 'v4': 4}
+
+
+def _batch_args(ps, B, noise, noise_variant, soft, rngs):
+    """the checks of a batch call: (ps, rngs) as lists of B entries"""
+    if soft and noise > 0 and noise_variant not in _VARIANTS:
+        raise NotImplementedError(f"noise variant '{noise_variant}' is not implemented (yet)")      # :264-266
+    ps = list(ps) if isinstance(ps, (list, tuple)) else [ps] * B
+    rngs = [RNG] * B if rngs is None else list(rngs)
+    if len(ps) != B or len(rngs) != B:
+        raise ValueError('ps, pcs and rngs must have one entry per cloud')
+    return ps, rngs
+
+
+def simulate_fog_batch_device(ps, points, cloud_offsets, noise, gain=False, noise_variant='v1', hard=True, soft=True, *,
+                              engine=None, rngs=None):
+    """
+    The engine call of simulate_fog_batch on device-resident clouds: points CUDA float32 (N, F), cloud b at rows
+    cloud_offsets[b] .. cloud_offsets[b + 1].  Steps the generators exactly as simulate_fog_batch (one integers draw
+    per cloud, then one draw per fog point; the fog counts come from a first pass that draws nothing, one synchronising
+    copy) and returns fog_batch_params' dict (points float64 (N, F), fog_mask, info; None for an empty batch).
+    """
+    off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+    B = off.shape[0] - 1
+    ps, rngs = _batch_args(ps, B, noise, noise_variant, soft, rngs)
+    if B == 0:
+        return None
+    eng = engine or default_engine()
+    d_pts = points
+    N = int(off[-1])
     alpha = np.array([p.alpha for p in ps], dtype=np.float64)
     beta = np.array([p.beta for p in ps], dtype=np.float64)
     beta_0 = np.array([p.beta_0 for p in ps], dtype=np.float64)
@@ -310,7 +352,7 @@ def simulate_fog_batch(ps, pcs, noise, gain=False, noise_variant='v1', hard=True
                 unique.append(p)
             index[b] = keys[k]
         luts = eng.fog_integral_tables(unique)
-    variant = variants.get(noise_variant, 1)
+    variant = _VARIANTS.get(noise_variant, 1)
     kw = dict(hard=hard, soft=soft, gain=gain, noise=int(noise), noise_variant=variant)
 
     def run(**extra):
@@ -342,19 +384,4 @@ def simulate_fog_batch(ps, pcs, noise, gain=False, noise_variant='v1', hard=True
                     _pcg64_advance(g, int(cnt[b]))
             res = run(rng_states=states)
     eng.check()
-    aug_all = res['points'].cpu().numpy()
-    info_all = res['info'].cpu().numpy()
-    mask_all = res['fog_mask'].cpu().numpy().astype(bool)
-    out = []
-    for b in range(B):
-        aug = aug_all[off[b]:off[b + 1]]
-        if not soft:
-            out.append((aug.astype(np.float32), None, None))
-            continue
-        info = info_all[b]
-        c = int(info[2])
-        fog_pc = aug[mask_all[off[b]:off[b + 1]]] if c > 0 else None
-        out.append((aug, fog_pc, {'min_fog_response': float(info[0]) if c else np.inf,
-                                  'max_fog_response': float(info[1]) if c else 0,
-                                  'num_fog_responses': c}))
-    return out
+    return res

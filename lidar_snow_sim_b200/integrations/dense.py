@@ -15,12 +15,14 @@ on the device once per (mode, pair) and cached.
     aug = OnTheFlyWeather(dataset_cfg, rainfall_rates=[...])        # in DenseDataset.__init__
     points = aug(points, training=self.training)                    # replaces dense_dataset.py:749-837
 """
+import math
 import random
 
 import numpy as np
 
 from ..engine import default_engine
-from ..fog.simulation import ParameterSet, simulate_fog
+from ..fog.haze import SENSOR_CONSTANTS, BetaRadomization
+from ..fog.simulation import ParameterSet, simulate_fog, simulate_fog_batch_device
 from ..snowfall.precompute import SNOWFALL_RATES, TERMINAL_VELOCITIES, get_fov_flag
 
 # the (snowfall_rate, terminal_velocity) pairs DenseDataset draws its rain rate from (dense_dataset.py:91-92): eight
@@ -310,6 +312,17 @@ def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None,
     if alpha == '0.000' or float(alpha) == 0.0:
         return points
     p = ParameterSet(alpha=float(alpha), gamma=0.000001)
+    soft, hard, gain, fog_noise_variant = _cvl_options(dataset_cfg)
+    points, _, _ = simulate_fog(p, pc=points, noise=10, gain=gain, noise_variant=fog_noise_variant, soft=soft, hard=hard,
+                                engine=engine, lut=lut, lut_dir=lut_dir, rng=rng)
+    return points
+
+
+FOG_ALPHAS = ['0.000', '0.005', '0.010', '0.020', '0.030', '0.060']           # dense_dataset.py:628
+
+
+def _cvl_options(dataset_cfg):
+    """foggify's CVL keys (dense_dataset.py:994-1006): (soft, hard, gain, noise variant)"""
     soft, hard, gain, fog_noise_variant = True, True, False, 'v1'
     if 'FOG_GAIN' in dataset_cfg:
         gain = dataset_cfg['FOG_GAIN']
@@ -319,9 +332,196 @@ def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None,
         soft = dataset_cfg['FOG_SOFT']
     if 'FOG_HARD' in dataset_cfg:
         hard = dataset_cfg['FOG_HARD']
-    points, _, _ = simulate_fog(p, pc=points, noise=10, gain=gain, noise_variant=fog_noise_variant, soft=soft, hard=hard,
-                                engine=engine, lut=lut, lut_dir=lut_dir, rng=rng)
-    return points
+    return soft, hard, gain, fog_noise_variant
+
+
+def _slot_rows(off, lengths, sel, dev):
+    """(rows, sub): the first lengths[b] rows of every selected slot b (slots start at off[b]) and their offsets"""
+    import torch
+    b = np.flatnonzero(sel)
+    sub = np.concatenate([[0], np.cumsum(lengths[b])]).astype(np.int64)
+    shift = torch.from_numpy(off[b] - sub[:-1]).to(dev)
+    rows = torch.arange(int(sub[-1]), device=dev) + torch.repeat_interleave(
+        shift, torch.from_numpy(lengths[b]).to(dev), output_size=int(sub[-1]))
+    return rows, sub
+
+
+class FogAugmentation:
+    """
+    The FOG_AUGMENTATION / FOG_AUGMENTATION_AFTER keys of `DenseDataset.__getitem__` (dense_dataset.py:618-675, 906-918)
+    and `foggify` (:967-1014) on a batch of device-resident clouds, with the dataset's curriculum bookkeeping
+    (curriculum_stage, current_iteration, iteration_increment, total_iterations; init_curriculum, :115-119) and its
+    `random_generator` for the 'uniform' schedule.
+
+        fog = FogAugmentation(dataset_cfg, random_generator=self.random_generator)    # in DenseDataset.__init__
+        fog.init_curriculum(it, epochs, workers, len(dataset))
+        r = fog.batch(points, offsets, counts)            # FOG_AUGMENTATION, before the row selection and LISA
+        ...                                               # r['mor'] feeds data_augmentor_batch(mor=...) / LIMIT_BY_MOR
+        r2 = fog.after_batch(rows, offsets, counts)       # FOG_AUGMENTATION_AFTER, on prepare_data_batch's rows
+
+    DENSE: the reference reads FOG_AUGMENTATION's clouds from files pre-computed per alpha
+    (`<lidar_folder>_DENSE_beta_<alpha>/<id>.bin`, :969-975); here haze_point_cloud is computed on the device for both
+    keys, as the reference computes it on the fly for FOG_AUGMENTATION_AFTER (:977-985): BetaRadomization(alpha, seed=0)
+    reseeds NumPy's global RandomState per sample, so every cloud draws from the same state (SnowfallEngine.haze_batch),
+    and NumPy's state ends as after the last sample.  CVL: simulate_fog(ParameterSet(alpha, gamma=1e-6), noise=10, ...)
+    with FOG_GAIN / FOG_NOISE_VARIANT / FOG_SOFT / FOG_HARD, the fog module's generator stepped as the per-sample calls
+    step it, integral tables generated on the device (lut='device').
+    Rows stay float32 by default (the reference continues in float64; out_dtype=torch.float64 keeps them).
+    """
+
+    def __init__(self, dataset_cfg, random_generator=None, lut=None, engine=None):
+        if lut not in (None, 'device'):
+            raise ValueError("lut: the batch generates the integral tables on the device (None or 'device')")
+        self.cfg = dataset_cfg
+        self.random_generator = np.random.default_rng() if random_generator is None else random_generator
+        self.engine = engine
+        self.curriculum_stage = 0                       # dense_dataset.py:84-87
+        self.total_iterations = -1
+        self.current_iteration = -1
+        self.iteration_increment = -1
+        self._last = None
+
+    def init_curriculum(self, it, epochs, workers, length):
+        """DenseDataset.init_curriculum (dense_dataset.py:115-119), length = len(dataset)"""
+        self.current_iteration = it
+        self.iteration_increment = workers
+        self.total_iterations = epochs * length
+
+    def _engine(self):
+        if self.engine is None:
+            self.engine = default_engine()
+        return self.engine
+
+    def _active(self, training):
+        return bool(training and (self.cfg.get('FOG_AUGMENTATION') or self.cfg.get('FOG_AUGMENTATION_AFTER')))
+
+    def draw(self):
+        """dense_dataset.py:620-671 for one sample: (curriculum_stage, alpha, method, mor)"""
+        cfg = self.cfg
+        s = cfg['FOG_AUGMENTATION'] if cfg.get('FOG_AUGMENTATION') else cfg['FOG_AUGMENTATION_AFTER']
+        alphas = cfg['FOG_ALPHAS'] if 'FOG_ALPHAS' in cfg else FOG_ALPHAS
+        method, schedule = s.split('_')[0], s.split('_')[-1]
+        assert (method in ['CVL', 'DENSE']), f'unknown augmentation schedule {schedule}'
+        if schedule == 'curriculum':
+            progress = self.current_iteration / self.total_iterations
+            ratio = 1 / len(alphas)
+            stage = math.floor(progress / ratio)
+        elif schedule == 'uniform':
+            stage = int(self.random_generator.integers(low=0, high=len(alphas)))
+        elif schedule == 'fixed':
+            stage = len(alphas) - 1
+            if 'FOG_ALPHA' in cfg:
+                target = cfg['FOG_ALPHA']
+                stage = min(range(len(alphas)), key=lambda i: abs(float(alphas[i]) - target))
+        else:
+            raise ValueError(f'unknown augmentation schedule "{schedule}"')
+        assert (0 <= stage <= len(alphas)), f'curriculum stage {stage} out of range {len(alphas)}'
+        alpha = alphas[stage]
+        mor = np.inf if alpha == '0.000' else np.log(20) / float(alpha)
+        return stage, alpha, method, mor
+
+    def draw_batch(self, B, training=True):
+        """draw() for B samples in turn, each followed by the bookkeeping of the foggify calls its sample makes (one per
+        FOG_AUGMENTATION, one per FOG_AUGMENTATION_AFTER key, :1011-1012).  Returns (alphas, methods, mor (B,))."""
+        alphas, methods, mor = [None] * B, [None] * B, np.full(B, np.inf)
+        if not self._active(training):
+            return alphas, methods, mor
+        calls = (1 if self.cfg.get('FOG_AUGMENTATION') else 0) + (1 if 'FOG_AUGMENTATION_AFTER' in self.cfg else 0)
+        for b in range(B):
+            stage, alphas[b], methods[b], mor[b] = self.draw()
+            for _ in range(calls):
+                self.curriculum_stage = stage
+                self.current_iteration += self.iteration_increment
+        return alphas, methods, mor
+
+    def batch(self, points, cloud_offsets, counts=None, training=True, out_dtype=None):
+        """
+        The FOG_AUGMENTATION block for B samples: points CUDA float32 (N, F >= 4), cloud b at rows cloud_offsets[b] ..
+        (+ counts[b], CUDA int32 (B,); None: whole slots).  Draws every sample (draw_batch), then fogs the samples whose
+        alpha is not '0.000'.  Returns dict(points (M, F) out_dtype (default float32), offsets (B + 1,) int64 host with
+        slots of n_b + n_b // 20 + 1 rows (a DENSE cloud can grow by its random scatter rows), counts (B,) int32 CUDA,
+        mor (B,) float64 host, alpha, method (B lists; None when the block draws nothing)).  Without FOG_AUGMENTATION
+        the rows pass through in their slots.
+        """
+        import torch
+        out_dtype = torch.float32 if out_dtype is None else out_dtype
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        alphas, methods, mor = self.draw_batch(off.shape[0] - 1, training)
+        self._last = (alphas, methods)
+        if self._active(training) and self.cfg.get('FOG_AUGMENTATION'):
+            res = self._foggify(points, off, counts, alphas, methods, out_dtype)
+        else:
+            res = self._passthrough(points, off, counts, out_dtype)
+        res.update(mor=mor, alpha=alphas, method=methods)
+        return res
+
+    def after_batch(self, points, cloud_offsets, counts=None, training=True, out_dtype=None):
+        """
+        FOG_AUGMENTATION_AFTER (dense_dataset.py:906-918): foggify(on_the_fly=True) with the alphas the last batch()
+        drew for the same samples, on prepare_data_batch's rows (whose voxels were made before, so these rows do not
+        reach them, as in the reference).  Returns dict(points, offsets, counts) as batch().
+        """
+        import torch
+        out_dtype = torch.float32 if out_dtype is None else out_dtype
+        off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        if not (training and 'FOG_AUGMENTATION_AFTER' in self.cfg and self._last is not None):
+            return self._passthrough(points, off, counts, out_dtype)
+        alphas, methods = self._last
+        if len(alphas) != off.shape[0] - 1:
+            raise ValueError(f'after_batch: {off.shape[0] - 1} clouds, the last batch() drew {len(alphas)} samples')
+        return self._foggify(points, off, counts, alphas, methods, out_dtype)
+
+    @staticmethod
+    def _passthrough(points, off, counts, out_dtype):
+        import torch
+        if counts is None:
+            counts = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
+        return dict(points=points.to(out_dtype), offsets=off, counts=counts)
+
+    def _foggify(self, points, off, counts, alphas, methods, out_dtype):
+        import torch
+        B = off.shape[0] - 1
+        if not (isinstance(points, torch.Tensor) and points.is_cuda and points.dtype == torch.float32 and
+                points.dim() == 2 and points.shape[1] >= 4 and points.shape[0] == int(off[-1])):
+            raise ValueError('FogAugmentation needs CUDA float32 (N, F >= 4) rows in the slots of cloud_offsets')
+        dev, F = points.device, points.shape[1]
+        slot = np.diff(off)
+        if counts is None:
+            counts = torch.from_numpy(slot.astype(np.int32)).to(dev)
+        new_slot = slot + slot // 20 + 1
+        new_off = np.concatenate([[0], np.cumsum(new_slot)]).astype(np.int64)
+        out = torch.zeros((int(new_off[-1]), F), dtype=out_dtype, device=dev)
+        out_counts = counts.clone()
+        fog = np.array([a is not None and a != '0.000' for a in alphas], dtype=bool)
+        dense = fog & np.array([m == 'DENSE' for m in methods], dtype=bool)
+        cvl = fog & ~dense
+        if (~dense).any():                              # clear and CVL clouds keep their rows' places
+            src, _ = _slot_rows(off, slot, ~dense, dev)
+            dst, _ = _slot_rows(new_off, slot, ~dense, dev)
+            out[dst] = points[src].to(out_dtype)
+        eng = self._engine()
+        if dense.any():
+            sel = np.flatnonzero(dense)
+            rows, sub = _slot_rows(off, slot, dense, dev)
+            br = BetaRadomization(beta=float(alphas[sel[0]]), seed=0)      # the same parameters for every alpha
+            br.propagate_in_time(10)
+            n, g, dmin = SENSOR_CONSTANTS['Velodyne HDL-64E S3D']
+            b_dev = torch.from_numpy(sel).to(dev)
+            r = eng.haze_batch(points[rows], sub, [float(alphas[b]) for b in sel], br.fourier(), n, g, dmin, 0.05,
+                               counts=counts[b_dev], state=np.random.get_state(), out_dtype=out_dtype)
+            dst, _ = _slot_rows(new_off, new_slot, dense, dev)
+            out[dst] = r['points']
+            out_counts[b_dev] = r['counts']
+        if cvl.any():
+            sel = np.flatnonzero(cvl)
+            valid = counts.cpu().numpy().astype(np.int64)
+            src, sub = _slot_rows(off, valid, cvl, dev)
+            soft, hard, gain, variant = _cvl_options(self.cfg)
+            ps = [ParameterSet(alpha=float(alphas[b]), gamma=0.000001) for b in sel]
+            res = simulate_fog_batch_device(ps, points[src].contiguous(), sub, 10, gain, variant, hard, soft, engine=eng)
+            dst, _ = _slot_rows(new_off, valid, cvl, dev)
+            out[dst] = res['points'].to(out_dtype)
+        return dict(points=out, offsets=new_off, counts=out_counts)
 
 
 def dror_filter(points, dataset_cfg, split, engine=None):
