@@ -501,6 +501,10 @@ LSS_API lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_clou
  *   out_f64         != 0: d_out_points float64, else float32;  out_label != 0: n_features + 1 columns, else n_features
  *   d_out_points    cloud b's rows at the front of its output slot, which starts at row sum_{c < b} (n_c + n_c / 20 + 1),
  *                   n_c the slot lengths; d_out_counts[b] rows
+ *   d_out_counts    int32[n_clouds] device: rows per cloud, or -1 where the reference raises OverflowError('Range
+ *                   exceeds valid bounds'): a random scatter candidate (h_beta[b] > 0) whose min(d_max, d) is NaN or
+ *                   infinite (a NaN intensity, I = -g, a non-finite beta field from y / x or z).  Such a cloud's output
+ *                   rows are undefined and its state is the start state after its 2 N' lost words.
  *   d_mt_state_out  uint32[n_clouds * 625] device: each cloud's state after its draws (key, pos)
  *   d_workspace     lss_haze_workspace_bytes(n_total, n_clouds) bytes.  Asynchronous on `stream`, no synchronisation.     */
 LSS_API lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -510,6 +514,9 @@ LSS_API lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_fe
                                   int out_label, void *d_out_points, int32_t *d_out_counts, uint32_t *d_mt_state_out,
                                   void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_haze_workspace_bytes(int64_t n_total, int n_clouds);
+/* test hook: the DENSE haze's correctly rounded float32 np.tan (fn 0) or np.log (fn 1) of n float32 device values, as
+ * lss_haze_batch computes the beta field's tangent and d_max's logarithm                                             */
+LSS_API lss_status lss_debug_haze_round(lss_engine *e, int fn, const float *d_x, int64_t n, float *d_out, void *stream);
 
 /* ---- DROR snow removal ------------------------------------------------------------------------------------------------
  * Dynamic Radius Outlier Removal, dynamic_radius_outlier_filter (lib/cadc_devkit/other/dror.py:288-334), for every cloud of

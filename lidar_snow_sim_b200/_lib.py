@@ -121,6 +121,7 @@ SIGNATURES = [
     ('lss_haze_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double,
                                   _c.c_double, _c.c_double, _P, _P, _c.c_int, _c.c_int, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_haze_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_debug_haze_round', _c.c_int, [_P, _c.c_int, _P, _c.c_int64, _P, _P]),
     ('lss_dror_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_int, _c.c_double,
                                   _c.c_uint32, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_dror_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),

@@ -16,13 +16,15 @@
 //   k_hz_det        class "d > dmin" (count); the beta field and d_max of those rows         -> scan: N'
 //   k_hz_classify   rank among detectable rows: lost; classes stable / cloud row (count) and candidate (count)
 //                                                                                           -> scans: S, C, K
+//                   a candidate whose min(d_max, d) (NaN propagating, as np.min) is not finite flags its cloud: legacy
+//                   uniform(high=...) raises OverflowError('Range exceeds valid bounds') there, before any d_rand draw
 //   k_hz_scatter    stable rows and cloud rows written at their ranks; candidates draw d_rand at 2 N' + 2 rank; kept
 //                   candidates (count)                                                      -> scan: K'
 //   k_hz_kept       the kept candidates' row indices, compacted in order
 //   k_hz_chain      one CTA per cloud: mt_chain (mt19937.cuh) for permutation(K') from its own key block and pos;
-//                   the cloud's final state
+//                   the cloud's final state (a flagged cloud: after its 2 N' lost words, no chain, K' set to 0)
 //   k_shuffle       (mt19937.cuh) the permutations
-//   k_hz_random     the first int(fraction K') kept candidates in permutation order; the counts
+//   k_hz_random     the first int(fraction K') kept candidates in permutation order; the counts (-1: flagged)
 //
 // Arithmetic as NumPy does it: d = sqrt(x*x + y*y + z*z) in float32 (no contraction), y / x and n / (I + g) in float32,
 // tan and log of a float32 correctly rounded to float32 (float64 rounded once; arguments near a rounding boundary from
@@ -55,6 +57,7 @@ struct HazeArgs {
     const uint32_t *stream;                 // raw key words, block after block
     SegTiles det, sc, cand, kept;
     int32_t *n_det, *n_stable, *n_cloud, *n_cand, *n_kept;   // [B] each
+    int32_t *bad;                           // [B] != 0: a candidate's uniform(high=...) raises (zeroed by k_hz_det)
     uint8_t *code;                          // [N]
     double *rbeta, *dmax, *drand;           // [N]
     int32_t *kidx;                          // [N] kept candidates' row indices, at the front of each slot
@@ -91,6 +94,23 @@ __device__ __forceinline__ float hz_round(double t, float x, const uint32_t *arg
     return (odd && x < 0.0f) ? -r : r;
 }
 
+// np.tan and np.log of a float32, correctly rounded
+__device__ __forceinline__ float hz_tan(float x)
+{
+    return hz_round(tan((double)x), x, haze_tan_arg, haze_tan_val, HAZE_TAN_N, true);
+}
+
+__device__ __forceinline__ float hz_log(float x)
+{
+    return hz_round(log((double)x), x, haze_log_arg, haze_log_val, HAZE_LOG_N, false);
+}
+
+__global__ void k_hz_debug_round(int fn, const float *x, float *out, int64_t n)
+{
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) out[i] = fn == 0 ? hz_tan(x[i]) : hz_log(x[i]);
+}
+
 // float64 word pair -> legacy random_double: (a >> 5, b >> 6), 53 bits
 __device__ __forceinline__ double hz_double(const uint32_t *stream, int64_t raw)
 {
@@ -121,7 +141,7 @@ __device__ __forceinline__ void hz_field(const HazeArgs &a, int b, int64_t g, co
     const float x = row[0], y = row[1], z = row[2], I = row[3];
     const float fwd = x == 0.0f ? 0.0001f : x;
     const float q = __fdiv_rn(y, fwd);
-    const float ang = a.angle ? a.angle[g] : hz_round(tan((double)q), q, haze_tan_arg, haze_tan_val, HAZE_TAN_N, true);
+    const float ang = a.angle ? a.angle[g] : hz_tan(q);
     const double an = (double)ang, h = (double)z;
     double field = 0.0;
     for (int k = 0; k < a.n_comp; k++) {
@@ -133,7 +153,7 @@ __device__ __forceinline__ void hz_field(const HazeArgs &a, int b, int64_t g, co
     }
     const double beta = __dadd_rn(field, a.beta[b]);
     const float v = __fdiv_rn(a.n_noise, __fadd_rn(I, a.gain));
-    const float lg = hz_round(log((double)v), v, haze_log_arg, haze_log_val, HAZE_LOG_N, false);
+    const float lg = hz_log(v);
     a.rbeta[g] = beta;
     a.dmax[g] = -__ddiv_rn((double)lg, __dmul_rn(2.0, beta));
 }
@@ -141,6 +161,7 @@ __device__ __forceinline__ void hz_field(const HazeArgs &a, int b, int64_t g, co
 __global__ void __launch_bounds__(HTILE) k_hz_det(HazeArgs a)
 {
     const int b = blockIdx.y, tile = blockIdx.x;
+    if (tile == 0 && threadIdx.x == 0) a.bad[b] = 0;
     if (tile >= a.det.tile_base[b + 1] - a.det.tile_base[b]) return;
     const int i = tile * HTILE + threadIdx.x;
     int cls = -1;
@@ -184,7 +205,11 @@ __global__ void __launch_bounds__(HTILE) k_hz_classify(HazeArgs a)
             const bool cloud_mask = dnew < dd && !lost;
             if (dd < dmax) { code |= HZ_STABLE; sc = 0; }
             else if (dmax < dd && cloud_mask) { code |= HZ_CLOUD; sc = 1; }
-            if (!cloud_mask && !lost) { code |= HZ_CAND; cand = 0; }
+            if (!cloud_mask && !lost) {
+                code |= HZ_CAND;
+                cand = 0;
+                if (!isfinite(isnan(dmax) ? dmax : fmin(dmax, dd))) a.bad[b] = 1;     // NaN kept, as np.min
+            }
         }
         a.code[g] = code;
     } else if (i < hz_rows(a, b)) {
@@ -271,11 +296,15 @@ struct OneCloud {                            // the chain of one cloud of n rows
 __global__ void __launch_bounds__(MT_TPB, 1) k_hz_chain(HazeArgs a, int32_t *J, uint32_t *state_out)
 {
     const int b = blockIdx.x;
-    const int64_t q = (int64_t)a.pos0 + 2 * (int64_t)a.n_det[b] + 2 * (int64_t)a.n_cand[b];
+    // a flagged cloud stops after its lost draws: no d_rand, no permutation (its K' becomes 0 for k_shuffle and
+    // k_hz_random; only this CTA's thread 0 writes it, and no thread reads it for a flagged cloud)
+    const bool bad = a.bad[b] != 0;
+    const int64_t q = (int64_t)a.pos0 + 2 * (int64_t)a.n_det[b] + (bad ? 0 : 2 * (int64_t)a.n_cand[b]);
     const int64_t kb = q == 0 ? 0 : (q - 1) / MT_N;
     const uint32_t *key = a.stream + kb * MT_N;
-    mt_chain(OneCloud{a.n_kept[b], a.off[b]}, [&](int t) { return key[t]; }, (int)(q - kb * MT_N), J,
+    mt_chain(OneCloud{bad ? 0 : a.n_kept[b], a.off[b]}, [&](int t) { return key[t]; }, (int)(q - kb * MT_N), J,
              state_out + (int64_t)b * (MT_N + 1));
+    if (bad && threadIdx.x == 0) a.n_kept[b] = 0;
 }
 
 __global__ void __launch_bounds__(256) k_hz_random(HazeArgs a)
@@ -285,7 +314,7 @@ __global__ void __launch_bounds__(256) k_hz_random(HazeArgs a)
     const bool beta0 = a.beta[b] == 0.0;
     const int m = beta0 ? 0 : (int)(a.fraction * (double)a.n_kept[b]);
     const int S = a.n_stable[b], C = a.n_cloud[b];
-    if (j == 0) a.out_cnt[b] = beta0 ? a.n_det[b] : S + C + m;
+    if (j == 0) a.out_cnt[b] = a.bad[b] ? -1 : beta0 ? a.n_det[b] : S + C + m;
     if (j >= m) return;
     const int64_t base = a.off[b];
     const int i = a.kidx[base + a.P[base + j]];
@@ -314,7 +343,7 @@ HazeLayout hz_layout(int64_t n_total, int n_clouds, int64_t n_max)
     L.sc = o;      o += seg_ws_bytes(N, n_clouds, HTILE, 2);
     L.cand = o;    o += seg_ws_bytes(N, n_clouds, HTILE, 1);
     L.kept = o;    o += seg_ws_bytes(N, n_clouds, HTILE, 1);
-    L.totals = o;  o = align_up(o + 5 * B * 4, 256);
+    L.totals = o;  o = align_up(o + 6 * B * 4, 256);
     L.code = o;    o = align_up(o + N, 256);
     L.rbeta = o;   o = align_up(o + N * 8, 256);
     L.dmax = o;    o = align_up(o + N * 8, 256);
@@ -399,6 +428,7 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
     a.sc.tile_base = a.cand.tile_base = a.kept.tile_base = a.det.tile_base;
     int32_t *tot = (int32_t *)(ws + L.totals);
     a.n_det = tot; a.n_stable = tot + B; a.n_cloud = tot + 2 * B; a.n_cand = tot + 3 * B; a.n_kept = tot + 4 * B;
+    a.bad = tot + 5 * B;
     a.det.total[0] = a.n_det;
     a.sc.total[0] = a.n_stable; a.sc.total[1] = a.n_cloud;
     a.cand.total[0] = a.n_cand;
@@ -433,7 +463,7 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
         LSS_CUDA_CHECK(e, lss_launch(e, k_hz_kept, gt, HTILE, 0, st, a));
     } else {
         ZeroRegions z;
-        z.add(tot, sizeof(int32_t) * 5 * B);
+        z.add(tot, sizeof(int32_t) * 6 * B);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
     int32_t *J = (int32_t *)(ws + L.J);
@@ -443,6 +473,16 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
                                      ShufArgs{a.off, a.n_kept, J, (unsigned long long *)(ws + L.R), a.P}));
     const unsigned mx = (unsigned)((g.max_n / 20 + 256) / 256);
     LSS_CUDA_CHECK(e, lss_launch(e, k_hz_random, dim3(mx, B), 256, 0, st, a));
+    return LSS_OK;
+}
+
+lss_status lss_debug_haze_round(lss_engine *e, int fn, const float *d_x, int64_t n, float *d_out, void *stream)
+{
+    if (!e || !d_x || !d_out || n < 0 || (fn != 0 && fn != 1)) return LSS_ERR_INVALID_ARG;
+    if (n == 0) return LSS_OK;
+    DeviceGuard g(e->device);
+    LSS_CUDA_CHECK(e, lss_launch(e, k_hz_debug_round, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, fn,
+                                 d_x, d_out, n));
     return LSS_OK;
 }
 

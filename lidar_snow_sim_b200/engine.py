@@ -580,8 +580,11 @@ class SnowfallEngine:
         per row to use instead of the device's correctly rounded one.  Returns dict(points (M, F + label) out_dtype with
         cloud b's rows at offsets[b] (M = offsets[B], slots of n_b + n_b // 20 + 1 rows), offsets int64 numpy (B + 1,),
         counts int32 CUDA (B,), states uint32 numpy (B, 625) each cloud's final key and pos).  The one synchronisation
-        is the copy of the states; NumPy's global state is then set to the last cloud's (the cached Gaussian as `state`
-        has it, as no Gaussian is drawn).
+        is the copy of the states and counts; NumPy's global state is then set to the last cloud's (the cached Gaussian
+        as `state` has it, as no Gaussian is drawn).  Where the reference raises OverflowError('Range exceeds valid
+        bounds') -- a random scatter candidate whose min(d_max, d) is NaN or infinite, e.g. from a NaN intensity, I = -g
+        or a non-finite y / x or z -- this raises it for the first such cloud, with NumPy's global state set to that
+        cloud's (after its lost draws).
         """
         off, B, N = _cloud_offsets(cloud_offsets)
         _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=4)
@@ -610,17 +613,24 @@ class SnowfallEngine:
         n = np.diff(off)
         out_off = np.zeros(B + 1, np.int64)
         np.cumsum(n + n // 20 + 1, out=out_off[1:])
-        out = _outputs(None, self.device, points=((int(out_off[-1]), Fo), out_dtype), counts=((B,), torch.int32),
-                       states=((B, 625), torch.int32))
+        out = _outputs(None, self.device, points=((int(out_off[-1]), Fo), out_dtype))
+        tail = torch.empty(B * 626, dtype=torch.int32, device=self.device)     # states then counts: one copy back
+        out['states'], out['counts'] = tail[:B * 625].view(B, 625), tail[B * 625:]
         ws = self._scratch('haze', self.lib.lss_haze_workspace_bytes(N, B))
         self._call('lss_haze_batch', points, F, _ptr(off), counts, B, _ptr(betas), _ptr(four), four.shape[0],
                    float(noise_level), float(gain), float(dmin), float(fraction_random), _ptr(words), angle,
                    1 if out_dtype == torch.float64 else 0, 1 if label else 0, out['points'], out['counts'],
                    out['states'], ws, ws.numel())
-        states = out['states'].cpu().numpy().view(np.uint32)
+        h = tail.cpu().numpy()
+        states = h[:B * 625].view(np.uint32).reshape(B, 625)
+        bad = np.flatnonzero(h[B * 625:] < 0)
         if B > 0:
             _, _, _, has_gauss, gauss = state
-            np.random.set_state(('MT19937', states[-1, :624].copy(), int(states[-1, 624]), has_gauss, gauss))
+            last = int(bad[0]) if bad.size else B - 1
+            np.random.set_state(('MT19937', states[last, :624].copy(), int(states[last, 624]), has_gauss, gauss))
+        if bad.size:
+            # the reference's np.random.uniform(high=scatter_max[...]) on a NaN or infinite bound, after the lost draws
+            raise OverflowError('Range exceeds valid bounds')
         return {'points': out['points'], 'offsets': out_off, 'counts': out['counts'], 'states': states}
 
     def dror_batch(self, points, cloud_offsets, alpha=0.16, beta=3.0, k_min=3, sr_min=0.04, counts=None, crop=False,

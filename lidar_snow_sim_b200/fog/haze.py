@@ -55,7 +55,9 @@ class BetaRadomization:
 
 def haze_point_cloud(pts_3D, beta_radomization, arguments, *, engine=None, angle=None):
     """lidar_foggification.py:61-149 on one cloud (N, F >= 4), NumPy's global RandomState as the stream.  `arguments`
-    needs sensor_type and fraction_random.  angle: optional float32 (N,) tangents to replay (see the module doc)."""
+    needs sensor_type and fraction_random.  angle: optional float32 (N,) tangents to replay (see the module doc).
+    Raises the reference's OverflowError('Range exceeds valid bounds') where its uniform draw of d_rand meets a NaN or
+    infinite bound, NumPy's global state left after the lost draws as the reference leaves it."""
     sensor = getattr(arguments, 'sensor_type', None)
     if sensor not in SENSOR_CONSTANTS:
         # the reference leaves n, g, dmin None and fails in its first comparison

@@ -105,8 +105,10 @@ def haze(pts, beta, fourier, state, sensor=(0.04, 0.45, 2), fraction_random=0.05
     """
     One cloud: pts float32 (N, F >= 4); beta the scalar of BetaRadomization; fourier (n, 6) fa, fh, oa, oh, ih, ia;
     state np.random.get_state() the draws start from; angle optional float32 (N,) per input row.  Returns dict(rows
-    float64 (M, F + 1), n_det, n_stable, n_cloud, n_cand, n_kept, perm (K',) int64, state (final get_state() tuple),
-    tuple_branch (beta == 0)).
+    float64 (M, F + 1), exponent (M,) the x of each row's attenuation exp(-x) (beta d, beta d_new or beta d_rand), n_det,
+    n_stable, n_cloud, n_cand, n_kept, perm (K',) int64, state (final get_state() tuple), tuple_branch (beta == 0)).
+    Raises OverflowError('Range exceeds valid bounds') where the reference's np.random.uniform(high=min(d_max, d)) meets
+    a NaN or infinite bound, with the state after the lost draws as its `state` attribute.
     """
     n_noise, gain, dmin = sensor
     pts = np.asarray(pts, np.float32)
@@ -127,15 +129,22 @@ def haze(pts, beta, fourier, state, sensor=(0.04, 0.45, 2), fraction_random=0.05
         rows = np.zeros((Np, F + 1))
         rows[:, 0:4] = p[:, 0:4]
         key, pos = st.block_at(2 * Np)
-        res.update(rows=rows, n_stable=Np, n_cloud=0, n_cand=0, n_kept=0, perm=np.zeros(0, np.int64),
-                   state=(state[0], key, pos, state[3], state[4]))
+        res.update(rows=rows, exponent=np.zeros(Np), n_stable=Np, n_cloud=0, n_cand=0, n_kept=0,
+                   perm=np.zeros(0, np.int64), state=(state[0], key, pos, state[3], state[4]))
         return res
     cloud_mask = (d_new < dd) & ~lost
     stable = np.flatnonzero(dd < d_max)
     cloud = np.flatnonzero((d_max < dd) & cloud_mask)
     cand = np.flatnonzero(~cloud_mask & ~lost)
     K = cand.size
-    d_rand = 0.0 + np.minimum(d_max, dd)[cand] * st.doubles(2 * Np, K)
+    high = np.minimum(d_max, dd)[cand]
+    if not np.all(np.isfinite(high)):
+        # legacy uniform checks its range before drawing: the reference raises after the lost draws
+        err = OverflowError('Range exceeds valid bounds')
+        key, pos = st.block_at(2 * Np)
+        err.state = (state[0], key, pos, state[3], state[4])
+        raise err
+    d_rand = 0.0 + high * st.doubles(2 * Np, K)
     keep = d_rand > dmin
     kept, d_rand = cand[keep], d_rand[keep]
     Kp = kept.size
@@ -155,8 +164,9 @@ def haze(pts, beta, fourier, state, sensor=(0.04, 0.45, 2), fraction_random=0.05
         return out
 
     rows = np.concatenate([block(stable, None, 0), block(cloud, d_new[cloud], 1), block(chosen, d_rc, 2)])
-    res.update(rows=rows, n_stable=stable.size, n_cloud=cloud.size, n_cand=K, n_kept=Kp, perm=perm,
-               state=(state[0], key, pos, state[3], state[4]))
+    exponent = np.concatenate([rb[stable] * dd[stable], rb[cloud] * d_new[cloud], rb[chosen] * d_rc])
+    res.update(rows=rows, exponent=exponent, n_stable=stable.size, n_cloud=cloud.size, n_cand=K, n_kept=Kp,
+               perm=perm, state=(state[0], key, pos, state[3], state[4]))
     return res
 
 
