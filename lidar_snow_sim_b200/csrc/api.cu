@@ -295,10 +295,23 @@ lss_status lss_snowfall_batch_slots(lss_engine *e, int table_id, const float *d_
     return lss_snowfall_run(e, a, (cudaStream_t)stream);
 }
 
+// lss_noise_threshold_poly's workspace: the device cloud offsets, then the pre-pass's own of pre_bytes
+static int64_t *poly_carve(WsCarve &c, void *&pre, int64_t &pre_bytes, int64_t n_total, int n_clouds)
+{
+    int64_t *off = c.take<int64_t>(n_clouds + 1);
+    pre_bytes = lss_prepass_ws_bytes(n_total, n_clouds);
+    pre = c.take<char>(pre_bytes);
+    return off;
+}
+
 int64_t lss_prepass_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return lss_prepass_ws_bytes(n_total, n_clouds) + 256 + (int64_t)(n_clouds + 1) * 8;
+    WsCarve c;
+    void *pre;
+    int64_t pre_bytes;
+    poly_carve(c, pre, pre_bytes, n_total, n_clouds);
+    return c.used;
 }
 
 lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets, int n_clouds,
@@ -313,10 +326,11 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
     DeviceGuard g(e->device);
     if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, n_clouds, h_plane_in != nullptr)) return rc;
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t off_bytes = align_up((int64_t)(n_clouds + 1) * 8, 256);
-    if (workspace_bytes < off_bytes + lss_prepass_ws_bytes(geo.n, n_clouds))
-        return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
-    int64_t *d_off = (int64_t *)d_workspace;
+    WsCarve c{(char *)d_workspace};
+    void *d_pre;
+    int64_t pre_bytes;
+    int64_t *d_off = poly_carve(c, d_pre, pre_bytes, geo.n, n_clouds);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), st));
     PrepassIO io;
     io.h_plane_in = h_plane_in;
@@ -326,7 +340,7 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
     io.d_fit_out = d_fit_out;
     io.d_ymins_out = d_ymins_out;
     return lss_prepass_run(e, d_points, d_off, nullptr, h_cloud_offsets, n_clouds, 0.5, noise_floor, 0, 0, 1, io,
-                           (char *)d_workspace + off_bytes, workspace_bytes - off_bytes, nullptr, st);
+                           d_pre, pre_bytes, nullptr, st);
 }
 
 lss_status lss_check_async(lss_engine *e, void *stream)

@@ -138,6 +138,20 @@ void lss_host_pipe_free(lss_engine *e);
 
 inline int64_t align_up(int64_t v, int64_t al) { return (v + al - 1) / al * al; }
 
+// Consecutive 256-byte-aligned regions of a workspace.  With base == nullptr it only counts, so the same code sizes a
+// workspace (the *_workspace_bytes query) and hands out its regions (the call).
+struct WsCarve {
+    char *base = nullptr;
+    int64_t used = 0;
+    // pointer to the next region of `count` T (null while counting); a count of 0 takes no bytes
+    template <typename T> T *take(int64_t count)
+    {
+        T *p = base ? (T *)(base + used) : nullptr;
+        used = align_up(used + count * (int64_t)sizeof(T), 256);
+        return p;
+    }
+};
+
 // Every kernel launch of the library goes through here, so that lss_launch_count() counts exactly what is enqueued.
 template <typename... P, typename... A>
 [[nodiscard]] inline cudaError_t lss_launch(lss_engine *e, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem,
@@ -387,5 +401,7 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
 // entry points call it before their own first enqueue.
 lss_status lss_prepass_check(lss_engine *e, const int64_t *h_cloud_off, int n_clouds, bool plane_given);
 int64_t lss_snowfall_ws_bytes(int64_t n_total, int n_clouds);
-// byte offset, inside the snowfall workspace, of the device copy of the cloud offsets (int64[n_clouds + 1]) a call uploads
-int64_t lss_snowfall_ws_cloud_off(int64_t n_total, int n_clouds);
+// The regions of lss_snowfall_run's workspace (beam.cuh's DevArgs), among them the device copy of the cloud offsets
+// (a.cloud_off) a call uploads.  Returns the scan schedule's region; `prepass` receives the pre-pass's workspace.
+struct DevArgs;
+int *lss_snowfall_carve(WsCarve &c, DevArgs &a, void *&prepass, int64_t n_total, int n_clouds);

@@ -279,25 +279,21 @@ cudaError_t sort_bytes(int64_t n, int n_clouds, size_t *bytes)
                                            (int)n, 0, end_bit(n_clouds));
 }
 
-struct DrorLayout { int64_t stats, off, tiles, seg, keys, rows, skeys, srows, packed, thr, sort, total; };
-
-DrorLayout dror_layout(int64_t n, int n_clouds, size_t sort_tmp)
+// The workspace, region by region; returns the radix sort's scratch.  The 32-byte work statistics stay at offset 0: the
+// Python engine reads them there.
+void *dror_carve(WsCarve &c, DrorArgs &a, int64_t n, int n_clouds, size_t sort_tmp)
 {
-    DrorLayout L;
-    int64_t o = 0;
-    L.stats = o;     o = align_up(o + 32, 256);
-    L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.tiles = o;     o += seg_ws_bytes(n, n_clouds, DTILE, 2);
-    L.seg = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
-    L.keys = o;      o = align_up(o + n * 8, 256);
-    L.rows = o;      o = align_up(o + n * 4, 256);
-    L.skeys = o;     o = align_up(o + n * 8, 256);
-    L.srows = o;     o = align_up(o + n * 4, 256);
-    L.packed = o;    o = align_up(o + n * 16, 256);
-    L.thr = o;       o = align_up(o + n * 8, 256);
-    L.sort = o;      o = align_up(o + (int64_t)sort_tmp, 256);
-    L.total = o;
-    return L;
+    a.stats = c.take<unsigned long long>(4);
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.tiles = seg_take(c, n, n_clouds, DTILE, 2);
+    a.seg = c.take<int32_t>(n_clouds + 1);
+    a.keys = c.take<unsigned long long>(n);
+    a.rows = c.take<int32_t>(n);
+    a.skeys = c.take<unsigned long long>(n);
+    a.srows = c.take<int32_t>(n);
+    a.packed = c.take<float4>(n);
+    a.thr = c.take<float2>(n);
+    return c.take<char>((int64_t)sort_tmp);
 }
 
 }  // namespace
@@ -309,7 +305,10 @@ int64_t lss_dror_workspace_bytes(int64_t n_total, int n_clouds)
     if (n_total < 0 || n_clouds < 0 || n_total >= (1LL << 31) || n_clouds > 65535) return -1;
     size_t tmp = 0;
     if (sort_bytes(n_total, n_clouds, &tmp) != cudaSuccess) return -1;
-    return dror_layout(n_total, n_clouds, tmp).total;
+    WsCarve c;
+    DrorArgs a;
+    dror_carve(c, a, n_total, n_clouds, tmp);
+    return c.used;
 }
 
 lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -335,36 +334,27 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
     cudaStream_t st = (cudaStream_t)stream;
     size_t sort_tmp = 0;
     LSS_CUDA_CHECK(e, sort_bytes(N, B, &sort_tmp));
-    const DrorLayout L = dror_layout(N, B, sort_tmp);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    DrorArgs a;
+    WsCarve c{(char *)d_workspace};
+    void *sort_ws = dror_carve(c, a, N, B, sort_tmp);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
 
-    char *ws = (char *)d_workspace;
-    DrorArgs a;
     a.pts = d_points;
     a.F = n_features;
     a.n_clouds = B;
-    a.cloud_off = (const int64_t *)(ws + L.off);
     a.cloud_cnt = d_cloud_counts;
     a.sr_coef = alpha_deg * beta * LSS_PI / 180;             // dror.py:318, evaluated left to right in float64
     a.sr_min = sr_min;
     a.k_need = k_min + 1;
     a.cube = (flags & LSS_DROR_CUBE) ? 1 : 0;
-    a.keys = (unsigned long long *)(ws + L.keys);
-    a.rows = (int32_t *)(ws + L.rows);
-    a.skeys = (const unsigned long long *)(ws + L.skeys);
-    a.srows = (const int32_t *)(ws + L.srows);
-    a.seg = (int32_t *)(ws + L.seg);
-    a.packed = (float4 *)(ws + L.packed);
-    a.thr = (float2 *)(ws + L.thr);
     a.keep = d_out_keep;
-    a.tiles = seg_tiles(ws + L.tiles, B);
     a.tiles.total[0] = d_out_n_snow;
     a.tiles.total[1] = d_out_counts;
     a.out_pts = d_out_points;
-    a.stats = (flags & LSS_DROR_WORK_STATS) ? (unsigned long long *)(ws + L.stats) : nullptr;
+    if (!(flags & LSS_DROR_WORK_STATS)) a.stats = nullptr;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
                                          (int32_t *)a.tiles.tile_base, st));
     if (a.stats) {
         ZeroRegions z;
@@ -377,7 +367,7 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
             const dim3 g256((unsigned)((g.max_n + 255) / 256), B), gt((unsigned)((g.max_n + DTILE - 1) / DTILE), B);
             LSS_CUDA_CHECK(e, lss_launch(e, k_dror_key, g256, 256, 0, st, a));
             size_t tmp = sort_tmp;
-            LSS_CUDA_CHECK(e, cub::DeviceRadixSort::SortPairs(ws + L.sort, tmp, (const unsigned long long *)a.keys,
+            LSS_CUDA_CHECK(e, cub::DeviceRadixSort::SortPairs(sort_ws, tmp, (const unsigned long long *)a.keys,
                                                               (unsigned long long *)a.skeys, (const int32_t *)a.rows,
                                                               (int32_t *)a.srows, (int)N, 0, end_bit(B), st));
             e->launches++;                                   // the sort's kernels count as one launch

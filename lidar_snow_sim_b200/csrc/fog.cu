@@ -291,21 +291,19 @@ __global__ void k_fog_info(FogArgs a, int B, double *info_out)
     info_out[3 * b + 2] = (double)cnt;
 }
 
-struct FogLayout { int64_t off, seg, seg_total, info, rng, par, total; };
-
-// per_cloud: room for the per-cloud parameters of lss_fog_batch_params behind lss_fog_batch's regions
-FogLayout fog_layout(int64_t n_total, int n_clouds, bool per_cloud = false)
+// The workspace, region by region; returns the noise generators' region.  per_cloud: room for the per-cloud parameters
+// of lss_fog_batch_params (B x (alpha, beta, beta_0), then B table indices) behind lss_fog_batch's regions.
+unsigned long long *fog_carve(WsCarve &c, FogArgs &a, int64_t n_total, int n_clouds, bool per_cloud)
 {
-    FogLayout L;
-    int64_t o = 0;
-    L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.seg = o;       o += seg_ws_bytes(n_total, n_clouds, FOG_TILE, 1);
-    L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 4, 256);
-    L.info = o;      o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
-    L.rng = o;       o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
-    L.par = o;       if (per_cloud) o = align_up(o + (int64_t)n_clouds * (3 * 8 + 4), 256);
-    L.total = o;
-    return L;
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.seg = seg_take(c, n_total, n_clouds, FOG_TILE, 1);
+    a.seg.total[0] = c.take<int32_t>(n_clouds);
+    a.info = c.take<unsigned long long>((int64_t)n_clouds * 4);
+    unsigned long long *rng = c.take<unsigned long long>((int64_t)n_clouds * 4);
+    char *par = c.take<char>(per_cloud ? (int64_t)n_clouds * (3 * 8 + 4) : 0);
+    a.cloud_par = per_cloud ? (const double *)par : nullptr;
+    a.cloud_lut = per_cloud && par ? (const int32_t *)(par + (int64_t)n_clouds * 3 * 8) : nullptr;
+    return rng;
 }
 
 // per-cloud fog parameters of lss_fog_batch_params (host arrays); null for lss_fog_batch
@@ -348,23 +346,18 @@ lss_status fog_run(lss_engine *e, const float *d_points, int n_features, const i
     }
     const int64_t N = g.n;
     if (!d_points && N > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
-    const FogLayout L = fog_layout(N, B, pc != nullptr);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    FogArgs a;
+    WsCarve c{(char *)d_workspace};
+    unsigned long long *rng = fog_carve(c, a, N, B, pc != nullptr);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
 
-    FogArgs a;
     a.pts = d_points;
     a.F = n_features;
-    a.cloud_off = (const int64_t *)(ws + L.off);
-    a.seg = seg_tiles(ws + L.seg, B);
-    a.seg.total[0] = (int32_t *)(ws + L.seg_total);
     a.lut = d_lut;
     a.alpha = alpha; a.beta = beta; a.beta_0 = beta_0;
-    a.cloud_par = pc ? (const double *)(ws + L.par) : nullptr;
-    a.cloud_lut = pc ? (const int32_t *)(ws + L.par + (int64_t)B * 3 * 8) : nullptr;
     a.hard = (flags & LSS_FOG_HARD) ? 1 : 0;
     a.soft = soft ? 1 : 0;
     a.gain = (soft && (flags & LSS_FOG_GAIN)) ? 1 : 0;
@@ -375,18 +368,17 @@ lss_status fog_run(lss_engine *e, const float *d_points, int n_features, const i
     a.out = d_out;
     a.mask = d_out_fog_mask;
     a.rank = d_out_rank;
-    a.info = (unsigned long long *)(ws + L.info);
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
                                          (int32_t *)a.seg.tile_base, st));
-    if (pc) LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.par, par.data(), par.size(), st));
+    if (pc) LSS_CUDA_CHECK(e, lss_stage_upload(e, (double *)a.cloud_par, par.data(), par.size(), st));
     if (h_rng_state && soft && noise > 0 && noise_variant != 4 && !d_ext_noise) {
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.rng, h_rng_state, sizeof(uint64_t) * 4 * B, st));
-        a.rng = (const unsigned long long *)(ws + L.rng);
+        LSS_CUDA_CHECK(e, lss_stage_upload(e, rng, h_rng_state, sizeof(uint64_t) * 4 * B, st));
+        a.rng = rng;
     }
     {
         ZeroRegions z;
-        z.add(ws + L.info, (size_t)B * 4 * 8);
+        z.add(a.info, (size_t)B * 4 * 8);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
     const dim3 grid((unsigned)((g.max_n + FOG_TILE - 1) / FOG_TILE), B);
@@ -410,13 +402,19 @@ lss_status fog_run(lss_engine *e, const float *d_points, int n_features, const i
 int64_t lss_fog_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return fog_layout(n_total, n_clouds).total;
+    WsCarve c;
+    FogArgs a;
+    fog_carve(c, a, n_total, n_clouds, false);
+    return c.used;
 }
 
 int64_t lss_fog_batch_params_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return fog_layout(n_total, n_clouds, true).total;
+    WsCarve c;
+    FogArgs a;
+    fog_carve(c, a, n_total, n_clouds, true);
+    return c.used;
 }
 
 lss_status lss_fog_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,

@@ -290,16 +290,11 @@ LutTable lut_table(const lss_fog_table_params &q)
     return p;
 }
 
-struct LutLayout { int64_t tables, f, total; };
-
-LutLayout lut_layout(int n, int T)
+// The workspace: the tables' constants [T], then the response integrals f [T * n]
+void lut_carve(WsCarve &c, LutTable *&tables, double *&f, int n, int T)
 {
-    LutLayout L;
-    int64_t o = 0;
-    L.tables = o; o = align_up(o + (int64_t)T * (int64_t)sizeof(LutTable), 256);
-    L.f = o;      o = align_up(o + (int64_t)T * n * 8, 256);
-    L.total = o;
-    return L;
+    tables = c.take<LutTable>(T);
+    f = c.take<double>((int64_t)T * n);
 }
 
 }  // namespace
@@ -307,7 +302,11 @@ LutLayout lut_layout(int n, int T)
 int64_t lss_fog_integral_tables_workspace_bytes(int n, int n_tables)
 {
     if (n < 3 || n > LUT_MAX_N || n_tables <= 0) return -1;
-    return lut_layout(n, n_tables).total;
+    WsCarve c;
+    LutTable *tables;
+    double *f;
+    lut_carve(c, tables, f, n, n_tables);
+    return c.used;
 }
 
 lss_status lss_fog_integral_tables(lss_engine *e, const lss_fog_table_params *h_params, int n_tables, double *d_out,
@@ -317,18 +316,18 @@ lss_status lss_fog_integral_tables(lss_engine *e, const lss_fog_table_params *h_
     LutGrid g;
     if (const char *why = lut_grid(h_params, n_tables, g)) return lss_fail(e, LSS_ERR_INVALID_ARG, why);
     if (!d_out || !d_workspace) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    const LutLayout L = lut_layout(g.n, n_tables);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    WsCarve c{(char *)d_workspace};
+    LutTable *d_tables;
+    double *d_f;
+    lut_carve(c, d_tables, d_f, g.n, n_tables);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     std::vector<LutTable> tables(n_tables);
     for (int t = 0; t < n_tables; t++) tables[t] = lut_table(h_params[t]);
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    const LutTable *d_tables = (const LutTable *)(ws + L.tables);
-    double *d_f = (double *)(ws + L.f);
     const size_t smem_resp = (size_t)g.n * 2 * sizeof(double);
     LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_fog_response, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_resp));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.tables, tables.data(), sizeof(LutTable) * n_tables, st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_tables, tables.data(), sizeof(LutTable) * n_tables, st));
     KernelTimer kt(e, LSS_K_FOG_LUT, st);
     LSS_CUDA_CHECK(e, lss_launch(e, k_fog_response, dim3(g.n_used, n_tables), LUT_TPB, smem_resp, st, d_tables, g, d_f));
     LSS_CUDA_CHECK(e, lss_launch(e, k_fog_table, n_tables, LUT_TPB, (size_t)g.n_used * sizeof(int), st, d_tables, g,

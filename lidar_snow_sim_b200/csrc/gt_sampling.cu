@@ -310,17 +310,12 @@ __global__ void __launch_bounds__(GT_TILE) k_gt_paste(PasteArgs a, int n_clouds)
     store_row(a, p, a.out_off[b] + a.n_obj_rows_b[b] + r, b, p[0], p[1], p[2]);
 }
 
-struct PasteLayout { int64_t off, seg, kept, code, total; };
-
-PasteLayout paste_layout(int64_t n, int B)
+void paste_carve(WsCarve &c, PasteArgs &a, int64_t n, int B)
 {
-    PasteLayout L;
-    L.off = 0;
-    L.seg = align_up(L.off + 8 * (int64_t)(B + 1), 256);     // the SegTiles region starts with its tile bases
-    L.kept = align_up(L.seg + seg_ws_bytes(n, B, GT_TILE, 1), 256);
-    L.code = align_up(L.kept + 4 * (int64_t)B, 256);
-    L.total = align_up(L.code + n, 256);
-    return L;
+    a.off = c.take<int64_t>(B + 1);
+    a.seg = seg_take(c, n, B, GT_TILE, 1);
+    a.kept = c.take<int32_t>(B);
+    a.code = c.take<uint8_t>(n);
 }
 
 }  // namespace
@@ -354,7 +349,10 @@ lss_status lss_gt_collide_batch(lss_engine *e, int n_clouds, int n_classes, cons
 int64_t lss_gt_paste_workspace_bytes(const int64_t *h_cloud_offsets, int n_clouds)
 {
     if (!h_cloud_offsets || n_clouds < 0) return -1;
-    return paste_layout(h_cloud_offsets[n_clouds], n_clouds).total;
+    WsCarve c;
+    PasteArgs a{};
+    paste_carve(c, a, h_cloud_offsets[n_clouds], n_clouds);
+    return c.used;
 }
 
 lss_status lss_gt_paste_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -378,23 +376,20 @@ lss_status lss_gt_paste_batch(lss_engine *e, const float *d_points, int n_featur
         (max_rm_boxes > 0 && !d_rm_boxes))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
     if (n_objects == 0 && n_object_rows > 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "object rows without objects");
-    const PasteLayout L = paste_layout(g.n, B);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    PasteArgs a{};
+    WsCarve c{(char *)d_workspace};
+    paste_carve(c, a, g.n, B);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    PasteArgs a{};
-    a.pts = d_points; a.F = n_features; a.off = (const int64_t *)(ws + L.off); a.cnt = d_cloud_counts;
+    a.pts = d_points; a.F = n_features; a.cnt = d_cloud_counts;
     a.rm = d_rm_boxes; a.rm_off = d_rm_offsets; a.ops = d_ops; a.max_ops = max_ops;
     a.db = d_db; a.obj = d_objects; a.obj_shift = d_object_shift; a.n_obj = n_objects; a.n_obj_rows = n_object_rows;
     a.out_off = d_out_offsets; a.n_obj_rows_b = d_object_rows;
-    a.code = (uint8_t *)(ws + L.code);
-    a.seg = seg_tiles(ws + L.seg, B);
-    a.kept = (int32_t *)(ws + L.kept);
     a.seg.total[0] = a.kept;
     a.out = d_out; a.counts = d_counts;
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.seg, g.tile_base.data(), sizeof(int32_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * (B + 1), st));
     const int64_t obj_blocks = (n_object_rows + GT_TILE - 1) / GT_TILE;
     const int64_t scene_tiles = (g.max_n + GT_TILE - 1) / GT_TILE;
     if (g.max_n > 0) {

@@ -324,37 +324,33 @@ __global__ void __launch_bounds__(256) k_hz_random(HazeArgs a)
     hz_write(a, a.out_off[b] + S + C + j, row, dr, d, __dmul_rn((double)row[3], exp(__dmul_rn(-a.rbeta[g], dr))), 2);
 }
 
-struct HazeLayout { int64_t off, out_off, beta, state, det, sc, cand, kept, totals, code, rbeta, dmax, drand, kidx, J, P, R,
-                    stream, total; };
-
 // key blocks the stream needs: every chain starts at raw word pos + 2 N' + 2 K <= 624 + 4 n_max
 int64_t hz_stream_blocks(int64_t n_max) { return (MT_N + 4 * n_max) / MT_N + 1; }
 
-HazeLayout hz_layout(int64_t n_total, int n_clouds, int64_t n_max)
+// The workspace, region by region, into the kernels' arguments and the shuffle's; returns the region the MT19937 state is
+// uploaded to.  The totals region holds six [B] arrays (n_det first); the stream is sized for clouds of up to n_max rows.
+uint32_t *hz_carve(WsCarve &c, HazeArgs &a, ShufArgs &sa, int64_t n_total, int n_clouds, int64_t n_max)
 {
-    HazeLayout L;
-    int64_t o = 0;
     const int64_t N = n_total, B = n_clouds;
-    L.off = o;     o = align_up(o + (B + 1) * 8, 256);
-    L.out_off = o; o = align_up(o + (B + 1) * 8, 256);
-    L.beta = o;    o = align_up(o + B * 8, 256);
-    L.state = o;   o = align_up(o + (MT_N + 1) * 4, 256);
-    L.det = o;     o += seg_ws_bytes(N, n_clouds, HTILE, 1);
-    L.sc = o;      o += seg_ws_bytes(N, n_clouds, HTILE, 2);
-    L.cand = o;    o += seg_ws_bytes(N, n_clouds, HTILE, 1);
-    L.kept = o;    o += seg_ws_bytes(N, n_clouds, HTILE, 1);
-    L.totals = o;  o = align_up(o + 6 * B * 4, 256);
-    L.code = o;    o = align_up(o + N, 256);
-    L.rbeta = o;   o = align_up(o + N * 8, 256);
-    L.dmax = o;    o = align_up(o + N * 8, 256);
-    L.drand = o;   o = align_up(o + N * 8, 256);
-    L.kidx = o;    o = align_up(o + N * 4, 256);
-    L.J = o;       o = align_up(o + N * 4, 256);
-    L.P = o;       o = align_up(o + N * 4, 256);
-    L.R = o;       o = align_up(o + N * 8, 256);
-    L.stream = o;  o = align_up(o + hz_stream_blocks(n_max) * MT_N * 4, 256);
-    L.total = o;
-    return L;
+    a.off = c.take<int64_t>(B + 1);
+    a.out_off = c.take<int64_t>(B + 1);
+    a.beta = c.take<double>(B);
+    uint32_t *state = c.take<uint32_t>(MT_N + 1);
+    a.det = seg_take(c, N, n_clouds, HTILE, 1);
+    a.sc = seg_take(c, N, n_clouds, HTILE, 2);
+    a.cand = seg_take(c, N, n_clouds, HTILE, 1);
+    a.kept = seg_take(c, N, n_clouds, HTILE, 1);
+    a.n_det = c.take<int32_t>(6 * B);
+    a.code = c.take<uint8_t>(N);
+    a.rbeta = c.take<double>(N);
+    a.dmax = c.take<double>(N);
+    a.drand = c.take<double>(N);
+    a.kidx = c.take<int32_t>(N);
+    sa.J = c.take<int32_t>(N);
+    a.P = sa.P = c.take<int32_t>(N);
+    sa.R = c.take<unsigned long long>(N);
+    a.stream = c.take<uint32_t>(hz_stream_blocks(n_max) * MT_N);
+    return state;
 }
 
 }  // namespace
@@ -364,7 +360,11 @@ extern "C" {
 int64_t lss_haze_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return hz_layout(n_total, n_clouds, n_total).total;
+    WsCarve c;
+    HazeArgs a{};
+    ShufArgs sa{};
+    hz_carve(c, a, sa, n_total, n_clouds, n_total);
+    return c.used;
 }
 
 lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -393,25 +393,23 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
         if (h_beta[b] == 0.0 && n_features != 4)        // the reference copies 4 columns into the F + 1 of its tuple
             return lss_fail(e, LSS_ERR_INVALID_ARG, "beta 0 (the tuple branch) needs n_features == 4");
     }
-    const HazeLayout L = hz_layout(g.n, B, g.max_n);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    HazeArgs a{};
+    ShufArgs sa{};
+    WsCarve c{(char *)d_workspace};
+    uint32_t *d_state = hz_carve(c, a, sa, g.n, B, g.max_n);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
 
     std::vector<int64_t> out_off(B + 1, 0);
     for (int b = 0; b < B; b++) {
         const int64_t n = h_cloud_offsets[b + 1] - h_cloud_offsets[b];
         out_off[b + 1] = out_off[b] + n + n / 20 + 1;
     }
-    HazeArgs a{};
     a.pts = d_points;
     a.F = n_features;
-    a.off = (const int64_t *)(ws + L.off);
     a.cnt = d_cloud_counts;
-    a.out_off = (const int64_t *)(ws + L.out_off);
-    a.beta = (const double *)(ws + L.beta);
     a.angle = d_angle;
     a.n_comp = n_components;
     for (int k = 0; k < 6 * n_components; k++) a.four[k] = h_fourier[k];
@@ -420,37 +418,26 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
     a.dmin = dmin;
     a.fraction = fraction_random;
     a.pos0 = (int)h_mt_state[MT_N];
-    a.stream = (const uint32_t *)(ws + L.stream);
-    a.det = seg_tiles(ws + L.det, B);
-    a.sc = seg_tiles(ws + L.sc, B);
-    a.cand = seg_tiles(ws + L.cand, B);
-    a.kept = seg_tiles(ws + L.kept, B);
     a.sc.tile_base = a.cand.tile_base = a.kept.tile_base = a.det.tile_base;
-    int32_t *tot = (int32_t *)(ws + L.totals);
-    a.n_det = tot; a.n_stable = tot + B; a.n_cloud = tot + 2 * B; a.n_cand = tot + 3 * B; a.n_kept = tot + 4 * B;
+    int32_t *tot = a.n_det;
+    a.n_stable = tot + B; a.n_cloud = tot + 2 * B; a.n_cand = tot + 3 * B; a.n_kept = tot + 4 * B;
     a.bad = tot + 5 * B;
     a.det.total[0] = a.n_det;
     a.sc.total[0] = a.n_stable; a.sc.total[1] = a.n_cloud;
     a.cand.total[0] = a.n_cand;
     a.kept.total[0] = a.n_kept;
-    a.code = (uint8_t *)(ws + L.code);
-    a.rbeta = (double *)(ws + L.rbeta);
-    a.dmax = (double *)(ws + L.dmax);
-    a.drand = (double *)(ws + L.drand);
-    a.kidx = (int32_t *)(ws + L.kidx);
-    a.P = (int32_t *)(ws + L.P);
     a.out = d_out_points;
     a.out_f64 = out_f64 ? 1 : 0;
     a.out_label = out_label ? 1 : 0;
     a.out_cnt = d_out_counts;
 
-    int64_t *d_off = (int64_t *)(ws + L.off);
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)a.det.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.out_off, out_off.data(), sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.beta, h_beta, sizeof(double) * B, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.state, h_mt_state, sizeof(uint32_t) * (MT_N + 1), st));
-    LSS_CUDA_CHECK(e, lss_launch(e, k_hz_stream, 1, MT_TPB, 0, st, (const uint32_t *)(ws + L.state),
-                                 (int)hz_stream_blocks(g.max_n), (uint32_t *)(ws + L.stream)));
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.off, (int32_t *)a.det.tile_base,
+                                         st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.out_off, out_off.data(), sizeof(int64_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (double *)a.beta, h_beta, sizeof(double) * B, st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_state, h_mt_state, sizeof(uint32_t) * (MT_N + 1), st));
+    LSS_CUDA_CHECK(e, lss_launch(e, k_hz_stream, 1, MT_TPB, 0, st, (const uint32_t *)d_state,
+                                 (int)hz_stream_blocks(g.max_n), (uint32_t *)a.stream));
     const dim3 gt((unsigned)(g.max_n > 0 ? (g.max_n + HTILE - 1) / HTILE : 1), B);
     if (g.max_n > 0) {
         LSS_CUDA_CHECK(e, lss_launch(e, k_hz_det, gt, HTILE, 0, st, a));
@@ -466,11 +453,10 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
         z.add(tot, sizeof(int32_t) * 6 * B);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
-    int32_t *J = (int32_t *)(ws + L.J);
-    LSS_CUDA_CHECK(e, lss_launch(e, k_hz_chain, B, MT_TPB, 0, st, a, J, d_mt_state_out));
-    if (g.max_n > 0)
-        LSS_CUDA_CHECK(e, lss_launch(e, k_shuffle, B, SHUF_TPB, 0, st,
-                                     ShufArgs{a.off, a.n_kept, J, (unsigned long long *)(ws + L.R), a.P}));
+    LSS_CUDA_CHECK(e, lss_launch(e, k_hz_chain, B, MT_TPB, 0, st, a, sa.J, d_mt_state_out));
+    sa.cloud_off = a.off;
+    sa.cloud_cnt = a.n_kept;
+    if (g.max_n > 0) LSS_CUDA_CHECK(e, lss_launch(e, k_shuffle, B, SHUF_TPB, 0, st, sa));
     const unsigned mx = (unsigned)((g.max_n / 20 + 256) / 256);
     LSS_CUDA_CHECK(e, lss_launch(e, k_hz_random, dim3(mx, B), 256, 0, st, a));
     return LSS_OK;

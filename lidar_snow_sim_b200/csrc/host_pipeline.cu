@@ -21,7 +21,7 @@
 #include <cstdlib>
 #include <vector>
 
-#include "common.cuh"
+#include "beam.cuh"
 
 struct PipeSlot {
     bool busy = false;
@@ -272,10 +272,13 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
         if (ce == cudaSuccess) ce = cudaStreamWaitEvent(p->s_d2h, ev_beam, 0);
         if (ce == cudaSuccess && nr > 0) {
             if (h_out_dev) {        // page-locked result buffer: only the kept rows travel (see k_copy_rows_out)
-                // cloud offsets of this chunk on the device: the snowfall stage uploaded them to the head of its workspace
-                const int64_t *d_off_chunk = (const int64_t *)(ws + lss_snowfall_ws_cloud_off(nr, nb));
+                // cloud offsets of this chunk on the device: the snowfall stage uploaded them into its workspace
+                WsCarve wc{ws};
+                DevArgs da;
+                void *prepass;
+                lss_snowfall_carve(wc, da, prepass, nr, nb);
                 ce = lss_launch(e, k_copy_rows_out, dim3(COPY_OUT_BLOCKS, nb), 256, 0, p->s_d2h, sl.d_out + r0 * 5,
-                                d_off_chunk, sl.d_counts + b0, h_out_dev + r0 * 5);
+                                da.cloud_off, sl.d_counts + b0, h_out_dev + r0 * 5);
             } else {
                 ce = cudaMemcpyAsync(h_out_points + r0 * 5, sl.d_out + r0 * 5, (size_t)nr * 5 * sizeof(float),
                                      cudaMemcpyDeviceToHost, p->s_d2h);

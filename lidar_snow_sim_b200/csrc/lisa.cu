@@ -329,20 +329,15 @@ void lisa_constants(int mode, double rain_rate, double min_diameter, double r_ma
     a.p_min = 0.9 * libm_pow(r_max, -2.0);                                    // :58
 }
 
-struct LisaLayout { int64_t off, seg, cloud, res, label, code, total; };
-
-LisaLayout lisa_layout(int64_t n, int n_clouds)
+// The workspace, region by region: device cloud offsets, segment tiles, per-cloud constants, results, labels, codes
+void lisa_carve(WsCarve &c, LisaBatchArgs &a, int64_t n, int n_clouds)
 {
-    LisaLayout L;
-    int64_t o = 0;
-    L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.seg = o;       o += seg_ws_bytes(n, n_clouds, LISA_TILE, 2);
-    L.cloud = o;     o = align_up(o + (int64_t)n_clouds * (int64_t)sizeof(LisaCloud), 256);
-    L.res = o;       o = align_up(o + n * 16, 256);
-    L.label = o;     o = align_up(o + n, 256);
-    L.code = o;      o = align_up(o + n, 256);
-    L.total = o;
-    return L;
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.seg = seg_take(c, n, n_clouds, LISA_TILE, 2);
+    a.cloud = c.take<LisaCloud>(n_clouds);
+    a.res = c.take<float4>(n);
+    a.label = c.take<uint8_t>(n);
+    a.code = c.take<uint8_t>(n);
 }
 
 }  // namespace
@@ -386,7 +381,10 @@ extern "C" lss_status lss_lisa_batch(lss_engine *e, const double *d_points, int 
 extern "C" int64_t lss_lisa_cloud_batch_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return lisa_layout(n_total, n_clouds).total;
+    WsCarve c;
+    LisaBatchArgs a;
+    lisa_carve(c, a, n_total, n_clouds);
+    return c.used;
 }
 
 extern "C" lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points, int n_features,
@@ -437,33 +435,27 @@ extern "C" lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points,
         c.alpha = h_alpha[b];
         c.seed = h_seed ? h_seed[b] : 0;
     }
-    const LisaLayout L = lisa_layout(N, B);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    LisaBatchArgs a;
+    WsCarve c{(char *)d_workspace};
+    lisa_carve(c, a, N, B);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
 
-    LisaBatchArgs a;
     a.base = base;
     a.pts = d_points;
     a.F = n_features;
     a.n_clouds = B;
     a.n_total = N;
-    a.cloud_off = (const int64_t *)(ws + L.off);
     a.cloud_cnt = d_cloud_counts;
-    a.cloud = (const LisaCloud *)(ws + L.cloud);
-    a.res = (float4 *)(ws + L.res);
-    a.label = (uint8_t *)(ws + L.label);
-    a.code = (uint8_t *)(ws + L.code);
-    a.seg = seg_tiles(ws + L.seg, B);
     a.seg.total[0] = d_out_counts;
     a.seg.total[1] = d_out_n_lost;
     a.out = d_out_points;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
                                          (int32_t *)a.seg.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.cloud, cloud.data(), sizeof(LisaCloud) * cloud.size(), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (LisaCloud *)a.cloud, cloud.data(), sizeof(LisaCloud) * cloud.size(), st));
     KernelTimer kt(e, LSS_K_LISA, st);
     if (g.max_n > 0) {
         const unsigned blocks = (unsigned)std::min<long long>((N + 7) / 8, (long long)e->n_sm * 64);

@@ -97,10 +97,10 @@ __global__ void __launch_bounds__(MIE_TPB) k_mie(const MieRow *rows, int n_rows,
 
 struct MiePlan {
     std::vector<MieRow> rows;                   // in launch order
-    int64_t off_rows, off_d, total;
+    int64_t d_words;                            // D storage of all rows
 };
 
-// checks the arguments, derives every row and the workspace layout; nullptr on success, else the reason
+// checks the arguments, derives every row and its D storage; nullptr on success, else the reason
 const char *mie_plan(const double *h_m, const double *h_wl, int T, const double *h_d, int nd, MiePlan &P)
 {
     if (!h_m || !h_wl || !h_d) return "null argument";
@@ -133,18 +133,21 @@ const char *mie_plan(const double *h_m, const double *h_wl, int T, const double 
         return (int64_t)a.n_mx + a.n_stop > (int64_t)b.n_mx + b.n_stop;
     });
     // D storage: each warp's rows interleaved, as long as its longest n_stop
-    int64_t d_words = 0;
+    P.d_words = 0;
     for (size_t w = 0; w < P.rows.size(); w += MIE_TPB) {
         int32_t longest = 0;
         for (size_t k = w; k < std::min(P.rows.size(), w + MIE_TPB); k++) longest = std::max(longest, P.rows[k].n_stop);
-        for (size_t k = w; k < std::min(P.rows.size(), w + MIE_TPB); k++) P.rows[k].d_off = d_words + (int64_t)(k - w);
-        d_words += (int64_t)longest * MIE_TPB;
+        for (size_t k = w; k < std::min(P.rows.size(), w + MIE_TPB); k++) P.rows[k].d_off = P.d_words + (int64_t)(k - w);
+        P.d_words += (int64_t)longest * MIE_TPB;
     }
-    int64_t o = 0;
-    P.off_rows = o; o = align_up(o + (int64_t)(P.rows.size() * sizeof(MieRow)), 256);
-    P.off_d = o;    o = align_up(o + d_words * 8, 256);
-    P.total = o;
     return nullptr;
+}
+
+// The workspace: the rows, then their D storage
+void mie_carve(WsCarve &c, const MiePlan &P, MieRow *&rows, double *&d)
+{
+    rows = c.take<MieRow>((int64_t)P.rows.size());
+    d = c.take<double>(P.d_words);
 }
 
 }  // namespace
@@ -154,7 +157,11 @@ int64_t lss_mie_tables_workspace_bytes(const double *h_refractive_index, const d
 {
     MiePlan P;
     if (mie_plan(h_refractive_index, h_wavelength_nm, n_tables, h_diameter_nm, n_diameters, P)) return -1;
-    return P.total;
+    WsCarve c;
+    MieRow *rows;
+    double *d;
+    mie_carve(c, P, rows, d);
+    return c.used;
 }
 
 lss_status lss_mie_tables(lss_engine *e, const double *h_refractive_index, const double *h_wavelength_nm, int n_tables,
@@ -166,14 +173,17 @@ lss_status lss_mie_tables(lss_engine *e, const double *h_refractive_index, const
     if (const char *why = mie_plan(h_refractive_index, h_wavelength_nm, n_tables, h_diameter_nm, n_diameters, P))
         return lss_fail(e, LSS_ERR_INVALID_ARG, why);
     if (!d_out || !d_workspace) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    if (workspace_bytes < P.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    WsCarve c{(char *)d_workspace};
+    MieRow *d_rows;
+    double *d_d;
+    mie_carve(c, P, d_rows, d_d);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
     const int n_rows = (int)P.rows.size();
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + P.off_rows, P.rows.data(), sizeof(MieRow) * P.rows.size(), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_rows, P.rows.data(), sizeof(MieRow) * P.rows.size(), st));
     KernelTimer kt(e, LSS_K_MIE, st);
-    LSS_CUDA_CHECK(e, lss_launch(e, k_mie, (n_rows + MIE_TPB - 1) / MIE_TPB, MIE_TPB, 0, st,
-                                 (const MieRow *)(ws + P.off_rows), n_rows, (double *)(ws + P.off_d), d_out));
+    LSS_CUDA_CHECK(e, lss_launch(e, k_mie, (n_rows + MIE_TPB - 1) / MIE_TPB, MIE_TPB, 0, st, (const MieRow *)d_rows, n_rows,
+                                 d_d, d_out));
     return LSS_OK;
 }

@@ -390,11 +390,9 @@ __global__ void __launch_bounds__(256) k_pa_fps(const int64_t *jobs, const doubl
     }
 }
 
-struct PaLayout { int64_t off, box_off, tile_base, tc_base, tile_cnt, total; };
-
-// partition workspace: cloud offsets, box offsets, tile bases, tile-counter bases, the tile counters
-bool pa_layout(const int64_t *h_off, const int64_t *h_box_off, int B, PaLayout &L, std::vector<int32_t> &tile_base,
-               std::vector<int64_t> &tc_base)
+// host tile bases and tile-counter bases of a batch; false for bad box offsets or clouds
+bool pa_tiles(const int64_t *h_off, const int64_t *h_box_off, int B, std::vector<int32_t> &tile_base,
+              std::vector<int64_t> &tc_base)
 {
     tile_base.assign((size_t)B + 1, 0);
     tc_base.assign((size_t)B + 1, 0);
@@ -405,28 +403,29 @@ bool pa_layout(const int64_t *h_off, const int64_t *h_box_off, int B, PaLayout &
         tile_base[b + 1] = tile_base[b] + (int32_t)nt;
         tc_base[b + 1] = tc_base[b] + nt * (m * PA_PARTS + 1);
     }
-    int64_t o = 0;
-    L.off = o;       o = align_up(o + (int64_t)(B + 1) * 8, 256);
-    L.box_off = o;   o = align_up(o + (int64_t)(B + 1) * 8, 256);
-    L.tile_base = o; o = align_up(o + (int64_t)(B + 1) * 4, 256);
-    L.tc_base = o;   o = align_up(o + (int64_t)(B + 1) * 8, 256);
-    L.tile_cnt = o;  o = align_up(o + tc_base[B] * 4, 256);
-    L.total = o;
     return true;
 }
 
-struct PaApplyLayout { int64_t members, fps_rows, fps_dist, fps_out, total; };
-
-PaApplyLayout pa_apply_layout(int64_t base, int64_t n_members, int64_t n_fps_rows, int64_t n_fps_out)
+// partition workspace: cloud offsets, box offsets, tile bases, tile-counter bases, the tile counters
+void pa_carve(WsCarve &c, PartArgs &a, int B, int64_t n_tile_cnt)
 {
-    PaApplyLayout L;
-    int64_t o = align_up(base, 256);
-    L.members = o;   o = align_up(o + n_members * 4, 256);
-    L.fps_rows = o;  o = align_up(o + n_fps_rows * 32, 256);
-    L.fps_dist = o;  o = align_up(o + n_fps_rows * 8, 256);
-    L.fps_out = o;   o = align_up(o + n_fps_out * 32, 256);
-    L.total = o;
-    return L;
+    a.off = c.take<int64_t>(B + 1);
+    a.box_off = c.take<int64_t>(B + 1);
+    a.tile_base = c.take<int32_t>(B + 1);
+    a.tc_base = c.take<int64_t>(B + 1);
+    a.tile_cnt = c.take<int>(n_tile_cnt);
+}
+
+// apply workspace: the partition's (the apply step reads what the partition left there), then the class members, the
+// FPS input rows (x, y, z, i), their distances and the FPS output rows
+void pa_apply_carve(WsCarve &c, PartArgs &a, double *&fps_rows, double *&fps_dist, double *&fps_out, int B,
+                    int64_t n_tile_cnt, int64_t n_members, int64_t n_fps_rows, int64_t n_fps_out)
+{
+    pa_carve(c, a, B, n_tile_cnt);
+    a.members = c.take<int32_t>(n_members);
+    fps_rows = c.take<double>(n_fps_rows * 4);
+    fps_dist = c.take<double>(n_fps_rows);
+    fps_out = c.take<double>(n_fps_out * 4);
 }
 
 size_t pa_smem_bytes(int max_boxes, bool scatter)
@@ -437,12 +436,12 @@ size_t pa_smem_bytes(int max_boxes, bool scatter)
 
 lss_status pa_common(lss_engine *e, const float *d_points, int n_features, const int64_t *h_off, int B,
                      const double *d_planes, const int32_t *d_nparts, const int64_t *h_box_off, BatchGeometry &g,
-                     PaLayout &L, std::vector<int32_t> &tile_base, std::vector<int64_t> &tc_base, int &max_boxes)
+                     std::vector<int32_t> &tile_base, std::vector<int64_t> &tc_base, int &max_boxes)
 {
     if (lss_status rc = lss_batch_geometry(e, h_off, B, PA_TILE, g)) return rc;
     if (!h_box_off || h_box_off[0] != 0) return lss_fail(e, LSS_ERR_INVALID_ARG, "box_offsets must start at 0");
     if (n_features < 3) return lss_fail(e, LSS_ERR_INVALID_ARG, "n_features >= 3 required");
-    if (!pa_layout(h_off, h_box_off, B, L, tile_base, tc_base))
+    if (!pa_tiles(h_off, h_box_off, B, tile_base, tc_base))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "box_offsets must be non-decreasing, at most 256 boxes per cloud");
     max_boxes = 0;
     for (int b = 0; b < B; b++) max_boxes = std::max(max_boxes, (int)(h_box_off[b + 1] - h_box_off[b]));
@@ -452,20 +451,15 @@ lss_status pa_common(lss_engine *e, const float *d_points, int n_features, const
 }
 
 PartArgs pa_args(const float *d_points, int F, const int32_t *d_counts, const double *d_planes, const int32_t *d_nparts,
-                 int f64, char *ws, const PaLayout &L)
+                 int f64)
 {
     PartArgs a;
     a.pts = d_points;
     a.F = F;
-    a.off = (const int64_t *)(ws + L.off);
     a.cnt = d_counts;
     a.planes = d_planes;
     a.nparts = d_nparts;
-    a.box_off = (const int64_t *)(ws + L.box_off);
-    a.tile_base = (const int32_t *)(ws + L.tile_base);
-    a.tc_base = (const int64_t *)(ws + L.tc_base);
     a.f64 = f64 ? 1 : 0;
-    a.tile_cnt = (int *)(ws + L.tile_cnt);
     a.totals = nullptr;
     a.class_start = nullptr;
     a.members = nullptr;
@@ -479,11 +473,13 @@ extern "C" {
 int64_t lss_pa_partition_workspace_bytes(const int64_t *h_cloud_offsets, const int64_t *h_box_offsets, int n_clouds)
 {
     if (!h_cloud_offsets || !h_box_offsets || n_clouds < 0) return -1;
-    PaLayout L;
     std::vector<int32_t> tb;
     std::vector<int64_t> tc;
-    if (!pa_layout(h_cloud_offsets, h_box_offsets, n_clouds, L, tb, tc)) return -1;
-    return L.total;
+    if (!pa_tiles(h_cloud_offsets, h_box_offsets, n_clouds, tb, tc)) return -1;
+    WsCarve c;
+    PartArgs a;
+    pa_carve(c, a, n_clouds, tc[n_clouds]);
+    return c.used;
 }
 
 lss_status lss_pa_partition_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -493,26 +489,26 @@ lss_status lss_pa_partition_batch(lss_engine *e, const float *d_points, int n_fe
 {
     if (!e) return LSS_ERR_INVALID_ARG;
     BatchGeometry g;
-    PaLayout L;
     std::vector<int32_t> tile_base;
     std::vector<int64_t> tc_base;
     int max_boxes = 0;
     const int B = n_clouds;
-    if (lss_status rc = pa_common(e, d_points, n_features, h_cloud_offsets, B, d_planes, d_nparts, h_box_offsets, g, L,
+    if (lss_status rc = pa_common(e, d_points, n_features, h_cloud_offsets, B, d_planes, d_nparts, h_box_offsets, g,
                                   tile_base, tc_base, max_boxes))
         return rc;
     if (!d_workspace || (B > 0 && !d_class_totals)) return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    PartArgs a = pa_args(d_points, n_features, d_cloud_counts, d_planes, d_nparts, boxes_f64);
+    WsCarve c{(char *)d_workspace};
+    pa_carve(c, a, B, tc_base[B]);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    PartArgs a = pa_args(d_points, n_features, d_cloud_counts, d_planes, d_nparts, boxes_f64, ws, L);
     a.totals = d_class_totals;
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.box_off, h_box_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.tile_base, tile_base.data(), sizeof(int32_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.tc_base, tc_base.data(), sizeof(int64_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.box_off, h_box_offsets, sizeof(int64_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int32_t *)a.tile_base, tile_base.data(), sizeof(int32_t) * (B + 1), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.tc_base, tc_base.data(), sizeof(int64_t) * (B + 1), st));
     KernelTimer kt(e, LSS_K_PA, st);
     if (g.max_n > 0) {
         const size_t smem = pa_smem_bytes(max_boxes, false);
@@ -531,9 +527,15 @@ lss_status lss_pa_partition_batch(lss_engine *e, const float *d_points, int n_fe
 int64_t lss_pa_apply_workspace_bytes(const int64_t *h_cloud_offsets, const int64_t *h_box_offsets, int n_clouds,
                                      int64_t n_members, int64_t n_fps_rows, int64_t n_fps_out)
 {
-    const int64_t base = lss_pa_partition_workspace_bytes(h_cloud_offsets, h_box_offsets, n_clouds);
-    if (base < 0 || n_members < 0 || n_fps_rows < 0 || n_fps_out < 0) return -1;
-    return pa_apply_layout(base, n_members, n_fps_rows, n_fps_out).total;
+    if (!h_cloud_offsets || !h_box_offsets || n_clouds < 0 || n_members < 0 || n_fps_rows < 0 || n_fps_out < 0) return -1;
+    std::vector<int32_t> tb;
+    std::vector<int64_t> tc;
+    if (!pa_tiles(h_cloud_offsets, h_box_offsets, n_clouds, tb, tc)) return -1;
+    WsCarve c;
+    PartArgs a;
+    double *fps_rows, *fps_dist, *fps_out;
+    pa_apply_carve(c, a, fps_rows, fps_dist, fps_out, n_clouds, tc[n_clouds], n_members, n_fps_rows, n_fps_out);
+    return c.used;
 }
 
 lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -547,12 +549,11 @@ lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int n_featur
 {
     if (!e) return LSS_ERR_INVALID_ARG;
     BatchGeometry g;
-    PaLayout L;
     std::vector<int32_t> tile_base;
     std::vector<int64_t> tc_base;
     int max_boxes = 0;
     const int B = n_clouds;
-    if (lss_status rc = pa_common(e, d_points, n_features, h_cloud_offsets, B, d_planes, d_nparts, h_box_offsets, g, L,
+    if (lss_status rc = pa_common(e, d_points, n_features, h_cloud_offsets, B, d_planes, d_nparts, h_box_offsets, g,
                                   tile_base, tc_base, max_boxes))
         return rc;
     if (n_features != 4) return lss_fail(e, LSS_ERR_INVALID_ARG, "n_features == 4 required");
@@ -561,15 +562,15 @@ lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int n_featur
     if (!d_workspace || (B > 0 && !d_class_start) || (n_out > 0 && (!d_out || !d_segs)) ||
         (n_fps_jobs > 0 && (!d_fps_segs || !d_fps_jobs)))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
-    const PaApplyLayout A = pa_apply_layout(L.total, n_members, n_fps_rows, n_fps_out);
-    if (workspace_bytes < A.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    PartArgs a = pa_args(d_points, n_features, d_cloud_counts, d_planes, d_nparts, boxes_f64);
+    WsCarve c{(char *)d_workspace};
+    double *d_fps_rows, *d_fps_dist, *d_fps_out;
+    pa_apply_carve(c, a, d_fps_rows, d_fps_dist, d_fps_out, B, tc_base[B], n_members, n_fps_rows, n_fps_out);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    PartArgs a = pa_args(d_points, n_features, d_cloud_counts, d_planes, d_nparts, boxes_f64, ws, L);
     a.class_start = d_class_start;
-    a.members = (int32_t *)(ws + A.members);
     KernelTimer kt(e, LSS_K_PA, st);
     if (g.max_n > 0 && n_members > 0) {
         const size_t smem = pa_smem_bytes(max_boxes, true);
@@ -583,19 +584,18 @@ lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int n_featur
     m.members = a.members;
     m.class_start = d_class_start;
     m.steps = d_steps;
-    m.fps_rows = (const double *)(ws + A.fps_out);
+    m.fps_rows = d_fps_out;
     m.noise = d_noise;
     m.normals = d_normals;
     if (n_fps_jobs > 0 && n_fps_rows > 0) {
         m.segs = d_fps_segs;
         m.n_segs = n_fps_segs;
         m.n_dst = n_fps_rows;
-        m.dst64 = (double *)(ws + A.fps_rows);
+        m.dst64 = d_fps_rows;
         m.dst32 = nullptr;
         LSS_CUDA_CHECK(e, lss_launch(e, k_pa_emit, (unsigned)((n_fps_rows + 255) / 256), 256, 0, st, m));
         LSS_CUDA_CHECK(e, lss_launch(e, k_pa_fps, (unsigned)n_fps_jobs, 256, 0, st, d_fps_jobs,
-                                     (const double *)(ws + A.fps_rows), (double *)(ws + A.fps_dist),
-                                     (double *)(ws + A.fps_out)));
+                                     (const double *)d_fps_rows, d_fps_dist, d_fps_out));
     }
     if (n_out > 0) {
         m.segs = d_segs;

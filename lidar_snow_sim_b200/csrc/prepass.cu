@@ -712,29 +712,35 @@ __global__ void k_poly_solve(PreArgs a, double *poly_out /* [B*3] or null */, do
 
 }  // namespace
 
-struct PrepassLayout { int64_t cp, rec_cnt, win, stage, tile_cnt, tile_base, trial, partial, plane_in, ymins, ymins_in, total; int max_blocks; };
-
-static PrepassLayout prepass_layout(int64_t n_total, int n_clouds)
+// The workspace, region by region.  The staging region is reused for the histogram records (8 + 1 bytes per row).
+// plane_in / ymins_in: where a caller's planes [B * 4] and bin picks [B * HIST_NX] are uploaded.
+static void prepass_carve(WsCarve &c, PreArgs &a, double *&plane_in, int32_t *&ymins_in, int64_t n_total, int n_clouds)
 {
-    PrepassLayout L;
-    L.max_blocks = 64;
-    int64_t o = 0;
-    L.cp = o;       o = align_up(o + (int64_t)sizeof(CloudPre) * n_clouds, 256);
-    L.rec_cnt = o;  o = align_up(o + (int64_t)n_clouds * 4, 256);
-    L.win = o;      o = align_up(o + n_total * 3 * 4, 256);
-    L.stage = o;    o = align_up(o + n_total * 3 * 4, 256);    // then the histogram records: 8 + 1 B per row
-    L.tile_cnt = o; o = align_up(o + (n_total / 32 + n_clouds + 2) * 4, 256);
-    L.tile_base = o; o = align_up(o + (int64_t)(n_clouds + 1) * 4, 256);
-    L.trial = o;    o = align_up(o + (int64_t)n_clouds * RANSAC_T * 8 * 8, 256);
-    L.partial = o;  o = align_up(o + (int64_t)n_clouds * L.max_blocks * 16 * 8, 256);
-    L.plane_in = o; o = align_up(o + (int64_t)n_clouds * 4 * 8, 256);
-    L.ymins = o;    o = align_up(o + (int64_t)n_clouds * HIST_NX * 4, 256);
-    L.ymins_in = o; o = align_up(o + (int64_t)n_clouds * HIST_NX * 4, 256);
-    L.total = o;
-    return L;
+    a.max_blocks = 64;
+    a.cp = c.take<CloudPre>(n_clouds);
+    a.rec_cnt = c.take<int>(n_clouds);
+    a.win = c.take<float>(n_total * 3);
+    a.stage = c.take<float>(n_total * 3);
+    a.rec_norm = (double *)a.stage;
+    a.rec_bin = a.stage ? (unsigned char *)a.stage + n_total * 8 : nullptr;
+    a.tile_cnt = c.take<int>(n_total / 32 + n_clouds + 2);
+    a.tile_base = c.take<int32_t>(n_clouds + 1);
+    a.trial = c.take<double>((int64_t)n_clouds * RANSAC_T * 8);
+    a.partial = c.take<double>((int64_t)n_clouds * a.max_blocks * 16);
+    plane_in = c.take<double>((int64_t)n_clouds * 4);
+    a.ymins = c.take<int32_t>((int64_t)n_clouds * HIST_NX);
+    ymins_in = c.take<int32_t>((int64_t)n_clouds * HIST_NX);
 }
 
-int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds) { return prepass_layout(n_total, n_clouds).total; }
+int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds)
+{
+    WsCarve c;
+    PreArgs a;
+    double *plane_in;
+    int32_t *ymins_in;
+    prepass_carve(c, a, plane_in, ymins_in, n_total, n_clouds);
+    return c.used;
+}
 
 // dynamic shared memory of k_window_gather_mad: the prefix of the tile counts of the largest cloud
 static size_t gather_dyn_smem(int64_t max_n) { return sizeof(int) * ((size_t)(max_n + 31) / 32 + 2); }
@@ -785,11 +791,13 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     double *d_poly_out = io.d_poly_out, *d_plane_out = io.d_plane_out;
     const int B = n_clouds;
     const int64_t N = h_cloud_off[B];
-    const PrepassLayout L = prepass_layout(N, B);
-    if (lss_status rc = lss_prepass_check(e, h_cloud_off, B, h_plane_in != nullptr)) return rc;
-    if (ws_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "pre-pass workspace too small");
-    char *ws = (char *)d_ws;
     PreArgs a;
+    WsCarve c{(char *)d_ws};
+    double *d_plane;
+    int32_t *d_ymins_in;
+    prepass_carve(c, a, d_plane, d_ymins_in, N, B);
+    if (lss_status rc = lss_prepass_check(e, h_cloud_off, B, h_plane_in != nullptr)) return rc;
+    if (ws_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "pre-pass workspace too small");
     a.pts = d_pts;
     a.cloud_off = d_cloud_off;
     a.cloud_cnt = d_cloud_cnt;
@@ -801,37 +809,24 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     a.noise_floor = noise_floor;
     a.flat_earth = flat_earth;
     a.have_plane = h_plane_in != nullptr;
-    a.cp = (CloudPre *)(ws + L.cp);
-    a.win = (float *)(ws + L.win);
-    a.stage = (float *)(ws + L.stage);
-    a.tile_cnt = (int *)(ws + L.tile_cnt);
-    a.tile_base = (const int32_t *)(ws + L.tile_base);
-    a.rec_norm = (double *)(ws + L.stage);
-    a.rec_bin = (unsigned char *)(ws + L.stage + N * 8);
-    a.rec_cnt = (int *)(ws + L.rec_cnt);
-    a.trial = (double *)(ws + L.trial);
-    a.partial = (double *)(ws + L.partial);
-    a.max_blocks = L.max_blocks;
     a.status = e->d_status;
-    a.ymins = (int32_t *)(ws + L.ymins);
     a.ymins_in = nullptr;
     if (io.h_ymins_in) {
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.ymins_in, io.h_ymins_in, sizeof(int32_t) * HIST_NX * B, stream));
-        a.ymins_in = (const int32_t *)(ws + L.ymins_in);
+        LSS_CUDA_CHECK(e, lss_stage_upload(e, d_ymins_in, io.h_ymins_in, sizeof(int32_t) * HIST_NX * B, stream));
+        a.ymins_in = d_ymins_in;
     }
     if (cloudpre_out) *cloudpre_out = a.cp;
     const int64_t max_n = largest_cloud(h_cloud_off, B);
-    int nblk = (int)std::min<int64_t>(L.max_blocks, std::max<int64_t>(1, (max_n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
+    int nblk = (int)std::min<int64_t>(a.max_blocks, std::max<int64_t>(1, (max_n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
 
     {
         ZeroRegions z;
-        z.add(a.cp, (size_t)(L.rec_cnt - L.cp) + sizeof(int) * B);     // CloudPre records and record cursors
+        z.add(a.cp, (size_t)((char *)a.rec_cnt - (char *)a.cp) + sizeof(int) * B);   // CloudPre records and record cursors
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
     }
     {
         KernelTimer kt(e, LSS_K_PREPASS, stream);
         if (h_plane_in) {
-            double *d_plane = (double *)(ws + L.plane_in);
             LSS_CUDA_CHECK(e, lss_stage_upload(e, d_plane, h_plane_in, sizeof(double) * 4 * B, stream));
             LSS_CUDA_CHECK(e, lss_launch(e, k_set_plane, (B + 127) / 128, 128, 0, stream, a, d_plane));
         } else {

@@ -102,21 +102,18 @@ __global__ void __launch_bounds__(256) k_gather(const float *src, int F, const i
     for (int c = 0; c < F; c++) d[c] = s[c];
 }
 
-struct ProcLayout { int64_t off, seg, rows, J, P, R, vox, total; };
-
-ProcLayout proc_layout(int64_t n_total, int n_clouds, int n_features_out)
+// The workspace: cloud offsets, segment tiles, the encoded rows (the shuffle's input), the shuffle's draws J, permutation P
+// and reservations R; returns voxelize's own workspace of vox_bytes behind them
+void *proc_carve(WsCarve &c, EncArgs &ea, ShufArgs &sa, int64_t n_total, int n_clouds, int n_features_out,
+                 int64_t vox_bytes)
 {
-    ProcLayout L;
-    int64_t o = 0;
-    L.off = o;  o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.seg = o;  o += seg_ws_bytes(n_total, n_clouds, PTILE, 1);
-    L.rows = o; o = align_up(o + n_total * n_features_out * 4, 256);
-    L.J = o;    o = align_up(o + n_total * 4, 256);
-    L.P = o;    o = align_up(o + n_total * 4, 256);
-    L.R = o;    o = align_up(o + n_total * 8, 256);
-    L.vox = o;
-    L.total = o;
-    return L;
+    ea.cloud_off = sa.cloud_off = c.take<int64_t>(n_clouds + 1);
+    ea.seg = seg_take(c, n_total, n_clouds, PTILE, 1);
+    ea.out = c.take<float>(n_total * n_features_out);
+    sa.J = c.take<int32_t>(n_total);
+    sa.P = c.take<int32_t>(n_total);
+    sa.R = c.take<unsigned long long>(n_total);
+    return c.take<char>(vox_bytes);
 }
 
 // draws + swaps of every cloud of the batch into P (the geometry is on the device already)
@@ -147,10 +144,13 @@ int64_t lss_processor_workspace_bytes(int64_t n_total, int n_clouds, int n_featu
                                       int max_voxels)
 {
     if (n_total < 0 || n_clouds < 0 || n_features_out < 0 || max_points_per_voxel < 0 || max_voxels < 0) return -1;
-    const ProcLayout L = proc_layout(n_total, n_clouds, n_features_out);
-    if (max_voxels == 0) return L.total;
-    const int64_t v = lss_voxelize_workspace_bytes(n_total, n_clouds, max_points_per_voxel, max_voxels);
-    return v < 0 ? -1 : L.total + v;
+    const int64_t v = max_voxels == 0 ? 0 : lss_voxelize_workspace_bytes(n_total, n_clouds, max_points_per_voxel, max_voxels);
+    if (v < 0) return -1;
+    WsCarve c;
+    EncArgs ea;
+    ShufArgs sa;
+    proc_carve(c, ea, sa, n_total, n_clouds, n_features_out, v);
+    return c.used;
 }
 
 lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts,
@@ -163,15 +163,17 @@ lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_cloud_offset
     if (!h_mt_state || !d_mt_state_out || !d_workspace || (g.n > 0 && !d_out_perm))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "null argument");
     if (lss_status rc = check_state(e, h_mt_state)) return rc;
-    const ProcLayout L = proc_layout(g.n, n_clouds, 0);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    WsCarve c{(char *)d_workspace};
+    EncArgs ea;
+    ShufArgs sa;
+    proc_carve(c, ea, sa, g.n, n_clouds, 0, 0);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    int64_t *d_off = (int64_t *)(ws + L.off);
+    int64_t *d_off = (int64_t *)sa.cloud_off;
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), st));
-    return run_permutations(e, d_off, d_cloud_counts, n_clouds, g.max_n, h_mt_state, d_mt_state_out,
-                            (int32_t *)(ws + L.J), d_out_perm, (unsigned long long *)(ws + L.R), st);
+    return run_permutations(e, d_off, d_cloud_counts, n_clouds, g.max_n, h_mt_state, d_mt_state_out, sa.J, d_out_perm,
+                            sa.R, st);
 }
 
 lss_status lss_processor_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -216,19 +218,19 @@ lss_status lss_processor_batch(lss_engine *e, const float *d_points, int n_featu
             return lss_fail(e, LSS_ERR_INVALID_ARG, "max_points_per_voxel > 0, max_voxels > 0 required");
         for (int k = 0; k < 6; k++) vrange[k] = (float)h_point_cloud_range[k];
     }
-    const ProcLayout L = proc_layout(g.n, n_clouds, n_features_out);
     const int64_t vox_bytes = voxels ? lss_voxelize_workspace_bytes(g.n, n_clouds, max_points_per_voxel, max_voxels) : 0;
-    if (vox_bytes < 0 || workspace_bytes < L.total + vox_bytes) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    if (vox_bytes < 0) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    ShufArgs sa;
+    WsCarve c{(char *)d_workspace};
+    void *d_vox_ws = proc_carve(c, ea, sa, g.n, n_clouds, n_features_out, vox_bytes);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     const int B = n_clouds;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    int64_t *d_off = (int64_t *)(ws + L.off);
-    ea.cloud_off = d_off;
+    int64_t *d_off = (int64_t *)ea.cloud_off;
     ea.cloud_cnt = d_cloud_counts;
-    ea.seg = seg_tiles(ws + L.seg, B);
     ea.seg.total[0] = d_out_counts;
-    ea.out = shuffle ? (float *)(ws + L.rows) : d_out_points;
+    if (!shuffle) ea.out = d_out_points;
     if (B > 0) {
         LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)ea.seg.tile_base, st));
         const dim3 gt((unsigned)(g.max_n > 0 ? (g.max_n + PTILE - 1) / PTILE : 1), B);
@@ -237,21 +239,20 @@ lss_status lss_processor_batch(lss_engine *e, const float *d_points, int n_featu
         LSS_CUDA_CHECK(e, lss_launch(e, k_enc_write, gt, PTILE, 0, st, ea));
     }
     if (shuffle) {
-        int32_t *P = (int32_t *)(ws + L.P);
-        if (lss_status rc = run_permutations(e, d_off, d_out_counts, B, g.max_n, h_mt_state, d_mt_state_out,
-                                             (int32_t *)(ws + L.J), P, (unsigned long long *)(ws + L.R), st))
+        if (lss_status rc = run_permutations(e, d_off, d_out_counts, B, g.max_n, h_mt_state, d_mt_state_out, sa.J, sa.P,
+                                             sa.R, st))
             return rc;
         if (g.max_n > 0) {
             const dim3 g256((unsigned)((g.max_n + 255) / 256), B);
             LSS_CUDA_CHECK(e, lss_launch(e, k_gather, g256, 256, 0, st, (const float *)ea.out, n_features_out, d_off,
-                                         (const int32_t *)d_out_counts, (const int32_t *)P, d_out_points));
+                                         (const int32_t *)d_out_counts, (const int32_t *)sa.P, d_out_points));
         }
     }
     if (voxels) {
         const float vs[3] = {h_voxel_size[0], h_voxel_size[1], h_voxel_size[2]};
         return lss_voxelize_batch(e, d_out_points, n_features_out, h_cloud_offsets, d_out_counts, B, vrange, vs,
                                   max_points_per_voxel, max_voxels, 0, d_out_voxels, d_out_coords, d_out_num_points,
-                                  d_out_n_voxels, ws + L.total, workspace_bytes - L.total, stream);
+                                  d_out_n_voxels, d_vox_ws, vox_bytes, stream);
     }
     return LSS_OK;
 }

@@ -240,23 +240,17 @@ __global__ void __launch_bounds__(1024) k_count(SampArgs a)
     if (tid == 0) a.counts[p] = run_cnt;
 }
 
-struct SampLayout { int64_t cand, state, hkey, hhead, next, flags, total; int H; };
-
-SampLayout samp_layout(int n_planes, int64_t M)
+void samp_carve(WsCarve &c, SampArgs &a, int n_planes, int64_t M)
 {
-    SampLayout L;
     int H = 1;
     while (H < 2 * M) H <<= 1;
-    L.H = H;
-    int64_t o = 0;
-    L.cand = o;      o = align_up(o + (int64_t)n_planes * M * 3 * 8, 256);
-    L.state = o;     o = align_up(o + (int64_t)n_planes * M, 256);
-    L.hkey = o;      o = align_up(o + (int64_t)n_planes * H * 8, 256);
-    L.hhead = o;     o = align_up(o + (int64_t)n_planes * H * 4, 256);
-    L.next = o;      o = align_up(o + (int64_t)n_planes * M * 4, 256);
-    L.flags = o;     o = align_up(o + (int64_t)n_planes * 4, 256);
-    L.total = o;
-    return L;
+    a.H = H;
+    a.cand = c.take<double>((int64_t)n_planes * M * 3);
+    a.state = c.take<unsigned char>((int64_t)n_planes * M);
+    a.hkey = c.take<unsigned long long>((int64_t)n_planes * H);
+    a.hhead = c.take<int>((int64_t)n_planes * H);
+    a.next = c.take<int>((int64_t)n_planes * M);
+    a.flags = c.take<int>(n_planes);
 }
 
 }  // namespace
@@ -266,7 +260,10 @@ extern "C" {
 int64_t lss_sample_particles_workspace_bytes(int n_planes, int64_t n_candidates)
 {
     if (n_planes <= 0 || n_candidates <= 0) return -1;
-    return samp_layout(n_planes, n_candidates).total;
+    WsCarve c;
+    SampArgs a;
+    samp_carve(c, a, n_planes, n_candidates);
+    return c.used;
 }
 
 lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ratio, double precipitation_rate, double R_0,
@@ -282,14 +279,14 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
     if (distribution == 0) rate = 25.5 * pow(precipitation_rate, -0.48);        // sampling.py:81-87
     else if (distribution == 1) rate = 22.9 * pow(precipitation_rate, -0.45);   // sampling.py:72-78
     else return lss_fail(e, LSS_ERR_INVALID_ARG, "Distribution model unknown.");
-    const SampLayout L = samp_layout(n_planes, n_candidates);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "sampler workspace too small");
+    SampArgs a;
+    WsCarve c{(char *)d_workspace};
+    samp_carve(c, a, n_planes, n_candidates);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "sampler workspace too small");
     int dev_prev = -1;
     cudaGetDevice(&dev_prev);
     if (dev_prev != e->device) cudaSetDevice(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
-    SampArgs a;
     a.n_planes = n_planes;
     a.M = (int)n_candidates;
     a.R0 = R_0;
@@ -297,20 +294,13 @@ lss_status lss_sample_particles(lss_engine *e, int n_planes, double occupancy_ra
     a.scale_mm = (1 / rate) * 10;                                                 // sampling.py:115,154
     a.target_area = occupancy_ratio * 3.141592653589793 * (R_0 * R_0);           // sampling.py:124
     a.seed = seed;
-    a.cand = (double *)(ws + L.cand);
-    a.state = (unsigned char *)(ws + L.state);
-    a.hkey = (unsigned long long *)(ws + L.hkey);
-    a.hhead = (int *)(ws + L.hhead);
-    a.next = (int *)(ws + L.next);
-    a.H = L.H;
     a.out = d_xyr_out;
     a.cap = capacity_per_plane;
     a.counts = d_counts;
-    a.flags = (int *)(ws + L.flags);
     lss_status rc = LSS_OK;
     do {
-        if (cudaMemsetAsync(a.hkey, 0xff, (size_t)n_planes * L.H * 8, st) != cudaSuccess ||
-            cudaMemsetAsync(a.hhead, 0xff, (size_t)n_planes * L.H * 4, st) != cudaSuccess ||
+        if (cudaMemsetAsync(a.hkey, 0xff, (size_t)n_planes * a.H * 8, st) != cudaSuccess ||
+            cudaMemsetAsync(a.hhead, 0xff, (size_t)n_planes * a.H * 4, st) != cudaSuccess ||
             cudaMemsetAsync(a.flags, 0, (size_t)n_planes * 4, st) != cudaSuccess) {
             rc = lss_fail(e, LSS_ERR_CUDA, "sampler memset failed");
             break;

@@ -19,18 +19,14 @@ struct SegTiles {
     int32_t *total[SEG_MAX_K];     // per class: [B] rows of the class in each cloud, written by k_seg_scan unless null
 };
 
-// Workspace of a SegTiles: tile bases [B + 1], then the tile counters for at most n_total / tile + B + 1 tiles
+// One workspace region of a SegTiles: tile bases [B + 1], then the tile counters for at most n_total / tile + B + 1 tiles
 // (>= the sum over clouds of ceil(n_b / tile)).  The totals live where each feature wants them.
-inline int64_t seg_ws_bytes(int64_t n_total, int n_clouds, int tile, int K)
+inline SegTiles seg_take(WsCarve &c, int64_t n_total, int n_clouds, int tile, int K)
 {
-    return align_up((int64_t)(n_clouds + 1) * 4 + (n_total / tile + n_clouds + 1) * K * 4, 256);
-}
-
-inline SegTiles seg_tiles(void *ws, int n_clouds)
-{
+    int32_t *p = c.take<int32_t>((int64_t)(n_clouds + 1) + (n_total / tile + n_clouds + 1) * K);
     SegTiles s{};
-    s.tile_base = (const int32_t *)ws;
-    s.tile = (int *)ws + (n_clouds + 1);
+    s.tile_base = p;
+    s.tile = p ? p + (n_clouds + 1) : nullptr;
     return s;
 }
 

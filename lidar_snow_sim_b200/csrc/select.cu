@@ -246,24 +246,19 @@ cudaError_t sl_sort_bytes(int64_t n, int n_clouds, size_t *bytes)
                                            (int)n, 0, key_end_bit(n_clouds));
 }
 
-struct SlLayout { int64_t off_in, off_o, seg, n_master, keys, rows, skeys, srows, code, sort, total; };
-
-SlLayout sl_layout(int64_t n_out, int n_clouds, size_t sort_tmp)
+// The workspace, region by region; returns the radix sort's scratch.  off_l holds both input slots' offsets (off_s after).
+void *sl_carve(WsCarve &c, SlArgs &a, int64_t n_out, int n_clouds, size_t sort_tmp)
 {
-    SlLayout L;
-    int64_t o = 0;
-    L.off_in = o;    o = align_up(o + (int64_t)(n_clouds + 1) * 16, 256);
-    L.off_o = o;     o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.seg = o;       o += seg_ws_bytes(n_out, n_clouds, STILE, 2);
-    L.n_master = o;  o = align_up(o + (int64_t)n_clouds * 4, 256);
-    L.keys = o;      o = align_up(o + n_out * 8, 256);
-    L.rows = o;      o = align_up(o + n_out * 4, 256);
-    L.skeys = o;     o = align_up(o + n_out * 8, 256);
-    L.srows = o;     o = align_up(o + n_out * 4, 256);
-    L.code = o;      o = align_up(o + n_out, 256);
-    L.sort = o;      o = align_up(o + (int64_t)sort_tmp, 256);
-    L.total = o;
-    return L;
+    a.off_l = c.take<int64_t>((int64_t)(n_clouds + 1) * 2);
+    a.off_o = c.take<int64_t>(n_clouds + 1);
+    a.seg = seg_take(c, n_out, n_clouds, STILE, 2);
+    a.n_master = c.take<int32_t>(n_clouds);
+    a.keys = c.take<unsigned long long>(n_out);
+    a.rows = c.take<int32_t>(n_out);
+    a.skeys = c.take<unsigned long long>(n_out);
+    a.srows = c.take<int32_t>(n_out);
+    a.code = c.take<uint8_t>(n_out);
+    return c.take<char>((int64_t)sort_tmp);
 }
 
 // output slots: max of the two input slots, cloud by cloud (both offset arrays already checked)
@@ -275,18 +270,12 @@ std::vector<int64_t> sl_out_offsets(const int64_t *off_l, const int64_t *off_s, 
     return o;
 }
 
-struct FovLayout { int64_t off, seg, shape, code, total; };
-
-FovLayout fov_layout(int64_t n, int n_clouds)
+void fov_carve(WsCarve &c, FovArgs &a, int64_t n, int n_clouds)
 {
-    FovLayout L;
-    int64_t o = 0;
-    L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.seg = o;       o += seg_ws_bytes(n, n_clouds, STILE, 2);
-    L.shape = o;     o = align_up(o + (int64_t)n_clouds * 8, 256);
-    L.code = o;      o = align_up(o + n, 256);
-    L.total = o;
-    return L;
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.seg = seg_take(c, n, n_clouds, STILE, 2);
+    a.shape = c.take<int2>(n_clouds);
+    a.code = c.take<uint8_t>(n);
 }
 
 bool overlaps(const void *a, int64_t a_bytes, const void *b, int64_t b_bytes)
@@ -308,7 +297,10 @@ int64_t lss_strongest_last_batch_workspace_bytes(const int64_t *h_last_offsets, 
     if (n_out >= (1LL << 31)) return -1;
     size_t tmp = 0;
     if (sl_sort_bytes(n_out, n_clouds, &tmp) != cudaSuccess) return -1;
-    return sl_layout(n_out, n_clouds, tmp).total;
+    WsCarve c;
+    SlArgs a;
+    sl_carve(c, a, n_out, n_clouds, tmp);
+    return c.used;
 }
 
 lss_status lss_strongest_last_batch(lss_engine *e, const float *d_last, const int64_t *h_last_offsets,
@@ -339,50 +331,41 @@ lss_status lss_strongest_last_batch(lss_engine *e, const float *d_last, const in
     cudaStream_t st = (cudaStream_t)stream;
     size_t sort_tmp = 0;
     LSS_CUDA_CHECK(e, sl_sort_bytes(N, B, &sort_tmp));
-    const SlLayout L = sl_layout(N, B, sort_tmp);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    SlArgs a;
+    WsCarve c{(char *)d_workspace};
+    void *sort_ws = sl_carve(c, a, N, B, sort_tmp);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
 
-    char *ws = (char *)d_workspace;
     std::vector<int64_t> off_in((size_t)2 * (B + 1));
     std::copy(h_last_offsets, h_last_offsets + B + 1, off_in.begin());
     std::copy(h_strongest_offsets, h_strongest_offsets + B + 1, off_in.begin() + B + 1);
-    SlArgs a;
     a.last = d_last;
     a.strongest = d_strongest;
     a.F = n_features;
     a.n_clouds = B;
-    a.off_l = (const int64_t *)(ws + L.off_in);
     a.off_s = a.off_l + (B + 1);
     a.cnt_l = d_last_counts;
     a.cnt_s = d_strongest_counts;
-    a.off_o = (const int64_t *)(ws + L.off_o);
     a.min_dist = (float)min_dist;                              // NumPy 2 compares the float32 norms in float32
-    a.n_master = (int32_t *)(ws + L.n_master);
     a.is_strongest = d_out_master_is_strongest;
     a.out_counts = d_out_counts;
-    a.keys = (unsigned long long *)(ws + L.keys);
-    a.rows = (int32_t *)(ws + L.rows);
-    a.skeys = (const unsigned long long *)(ws + L.skeys);
-    a.srows = (const int32_t *)(ws + L.srows);
     a.n_sorted = (int)N;
-    a.code = (uint8_t *)(ws + L.code);
     a.mask = d_out_mask;
-    a.seg = seg_tiles(ws + L.seg, B);
     a.seg.total[0] = d_out_counts;
     a.seg.total[1] = nullptr;
     a.out = d_out_points;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, off_o.data(), B, go.tile_base, (int64_t *)(ws + L.off_o),
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, off_o.data(), B, go.tile_base, (int64_t *)a.off_o,
                                          (int32_t *)a.seg.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.off_in, off_in.data(), sizeof(int64_t) * off_in.size(), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.off_l, off_in.data(), sizeof(int64_t) * off_in.size(), st));
     KernelTimer kt(e, LSS_K_SELECT, st);
     const dim3 grow((unsigned)std::max<int64_t>((go.max_n + SBLOCK - 1) / SBLOCK, 1), B);
     LSS_CUDA_CHECK(e, lss_launch(e, k_sl_key, grow, SBLOCK, 0, st, a));
     if (go.max_n > 0) {
         const dim3 gt((unsigned)((go.max_n + STILE - 1) / STILE), B);
         size_t tmp = sort_tmp;
-        LSS_CUDA_CHECK(e, cub::DeviceRadixSort::SortPairs(ws + L.sort, tmp, (const unsigned long long *)a.keys,
+        LSS_CUDA_CHECK(e, cub::DeviceRadixSort::SortPairs(sort_ws, tmp, (const unsigned long long *)a.keys,
                                                           (unsigned long long *)a.skeys, (const int32_t *)a.rows,
                                                           (int32_t *)a.srows, (int)N, 0, key_end_bit(B), st));
         e->launches++;                                         // the sort's kernels count as one launch
@@ -398,7 +381,10 @@ lss_status lss_strongest_last_batch(lss_engine *e, const float *d_last, const in
 int64_t lss_camera_fov_batch_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return fov_layout(n_total, n_clouds).total;
+    WsCarve c;
+    FovArgs a;
+    fov_carve(c, a, n_total, n_clouds);
+    return c.used;
 }
 
 lss_status lss_camera_fov_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -418,34 +404,30 @@ lss_status lss_camera_fov_batch(lss_engine *e, const float *d_points, int n_feat
     if (overlaps(d_out_points, row_bytes, d_points, row_bytes))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "d_out_points must not alias d_points");
     if (!e->has_camera) return lss_fail(e, LSS_ERR_NO_SENSOR, "camera calibration not set");
-    const FovLayout L = fov_layout(N, B);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    FovArgs a;
+    WsCarve c{(char *)d_workspace};
+    fov_carve(c, a, N, B);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if (B == 0) return LSS_OK;
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    char *ws = (char *)d_workspace;
     std::vector<int32_t> shape((size_t)2 * B);
     for (int b = 0; b < B; b++) {
         shape[2 * b] = h_img_shape ? h_img_shape[2 * b] : e->camera.img_h;
         shape[2 * b + 1] = h_img_shape ? h_img_shape[2 * b + 1] : e->camera.img_w;
     }
-    FovArgs a;
     a.pts = d_points;
     a.F = n_features;
-    a.cloud_off = (const int64_t *)(ws + L.off);
     a.cloud_cnt = d_cloud_counts;
     a.camera = e->d_camera;
-    a.shape = (const int2 *)(ws + L.shape);
-    a.code = (uint8_t *)(ws + L.code);
     a.mask = d_out_mask;
-    a.seg = seg_tiles(ws + L.seg, B);
     a.seg.total[0] = d_out_counts;
     a.seg.total[1] = nullptr;
     a.out = d_out_points;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)(ws + L.off),
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
                                          (int32_t *)a.seg.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.shape, shape.data(), sizeof(int32_t) * shape.size(), st));
+    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int2 *)a.shape, shape.data(), sizeof(int32_t) * shape.size(), st));
     KernelTimer kt(e, LSS_K_SELECT, st);
     if (g.max_n > 0) {
         const dim3 gt((unsigned)((g.max_n + STILE - 1) / STILE), B);

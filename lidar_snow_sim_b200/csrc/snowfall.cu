@@ -330,60 +330,55 @@ __global__ void __launch_bounds__(TILE) k_scatter(const float *__restrict__ aug,
     }
 }
 
-struct WsLayout {
-    int64_t aug, keep_d, keep_i, keep_tag, code_keep, code_all, nocc, hist_keep, hist_all, hist_rows, cloud_off, tile_base,
-        order, thresh, counters, counters_bytes, list, chunks_per_class, chunk_tab, sched, sched_tiles, prepass, prepass_bytes, total;
-};
-
 int64_t hit_cap(int64_t n_total) { return std::min<int64_t>(n_total * HIT_SLOTS_PER_BEAM + 4096, 0x7fffffff); }
 
-WsLayout ws_layout(int64_t n_total, int n_clouds)
-{
-    WsLayout w;
-    w.hist_rows = n_total / TILE + (int64_t)n_clouds + 1;          // >= sum over clouds of ceil(n_b / TILE)
-    w.sched_tiles = n_total / 32 + (int64_t)n_clouds + 1;          // >= sum over clouds of ceil(n_b / 32)
-    int64_t o = 0;
-    w.aug = o;        o = align_up(o + n_total * 5 * 4, 256);
-    w.keep_d = o;     o = align_up(o + n_total * 4, 256);           // keep record: range | intensity | tag
-    w.keep_i = o;     o = align_up(o + n_total * 4, 256);
-    w.keep_tag = o;   o = align_up(o + n_total, 256);
-    w.code_keep = o;  o = align_up(o + n_total, 256);
-    w.code_all = o;   o = align_up(o + n_total, 256);
-    w.nocc = o;       o = align_up(o + n_total * 4, 256);
-    w.hist_keep = o;  o = align_up(o + w.hist_rows * NBINS * 4, 256);
-    w.hist_all = o;   o = align_up(o + w.hist_rows * NBINS * 4, 256);
-    w.cloud_off = o;  o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    w.tile_base = o;  o = align_up(o + (int64_t)(n_clouds + 1) * 2 * 4, 256);   // scatter tiles, then warp tiles
-    w.order = o;      o = align_up(o + (int64_t)n_clouds * LSS_N_CHANNELS * 4, 256);
-    w.thresh = o;     o = align_up(o + (int64_t)n_clouds * 3 * 8, 256);
-    // counters: int[B*2] | unsigned att_cnt[B*64] | unsigned long long att_sum[B]
-    w.counters_bytes = align_up((int64_t)n_clouds * 2 * 4, 8) + (int64_t)n_clouds * LSS_N_CHANNELS * 4 + (int64_t)n_clouds * 8;
-    w.counters = o;   o = align_up(o + w.counters_bytes, 256);
-    // list header | solve list chunks (every beam may have occluders; each class leaves at most one chunk partly filled)
-    //   | hit records a1 | a2 | range (float64 each, HIT_SLOTS_PER_BEAM slots per beam of the batch + 4096)
-    w.chunks_per_class = (n_total + LIST_CHUNK - 1) / LIST_CHUNK;
-    w.list = o;       o = align_up(o + LIST_HDR_BYTES +
-                                   (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK * (int64_t)sizeof(SolveItem) +
-                                   hit_cap(n_total) * 3 * 8, 256);
-    // chunk table of the solve list: LIST_CLASSES x chunks_per_class ids
-    w.chunk_tab = o;  o = align_up(o + (int64_t)LIST_CLASSES * w.chunks_per_class * 4, 256);
-    // scan schedule: bin counts and cursors | warp-tile entries, unsorted + sorted
-    w.sched = o;      o = align_up(o + (int64_t)SCHED_BINS * 2 * 4 + 2 * w.sched_tiles * 8, 256);
-    w.prepass_bytes = lss_prepass_ws_bytes(n_total, n_clouds);
-    w.prepass = o;    o = align_up(o + w.prepass_bytes, 256);
-    w.total = o;
-    return w;
-}
+int64_t sched_tiles(int64_t n_total, int n_clouds) { return n_total / 32 + (int64_t)n_clouds + 1; }   // >= sum of ceil(n_b / 32)
+
+// counters region: int[B*2] | unsigned att_cnt[B*64] | unsigned long long att_sum[B]
+int64_t att_cnt_off(int n_clouds) { return align_up((int64_t)n_clouds * 2 * 4, 8); }
+int64_t counters_bytes(int n_clouds) { return att_cnt_off(n_clouds) + (int64_t)n_clouds * (LSS_N_CHANNELS * 4 + 8); }
 
 }  // namespace
+
+int *lss_snowfall_carve(WsCarve &c, DevArgs &a, void *&prepass, int64_t n_total, int n_clouds)
+{
+    const int64_t hist_rows = n_total / TILE + (int64_t)n_clouds + 1;          // >= sum over clouds of ceil(n_b / TILE)
+    a.aug = c.take<float>(n_total * 5);
+    a.keep_d = c.take<float>(n_total);
+    a.keep_i = c.take<float>(n_total);
+    a.keep_tag = c.take<uint8_t>(n_total);
+    a.code_keep = c.take<uint8_t>(n_total);
+    a.code_all = c.take<uint8_t>(n_total);
+    a.nocc = c.take<int32_t>(n_total);
+    a.hist_keep = c.take<unsigned>(hist_rows * NBINS);
+    a.hist_all = c.take<unsigned>(hist_rows * NBINS);
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.tile_base = c.take<int32_t>((int64_t)(n_clouds + 1) * 2);               // scatter tiles, then warp tiles
+    a.order = c.take<int32_t>((int64_t)n_clouds * LSS_N_CHANNELS);
+    a.thresh = c.take<double>((int64_t)n_clouds * 3);
+    a.counters = (int *)c.take<char>(counters_bytes(n_clouds));
+    // list header | solve list chunks (every beam may have occluders; each class leaves at most one chunk partly filled)
+    //   | hit records a1 | a2 | range (float64 each, HIT_SLOTS_PER_BEAM slots per beam of the batch + 4096)
+    a.chunks_per_class = (int)((n_total + LIST_CHUNK - 1) / LIST_CHUNK);
+    a.hit_cap = (int)hit_cap(n_total);
+    a.hdr = (int *)c.take<char>(LIST_HDR_BYTES + (a.chunks_per_class + LIST_CLASSES) * LIST_CHUNK * (int64_t)sizeof(SolveItem) +
+                                (int64_t)a.hit_cap * 3 * 8);
+    a.chunk_tab = c.take<int>((int64_t)LIST_CLASSES * a.chunks_per_class);   // LIST_CLASSES x chunks_per_class chunk ids
+    // scan schedule: bin counts and cursors | warp-tile entries, unsorted + sorted
+    int *sched = (int *)c.take<char>((int64_t)SCHED_BINS * 2 * 4 + 2 * sched_tiles(n_total, n_clouds) * 8);
+    prepass = c.take<char>(lss_prepass_ws_bytes(n_total, n_clouds));
+    return sched;
+}
 
 int64_t lss_snowfall_ws_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return ws_layout(n_total, n_clouds).total;
+    WsCarve c;
+    DevArgs a;
+    void *prepass;
+    lss_snowfall_carve(c, a, prepass, n_total, n_clouds);
+    return c.used;
 }
-
-int64_t lss_snowfall_ws_cloud_off(int64_t n_total, int n_clouds) { return ws_layout(n_total, n_clouds).cloud_off; }
 
 lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t stream)
 {
@@ -396,8 +391,11 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     for (int k = 0; k < B * LSS_N_CHANNELS; k++)
         if (s.h_order[k] < 0 || s.h_order[k] >= s.ts->n_planes)
             return lss_fail(e, LSS_ERR_NO_TABLE, "order[] names a plane that is not in the table set");
-    const WsLayout w = ws_layout(N, B);
-    if (s.workspace_bytes < w.total || !s.d_workspace) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    DevArgs a;
+    WsCarve c{(char *)s.d_workspace};
+    void *d_prepass_ws;
+    int *d_sched_hist = lss_snowfall_carve(c, a, d_prepass_ws, N, B);
+    if (s.workspace_bytes < c.used || !s.d_workspace) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     if ((s.flags & LSS_FLAG_THRESHOLD_FILTER) && !s.h_thresh_poly && !(s.flags & LSS_FLAG_DEVICE_PREPASS))
         return lss_fail(e, LSS_ERR_INVALID_ARG, "threshold filter needs h_thresh_poly or LSS_FLAG_DEVICE_PREPASS");
     if ((s.flags & LSS_FLAG_CAMERA_FOV) && !e->has_camera)
@@ -414,20 +412,14 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     if (device_prepass)
         if (lss_status rc = lss_prepass_check(e, s.h_cloud_offsets, B, s.h_plane_in != nullptr)) return rc;
 
-    char *ws = (char *)s.d_workspace;
-    float *d_aug = (float *)(ws + w.aug);
-    uint8_t *d_code_keep = (uint8_t *)(ws + w.code_keep);
     const bool want_all = s.d_out_full != nullptr;
-    uint8_t *d_code_all = want_all ? (uint8_t *)(ws + w.code_all) : nullptr;
-    int32_t *d_nocc_tmp = s.d_out_nocc ? (int32_t *)(ws + w.nocc) : nullptr;
-    unsigned *d_hist_keep = (unsigned *)(ws + w.hist_keep);
-    unsigned *d_hist_all = want_all ? (unsigned *)(ws + w.hist_all) : nullptr;
-    int64_t *d_off = (int64_t *)(ws + w.cloud_off);
-    int32_t *d_tile_base = (int32_t *)(ws + w.tile_base);
-    int32_t *d_order = (int32_t *)(ws + w.order);
-    double *d_thresh = (double *)(ws + w.thresh);
-    int *d_counters = (int *)(ws + w.counters);
-    unsigned *d_att_cnt = (unsigned *)(ws + w.counters + align_up((int64_t)B * 2 * 4, 8));
+    if (!want_all) a.code_all = nullptr, a.hist_all = nullptr;
+    if (!s.d_out_nocc) a.nocc = nullptr;
+    int64_t *d_off = (int64_t *)a.cloud_off;
+    int32_t *d_tile_base = (int32_t *)a.tile_base;
+    int32_t *d_order = (int32_t *)a.order;
+    double *d_thresh = (double *)a.thresh;
+    unsigned *d_att_cnt = (unsigned *)((char *)a.counters + att_cnt_off(B));
     unsigned long long *d_att_sum = (unsigned long long *)((char *)d_att_cnt + (int64_t)B * LSS_N_CHANNELS * 4);
 
     // d_tile_base: [0, B] first scatter tile of each cloud, [B + 1, 2 B + 1] first warp tile of each cloud
@@ -436,23 +428,21 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     LSS_CUDA_CHECK(e, lss_stage_upload(e, d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS, stream));
     if (s.h_thresh_poly)
         LSS_CUDA_CHECK(e, lss_stage_upload(e, d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B, stream));
-    int *d_list_hdr = (int *)(ws + w.list);                                 // (LIST_HDR_BYTES)
     {
         ZeroRegions z;
-        z.add(d_counters, w.counters_bytes);
+        z.add(a.counters, counters_bytes(B));
         z.add(s.d_out_stats, sizeof(double) * 4 * B);
         if (N == 0 || B == 0) {
             z.add(s.d_out_counts, sizeof(int32_t) * B);
             LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
             return LSS_OK;
         }
-        z.add(d_list_hdr, LIST_HDR_BYTES);                 // (the tile histograms are written whole by k_keep)
-        z.add(ws + w.chunk_tab, (size_t)LIST_CLASSES * w.chunks_per_class * 4);
-        z.add(ws + w.sched, (size_t)SCHED_BINS * 2 * 4);
+        z.add(a.hdr, LIST_HDR_BYTES);                     // (the tile histograms are written whole by k_keep)
+        z.add(a.chunk_tab, (size_t)LIST_CLASSES * a.chunks_per_class * 4);
+        z.add(d_sched_hist, (size_t)SCHED_BINS * 2 * 4);
         LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
     }
 
-    DevArgs a;
     a.rec = s.ts->d_rec;
     a.tan = s.ts->d_tan;
     a.plane_off = s.ts->d_plane_off;
@@ -465,10 +455,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.inv_w = s.ts->n_buckets / LSS_TWO_PI;
     a.pts = s.d_points;
     a.theta = s.d_theta;
-    a.cloud_off = d_off;
     a.cloud_cnt = s.d_cloud_counts;
-    a.order = d_order;
-    a.thresh = d_thresh;
     a.sensor = e->d_sensor;
     a.camera = e->d_camera;
     a.R = e->d_R;
@@ -476,24 +463,12 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     a.half_div = (s.beam_divergence_deg / 2) * (LSS_PI / 180.0);
     a.div_rad = div_rad;
     a.flags = s.flags;
-    a.aug = d_aug;
-    a.keep_d = (float *)(ws + w.keep_d);
-    a.keep_i = (float *)(ws + w.keep_i);
-    a.keep_tag = (uint8_t *)(ws + w.keep_tag);
-    a.code_keep = d_code_keep;
-    a.code_all = d_code_all;
-    a.nocc = d_nocc_tmp;
-    a.hist_keep = d_hist_keep;
-    a.hist_all = d_hist_all;
-    a.tile_base = d_tile_base;
     a.stats = s.d_out_stats;
-    a.counters = d_counters;
     a.att_cnt = d_att_cnt;
     a.att_sum = d_att_sum;
     a.status = e->d_status;
-    SolveItem *d_solve_list = (SolveItem *)(ws + w.list + LIST_HDR_BYTES);   // (chunks_per_class + LIST_CLASSES) chunks
-    a.hit_cap = (int)hit_cap(N);
-    a.hit_a1 = (double *)(d_solve_list + (w.chunks_per_class + LIST_CLASSES) * LIST_CHUNK);
+    SolveItem *d_solve_list = (SolveItem *)((char *)a.hdr + LIST_HDR_BYTES);   // (chunks_per_class + LIST_CLASSES) chunks
+    a.hit_a1 = (double *)(d_solve_list + (a.chunks_per_class + LIST_CLASSES) * LIST_CHUNK);
     a.hit_a2 = a.hit_a1 + a.hit_cap;
     a.hit_rho = a.hit_a2 + a.hit_cap;
     // Device pre-pass: plane + laser parameters + threshold polynomial (simulation.py:449-467), on the cloud as given.
@@ -513,7 +488,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
         io.h_ymins_in = s.h_ymins_in;
         io.d_poly_out = d_thresh;
         lss_status ps = lss_prepass_run(e, s.d_points, d_off, s.d_cloud_counts, s.h_cloud_offsets, B, 0.5, s.noise_floor, 0, 0, 1,
-                                io, ws + w.prepass, w.prepass_bytes, nullptr, side);
+                                io, d_prepass_ws, lss_prepass_ws_bytes(N, B), nullptr, side);
         const cudaError_t je = cudaEventRecord(ev_join, side);
         if (ps != LSS_OK || je != cudaSuccess) {
             cudaStreamWaitEvent(stream, ev_join, 0);                // never leave the side stream dangling
@@ -524,14 +499,10 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     {
         KernelTimer kt(e, LSS_K_SNOWFALL, stream);
         // 1. scan: all beams; the ones without occluders are finished, the others go to the solve list with their hits
-        a.hdr = d_list_hdr;
         a.items = d_solve_list;
-        a.chunk_tab = (int *)(ws + w.chunk_tab);
-        a.chunks_per_class = (int)w.chunks_per_class;
         {   // plane-major order of the warp tiles
-            int *d_sched_hist = (int *)(ws + w.sched);
             unsigned long long *d_ent = (unsigned long long *)(d_sched_hist + 2 * SCHED_BINS);
-            unsigned long long *d_sched = d_ent + w.sched_tiles;
+            unsigned long long *d_sched = d_ent + sched_tiles(N, B);
             const int max_wtiles = (int)((max_n + 31) / 32);
             ce = lss_launch(e, k_sched_key, dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B),
                             SCHED_KEY_TPB, 0, stream, s.d_points, d_off, s.d_cloud_counts, d_order, d_tile_base + B + 1,
@@ -549,7 +520,7 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
         // 2. solve: the listed beams, class by class, one warp per tile of 32 (persistent grid)
         if (ce == cudaSuccess) {
             KernelTimer ks(e, LSS_K_SOLVE, stream);
-            ce = lss_launch_solve(e, a, d_list_hdr + 1, stream);
+            ce = lss_launch_solve(e, a, a.hdr + 1, stream);
         }
     }
     if (ev_join) LSS_CUDA_CHECK(e, cudaStreamWaitEvent(stream, ev_join, 0));
@@ -560,20 +531,20 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     }
     {
         KernelTimer kt(e, LSS_K_SORT, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, d_hist_keep, d_tile_base, s.d_out_counts,
-                                     s.d_out_stats, d_counters, d_att_cnt, d_att_sum, e->d_sensor));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, a.hist_keep, d_tile_base, s.d_out_counts,
+                                     s.d_out_stats, a.counters, d_att_cnt, d_att_sum, e->d_sensor));
     }
     {
         KernelTimer kt(e, LSS_K_COMPACT, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, d_aug, d_code_keep, d_hist_keep, d_off,
+        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, a.aug, a.code_keep, a.hist_keep, d_off,
                                      s.d_cloud_counts, d_tile_base, s.d_out_points, nullptr, nullptr, nullptr));
     }
     if (want_all) {     // un-filtered, channel-sorted debug views (tests): full rows, original index, occluder counts
         KernelTimer kt(e, LSS_K_COMPACT, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, d_hist_all, d_tile_base, nullptr, nullptr, nullptr,
+        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, a.hist_all, d_tile_base, nullptr, nullptr, nullptr,
                                      nullptr, nullptr, nullptr));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, d_aug, d_code_all, d_hist_all, d_off,
-                                     s.d_cloud_counts, d_tile_base, s.d_out_full, d_nocc_tmp, s.d_out_nocc, s.d_out_perm));
+        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, a.aug, a.code_all, a.hist_all, d_off,
+                                     s.d_cloud_counts, d_tile_base, s.d_out_full, a.nocc, s.d_out_nocc, s.d_out_perm));
     }
     return LSS_OK;
 }

@@ -177,24 +177,20 @@ __global__ void __launch_bounds__(256) k_vox_write(VoxArgs a)
     }
 }
 
-struct VoxLayout { int64_t off, key, first, count, vid, slot_of, seg, seg_total, top, total, n_slots; };
+int64_t vox_slots(int64_t n_total, int n_clouds) { return 2 * n_total + n_clouds + 1; }
 
-VoxLayout vox_layout(int64_t n_total, int n_clouds, int max_points, int max_voxels)
+void vox_carve(WsCarve &c, VoxArgs &a, int64_t n_total, int n_clouds, int max_points, int max_voxels)
 {
-    VoxLayout L;
-    L.n_slots = 2 * n_total + n_clouds + 1;
-    int64_t o = 0;
-    L.off = o;       o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.key = o;       o = align_up(o + L.n_slots * 8, 256);
-    L.first = o;     o = align_up(o + L.n_slots * 4, 256);
-    L.count = o;     o = align_up(o + L.n_slots * 4, 256);
-    L.vid = o;       o = align_up(o + L.n_slots * 4, 256);
-    L.slot_of = o;   o = align_up(o + n_total * 4, 256);
-    L.seg = o;       o += seg_ws_bytes(n_total, n_clouds, VTILE, 1);
-    L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 4, 256);
-    L.top = o;       o = align_up(o + (int64_t)n_clouds * max_voxels * max_points * 4, 256);
-    L.total = o;
-    return L;
+    const int64_t n_slots = vox_slots(n_total, n_clouds);
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.h_key = c.take<unsigned long long>(n_slots);
+    a.h_first = c.take<int>(n_slots);
+    a.h_count = c.take<int>(n_slots);
+    a.h_vid = c.take<int>(n_slots);
+    a.slot_of = c.take<int>(n_total);
+    a.seg = seg_take(c, n_total, n_clouds, VTILE, 1);
+    a.seg.total[0] = c.take<int32_t>(n_clouds);
+    a.top = c.take<int>((int64_t)n_clouds * max_voxels * max_points);
 }
 
 cudaError_t fill32(lss_engine *e, void *p, unsigned long long words, uint32_t v, cudaStream_t st)
@@ -211,7 +207,10 @@ extern "C" {
 int64_t lss_voxelize_workspace_bytes(int64_t n_total, int n_clouds, int max_points_per_voxel, int max_voxels)
 {
     if (n_total < 0 || n_clouds < 0 || max_points_per_voxel <= 0 || max_voxels <= 0) return -1;
-    return vox_layout(n_total, n_clouds, max_points_per_voxel, max_voxels).total;
+    WsCarve c;
+    VoxArgs a;
+    vox_carve(c, a, n_total, n_clouds, max_points_per_voxel, max_voxels);
+    return c.used;
 }
 
 lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
@@ -233,9 +232,10 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
     if (N >= (1LL << 30)) return lss_fail(e, LSS_ERR_INVALID_ARG, "batch too large");
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
-    const VoxLayout L = vox_layout(N, B, max_points_per_voxel, max_voxels);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     VoxArgs a;
+    WsCarve c{(char *)d_workspace};
+    vox_carve(c, a, N, B, max_points_per_voxel, max_voxels);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
     a.pts = d_points;
     a.F = n_features;
     a.cloud_cnt = d_cloud_counts;
@@ -253,17 +253,6 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
         a.gs[j] = (int)nearbyintf(q);
         if (a.gs[j] <= 0 || q > 2.0e9f) return lss_fail(e, LSS_ERR_INVALID_ARG, "bad grid size");
     }
-    char *ws = (char *)d_workspace;
-    int64_t *d_off = (int64_t *)(ws + L.off);
-    a.cloud_off = d_off;
-    a.h_key = (unsigned long long *)(ws + L.key);
-    a.h_first = (int *)(ws + L.first);
-    a.h_count = (int *)(ws + L.count);
-    a.h_vid = (int *)(ws + L.vid);
-    a.slot_of = (int *)(ws + L.slot_of);
-    a.seg = seg_tiles(ws + L.seg, B);
-    a.seg.total[0] = (int32_t *)(ws + L.seg_total);
-    a.top = (int *)(ws + L.top);
     a.out_vox = d_out_voxels;
     a.out_coords = d_out_coords;
     a.out_num = d_out_num_points;
@@ -271,12 +260,14 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
 
     const size_t n_vox_all = (size_t)B * max_voxels;
     if (B == 0) return LSS_OK;
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)a.seg.tile_base, st));
+    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
+                                         (int32_t *)a.seg.tile_base, st));
     {
         KernelTimer kt(e, LSS_K_VOXEL, st);
-        LSS_CUDA_CHECK(e, fill32(e, a.h_key, (unsigned long long)L.n_slots * 2, 0xffffffffu, st));
-        LSS_CUDA_CHECK(e, fill32(e, a.h_first, (unsigned long long)L.n_slots, (uint32_t)INT_MAX, st));
-        LSS_CUDA_CHECK(e, fill32(e, a.h_count, (unsigned long long)L.n_slots, 0u, st));
+        const unsigned long long n_slots = (unsigned long long)vox_slots(N, B);
+        LSS_CUDA_CHECK(e, fill32(e, a.h_key, n_slots * 2, 0xffffffffu, st));
+        LSS_CUDA_CHECK(e, fill32(e, a.h_first, n_slots, (uint32_t)INT_MAX, st));
+        LSS_CUDA_CHECK(e, fill32(e, a.h_count, n_slots, 0u, st));
         LSS_CUDA_CHECK(e, fill32(e, a.top, (unsigned long long)n_vox_all * max_points_per_voxel, (uint32_t)INT_MAX, st));
         LSS_CUDA_CHECK(e, fill32(e, d_out_voxels, (unsigned long long)n_vox_all * max_points_per_voxel * n_features, 0u, st));
         LSS_CUDA_CHECK(e, fill32(e, d_out_coords, (unsigned long long)n_vox_all * 4, 0u, st));

@@ -141,22 +141,16 @@ __global__ void __launch_bounds__(WET_TILE) k_wet_scatter(WetArgs a)
     }
 }
 
-struct WetLayout { int64_t off, f_wet, cls, new_i, seg, seg_total, prepass, prepass_bytes, total; };
-
-WetLayout wet_layout(int64_t n_total, int n_clouds)
+// The workspace, region by region; returns the pre-pass's workspace
+void *wet_carve(WsCarve &c, WetArgs &a, int64_t n_total, int n_clouds)
 {
-    WetLayout L;
-    int64_t o = 0;
-    L.off = o;      o = align_up(o + (int64_t)(n_clouds + 1) * 8, 256);
-    L.f_wet = o;    o = align_up(o + (int64_t)n_clouds * 8, 256);
-    L.cls = o;      o = align_up(o + n_total, 256);
-    L.new_i = o;    o = align_up(o + n_total * 8, 256);
-    L.seg = o;      o += seg_ws_bytes(n_total, n_clouds, WET_TILE, 2);
-    L.seg_total = o; o = align_up(o + (int64_t)n_clouds * 2 * 4, 256);
-    L.prepass_bytes = lss_prepass_ws_bytes(n_total, n_clouds);
-    L.prepass = o;  o = align_up(o + L.prepass_bytes, 256);
-    L.total = o;
-    return L;
+    a.cloud_off = c.take<int64_t>(n_clouds + 1);
+    a.f_wet = c.take<double>(n_clouds);
+    a.cls = c.take<uint8_t>(n_total);
+    a.new_i = c.take<double>(n_total);
+    a.seg = seg_take(c, n_total, n_clouds, WET_TILE, 2);
+    a.seg.total[0] = c.take<int32_t>((int64_t)n_clouds * 2);                  // both classes' totals
+    return c.take<char>(lss_prepass_ws_bytes(n_total, n_clouds));
 }
 
 // latch_range: latch LSS_ERR_INTENSITY_RANGE for a cloud of >= 1000 ground points with a degenerate I/cos range
@@ -183,15 +177,13 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
         return LSS_OK;
     }
     if (!d_points) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
-    const WetLayout L = wet_layout(N, B);
-    if (workspace_bytes < L.total) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
-    if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, B, h_plane_in != nullptr)) return rc;
-    char *ws = (char *)d_workspace;
     WetArgs a;
-    a.seg = seg_tiles(ws + L.seg, B);
-    a.seg.total[0] = (int32_t *)(ws + L.seg_total);
+    WsCarve c{(char *)d_workspace};
+    void *d_prepass_ws = wet_carve(c, a, N, B);
+    if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, B, h_plane_in != nullptr)) return rc;
     a.seg.total[1] = a.seg.total[0] + B;
-    int64_t *d_off = (int64_t *)(ws + L.off);
+    int64_t *d_off = (int64_t *)a.cloud_off;
     LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)a.seg.tile_base, st));
     void *cp_ptr = nullptr;
     // the plane is fitted on the cloud as given; laser parameters over the |p.w+h| < delta band, float64 ranges
@@ -203,10 +195,9 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     io.d_ymins_out = d_out_ymins;
     io.range_min_ground = latch_range ? 1000 : INT_MAX;                       // augmentation.py:51-52 returns first
     if (lss_status rc = lss_prepass_run(e, d_points, d_off, d_cloud_counts, h_cloud_offsets, B, delta, noise_floor,
-                                        flat_earth, 1, 0, io, ws + L.prepass, L.prepass_bytes, &cp_ptr, st))
+                                        flat_earth, 1, 0, io, d_prepass_ws, lss_prepass_ws_bytes(N, B), &cp_ptr, st))
         return rc;
     a.pts = d_points;
-    a.cloud_off = d_off;
     a.cloud_cnt = d_cloud_counts;
     a.cp = (const CloudPre *)cp_ptr;
     a.delta = delta;
@@ -218,13 +209,10 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
             const double f = h_water_height[b] / pavement_depth;                // augmentation.py:122
             f_wet[b] = f < 0 ? 0 : (f > 1 ? 1 : f);
         }
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, ws + L.f_wet, f_wet.data(), sizeof(double) * B, st));
-        a.f_wet = (const double *)(ws + L.f_wet);
+        LSS_CUDA_CHECK(e, lss_stage_upload(e, (double *)a.f_wet, f_wet.data(), sizeof(double) * B, st));
     }
     a.flat_earth = flat_earth;
     a.replace = replace;
-    a.cls = (uint8_t *)(ws + L.cls);
-    a.new_i = (double *)(ws + L.new_i);
     a.out = d_out_points;
     a.out_i64 = d_out_intensity64;
     a.out_counts = d_out_counts;
@@ -250,7 +238,10 @@ extern "C" {
 int64_t lss_wet_ground_workspace_bytes(int64_t n_total, int n_clouds)
 {
     if (n_total < 0 || n_clouds < 0) return -1;
-    return wet_layout(n_total, n_clouds).total;
+    WsCarve c;
+    WetArgs a;
+    wet_carve(c, a, n_total, n_clouds);
+    return c.used;
 }
 
 lss_status lss_wet_ground_batch(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
