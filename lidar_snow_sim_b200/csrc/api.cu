@@ -331,7 +331,6 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
     int64_t pre_bytes;
     int64_t *d_off = poly_carve(c, d_pre, pre_bytes, geo.n, n_clouds);
     if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), st));
     PrepassIO io;
     io.h_plane_in = h_plane_in;
     io.h_ymins_in = h_ymins_in;
@@ -339,6 +338,12 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
     io.d_plane_out = d_plane_out;
     io.d_fit_out = d_fit_out;
     io.d_ymins_out = d_ymins_out;
+    io.staged = true;
+    StageDone stage_done;                   // one staging launch heads the chain; its ring slot is released at the end
+    StageList l;
+    l.upload(d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1));
+    lss_prepass_stage(l, io, d_pre, geo.n, n_clouds);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st, &stage_done));
     return lss_prepass_run(e, d_points, d_off, nullptr, h_cloud_offsets, n_clouds, 0.5, noise_floor, 0, 0, 1, io,
                            d_pre, pre_bytes, nullptr, st);
 }

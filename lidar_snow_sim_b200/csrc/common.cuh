@@ -162,6 +162,40 @@ template <typename... P, typename... A>
     return cudaGetLastError();
 }
 
+// Programmatic dependent launch (sm_90).  A kernel launched by lss_launch_pdl right after another kernel on the same
+// stream may start while that kernel drains: its CTAs are scheduled once every CTA of the predecessor has executed
+// lss_pdl_trigger() (or exited), and lss_pdl_wait() blocks until the predecessor has completed and its writes are
+// visible.  That hides the launch latency of the boundary and the predecessor's last partial wave.  Rules of the chains
+// launched this way:
+//   * the first kernel of a chain is a plain lss_launch (a full dependency on whatever came before it);
+//   * every kernel launched this way calls lss_pdl_wait() on EVERY path, before its first read of anything an earlier
+//     kernel wrote and before its first write of anything an earlier kernel may still read.  Only the caller's inputs
+//     may be read before it.  Because every CTA waits, a kernel's completion implies its predecessor's, so a wait
+//     covers the whole chain before it and an event recorded after the chain covers all of it;
+//   * an event record or event wait between two launches makes that edge a full dependency again.
+// Without the launch attribute (a plain launch) lss_pdl_wait() returns at once and lss_pdl_trigger() does nothing.
+__device__ __forceinline__ void lss_pdl_wait() { asm volatile("griddepcontrol.wait;\n" ::: "memory"); }
+__device__ __forceinline__ void lss_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory"); }
+
+template <typename... P, typename... A>
+[[nodiscard]] inline cudaError_t lss_launch_pdl(lss_engine *e, void (*kernel)(P...), dim3 grid, dim3 block, size_t smem,
+                                                cudaStream_t stream, A &&...args)
+{
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const cudaError_t err = cudaLaunchKernelEx(&cfg, kernel, std::forward<A>(args)...);
+    e->launches++;
+    return err;
+}
+
 // next side stream + a (fork, join) event pair, round robin; created on first use
 inline cudaError_t lss_side_stream(lss_engine *e, cudaStream_t *stream, cudaEvent_t *ev_fork, cudaEvent_t *ev_join)
 {
@@ -180,67 +214,134 @@ inline cudaError_t lss_side_stream(lss_engine *e, cudaStream_t *stream, cudaEven
     return cudaSuccess;
 }
 
-// Asynchronous host -> device upload of a small host array through the engine's pinned ring (stream ordered; the
-// caller's buffer may be reused as soon as this returns).  The transfer is a tiny kernel reading the mapped pinned slot,
-// not a cudaMemcpyAsync: a copy-engine transfer would queue behind the multi-megabyte chunk copies of the host pipeline
-// (host_pipeline.cu) and stall the kernels waiting for their 300 bytes of offsets.  `bytes` must be a multiple of 4.
-static __global__ void k_stage_copy(uint32_t *dst, const uint32_t *src, int n_words)
-{
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_words; i += gridDim.x * blockDim.x) dst[i] = src[i];
-}
-
-inline cudaError_t lss_stage_upload(lss_engine *e, void *dst, const void *src, size_t bytes, cudaStream_t stream)
-{
-    if (bytes == 0) return cudaSuccess;
-    if (bytes % 4 != 0 || ((uintptr_t)dst & 3) != 0) return cudaErrorInvalidValue;
-    lss_engine::StageSlot &sl = e->stage[e->stage_next];
-    e->stage_next = (e->stage_next + 1) % lss_engine::N_STAGE;
-    cudaError_t err;
-    if (!sl.done) {
-        if ((err = cudaEventCreateWithFlags(&sl.done, cudaEventDisableTiming)) != cudaSuccess) return err;
-    } else if ((err = cudaEventSynchronize(sl.done)) != cudaSuccess) {
-        return err;
-    }
-    if (sl.cap < bytes) {
-        if (sl.host) cudaFreeHost(sl.host);
-        sl.host = nullptr; sl.cap = 0;
-        const size_t cap = bytes < 4096 ? 4096 : bytes * 2;
-        if ((err = cudaHostAlloc(&sl.host, cap, cudaHostAllocMapped)) != cudaSuccess) return err;
-        sl.cap = cap;
-    }
-    memcpy(sl.host, src, bytes);
-    const int n_words = (int)(bytes / 4);
-    const int blocks = n_words >= 1 << 16 ? 64 : (n_words + 1023) / 1024;
-    if ((err = lss_launch(e, k_stage_copy, blocks, 256, 0, stream, (uint32_t *)dst, (const uint32_t *)sl.host, n_words)) !=
-        cudaSuccess)
-        return err;
-    return cudaEventRecord(sl.done, stream);
-}
-
-// Stream-ordered zero fill of up to 6 device regions in ONE kernel launch.  Not cudaMemsetAsync: memsets may be executed
-// by a copy engine, where they queue behind the host pipeline's multi-megabyte chunk copies.  Region sizes are multiples of 4 bytes, pointers 4-byte aligned.
+// Stream-ordered zero fill of device regions.  Not cudaMemsetAsync: memsets may be executed by a copy engine, where they
+// queue behind the host pipeline's multi-megabyte chunk copies.  Region sizes are multiples of 4 bytes, pointers 4-byte
+// aligned.
 struct ZeroRegions {
-    static constexpr int MAX = 6;
+    static constexpr int MAX = 8;
     uint32_t *p[MAX];
     unsigned long long words[MAX];
     int n = 0;
     void add(void *ptr, size_t bytes) { if (ptr && bytes) { p[n] = (uint32_t *)ptr; words[n] = (bytes + 3) / 4; n++; } }
 };
-static __global__ void k_zero_regions(ZeroRegions r)
+
+// A call's staging: small host arrays to upload (offsets, orders, polynomials) and device regions to zero, enqueued by
+// lss_stage as ONE kernel launch.  The transfer is a tiny kernel reading the engine's mapped pinned ring, not a
+// cudaMemcpyAsync: a copy-engine transfer would queue behind the multi-megabyte chunk copies of the host pipeline
+// (host_pipeline.cu) and stall the kernels waiting for their 300 bytes of offsets, and a cudaMemcpyAsync from pageable
+// memory makes the host wait for the stream.  Upload sizes are multiples of 4 bytes, destinations 4-byte aligned.
+struct StageList {
+    static constexpr int MAX = 8;
+    uint32_t *dst[MAX];
+    const uint32_t *src[MAX];         // the caller's host array; lss_stage points it into the ring slot
+    unsigned long long words[MAX];
+    int n = 0;
+    bool bad = false;                 // too many uploads, or a size / alignment the copy cannot take
+    ZeroRegions zero;
+    void upload(void *d, const void *h, size_t bytes)
+    {
+        if (bytes == 0) return;
+        if (n == MAX || bytes % 4 != 0 || ((uintptr_t)d & 3) != 0) { bad = true; return; }
+        dst[n] = (uint32_t *)d; src[n] = (const uint32_t *)h; words[n] = bytes / 4; n++;
+    }
+};
+// grid (blocks, uploads + zero regions): row y < s.n copies upload y, the rows after it clear one zero region each.  Always
+// the first kernel of its chain (a plain launch); its dependents may be scheduled at once.
+static __global__ void k_stage_copy(StageList s)
 {
-    uint32_t *p = r.p[blockIdx.y];
-    const unsigned long long n = r.words[blockIdx.y];
+    lss_pdl_trigger();
+    const int r = blockIdx.y;
     const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
-    for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) p[i] = 0u;
+    const unsigned long long i0 = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < s.n) {
+        uint32_t *dst = s.dst[r];
+        const uint32_t *src = s.src[r];
+        for (unsigned long long i = i0; i < s.words[r]; i += stride) dst[i] = src[i];
+    } else {
+        uint32_t *p = s.zero.p[r - s.n];
+        for (unsigned long long i = i0; i < s.zero.words[r - s.n]; i += stride) p[i] = 0u;
+    }
 }
-inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStream_t stream)
+
+// Records a staging ring slot's `done` event on the stream when it goes out of scope: declared at the top of an entry
+// point and handed to lss_stage, it records after the call's last launch, on every return path.  An event record between
+// two kernels would make their edge a full dependency (lss_launch_pdl).
+struct StageDone {
+    cudaEvent_t ev = nullptr;
+    cudaStream_t stream = nullptr;
+    StageDone() = default;
+    StageDone(const StageDone &) = delete;
+    StageDone &operator=(const StageDone &) = delete;
+    ~StageDone() { if (ev) cudaEventRecord(ev, stream); }
+};
+
+// Enqueues the uploads and zero fills of `l` as one launch of k_stage_copy (nothing when the list is empty).  The host arrays
+// are copied into one slot of the engine's pinned ring before this returns, so the caller may reuse them at once.  A slot
+// is handed out again only after its `done` event, recorded after the copy, has completed: right after the launch when
+// `done` is null, else when `done` goes out of scope.
+inline cudaError_t lss_stage(lss_engine *e, StageList l, cudaStream_t stream, StageDone *done = nullptr)
 {
-    if (r.n == 0) return cudaSuccess;
+    if (l.bad) return cudaErrorInvalidValue;
+    if (l.n + l.zero.n == 0) return cudaSuccess;
+    size_t bytes = 0;
     unsigned long long mx = 0;
-    for (int i = 0; i < r.n; i++) mx = r.words[i] > mx ? r.words[i] : mx;
+    for (int k = 0; k < l.n; k++) {
+        bytes += (size_t)align_up((int64_t)l.words[k] * 4, 16);
+        mx = l.words[k] > mx ? l.words[k] : mx;
+    }
+    for (int k = 0; k < l.zero.n; k++) mx = l.zero.words[k] > mx ? l.zero.words[k] : mx;
+    cudaError_t err;
+    lss_engine::StageSlot *sl = nullptr;
+    if (bytes) {
+        sl = &e->stage[e->stage_next];
+        e->stage_next = (e->stage_next + 1) % lss_engine::N_STAGE;
+        if (!sl->done) {
+            if ((err = cudaEventCreateWithFlags(&sl->done, cudaEventDisableTiming)) != cudaSuccess) return err;
+        } else if ((err = cudaEventSynchronize(sl->done)) != cudaSuccess) {
+            return err;
+        }
+        if (sl->cap < bytes) {
+            if (sl->host) cudaFreeHost(sl->host);
+            sl->host = nullptr; sl->cap = 0;
+            const size_t cap = bytes < 4096 ? 4096 : bytes * 2;
+            if ((err = cudaHostAlloc(&sl->host, cap, cudaHostAllocMapped)) != cudaSuccess) return err;
+            sl->cap = cap;
+        }
+        size_t off = 0;
+        for (int k = 0; k < l.n; k++) {
+            char *h = (char *)sl->host + off;
+            memcpy(h, l.src[k], l.words[k] * 4);
+            l.src[k] = (const uint32_t *)h;
+            off += (size_t)align_up((int64_t)l.words[k] * 4, 16);
+        }
+    }
     const unsigned long long cap = 4ull * e->n_sm;
     const unsigned blocks = (unsigned)((mx + 1023) / 1024 < cap ? (mx + 1023) / 1024 : cap);
-    return lss_launch(e, k_zero_regions, dim3(blocks ? blocks : 1, r.n), 256, 0, stream, r);
+    if ((err = lss_launch(e, k_stage_copy, dim3(blocks ? blocks : 1, l.n + l.zero.n), 256, 0, stream, l)) != cudaSuccess)
+        return err;
+    if (!sl) return cudaSuccess;
+    if (!done) return cudaEventRecord(sl->done, stream);
+    if (done->ev && (err = cudaEventRecord(done->ev, done->stream)) != cudaSuccess) return err;
+    done->ev = sl->done;
+    done->stream = stream;
+    return cudaSuccess;
+}
+
+// Asynchronous host -> device upload of one small host array (one launch; the caller's buffer may be reused as soon as
+// this returns).  `bytes` must be a multiple of 4.
+inline cudaError_t lss_stage_upload(lss_engine *e, void *dst, const void *src, size_t bytes, cudaStream_t stream)
+{
+    StageList l;
+    l.upload(dst, src, bytes);
+    return lss_stage(e, l, stream);
+}
+
+// Stream-ordered zero fill of up to ZeroRegions::MAX device regions in ONE kernel launch.
+inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStream_t stream)
+{
+    StageList l;
+    l.zero = r;
+    return lss_stage(e, l, stream);
 }
 
 enum { LSS_K_SORT = 0, LSS_K_PREPASS = 1, LSS_K_SNOWFALL = 2, LSS_K_COMPACT = 3, LSS_K_FINALIZE = 4, LSS_K_WET = 5,
@@ -390,7 +491,12 @@ struct PrepassIO {
     // a cloud with at least this many ground points latches LSS_ERR_INTENSITY_RANGE when its I/cos range is degenerate
     // (the snowfall path fits from 3 ground points on; wet ground returns below 1000 first, augmentation.py:51-52)
     int range_min_ground = 3;
+    // the caller's staging launch already did what lss_prepass_stage adds (the pre-pass then enqueues no staging of its own)
+    bool staged = false;
 };
+// Adds the pre-pass's staging to a caller's StageList: the zero fill of its per-cloud records and the upload of io's host
+// inputs.  Folded into the caller's own staging launch (io.staged), it saves the pre-pass a launch at the head of its chain.
+void lss_prepass_stage(StageList &l, const PrepassIO &io, void *d_ws, int64_t n_total, int n_clouds);
 lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_cloud_off, const int32_t *d_cloud_cnt,
                            const int64_t *h_cloud_off, int n_clouds, double delta, double noise_floor, int flat_earth,
                            int range64, int raise_few_ground, const PrepassIO &io, void *d_ws, int64_t ws_bytes,

@@ -742,6 +742,18 @@ int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds)
     return c.used;
 }
 
+void lss_prepass_stage(StageList &l, const PrepassIO &io, void *d_ws, int64_t n_total, int n_clouds)
+{
+    WsCarve c{(char *)d_ws};
+    PreArgs a;
+    double *d_plane;
+    int32_t *d_ymins_in;
+    prepass_carve(c, a, d_plane, d_ymins_in, n_total, n_clouds);
+    l.zero.add(a.cp, (size_t)((char *)a.rec_cnt - (char *)a.cp) + sizeof(int) * n_clouds);   // records and record cursors
+    if (io.h_ymins_in) l.upload(d_ymins_in, io.h_ymins_in, sizeof(int32_t) * HIST_NX * n_clouds);
+    if (io.h_plane_in) l.upload(d_plane, io.h_plane_in, sizeof(double) * 4 * n_clouds);
+}
+
 // dynamic shared memory of k_window_gather_mad: the prefix of the tile counts of the largest cloud
 static size_t gather_dyn_smem(int64_t max_n) { return sizeof(int) * ((size_t)(max_n + 31) / 32 + 2); }
 
@@ -810,24 +822,20 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     a.flat_earth = flat_earth;
     a.have_plane = h_plane_in != nullptr;
     a.status = e->d_status;
-    a.ymins_in = nullptr;
-    if (io.h_ymins_in) {
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, d_ymins_in, io.h_ymins_in, sizeof(int32_t) * HIST_NX * B, stream));
-        a.ymins_in = d_ymins_in;
-    }
+    a.ymins_in = io.h_ymins_in ? d_ymins_in : nullptr;
     if (cloudpre_out) *cloudpre_out = a.cp;
     const int64_t max_n = largest_cloud(h_cloud_off, B);
     int nblk = (int)std::min<int64_t>(a.max_blocks, std::max<int64_t>(1, (max_n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
-
-    {
-        ZeroRegions z;
-        z.add(a.cp, (size_t)((char *)a.rec_cnt - (char *)a.cp) + sizeof(int) * B);   // CloudPre records and record cursors
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
+    if (!io.staged) {
+        StageList l;
+        lss_prepass_stage(l, io, d_ws, N, B);
+        LSS_CUDA_CHECK(e, lss_stage(e, l, stream));
     }
+    // Plain launches: next to the scan, a PDL chain here would park each kernel's CTAs on the SMs while the one before
+    // it runs, at the side stream's high priority, and the step measured slower (DESIGN.md section 8)
     {
         KernelTimer kt(e, LSS_K_PREPASS, stream);
         if (h_plane_in) {
-            LSS_CUDA_CHECK(e, lss_stage_upload(e, d_plane, h_plane_in, sizeof(double) * 4 * B, stream));
             LSS_CUDA_CHECK(e, lss_launch(e, k_set_plane, (B + 127) / 128, 128, 0, stream, a, d_plane));
         } else {
             const int max_tiles = (int)std::max<int64_t>(1, (max_n + WTILE - 1) / WTILE);

@@ -83,6 +83,8 @@ template <int K, int TILE>
 __global__ void __launch_bounds__(TILE) k_seg_count_codes(const uint8_t *code, const int64_t *cloud_off,
                                                           const int32_t *cloud_cnt, SegTiles s)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     const int b = blockIdx.y, tile = blockIdx.x;
     if (tile >= s.tile_base[b + 1] - s.tile_base[b]) return;
     const int i = tile * TILE + threadIdx.x;
@@ -98,6 +100,8 @@ __global__ void __launch_bounds__(TILE) k_seg_count_codes(const uint8_t *code, c
 template <int K>
 __global__ void __launch_bounds__(SEG_SCAN_TPB) k_seg_scan(SegTiles s)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     __shared__ __align__(16) int warp_sum[K][SEG_SCAN_TPB / 32];
     __shared__ int run[K];
     const int b = blockIdx.x;

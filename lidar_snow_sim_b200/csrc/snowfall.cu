@@ -44,6 +44,8 @@ __global__ void __launch_bounds__(SCHED_KEY_TPB) k_sched_key(const float *__rest
                                                             const int32_t *__restrict__ order, const int32_t *__restrict__ wtile_base,
                                                             unsigned long long *ent, int *hist)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     const int b = blockIdx.y, t = blockIdx.x * SCHED_KEY_TPB + threadIdx.x;
     const int64_t beg = cloud_off[b];
     const int n_slot = (int)(cloud_off[b + 1] - beg);
@@ -71,6 +73,8 @@ constexpr int SCHED_PER_THREAD = 2;
 __global__ void __launch_bounds__(256) k_sched_sort(const unsigned long long *__restrict__ in, unsigned long long *out,
                                                     int *hist, int n)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     __shared__ int base[SCHED_BINS], cnt[SCHED_BINS], blk[SCHED_BINS];
     const int first = blockIdx.x * (256 * SCHED_PER_THREAD);
     for (int c = threadIdx.x; c < SCHED_BINS; c += 256) cnt[c] = 0;
@@ -130,6 +134,8 @@ constexpr int KEEP_ROWS = TILE / KEEP_TPB;
 
 __global__ void __launch_bounds__(KEEP_TPB) k_keep(DevArgs a)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     __shared__ unsigned h_keep[NBINS], h_all[NBINS];
     __shared__ int s_cnt[2];
     const int b = blockIdx.y, tile = blockIdx.x;
@@ -219,6 +225,8 @@ __global__ void __launch_bounds__(1024) k_tile_scan(unsigned *hist, const int32_
                                                      const unsigned *att_cnt, const unsigned long long *att_sum,
                                                      const SensorConst *sensor)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     __shared__ unsigned bin_total[NBINS];
     __shared__ double att_term[LSS_N_CHANNELS];
     const int b = blockIdx.x;
@@ -296,6 +304,8 @@ __global__ void __launch_bounds__(TILE) k_scatter(const float *__restrict__ aug,
                                                    float *__restrict__ out, const int32_t *__restrict__ nocc_in,
                                                    int32_t *__restrict__ nocc_out, int32_t *__restrict__ perm_out)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     __shared__ unsigned warp_cnt[TILE / 32][NBINS];
     const int b = blockIdx.y, tile = blockIdx.x;
     const int64_t beg = cloud_off[b];
@@ -422,26 +432,33 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     unsigned *d_att_cnt = (unsigned *)((char *)a.counters + att_cnt_off(B));
     unsigned long long *d_att_sum = (unsigned long long *)((char *)d_att_cnt + (int64_t)B * LSS_N_CHANNELS * 4);
 
+    // One staging launch, the first of the call's chain: the host arrays (offsets, tile bases, orders, the polynomial when
+    // one is given, the pre-pass's inputs) and every zero fill.  Its ring slot is released after the call's last launch.
+    StageDone stage_done;
+    StageList l;
     // d_tile_base: [0, B] first scatter tile of each cloud, [B + 1, 2 B + 1] first warp tile of each cloud
     g.tile_base.insert(g.tile_base.end(), wg.tile_base.begin(), wg.tile_base.end());
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, s.h_cloud_offsets, B, g.tile_base, d_off, d_tile_base, stream));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS, stream));
-    if (s.h_thresh_poly)
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B, stream));
-    {
-        ZeroRegions z;
-        z.add(a.counters, counters_bytes(B));
-        z.add(s.d_out_stats, sizeof(double) * 4 * B);
-        if (N == 0 || B == 0) {
-            z.add(s.d_out_counts, sizeof(int32_t) * B);
-            LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
-            return LSS_OK;
-        }
-        z.add(a.hdr, LIST_HDR_BYTES);                     // (the tile histograms are written whole by k_keep)
-        z.add(a.chunk_tab, (size_t)LIST_CLASSES * a.chunks_per_class * 4);
-        z.add(d_sched_hist, (size_t)SCHED_BINS * 2 * 4);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, stream));
+    l.upload(d_off, s.h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload(d_tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    l.upload(d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS);
+    if (s.h_thresh_poly) l.upload(d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B);
+    l.zero.add(a.counters, counters_bytes(B));
+    l.zero.add(s.d_out_stats, sizeof(double) * 4 * B);
+    if (N == 0 || B == 0) {
+        l.zero.add(s.d_out_counts, sizeof(int32_t) * B);
+        LSS_CUDA_CHECK(e, lss_stage(e, l, stream, &stage_done));
+        return LSS_OK;
     }
+    l.zero.add(a.hdr, LIST_HDR_BYTES);                     // (the tile histograms are written whole by k_keep)
+    l.zero.add(a.chunk_tab, (size_t)LIST_CLASSES * a.chunks_per_class * 4);
+    l.zero.add(d_sched_hist, (size_t)SCHED_BINS * 2 * 4);
+    PrepassIO io;
+    io.h_plane_in = s.h_plane_in;
+    io.h_ymins_in = s.h_ymins_in;
+    io.d_poly_out = d_thresh;
+    io.staged = true;
+    if (device_prepass) lss_prepass_stage(l, io, d_prepass_ws, N, B);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, stream, &stage_done));
 
     a.rec = s.ts->d_rec;
     a.tan = s.ts->d_tan;
@@ -483,10 +500,6 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
         LSS_CUDA_CHECK(e, lss_side_stream(e, &side, &ev_fork, &ev_join));
         LSS_CUDA_CHECK(e, cudaEventRecord(ev_fork, stream));
         LSS_CUDA_CHECK(e, cudaStreamWaitEvent(side, ev_fork, 0));
-        PrepassIO io;
-        io.h_plane_in = s.h_plane_in;
-        io.h_ymins_in = s.h_ymins_in;
-        io.d_poly_out = d_thresh;
         lss_status ps = lss_prepass_run(e, s.d_points, d_off, s.d_cloud_counts, s.h_cloud_offsets, B, 0.5, s.noise_floor, 0, 0, 1,
                                 io, d_prepass_ws, lss_prepass_ws_bytes(N, B), nullptr, side);
         const cudaError_t je = cudaEventRecord(ev_join, side);
@@ -504,12 +517,12 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
             unsigned long long *d_ent = (unsigned long long *)(d_sched_hist + 2 * SCHED_BINS);
             unsigned long long *d_sched = d_ent + sched_tiles(N, B);
             const int max_wtiles = (int)((max_n + 31) / 32);
-            ce = lss_launch(e, k_sched_key, dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B),
-                            SCHED_KEY_TPB, 0, stream, s.d_points, d_off, s.d_cloud_counts, d_order, d_tile_base + B + 1,
-                            d_ent, d_sched_hist);
+            ce = lss_launch_pdl(e, k_sched_key, dim3((unsigned)((max_wtiles + SCHED_KEY_TPB - 1) / SCHED_KEY_TPB), (unsigned)B),
+                                SCHED_KEY_TPB, 0, stream, s.d_points, d_off, s.d_cloud_counts, d_order, d_tile_base + B + 1,
+                                d_ent, d_sched_hist);
             if (ce == cudaSuccess)
-                ce = lss_launch(e, k_sched_sort, (unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)),
-                                256, 0, stream, d_ent, d_sched, d_sched_hist, n_wtiles);
+                ce = lss_launch_pdl(e, k_sched_sort, (unsigned)((n_wtiles + 256 * SCHED_PER_THREAD - 1) / (256 * SCHED_PER_THREAD)),
+                                    256, 0, stream, d_ent, d_sched, d_sched_hist, n_wtiles);
             a.sched = d_sched;
             a.n_wtiles = n_wtiles;
         }
@@ -527,24 +540,24 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     LSS_CUDA_CHECK(e, ce);
     {
         KernelTimer kt(e, LSS_K_FINALIZE, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_keep, dim3(max_tiles, B), KEEP_TPB, 0, stream, a));
+        LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_keep, dim3(max_tiles, B), KEEP_TPB, 0, stream, a));
     }
     {
         KernelTimer kt(e, LSS_K_SORT, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, a.hist_keep, d_tile_base, s.d_out_counts,
-                                     s.d_out_stats, a.counters, d_att_cnt, d_att_sum, e->d_sensor));
+        LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_tile_scan, B, 1024, 0, stream, a.hist_keep, d_tile_base, s.d_out_counts,
+                                         s.d_out_stats, a.counters, d_att_cnt, d_att_sum, e->d_sensor));
     }
     {
         KernelTimer kt(e, LSS_K_COMPACT, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, a.aug, a.code_keep, a.hist_keep, d_off,
-                                     s.d_cloud_counts, d_tile_base, s.d_out_points, nullptr, nullptr, nullptr));
+        LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, a.aug, a.code_keep, a.hist_keep, d_off,
+                                         s.d_cloud_counts, d_tile_base, s.d_out_points, nullptr, nullptr, nullptr));
     }
     if (want_all) {     // un-filtered, channel-sorted debug views (tests): full rows, original index, occluder counts
         KernelTimer kt(e, LSS_K_COMPACT, stream);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_tile_scan, B, 1024, 0, stream, a.hist_all, d_tile_base, nullptr, nullptr, nullptr,
-                                     nullptr, nullptr, nullptr));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, a.aug, a.code_all, a.hist_all, d_off,
-                                     s.d_cloud_counts, d_tile_base, s.d_out_full, a.nocc, s.d_out_nocc, s.d_out_perm));
+        LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_tile_scan, B, 1024, 0, stream, a.hist_all, d_tile_base, nullptr, nullptr, nullptr,
+                                         nullptr, nullptr, nullptr));
+        LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_scatter, dim3(max_tiles, B), TILE, 0, stream, a.aug, a.code_all, a.hist_all, d_off,
+                                         s.d_cloud_counts, d_tile_base, s.d_out_full, a.nocc, s.d_out_nocc, s.d_out_perm));
     }
     return LSS_OK;
 }

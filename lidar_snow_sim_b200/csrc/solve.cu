@@ -151,9 +151,14 @@ __global__ void __launch_bounds__(SNOW_TPB, LSS_SCAN_CTAS) k_scan(DevArgs a)
     __shared__ int s_idx[SNOW_WARPS][32][SURV_CAP];                // plane-local particle index of each lane's survivors
     __shared__ unsigned s_hit[SNOW_WARPS][32];                     // bit r: survivor r of this lane is a hit
     const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    // Dependents (the solve kernel) are scheduled once every scan CTA has started, i.e. when the last wave is resident:
+    // their CTAs then take only the slots that retiring scan CTAs free.  Which rows a warp reads comes from the schedule,
+    // so everything after the index arithmetic waits for the kernels before.
+    lss_pdl_trigger();
     // this warp's tile from the plane-major schedule: the warps of a CTA may belong to different clouds (no block-wide
     // barrier below)
     const int st = blockIdx.x * SNOW_WARPS + wid;
+    lss_pdl_wait();
     if (st >= a.n_wtiles) return;
     const unsigned long long se = a.sched[st];
     const int b = (int)((se >> 32) & 0xffffu), w0 = (int)(unsigned)se;  // cloud, first row of this warp
@@ -450,6 +455,8 @@ __global__ void __launch_bounds__(SOLVE_TPB, SOLVE_CTAS_PER_SM) k_solve(DevArgs 
     // class c, s_tile0[LIST_CLASSES] = number of tiles; s_cnt[c] = listed beams of class c.
     __shared__ int s_tile0[LIST_CLASSES + 1];
     __shared__ int s_cnt[LIST_CLASSES];
+    lss_pdl_trigger();
+    lss_pdl_wait();                                                 // the class counts and the list come from the scan
     if (wid == 0) {
         int run = 0;
         for (int c0 = 0; c0 < LIST_CLASSES; c0 += 32) {
@@ -947,12 +954,19 @@ extern "C" lss_status lss_debug_solve_phases(lss_engine *e, int reset, uint64_t 
 #endif
 }
 
+// Both follow another kernel of the chain on the stream (lss_launch_pdl).  -DLSS_PDL_SOLVE=0 (LSS_NVCC_FLAGS) launches the
+// solve kernel plainly instead, to measure what its overlap with the scan's last wave buys.
+#ifndef LSS_PDL_SOLVE
+#define LSS_PDL_SOLVE 1
+#endif
 cudaError_t lss_launch_scan(lss_engine *e, const DevArgs &a, cudaStream_t stream)
 {
-    return lss_launch(e, k_scan, (unsigned)((a.n_wtiles + SNOW_WARPS - 1) / SNOW_WARPS), SNOW_TPB, 0, stream, a);
+    return lss_launch_pdl(e, k_scan, (unsigned)((a.n_wtiles + SNOW_WARPS - 1) / SNOW_WARPS), SNOW_TPB, 0, stream, a);
 }
 
 cudaError_t lss_launch_solve(lss_engine *e, const DevArgs &a, int *tile_cursor, cudaStream_t stream)
 {
-    return lss_launch(e, k_solve, (unsigned)(e->n_sm * SOLVE_CTAS_PER_SM), SOLVE_TPB, 0, stream, a, tile_cursor);
+    const unsigned grid = (unsigned)(e->n_sm * SOLVE_CTAS_PER_SM);
+    if (LSS_PDL_SOLVE) return lss_launch_pdl(e, k_solve, grid, SOLVE_TPB, 0, stream, a, tile_cursor);
+    return lss_launch(e, k_solve, grid, SOLVE_TPB, 0, stream, a, tile_cursor);
 }

@@ -72,6 +72,8 @@ __device__ __forceinline__ Fresnel fresnel_power(double ain, double nair, double
 
 __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     const int b = blockIdx.y;
     const CloudPre cp = a.cp[b];
     const int64_t beg = a.cloud_off[b];
@@ -114,6 +116,8 @@ __global__ void __launch_bounds__(WET_TPB) k_wet_points(WetArgs a)
 // rank inside the class.  Tile 0 of every cloud also writes the output count and the pass-through flag.
 __global__ void __launch_bounds__(WET_TILE) k_wet_scatter(WetArgs a)
 {
+    lss_pdl_trigger();
+    lss_pdl_wait();
     const int b = blockIdx.y, tile = blockIdx.x;
     const CloudPre &cp = a.cp[b];
     const int pass_code = wet_passthrough(cp);
@@ -184,8 +188,6 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     if (lss_status rc = lss_prepass_check(e, h_cloud_offsets, B, h_plane_in != nullptr)) return rc;
     a.seg.total[1] = a.seg.total[0] + B;
     int64_t *d_off = (int64_t *)a.cloud_off;
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)a.seg.tile_base, st));
-    void *cp_ptr = nullptr;
     // the plane is fitted on the cloud as given; laser parameters over the |p.w+h| < delta band, float64 ranges
     PrepassIO io;
     io.h_plane_in = h_plane_in;
@@ -194,6 +196,24 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     io.d_fit_out = d_out_fit;
     io.d_ymins_out = d_out_ymins;
     io.range_min_ground = latch_range ? 1000 : INT_MAX;                       // augmentation.py:51-52 returns first
+    io.staged = true;
+    // One staging launch heads the call's chain: offsets, tile bases, wetness per cloud and the pre-pass's staging.  Its
+    // ring slot is released after the call's last launch.
+    StageDone stage_done;
+    {
+        std::vector<double> f_wet(B);
+        for (int b = 0; b < B; b++) {
+            const double f = h_water_height[b] / pavement_depth;                // augmentation.py:122
+            f_wet[b] = f < 0 ? 0 : (f > 1 ? 1 : f);
+        }
+        StageList l;
+        l.upload(d_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+        l.upload((int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+        l.upload((double *)a.f_wet, f_wet.data(), sizeof(double) * B);
+        lss_prepass_stage(l, io, d_prepass_ws, N, B);
+        LSS_CUDA_CHECK(e, lss_stage(e, l, st, &stage_done));
+    }
+    void *cp_ptr = nullptr;
     if (lss_status rc = lss_prepass_run(e, d_points, d_off, d_cloud_counts, h_cloud_offsets, B, delta, noise_floor,
                                         flat_earth, 1, 0, io, d_prepass_ws, lss_prepass_ws_bytes(N, B), &cp_ptr, st))
         return rc;
@@ -203,14 +223,6 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     a.delta = delta;
     a.noise_floor = noise_floor;
     a.power_factor = power_factor;
-    {
-        std::vector<double> f_wet(B);
-        for (int b = 0; b < B; b++) {
-            const double f = h_water_height[b] / pavement_depth;                // augmentation.py:122
-            f_wet[b] = f < 0 ? 0 : (f > 1 ? 1 : f);
-        }
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, (double *)a.f_wet, f_wet.data(), sizeof(double) * B, st));
-    }
     a.flat_earth = flat_earth;
     a.replace = replace;
     a.out = d_out_points;
@@ -221,13 +233,13 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     const int nblk = (int)std::max<int64_t>(1, std::min<int64_t>(1024, (g.max_n + WET_TPB * 4 - 1) / (WET_TPB * 4)));
     {
         KernelTimer kt(e, LSS_K_WET, st);
-        LSS_CUDA_CHECK(e, lss_launch(e, k_wet_points, dim3(nblk, B), WET_TPB, 0, st, a));
+        LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_wet_points, dim3(nblk, B), WET_TPB, 0, st, a));
     }
     KernelTimer kt(e, LSS_K_COMPACT, st);
-    LSS_CUDA_CHECK(e, lss_launch(e, k_seg_count_codes<2, WET_TILE>, dim3(max_tiles, B), WET_TILE, 0, st, a.cls, a.cloud_off,
-                                 a.cloud_cnt, a.seg));
-    LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.seg));
-    LSS_CUDA_CHECK(e, lss_launch(e, k_wet_scatter, dim3(max_tiles, B), WET_TILE, 0, st, a));
+    LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_seg_count_codes<2, WET_TILE>, dim3(max_tiles, B), WET_TILE, 0, st, a.cls,
+                                     a.cloud_off, a.cloud_cnt, a.seg));
+    LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.seg));
+    LSS_CUDA_CHECK(e, lss_launch_pdl(e, k_wet_scatter, dim3(max_tiles, B), WET_TILE, 0, st, a));
     return LSS_OK;
 }
 
