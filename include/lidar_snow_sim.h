@@ -573,7 +573,7 @@ LSS_API int64_t lss_dror_workspace_bytes(int64_t n_total, int n_clouds);
  *                   each slot (n_master = max(n_l, n_s)), rows behind them untouched
  *   d_workspace     lss_strongest_last_batch_workspace_bytes(h_last_offsets, h_strongest_offsets, n_clouds) bytes; that
  *                   query needs a CUDA device (radix sort scratch) and returns -1 without one or for bad offsets
- * Exact: comparisons and integer counts only.  3 staging copies and 6 launches (the sort counted as one); no
+ * Exact: comparisons and integer counts only.  1 staging launch and 6 launches (the sort counted as one); no
  * allocation, no synchronisation.                                                                                        */
 LSS_API lss_status lss_strongest_last_batch(lss_engine *e, const float *d_last, const int64_t *h_last_offsets,
                                             const int32_t *d_last_counts, const float *d_strongest,
@@ -595,7 +595,7 @@ LSS_API int64_t lss_strongest_last_batch_workspace_bytes(const int64_t *h_last_o
  *   d_out_points    float32[n_total * n_features]: kept rows in order at the front of each slot.  Must not alias d_points.
  *   d_out_counts    int32[n_clouds];  d_out_mask  uint8[n_total] or NULL: the flag of every valid row
  *   d_workspace     lss_camera_fov_batch_workspace_bytes(n_total, n_clouds) bytes
- * LSS_ERR_NO_SENSOR without a camera.  3 staging copies and 3 kernels; no allocation, no synchronisation.              */
+ * LSS_ERR_NO_SENSOR without a camera.  1 staging launch and 3 kernels; no allocation, no synchronisation.              */
 LSS_API lss_status lss_camera_fov_batch(lss_engine *e, const float *d_points, int n_features, const int64_t *h_cloud_offsets,
                                         const int32_t *d_cloud_counts, int n_clouds, const int32_t *h_img_shape,
                                         float *d_out_points, int32_t *d_out_counts, uint8_t *d_out_mask,

@@ -338,7 +338,6 @@ lss_status lss_noise_threshold_poly(lss_engine *e, const float *d_points, const 
     io.d_plane_out = d_plane_out;
     io.d_fit_out = d_fit_out;
     io.d_ymins_out = d_ymins_out;
-    io.staged = true;
     StageDone stage_done;                   // one staging launch heads the chain; its ring slot is released at the end
     StageList l;
     l.upload(d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1));

@@ -214,52 +214,48 @@ inline cudaError_t lss_side_stream(lss_engine *e, cudaStream_t *stream, cudaEven
     return cudaSuccess;
 }
 
-// Stream-ordered zero fill of device regions.  Not cudaMemsetAsync: memsets may be executed by a copy engine, where they
-// queue behind the host pipeline's multi-megabyte chunk copies.  Region sizes are multiples of 4 bytes, pointers 4-byte
-// aligned.
-struct ZeroRegions {
-    static constexpr int MAX = 8;
-    uint32_t *p[MAX];
-    unsigned long long words[MAX];
-    int n = 0;
-    void add(void *ptr, size_t bytes) { if (ptr && bytes) { p[n] = (uint32_t *)ptr; words[n] = (bytes + 3) / 4; n++; } }
-};
-
 // A call's staging: small host arrays to upload (offsets, orders, polynomials) and device regions to zero, enqueued by
-// lss_stage as ONE kernel launch.  The transfer is a tiny kernel reading the engine's mapped pinned ring, not a
-// cudaMemcpyAsync: a copy-engine transfer would queue behind the multi-megabyte chunk copies of the host pipeline
-// (host_pipeline.cu) and stall the kernels waiting for their 300 bytes of offsets, and a cudaMemcpyAsync from pageable
-// memory makes the host wait for the stream.  Upload sizes are multiples of 4 bytes, destinations 4-byte aligned.
+// lss_stage as ONE kernel launch before the call's first kernel.  The transfer is a tiny kernel reading the engine's
+// mapped pinned ring, not a cudaMemcpyAsync: a copy-engine transfer would queue behind the multi-megabyte chunk copies of
+// the host pipeline (host_pipeline.cu) and stall the kernels waiting for their 300 bytes of offsets, and a cudaMemcpyAsync
+// from pageable memory makes the host wait for the stream.  The zero fills are not cudaMemsetAsync for the same reason: a
+// memset may be executed by a copy engine.  Upload sizes are multiples of 4 bytes; destinations and zero regions are 4-byte
+// aligned, and a zero region is cleared in whole 4-byte words.  The rows of the launch run concurrently, so no upload
+// destination or zero region of a list may overlap another.
 struct StageList {
-    static constexpr int MAX = 8;
+    static constexpr int MAX = 16;
     uint32_t *dst[MAX];
-    const uint32_t *src[MAX];         // the caller's host array; lss_stage points it into the ring slot
+    const uint32_t *src[MAX];         // the caller's host array (lss_stage points it into the ring slot); null: zero fill
     unsigned long long words[MAX];
     int n = 0;
-    bool bad = false;                 // too many uploads, or a size / alignment the copy cannot take
-    ZeroRegions zero;
+    bool bad = false;                 // too many rows, or a size / alignment the copy cannot take
     void upload(void *d, const void *h, size_t bytes)
     {
         if (bytes == 0) return;
-        if (n == MAX || bytes % 4 != 0 || ((uintptr_t)d & 3) != 0) { bad = true; return; }
+        if (n == MAX || !h || bytes % 4 != 0 || ((uintptr_t)d & 3) != 0) { bad = true; return; }
         dst[n] = (uint32_t *)d; src[n] = (const uint32_t *)h; words[n] = bytes / 4; n++;
     }
+    void zero(void *d, size_t bytes)  // nothing for a null region
+    {
+        if (!d || bytes == 0) return;
+        if (n == MAX || ((uintptr_t)d & 3) != 0) { bad = true; return; }
+        dst[n] = (uint32_t *)d; src[n] = nullptr; words[n] = (bytes + 3) / 4; n++;
+    }
 };
-// grid (blocks, uploads + zero regions): row y < s.n copies upload y, the rows after it clear one zero region each.  Always
-// the first kernel of its chain (a plain launch); its dependents may be scheduled at once.
+// grid (blocks, rows of the list): row y copies upload y, or clears zero region y.  Always the first kernel of its chain (a
+// plain launch); its dependents may be scheduled at once.
 static __global__ void k_stage_copy(StageList s)
 {
     lss_pdl_trigger();
     const int r = blockIdx.y;
     const unsigned long long stride = (unsigned long long)gridDim.x * blockDim.x;
     const unsigned long long i0 = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (r < s.n) {
-        uint32_t *dst = s.dst[r];
-        const uint32_t *src = s.src[r];
+    uint32_t *dst = s.dst[r];
+    const uint32_t *src = s.src[r];
+    if (src) {
         for (unsigned long long i = i0; i < s.words[r]; i += stride) dst[i] = src[i];
     } else {
-        uint32_t *p = s.zero.p[r - s.n];
-        for (unsigned long long i = i0; i < s.zero.words[r - s.n]; i += stride) p[i] = 0u;
+        for (unsigned long long i = i0; i < s.words[r]; i += stride) dst[i] = 0u;
     }
 }
 
@@ -282,14 +278,13 @@ struct StageDone {
 inline cudaError_t lss_stage(lss_engine *e, StageList l, cudaStream_t stream, StageDone *done = nullptr)
 {
     if (l.bad) return cudaErrorInvalidValue;
-    if (l.n + l.zero.n == 0) return cudaSuccess;
+    if (l.n == 0) return cudaSuccess;
     size_t bytes = 0;
     unsigned long long mx = 0;
     for (int k = 0; k < l.n; k++) {
-        bytes += (size_t)align_up((int64_t)l.words[k] * 4, 16);
+        if (l.src[k]) bytes += (size_t)align_up((int64_t)l.words[k] * 4, 16);
         mx = l.words[k] > mx ? l.words[k] : mx;
     }
-    for (int k = 0; k < l.zero.n; k++) mx = l.zero.words[k] > mx ? l.zero.words[k] : mx;
     cudaError_t err;
     lss_engine::StageSlot *sl = nullptr;
     if (bytes) {
@@ -309,6 +304,7 @@ inline cudaError_t lss_stage(lss_engine *e, StageList l, cudaStream_t stream, St
         }
         size_t off = 0;
         for (int k = 0; k < l.n; k++) {
+            if (!l.src[k]) continue;
             char *h = (char *)sl->host + off;
             memcpy(h, l.src[k], l.words[k] * 4);
             l.src[k] = (const uint32_t *)h;
@@ -317,31 +313,13 @@ inline cudaError_t lss_stage(lss_engine *e, StageList l, cudaStream_t stream, St
     }
     const unsigned long long cap = 4ull * e->n_sm;
     const unsigned blocks = (unsigned)((mx + 1023) / 1024 < cap ? (mx + 1023) / 1024 : cap);
-    if ((err = lss_launch(e, k_stage_copy, dim3(blocks ? blocks : 1, l.n + l.zero.n), 256, 0, stream, l)) != cudaSuccess)
-        return err;
+    if ((err = lss_launch(e, k_stage_copy, dim3(blocks ? blocks : 1, l.n), 256, 0, stream, l)) != cudaSuccess) return err;
     if (!sl) return cudaSuccess;
     if (!done) return cudaEventRecord(sl->done, stream);
     if (done->ev && (err = cudaEventRecord(done->ev, done->stream)) != cudaSuccess) return err;
     done->ev = sl->done;
     done->stream = stream;
     return cudaSuccess;
-}
-
-// Asynchronous host -> device upload of one small host array (one launch; the caller's buffer may be reused as soon as
-// this returns).  `bytes` must be a multiple of 4.
-inline cudaError_t lss_stage_upload(lss_engine *e, void *dst, const void *src, size_t bytes, cudaStream_t stream)
-{
-    StageList l;
-    l.upload(dst, src, bytes);
-    return lss_stage(e, l, stream);
-}
-
-// Stream-ordered zero fill of up to ZeroRegions::MAX device regions in ONE kernel launch.
-inline cudaError_t lss_zero_async(lss_engine *e, const ZeroRegions &r, cudaStream_t stream)
-{
-    StageList l;
-    l.zero = r;
-    return lss_stage(e, l, stream);
 }
 
 enum { LSS_K_SORT = 0, LSS_K_PREPASS = 1, LSS_K_SNOWFALL = 2, LSS_K_COMPACT = 3, LSS_K_FINALIZE = 4, LSS_K_WET = 5,
@@ -410,16 +388,6 @@ inline lss_status lss_batch_geometry(lss_engine *e, const int64_t *h_cloud_offse
     }
     g.n = h_cloud_offsets[n_clouds];
     return LSS_OK;
-}
-
-// Stream-ordered upload of a batch's cloud offsets [B + 1] and tile bases (any number of int32) to the device.
-inline cudaError_t lss_stage_geometry(lss_engine *e, const int64_t *h_cloud_offsets, int n_clouds,
-                                      const std::vector<int32_t> &tile_base, int64_t *d_off, int32_t *d_tile_base,
-                                      cudaStream_t stream)
-{
-    const cudaError_t err = lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), stream);
-    if (err != cudaSuccess) return err;
-    return lss_stage_upload(e, d_tile_base, tile_base.data(), sizeof(int32_t) * tile_base.size(), stream);
 }
 
 // implemented in tables.cu
@@ -491,11 +459,10 @@ struct PrepassIO {
     // a cloud with at least this many ground points latches LSS_ERR_INTENSITY_RANGE when its I/cos range is degenerate
     // (the snowfall path fits from 3 ground points on; wet ground returns below 1000 first, augmentation.py:51-52)
     int range_min_ground = 3;
-    // the caller's staging launch already did what lss_prepass_stage adds (the pre-pass then enqueues no staging of its own)
-    bool staged = false;
 };
 // Adds the pre-pass's staging to a caller's StageList: the zero fill of its per-cloud records and the upload of io's host
-// inputs.  Folded into the caller's own staging launch (io.staged), it saves the pre-pass a launch at the head of its chain.
+// inputs.  The pre-pass enqueues no staging of its own: every caller of lss_prepass_run must have added this to its own
+// staging launch, enqueued before it.
 void lss_prepass_stage(StageList &l, const PrepassIO &io, void *d_ws, int64_t n_total, int n_clouds);
 lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_cloud_off, const int32_t *d_cloud_cnt,
                            const int64_t *h_cloud_off, int n_clouds, double delta, double noise_floor, int flat_earth,

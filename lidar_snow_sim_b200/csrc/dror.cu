@@ -354,13 +354,15 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
     a.out_pts = d_out_points;
     if (!(flags & LSS_DROR_WORK_STATS)) a.stats = nullptr;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
-                                         (int32_t *)a.tiles.tile_base, st));
-    if (a.stats) {
-        ZeroRegions z;
-        z.add(a.stats, 32);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
+    StageList l;
+    l.upload((int64_t *)a.cloud_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.tiles.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    l.zero(a.stats, 32);                                     // (null without LSS_DROR_WORK_STATS)
+    if (g.max_n == 0) {
+        l.zero(d_out_counts, sizeof(int32_t) * B);
+        l.zero(d_out_n_snow, sizeof(int32_t) * B);
     }
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     {
         KernelTimer kt(e, LSS_K_DROR, st);
         if (g.max_n > 0) {
@@ -380,11 +382,6 @@ lss_status lss_dror_batch(lss_engine *e, const float *d_points, int n_features, 
                                          a.tiles));
             LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.tiles));
             if (d_out_points) LSS_CUDA_CHECK(e, lss_launch(e, k_dror_scatter, gt, DTILE, 0, st, a));
-        } else {
-            ZeroRegions z;
-            z.add(d_out_counts, sizeof(int32_t) * B);
-            z.add(d_out_n_snow, sizeof(int32_t) * B);
-            LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
         }
     }
     return LSS_OK;

@@ -369,18 +369,16 @@ lss_status fog_run(lss_engine *e, const float *d_points, int n_features, const i
     a.mask = d_out_fog_mask;
     a.rank = d_out_rank;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
-                                         (int32_t *)a.seg.tile_base, st));
-    if (pc) LSS_CUDA_CHECK(e, lss_stage_upload(e, (double *)a.cloud_par, par.data(), par.size(), st));
+    StageList l;
+    l.upload((int64_t *)a.cloud_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    if (pc) l.upload((double *)a.cloud_par, par.data(), par.size());
     if (h_rng_state && soft && noise > 0 && noise_variant != 4 && !d_ext_noise) {
-        LSS_CUDA_CHECK(e, lss_stage_upload(e, rng, h_rng_state, sizeof(uint64_t) * 4 * B, st));
+        l.upload(rng, h_rng_state, sizeof(uint64_t) * 4 * B);
         a.rng = rng;
     }
-    {
-        ZeroRegions z;
-        z.add(a.info, (size_t)B * 4 * 8);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
-    }
+    l.zero(a.info, (size_t)B * 4 * 8);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     const dim3 grid((unsigned)((g.max_n + FOG_TILE - 1) / FOG_TILE), B);
     if (N > 0) {
         KernelTimer kt(e, LSS_K_FOG, st);

@@ -327,7 +327,9 @@ lss_status lss_fog_integral_tables(lss_engine *e, const lss_fog_table_params *h_
     cudaStream_t st = (cudaStream_t)stream;
     const size_t smem_resp = (size_t)g.n * 2 * sizeof(double);
     LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_fog_response, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_resp));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_tables, tables.data(), sizeof(LutTable) * n_tables, st));
+    StageList l;
+    l.upload(d_tables, tables.data(), sizeof(LutTable) * n_tables);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     KernelTimer kt(e, LSS_K_FOG_LUT, st);
     LSS_CUDA_CHECK(e, lss_launch(e, k_fog_response, dim3(g.n_used, n_tables), LUT_TPB, smem_resp, st, d_tables, g, d_f));
     LSS_CUDA_CHECK(e, lss_launch(e, k_fog_table, n_tables, LUT_TPB, (size_t)g.n_used * sizeof(int), st, d_tables, g,

@@ -380,6 +380,11 @@ lss_status lss_gt_paste_batch(lss_engine *e, const float *d_points, int n_featur
     WsCarve c{(char *)d_workspace};
     paste_carve(c, a, g.n, B);
     if (workspace_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "workspace too small");
+    const int64_t obj_blocks = (n_object_rows + GT_TILE - 1) / GT_TILE;
+    const int64_t scene_tiles = (g.max_n + GT_TILE - 1) / GT_TILE;
+    int64_t gx = scene_tiles > obj_blocks ? scene_tiles : obj_blocks;
+    gx = gx > 0 ? gx : 1;                                     // block (0, B) writes the counts
+    if (gx > INT32_MAX) return lss_fail(e, LSS_ERR_INVALID_ARG, "too many object rows");
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     a.pts = d_points; a.F = n_features; a.cnt = d_cloud_counts;
@@ -388,22 +393,16 @@ lss_status lss_gt_paste_batch(lss_engine *e, const float *d_points, int n_featur
     a.out_off = d_out_offsets; a.n_obj_rows_b = d_object_rows;
     a.seg.total[0] = a.kept;
     a.out = d_out; a.counts = d_counts;
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * (B + 1), st));
-    const int64_t obj_blocks = (n_object_rows + GT_TILE - 1) / GT_TILE;
-    const int64_t scene_tiles = (g.max_n + GT_TILE - 1) / GT_TILE;
+    StageList l;
+    l.upload((int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * (B + 1));
+    if (g.max_n == 0) l.zero(a.kept, sizeof(int32_t) * (size_t)B);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     if (g.max_n > 0) {
         LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_gt_mark, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         LSS_CUDA_CHECK(e, lss_launch(e, k_gt_mark, dim3((unsigned)scene_tiles, B), GT_TILE, smem, st, a));
         LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<1>, B, SEG_SCAN_TPB, 0, st, a.seg));
-    } else {
-        ZeroRegions z;
-        z.add(a.kept, sizeof(int32_t) * (size_t)B);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
-    int64_t gx = scene_tiles > obj_blocks ? scene_tiles : obj_blocks;
-    gx = gx > 0 ? gx : 1;                                     // block (0, B) writes the counts
-    if (gx > INT32_MAX) return lss_fail(e, LSS_ERR_INVALID_ARG, "too many object rows");
     LSS_CUDA_CHECK(e, lss_launch(e, k_gt_paste, dim3((unsigned)gx, B + 1), GT_TILE, 0, st, a, B));
     return LSS_OK;
 }

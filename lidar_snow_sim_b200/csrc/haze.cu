@@ -431,11 +431,14 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
     a.out_label = out_label ? 1 : 0;
     a.out_cnt = d_out_counts;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.off, (int32_t *)a.det.tile_base,
-                                         st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.out_off, out_off.data(), sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (double *)a.beta, h_beta, sizeof(double) * B, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_state, h_mt_state, sizeof(uint32_t) * (MT_N + 1), st));
+    StageList l;
+    l.upload((int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.det.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    l.upload((int64_t *)a.out_off, out_off.data(), sizeof(int64_t) * (B + 1));
+    l.upload((double *)a.beta, h_beta, sizeof(double) * B);
+    l.upload(d_state, h_mt_state, sizeof(uint32_t) * (MT_N + 1));
+    if (g.max_n == 0) l.zero(tot, sizeof(int32_t) * 6 * B);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     LSS_CUDA_CHECK(e, lss_launch(e, k_hz_stream, 1, MT_TPB, 0, st, (const uint32_t *)d_state,
                                  (int)hz_stream_blocks(g.max_n), (uint32_t *)a.stream));
     const dim3 gt((unsigned)(g.max_n > 0 ? (g.max_n + HTILE - 1) / HTILE : 1), B);
@@ -448,10 +451,6 @@ lss_status lss_haze_batch(lss_engine *e, const float *d_points, int n_features, 
         LSS_CUDA_CHECK(e, lss_launch(e, k_hz_scatter, gt, HTILE, 0, st, a));
         LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<1>, B, SEG_SCAN_TPB, 0, st, a.kept));
         LSS_CUDA_CHECK(e, lss_launch(e, k_hz_kept, gt, HTILE, 0, st, a));
-    } else {
-        ZeroRegions z;
-        z.add(tot, sizeof(int32_t) * 6 * B);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
     LSS_CUDA_CHECK(e, lss_launch(e, k_hz_chain, B, MT_TPB, 0, st, a, sa.J, d_mt_state_out));
     sa.cloud_off = a.off;

@@ -223,9 +223,9 @@ extern "C" lss_status lss_snowfall_batch_host_submit(lss_engine *e, int table_id
     int *const engine_status = e->d_status;
     e->d_status = sl.d_status;                       // the kernels of this batch latch their errors per slot
     {
-        ZeroRegions z;
-        z.add(sl.d_status, sizeof(int));
-        ce = lss_zero_async(e, z, p->s_h2d);         // ordered before every chunk's "rows landed" event
+        StageList l;
+        l.zero(sl.d_status, sizeof(int));
+        ce = lss_stage(e, l, p->s_h2d);              // ordered before every chunk's "rows landed" event
         if (ce == cudaSuccess) ce = cudaEventRecord(sl.ev_start, p->s_h2d);
         if (ce != cudaSuccess) rc = lss_fail(e, LSS_ERR_CUDA, cudaGetErrorString(ce));
     }

@@ -453,9 +453,15 @@ extern "C" lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points,
     a.seg.total[1] = d_out_n_lost;
     a.out = d_out_points;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
-                                         (int32_t *)a.seg.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (LisaCloud *)a.cloud, cloud.data(), sizeof(LisaCloud) * cloud.size(), st));
+    StageList l;
+    l.upload((int64_t *)a.cloud_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    l.upload((LisaCloud *)a.cloud, cloud.data(), sizeof(LisaCloud) * cloud.size());
+    if (g.max_n == 0) {
+        l.zero(d_out_counts, sizeof(int32_t) * B);
+        l.zero(d_out_n_lost, sizeof(int32_t) * B);
+    }
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     KernelTimer kt(e, LSS_K_LISA, st);
     if (g.max_n > 0) {
         const unsigned blocks = (unsigned)std::min<long long>((N + 7) / 8, (long long)e->n_sm * 64);
@@ -465,11 +471,6 @@ extern "C" lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points,
                                      a.cloud_off, a.cloud_cnt, a.seg));
         LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.seg));
         LSS_CUDA_CHECK(e, lss_launch(e, k_lisa_scatter, gt, LISA_TILE, 0, st, a));
-    } else {
-        ZeroRegions z;
-        z.add(d_out_counts, sizeof(int32_t) * B);
-        z.add(d_out_n_lost, sizeof(int32_t) * B);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
     return LSS_OK;
 }

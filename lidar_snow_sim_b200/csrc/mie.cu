@@ -181,7 +181,9 @@ lss_status lss_mie_tables(lss_engine *e, const double *h_refractive_index, const
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     const int n_rows = (int)P.rows.size();
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_rows, P.rows.data(), sizeof(MieRow) * P.rows.size(), st));
+    StageList l;
+    l.upload(d_rows, P.rows.data(), sizeof(MieRow) * P.rows.size());
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     KernelTimer kt(e, LSS_K_MIE, st);
     LSS_CUDA_CHECK(e, lss_launch(e, k_mie, (n_rows + MIE_TPB - 1) / MIE_TPB, MIE_TPB, 0, st, (const MieRow *)d_rows, n_rows,
                                  d_d, d_out));

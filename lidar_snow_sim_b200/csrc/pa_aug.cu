@@ -505,10 +505,13 @@ lss_status lss_pa_partition_batch(lss_engine *e, const float *d_points, int n_fe
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     a.totals = d_class_totals;
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.box_off, h_box_offsets, sizeof(int64_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int32_t *)a.tile_base, tile_base.data(), sizeof(int32_t) * (B + 1), st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.tc_base, tc_base.data(), sizeof(int64_t) * (B + 1), st));
+    StageList l;
+    l.upload((int64_t *)a.off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int64_t *)a.box_off, h_box_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.tile_base, tile_base.data(), sizeof(int32_t) * (B + 1));
+    l.upload((int64_t *)a.tc_base, tc_base.data(), sizeof(int64_t) * (B + 1));
+    if (g.max_n == 0) l.zero(d_class_totals, sizeof(int32_t) * (size_t)(h_box_offsets[B] * PA_PARTS + B));
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     KernelTimer kt(e, LSS_K_PA, st);
     if (g.max_n > 0) {
         const size_t smem = pa_smem_bytes(max_boxes, false);
@@ -516,10 +519,6 @@ lss_status lss_pa_partition_batch(lss_engine *e, const float *d_points, int n_fe
         const dim3 gt((unsigned)((g.max_n + PA_TILE - 1) / PA_TILE), B);
         LSS_CUDA_CHECK(e, lss_launch(e, k_pa_count, gt, PA_TILE, smem, st, a));
         LSS_CUDA_CHECK(e, lss_launch(e, k_pa_scan, B, 1024, 0, st, a));
-    } else {
-        ZeroRegions z;
-        z.add(d_class_totals, sizeof(int32_t) * (size_t)(h_box_offsets[B] * PA_PARTS + B));
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
     return LSS_OK;
 }

@@ -749,7 +749,7 @@ void lss_prepass_stage(StageList &l, const PrepassIO &io, void *d_ws, int64_t n_
     double *d_plane;
     int32_t *d_ymins_in;
     prepass_carve(c, a, d_plane, d_ymins_in, n_total, n_clouds);
-    l.zero.add(a.cp, (size_t)((char *)a.rec_cnt - (char *)a.cp) + sizeof(int) * n_clouds);   // records and record cursors
+    l.zero(a.cp,(size_t)((char *)a.rec_cnt - (char *)a.cp) + sizeof(int) * n_clouds);   // records and record cursors
     if (io.h_ymins_in) l.upload(d_ymins_in, io.h_ymins_in, sizeof(int32_t) * HIST_NX * n_clouds);
     if (io.h_plane_in) l.upload(d_plane, io.h_plane_in, sizeof(double) * 4 * n_clouds);
 }
@@ -791,7 +791,8 @@ lss_status lss_prepass_check(lss_engine *e, const int64_t *h_cloud_off, int n_cl
     return LSS_ERR_INVALID_ARG;
 }
 
-// Runs the whole pre-pass for a batch.  d_poly_out / d_plane_out: device [B*3] / [B*4] (either may be null).
+// Runs the whole pre-pass for a batch.  The caller must have added lss_prepass_stage to its own staging launch, enqueued on
+// `stream` before this.  d_poly_out / d_plane_out: device [B*3] / [B*4] (either may be null).
 // h_plane_in: optional host [B*4] (w0, w1, w2, h) to use instead of the RANSAC estimate.
 // d_cloudpre_out: optional device pointer receiving the address of the per-cloud CloudPre records (for wet ground).
 lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_cloud_off, const int32_t *d_cloud_cnt,
@@ -826,11 +827,6 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     if (cloudpre_out) *cloudpre_out = a.cp;
     const int64_t max_n = largest_cloud(h_cloud_off, B);
     int nblk = (int)std::min<int64_t>(a.max_blocks, std::max<int64_t>(1, (max_n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
-    if (!io.staged) {
-        StageList l;
-        lss_prepass_stage(l, io, d_ws, N, B);
-        LSS_CUDA_CHECK(e, lss_stage(e, l, stream));
-    }
     // Plain launches: next to the scan, a PDL chain here would park each kernel's CTAs on the SMs while the one before
     // it runs, at the side stream's high priority, and the step measured slower (DESIGN.md section 8)
     {

@@ -171,7 +171,9 @@ lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_cloud_offset
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     int64_t *d_off = (int64_t *)sa.cloud_off;
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1), st));
+    StageList l;
+    l.upload(d_off, h_cloud_offsets, sizeof(int64_t) * (n_clouds + 1));
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     return run_permutations(e, d_off, d_cloud_counts, n_clouds, g.max_n, h_mt_state, d_mt_state_out, sa.J, d_out_perm,
                             sa.R, st);
 }
@@ -232,7 +234,10 @@ lss_status lss_processor_batch(lss_engine *e, const float *d_points, int n_featu
     ea.seg.total[0] = d_out_counts;
     if (!shuffle) ea.out = d_out_points;
     if (B > 0) {
-        LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, d_off, (int32_t *)ea.seg.tile_base, st));
+        StageList l;
+        l.upload(d_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+        l.upload((int32_t *)ea.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+        LSS_CUDA_CHECK(e, lss_stage(e, l, st));
         const dim3 gt((unsigned)(g.max_n > 0 ? (g.max_n + PTILE - 1) / PTILE : 1), B);
         LSS_CUDA_CHECK(e, lss_launch(e, k_enc_count, gt, PTILE, 0, st, ea));
         LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<1>, B, SEG_SCAN_TPB, 0, st, ea.seg));

@@ -356,9 +356,11 @@ lss_status lss_strongest_last_batch(lss_engine *e, const float *d_last, const in
     a.seg.total[1] = nullptr;
     a.out = d_out_points;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, off_o.data(), B, go.tile_base, (int64_t *)a.off_o,
-                                         (int32_t *)a.seg.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int64_t *)a.off_l, off_in.data(), sizeof(int64_t) * off_in.size(), st));
+    StageList l;
+    l.upload((int64_t *)a.off_o, off_o.data(), sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.seg.tile_base, go.tile_base.data(), sizeof(int32_t) * go.tile_base.size());
+    l.upload((int64_t *)a.off_l, off_in.data(), sizeof(int64_t) * off_in.size());
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     KernelTimer kt(e, LSS_K_SELECT, st);
     const dim3 grow((unsigned)std::max<int64_t>((go.max_n + SBLOCK - 1) / SBLOCK, 1), B);
     LSS_CUDA_CHECK(e, lss_launch(e, k_sl_key, grow, SBLOCK, 0, st, a));
@@ -425,19 +427,18 @@ lss_status lss_camera_fov_batch(lss_engine *e, const float *d_points, int n_feat
     a.seg.total[1] = nullptr;
     a.out = d_out_points;
 
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
-                                         (int32_t *)a.seg.tile_base, st));
-    LSS_CUDA_CHECK(e, lss_stage_upload(e, (int2 *)a.shape, shape.data(), sizeof(int32_t) * shape.size(), st));
+    StageList l;
+    l.upload((int64_t *)a.cloud_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    l.upload((int2 *)a.shape, shape.data(), sizeof(int32_t) * shape.size());
+    if (g.max_n == 0) l.zero(d_out_counts, sizeof(int32_t) * B);
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     KernelTimer kt(e, LSS_K_SELECT, st);
     if (g.max_n > 0) {
         const dim3 gt((unsigned)((g.max_n + STILE - 1) / STILE), B);
         LSS_CUDA_CHECK(e, lss_launch(e, k_fov, gt, STILE, 0, st, a));
         LSS_CUDA_CHECK(e, lss_launch(e, k_seg_scan<2>, B, SEG_SCAN_TPB, 0, st, a.seg));
         LSS_CUDA_CHECK(e, lss_launch(e, k_fov_scatter, gt, STILE, 0, st, a));
-    } else {
-        ZeroRegions z;
-        z.add(d_out_counts, sizeof(int32_t) * B);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
     }
     return LSS_OK;
 }

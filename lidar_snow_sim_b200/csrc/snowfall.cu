@@ -442,21 +442,20 @@ lss_status lss_snowfall_run(lss_engine *e, const SnowfallArgs &s, cudaStream_t s
     l.upload(d_tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
     l.upload(d_order, s.h_order, sizeof(int32_t) * B * LSS_N_CHANNELS);
     if (s.h_thresh_poly) l.upload(d_thresh, s.h_thresh_poly, sizeof(double) * 3 * B);
-    l.zero.add(a.counters, counters_bytes(B));
-    l.zero.add(s.d_out_stats, sizeof(double) * 4 * B);
+    l.zero(a.counters, counters_bytes(B));
+    l.zero(s.d_out_stats, sizeof(double) * 4 * B);
     if (N == 0 || B == 0) {
-        l.zero.add(s.d_out_counts, sizeof(int32_t) * B);
+        l.zero(s.d_out_counts, sizeof(int32_t) * B);
         LSS_CUDA_CHECK(e, lss_stage(e, l, stream, &stage_done));
         return LSS_OK;
     }
-    l.zero.add(a.hdr, LIST_HDR_BYTES);                     // (the tile histograms are written whole by k_keep)
-    l.zero.add(a.chunk_tab, (size_t)LIST_CLASSES * a.chunks_per_class * 4);
-    l.zero.add(d_sched_hist, (size_t)SCHED_BINS * 2 * 4);
+    l.zero(a.hdr, LIST_HDR_BYTES);                     // (the tile histograms are written whole by k_keep)
+    l.zero(a.chunk_tab, (size_t)LIST_CLASSES * a.chunks_per_class * 4);
+    l.zero(d_sched_hist, (size_t)SCHED_BINS * 2 * 4);
     PrepassIO io;
     io.h_plane_in = s.h_plane_in;
     io.h_ymins_in = s.h_ymins_in;
     io.d_poly_out = d_thresh;
-    io.staged = true;
     if (device_prepass) lss_prepass_stage(l, io, d_prepass_ws, N, B);
     LSS_CUDA_CHECK(e, lss_stage(e, l, stream, &stage_done));
 

@@ -260,8 +260,10 @@ lss_status lss_voxelize_batch(lss_engine *e, const float *d_points, int n_featur
 
     const size_t n_vox_all = (size_t)B * max_voxels;
     if (B == 0) return LSS_OK;
-    LSS_CUDA_CHECK(e, lss_stage_geometry(e, h_cloud_offsets, B, g.tile_base, (int64_t *)a.cloud_off,
-                                         (int32_t *)a.seg.tile_base, st));
+    StageList l;
+    l.upload((int64_t *)a.cloud_off, h_cloud_offsets, sizeof(int64_t) * (B + 1));
+    l.upload((int32_t *)a.seg.tile_base, g.tile_base.data(), sizeof(int32_t) * g.tile_base.size());
+    LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     {
         KernelTimer kt(e, LSS_K_VOXEL, st);
         const unsigned long long n_slots = (unsigned long long)vox_slots(N, B);

@@ -175,9 +175,9 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     DeviceGuard dg(e->device);
     cudaStream_t st = (cudaStream_t)stream;
     if (B == 0 || N == 0) {
-        ZeroRegions z;
-        z.add(d_out_counts, sizeof(int32_t) * B);
-        LSS_CUDA_CHECK(e, lss_zero_async(e, z, st));
+        StageList l;
+        l.zero(d_out_counts, sizeof(int32_t) * B);
+        LSS_CUDA_CHECK(e, lss_stage(e, l, st));
         return LSS_OK;
     }
     if (!d_points) return lss_fail(e, LSS_ERR_INVALID_ARG, "null points");
@@ -196,7 +196,6 @@ lss_status wet_ground_run(lss_engine *e, const float *d_points, const int64_t *h
     io.d_fit_out = d_out_fit;
     io.d_ymins_out = d_out_ymins;
     io.range_min_ground = latch_range ? 1000 : INT_MAX;                       // augmentation.py:51-52 returns first
-    io.staged = true;
     // One staging launch heads the call's chain: offsets, tile bases, wetness per cloud and the pre-pass's staging.  Its
     // ring slot is released after the call's last launch.
     StageDone stage_done;

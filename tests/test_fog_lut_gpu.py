@@ -181,11 +181,11 @@ def test_batch_params_rejects_bad_table_index(engine):
                                 [p.beta_0] * 3, [0, 0, 0])
 
 
-@pytest.mark.parametrize('name,expected', [('tables', 3), ('batch_params', 9)])
+@pytest.mark.parametrize('name,expected', [('tables', 3), ('batch_params', 6)])
 def test_launch_count(engine, name, expected):
     """lss_launch_count() rises by the kernels a call enqueues: the table generator uploads its parameters and runs
-    k_fog_response + k_fog_table; the per-cloud batch adds one parameter upload to lss_fog_batch's launches (offsets,
-    tile bases, zero fill, count, scan, apply, gain, info)."""
+    k_fog_response + k_fog_table; the per-cloud batch stages its offsets, tile bases, per-cloud parameters and zero fill
+    in one launch, then runs count, scan, apply, gain, info."""
     clouds = _clouds()
     off = np.concatenate([[0], np.cumsum([c.shape[0] for c in clouds])]).astype(np.int64)
     pts = torch.from_numpy(np.concatenate(clouds)).cuda()

@@ -244,8 +244,8 @@ def test_argument_errors(engine):
         engine.strongest_last_batch(pc, np.array([0, n // 2, n // 3, n]), pc, np.array([0, 1, 2, n]))
 
 
-def test_launch_count_is_fixed(engine):
-    """strongest / last: 3 staging copies + key, sort (one), match, count, scan, scatter; FOV: 3 staging copies + 3
+def test_launch_count_stages_once(engine):
+    """strongest / last: 1 staging launch + key, sort (one), match, count, scan, scatter; FOV: 1 staging launch + 3
     kernels -- whatever the batch."""
     for clouds in ([G['ps__subset']], [G['ps__dups'], G['ps__wrap'], G['ps__equal']]):
         pts = torch.from_numpy(np.concatenate(clouds)).cuda()
@@ -254,8 +254,8 @@ def test_launch_count_is_fixed(engine):
         pl = torch.from_numpy(np.concatenate(half)).cuda()
         before = engine.launch_count()
         engine.strongest_last_batch(pl, _offsets(half), pts, off)
-        assert engine.launch_count() - before == 9
+        assert engine.launch_count() - before == 7
         before = engine.launch_count()
         engine.camera_fov_batch(pts, off)
-        assert engine.launch_count() - before == 6
+        assert engine.launch_count() - before == 4
     engine.check()
