@@ -477,6 +477,46 @@ LSS_API lss_status lss_mt19937_permutations(lss_engine *e, const int64_t *h_clou
                                             uint32_t *d_mt_state_out, void *d_workspace, int64_t workspace_bytes,
                                             void *stream);
 
+/* ---- DATA_PROCESSOR: sample_points, and the farthest distance of FILTER_OUT_OF_MOR_BOXES ------------------------------
+ * DataProcessor.sample_points (data_processor.py:145-175) with NUM_POINTS k >= 0 on NumPy's legacy RandomState, for every
+ * cloud of a batch, optionally followed by shuffle_points (data_processor.py:93-103).  Per cloud of n rows with F rows whose
+ * distance np.linalg.norm(xyz) is not < 40 (NaN and inf included): k < n draws permutation(n - F) when k > F (the near
+ * rows' choice, then every far row), else permutation(n); k > n draws permutation(n) for the k - n extra rows; then
+ * np.random.shuffle of the k chosen indices, and with shuffle != 0 permutation(k).  A cloud with n == 0 < k or k - n > n
+ * is where the reference raises ValueError, before that cloud draws anything.
+ *   d_points         float32 (f64 == 0) or float64 rows [n_total * n_features], n_features >= 3 (x, y, z first)
+ *   d_cloud_counts   int32[n_clouds] device or NULL: valid rows per slot
+ *   h_f32_distance   int32[n_clouds] or NULL: with float64 rows, != 0 -> the cloud's distances in float32 (rows that hold
+ *                    float32 values where the reference's rows are float32); float32 rows always use float32
+ *   num_points       k in [0, 2^30); -1 (rows unchanged) is the caller's
+ *   h_run_offsets    int32[n_runs + 1], 0 .. n_clouds non-decreasing: run r is clouds [h_run_offsets[r], [r + 1]), whose
+ *                    draws continue one another from h_run_states[r]
+ *   h_run_states     uint32[n_runs * 625]: each run's start state, np.random.get_state()'s 624 key words then pos
+ *   d_out_points     rows of d_points' type [n_clouds * k * n_features]: cloud b's k rows at row b * k (undefined for a
+ *                    failing cloud and the later clouds of its run)
+ *   d_run_states_out uint32[n_runs * 625] device: each run's state after its last draw; at its first failing cloud, the
+ *                    state before that cloud
+ *   d_run_status     int32[2 * n_runs] device: per run the first failing cloud (-1: none) and the reason: 1 'a' cannot be
+ *                    empty unless no samples are taken, 2 Cannot take a larger sample than population when 'replace=False'
+ *   d_workspace      lss_sample_points_workspace_bytes(n_total, n_clouds, num_points, n_runs) bytes
+ * Asynchronous on `stream`, no synchronisation.                                                                           */
+LSS_API lss_status lss_sample_points_batch(lss_engine *e, const void *d_points, int f64, int n_features,
+                                           const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts, int n_clouds,
+                                           const int32_t *h_f32_distance, int num_points, int shuffle,
+                                           const int32_t *h_run_offsets, int n_runs, const uint32_t *h_run_states,
+                                           void *d_out_points, uint32_t *d_run_states_out, int32_t *d_run_status,
+                                           void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_sample_points_workspace_bytes(int64_t n_total, int n_clouds, int num_points, int n_runs);
+/* max(np.linalg.norm(points[:, 0:3], axis=1)) per cloud with Python's builtin max (dense_dataset.py:930): NaN when row 0's
+ * distance is NaN, else the largest non-NaN distance; -1 for an empty cloud (where builtin max raises ValueError).
+ * Arguments as lss_sample_points_batch; d_out_max float64[n_clouds] device; d_workspace
+ * lss_farthest_distance_workspace_bytes(n_clouds) bytes.  Asynchronous on `stream`.                                      */
+LSS_API lss_status lss_farthest_distance_batch(lss_engine *e, const void *d_points, int f64, int n_features,
+                                               const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts,
+                                               int n_clouds, const int32_t *h_f32_distance, double *d_out_max,
+                                               void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_farthest_distance_workspace_bytes(int n_clouds);
+
 /* ---- DENSE fog: haze_point_cloud -----------------------------------------------------------------------------------------
  * haze_point_cloud (lib/LiDAR_fog_sim/SeeingThroughFog/tools/DatasetFoggification/lidar_foggification.py:61-149) with
  * BetaRadomization.get_beta (beta_modification.py:116-147) for every cloud of a batch, every cloud drawing from the same

@@ -118,6 +118,12 @@ SIGNATURES = [
                                        _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_processor_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int, _c.c_int]),
     ('lss_mt19937_permutations', _c.c_int, [_P, _P, _P, _c.c_int, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_sample_points_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _c.c_int, _c.c_int, _P,
+                                           _c.c_int, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_sample_points_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int]),
+    ('lss_farthest_distance_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _c.c_int64,
+                                               _P]),
+    ('lss_farthest_distance_workspace_bytes', _c.c_int64, [_c.c_int]),
     ('lss_haze_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double,
                                   _c.c_double, _c.c_double, _P, _P, _c.c_int, _c.c_int, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_haze_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),

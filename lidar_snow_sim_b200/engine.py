@@ -568,6 +568,94 @@ class SnowfallEngine:
         _set_mt_state(state, out['state'])
         return out['perm']
 
+    def sample_points_batch(self, points, cloud_offsets, num_points, counts=None, shuffle=False, run_starts=None,
+                            run_states=None, f32_distance=None):
+        """
+        DataProcessor.sample_points (data_processor.py:145-175) with NUM_POINTS = num_points (>= 0) on NumPy's legacy
+        RandomState for every cloud, followed by shuffle_points' np.random.permutation when shuffle (lss_sample_points_batch,
+        current stream).  points: CUDA float32 or float64 (N, F >= 3); counts: optional CUDA int32 (B,) valid rows per
+        slot.  The clouds draw in batch order from NumPy's global state, or in runs: run_starts (R,) the first cloud of each
+        run (0 first, increasing) and run_states R np.random.get_state() tuples, each run continuing from its own state.
+        f32_distance: optional host bool (B,), with float64 rows: the clouds whose near / far test is taken in float32 (rows
+        holding float32 values).  Returns dict(points (B * num_points, F) of points' dtype, offsets num_points *
+        arange(B + 1) host int64, counts (B,) int32 CUDA, states (R, 625) uint32 host: each run's final key and pos).
+        The call synchronises once, for the copy of the final states and the status; NumPy's global state is then the last
+        run's (the cached Gaussian as that run's start state has it).  Where the reference raises ValueError (a cloud with
+        no rows and num_points > 0, or more than twice its rows), this raises it for the first such cloud, with NumPy's
+        state as it was before that cloud's draws.
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        if not (isinstance(points, torch.Tensor) and points.dtype in (torch.float32, torch.float64)):
+            raise ValueError('points: expected a float32 or float64 CUDA tensor')
+        _check_tensor('points', points, self.device, points.dtype, (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        k = int(num_points)
+        if not 0 <= k < 2 ** 30:
+            raise ValueError(f'num_points must be in [0, 2^30), got {k}')
+        if run_starts is None:
+            starts = np.zeros(1, np.int64)
+            run_states = [np.random.get_state()] if run_states is None else list(run_states)
+        else:
+            starts = np.ascontiguousarray(run_starts, dtype=np.int64).reshape(-1)
+            run_states = list(run_states or [])
+        R = starts.shape[0]
+        if (len(run_states) != R or starts[0] != 0 or np.any(np.diff(starts) <= 0) or starts[-1] >= max(B, 1)):
+            raise ValueError('run_starts: 0 first, increasing, below the number of clouds, one state per run')
+        words = np.empty((R, 625), np.uint32)
+        for r, st in enumerate(run_states):
+            if st[0] != 'MT19937' or not 0 <= int(st[2]) <= 624:
+                raise ValueError('run_states: MT19937 np.random.get_state() tuples with pos in [0, 624]')
+            words[r, :624] = np.asarray(st[1], dtype=np.uint32)
+            words[r, 624] = int(st[2])
+        run_off = np.append(starts, B).astype(np.int32)
+        f32 = None
+        if f32_distance is not None:
+            f32 = np.ascontiguousarray(f32_distance, dtype=np.int32).reshape(-1)
+            if f32.shape[0] != B:
+                raise ValueError(f'f32_distance: expected {B} flags, got {f32.shape[0]}')
+        F = points.shape[1]
+        out = _outputs(None, self.device, points=((B * k, F), points.dtype))
+        tail = torch.empty(R * 627, dtype=torch.int32, device=self.device)     # states then status: one copy back
+        ws = self._scratch('sample_points', self.lib.lss_sample_points_workspace_bytes(N, B, k, R))
+        self._call('lss_sample_points_batch', points, 1 if points.dtype == torch.float64 else 0, F, _ptr(off), counts, B,
+                   _ptr(f32), k, 1 if shuffle else 0, _ptr(run_off), R, _ptr(words), out['points'], tail[:R * 625],
+                   tail[R * 625:], ws, ws.numel())
+        h = tail.cpu().numpy()
+        states = h[:R * 625].view(np.uint32).reshape(R, 625)
+        status = h[R * 625:].reshape(R, 2)
+        failed = [r for r in range(R) if status[r, 0] >= 0]
+        last = min(failed, key=lambda r: status[r, 0]) if failed else R - 1
+        _, _, _, has_gauss, gauss = run_states[last]
+        np.random.set_state(('MT19937', states[last, :624].copy(), int(states[last, 624]), has_gauss, gauss))
+        if failed:
+            raise ValueError("'a' cannot be empty unless no samples are taken" if status[last, 1] == 1 else
+                             "Cannot take a larger sample than population when 'replace=False'")
+        return {'points': out['points'], 'offsets': np.arange(B + 1, dtype=np.int64) * k,
+                'counts': torch.full((B,), k, dtype=torch.int32, device=self.device), 'states': states}
+
+    def farthest_distance_batch(self, points, cloud_offsets, counts=None, f32_distance=None):
+        """
+        max(np.linalg.norm(points[:, 0:3], axis=1)) of every cloud with Python's builtin max, as FILTER_OUT_OF_MOR_BOXES
+        takes it (dense_dataset.py:930; lss_farthest_distance_batch, current stream): NaN when row 0's distance is NaN,
+        else the largest non-NaN distance; -1 for an empty cloud.  points, counts, f32_distance as sample_points_batch.
+        Returns a CUDA float64 (B,) tensor; float32 distances are exact in it.
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        if not (isinstance(points, torch.Tensor) and points.dtype in (torch.float32, torch.float64)):
+            raise ValueError('points: expected a float32 or float64 CUDA tensor')
+        _check_tensor('points', points, self.device, points.dtype, (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        f32 = None
+        if f32_distance is not None:
+            f32 = np.ascontiguousarray(f32_distance, dtype=np.int32).reshape(-1)
+            if f32.shape[0] != B:
+                raise ValueError(f'f32_distance: expected {B} flags, got {f32.shape[0]}')
+        out = torch.empty(B, dtype=torch.float64, device=self.device)
+        ws = self._scratch('farthest', self.lib.lss_farthest_distance_workspace_bytes(B))
+        self._call('lss_farthest_distance_batch', points, 1 if points.dtype == torch.float64 else 0, points.shape[1],
+                   _ptr(off), counts, B, _ptr(f32), out, ws, ws.numel())
+        return out
+
     def haze_batch(self, points, cloud_offsets, beta, fourier, noise_level=0.04, gain=0.45, dmin=2.0,
                    fraction_random=0.05, counts=None, state=None, angle=None, out_dtype=torch.float32, label=False):
         """

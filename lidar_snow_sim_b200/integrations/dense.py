@@ -358,6 +358,7 @@ class FogAugmentation:
         r = fog.batch(points, offsets, counts)            # FOG_AUGMENTATION, before the row selection and LISA
         ...                                               # r['mor'] feeds data_augmentor_batch(mor=...) / LIMIT_BY_MOR
         r2 = fog.after_batch(rows, offsets, counts)       # FOG_AUGMENTATION_AFTER, on prepare_data_batch's rows
+                                                          # (processor=proc: and sample_points again, for PointRCNN)
 
     DENSE: the reference reads FOG_AUGMENTATION's clouds from files pre-computed per alpha
     (`<lidar_folder>_DENSE_beta_<alpha>/<id>.bin`, :969-975); here haze_point_cloud is computed on the device for both
@@ -455,11 +456,20 @@ class FogAugmentation:
         res.update(mor=mor, alpha=alphas, method=methods)
         return res
 
-    def after_batch(self, points, cloud_offsets, counts=None, training=True, out_dtype=None):
+    def after_batch(self, points, cloud_offsets, counts=None, training=True, out_dtype=None, processor=None):
         """
         FOG_AUGMENTATION_AFTER (dense_dataset.py:906-918): foggify(on_the_fly=True) with the alphas the last batch()
         drew for the same samples, on prepare_data_batch's rows (whose voxels were made before, so these rows do not
         reach them, as in the reference).  Returns dict(points, offsets, counts) as batch().
+        processor: the dataset's DataProcessor.  When its queue has sample_points (NUM_POINTS k != -1, PointRCNN), every
+        cloud is then resampled to k rows as the reference does "because DENSE augmentation randomly drops points"
+        (:911-918): cloud b's rows at row b * k (offsets k * arange(B + 1)), and 'f32_distance' (host bool (B,)) marks
+        the clouds whose rows the reference holds in float32: the clear clouds, and the CVL clouds when FOG_SOFT is
+        false (simulate_fog's hard fog keeps the input's float32; its soft fog, the default, and haze_point_cloud return
+        float64).  The near / far test of each cloud is taken in that precision.  A DENSE-fogged cloud reseeds NumPy,
+        so its draws start from its haze's final state; every other cloud continues from the cloud before it, the first
+        from NumPy's state on entry.  NumPy's state ends as after the last cloud's draws.  The rows are exact with
+        out_dtype=torch.float64, as the reference keeps them.
         """
         import torch
         out_dtype = torch.float32 if out_dtype is None else out_dtype
@@ -469,7 +479,21 @@ class FogAugmentation:
         alphas, methods = self._last
         if len(alphas) != off.shape[0] - 1:
             raise ValueError(f'after_batch: {off.shape[0] - 1} clouds, the last batch() drew {len(alphas)} samples')
-        return self._foggify(points, off, counts, alphas, methods, out_dtype)
+        k = None if processor is None else processor.num_points()
+        if k is None or k == -1:
+            return self._foggify(points, off, counts, alphas, methods, out_dtype)
+        entry = np.random.get_state()                   # before BetaRadomization(seed=0) reseeds NumPy
+        res, dense, haze_states = self._foggify(points, off, counts, alphas, methods, torch.float64, want_states=True)
+        gauss = np.random.get_state()[3:]               # a haze's: the reseed clears the cached Gaussian
+        starts = sorted({0} | set(np.flatnonzero(dense).tolist()))
+        states = [('MT19937', haze_states[b][:624].copy(), int(haze_states[b][624])) + gauss if dense[b] else entry
+                  for b in starts]
+        fogged = np.array([a is not None and a != '0.000' for a in alphas], dtype=bool)
+        soft = bool(_cvl_options(self.cfg)[0])
+        f32 = ~fogged | (~dense & (not soft))             # clear clouds; CVL clouds when only the hard fog runs
+        r = self._engine().sample_points_batch(res['points'], res['offsets'], k, counts=res['counts'],
+                                               run_starts=starts, run_states=states, f32_distance=f32)
+        return dict(points=r['points'].to(out_dtype), offsets=r['offsets'], counts=r['counts'], f32_distance=f32)
 
     @staticmethod
     def _passthrough(points, off, counts, out_dtype):
@@ -478,7 +502,9 @@ class FogAugmentation:
             counts = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
         return dict(points=points.to(out_dtype), offsets=off, counts=counts)
 
-    def _foggify(self, points, off, counts, alphas, methods, out_dtype):
+    def _foggify(self, points, off, counts, alphas, methods, out_dtype, want_states=False):
+        """the fog of every cloud; with want_states also the DENSE-fogged clouds' mask and their haze's final states
+        (cloud index -> uint32 (625,))"""
         import torch
         B = off.shape[0] - 1
         if not (isinstance(points, torch.Tensor) and points.is_cuda and points.dtype == torch.float32 and
@@ -500,6 +526,7 @@ class FogAugmentation:
             dst, _ = _slot_rows(new_off, slot, ~dense, dev)
             out[dst] = points[src].to(out_dtype)
         eng = self._engine()
+        haze_states = {}
         if dense.any():
             sel = np.flatnonzero(dense)
             rows, sub = _slot_rows(off, slot, dense, dev)
@@ -512,6 +539,7 @@ class FogAugmentation:
             dst, _ = _slot_rows(new_off, new_slot, dense, dev)
             out[dst] = r['points']
             out_counts[b_dev] = r['counts']
+            haze_states = dict(zip(sel.tolist(), r['states']))
         if cvl.any():
             sel = np.flatnonzero(cvl)
             valid = counts.cpu().numpy().astype(np.int64)
@@ -521,7 +549,34 @@ class FogAugmentation:
             res = simulate_fog_batch_device(ps, points[src].contiguous(), sub, 10, gain, variant, hard, soft, engine=eng)
             dst, _ = _slot_rows(new_off, valid, cvl, dev)
             out[dst] = res['points'].to(out_dtype)
-        return dict(points=out, offsets=new_off, counts=out_counts)
+        res = dict(points=out, offsets=new_off, counts=out_counts)
+        return (res, dense, haze_states) if want_states else res
+
+
+def filter_out_of_mor_boxes_batch(points, offsets, counts, gt_boxes, dataset_cfg, f32_distance=None, engine=None):
+    """
+    The FILTER_OUT_OF_MOR_BOXES key of `DenseDataset.__getitem__` (dense_dataset.py:922-934) on B device-resident clouds:
+    each cloud's boxes whose centre distance is not below its farthest row's distance are dropped.  points CUDA float32
+    or float64 (N, F >= 3), cloud b's counts[b] rows at offsets[b]; gt_boxes None or one host array per cloud;
+    f32_distance as after_batch returns it (the clouds the reference holds in float32; None: the rows' precision).
+    The farthest distance is Python's builtin max over the rows' norms (NaN when row 0's is NaN, so every box is dropped;
+    else the largest non-NaN norm), taken on the device; the box mask on the host.  Returns the list of kept boxes.  An
+    empty cloud raises builtin max's ValueError, as in the reference.
+    """
+    import torch
+    if gt_boxes is None or not dataset_cfg.get('FILTER_OUT_OF_MOR_BOXES', False):
+        return gt_boxes
+    engine = engine or default_engine()
+    dist = engine.farthest_distance_batch(points, offsets, counts=counts, f32_distance=f32_distance).cpu().numpy()
+    kept = []
+    for b, boxes in enumerate(gt_boxes):
+        if dist[b] < 0:
+            raise ValueError('max() iterable argument is empty')
+        f32 = points.dtype != torch.float64 or (f32_distance is not None and f32_distance[b])
+        max_point_dist = (np.float32 if f32 else np.float64)(dist[b])
+        box_distances = np.linalg.norm(boxes[:, 0:3], axis=1)
+        kept.append(boxes[box_distances < max_point_dist])
+    return kept
 
 
 def dror_filter(points, dataset_cfg, split, engine=None):

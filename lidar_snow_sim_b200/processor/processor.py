@@ -5,9 +5,11 @@ OpenPCDet's PointFeatureEncoder (pcdet/datasets/processor/point_feature_encoder.
 global RandomState and the voxels -- runs in one engine call (SnowfallEngine.processor_batch); the boxes' range mask
 stays on the host, O(boxes).
 
-Supported queue entries: mask_points_and_boxes_outside_range, shuffle_points, transform_points_to_voxels(_placeholder)
-and calculate_grid_size, with the row steps in that order (dense_dataset.yaml's).  sample_points and
-downsample_depth_map raise NotImplementedError.  Only float32 rows are accepted.
+Supported queue entries: mask_points_and_boxes_outside_range, sample_points, shuffle_points,
+transform_points_to_voxels(_placeholder) and calculate_grid_size, with the row steps in that order (dense_dataset.yaml's
+and pointrcnn.yaml's).  sample_points runs in a second engine call (SnowfallEngine.sample_points_batch) that takes the
+shuffle with it; it needs a NUM_POINTS mapping, and no shipped config combines it with the voxels, so both raise
+NotImplementedError.  downsample_depth_map raises NotImplementedError.  Only float32 rows are accepted.
 """
 import numpy as np
 import torch
@@ -15,7 +17,7 @@ import torch
 from ..engine import default_engine
 
 XYZ = ('x', 'y', 'z')
-ROW_STEPS = ('mask_points_and_boxes_outside_range', 'shuffle_points', 'transform_points_to_voxels')
+ROW_STEPS = ('mask_points_and_boxes_outside_range', 'sample_points', 'shuffle_points', 'transform_points_to_voxels')
 GRID_STEPS = ('transform_points_to_voxels', 'transform_points_to_voxels_placeholder', 'calculate_grid_size')
 
 
@@ -100,8 +102,10 @@ class DataProcessor:
         steps = []
         for cur_cfg in processor_configs:
             name = _get(cur_cfg, 'NAME')
-            if name in ('sample_points', 'downsample_depth_map'):
+            if name == 'downsample_depth_map':
                 raise NotImplementedError(f'DATA_PROCESSOR entry {name!r} has no device implementation')
+            if name == 'sample_points' and not hasattr(_get(cur_cfg, 'NUM_POINTS'), 'keys'):
+                raise NotImplementedError('DATA_PROCESSOR: sample_points needs a NUM_POINTS mapping (train / test)')
             if name not in ROW_STEPS + GRID_STEPS:
                 raise AttributeError(f"'DataProcessor' object has no attribute {name!r}")
             if name in GRID_STEPS:
@@ -115,9 +119,16 @@ class DataProcessor:
         if steps != sorted(steps) or len(set(steps)) != len(steps):
             raise NotImplementedError('DATA_PROCESSOR: the row steps run once each, in the order '
                                       + ', '.join(ROW_STEPS))
+        if self._cfg('sample_points') is not None and self._cfg('transform_points_to_voxels') is not None:
+            raise NotImplementedError('DATA_PROCESSOR: sample_points with transform_points_to_voxels')
 
     def _cfg(self, name):
         return next((c for n, c in self.data_processor_queue if n == name), None)
+
+    def num_points(self):
+        """sample_points' NUM_POINTS for the mode, or None when the queue has no sample_points (-1: rows unchanged)"""
+        cfg = self._cfg('sample_points')
+        return None if cfg is None else int(_get(cfg, 'NUM_POINTS')[self.mode])
 
     def _box_mask(self, boxes):
         cfg = self._cfg('mask_points_and_boxes_outside_range')
@@ -136,6 +147,8 @@ class DataProcessor:
         (N, F_out) rows at the front of the slots 'offsets' (host int64 (B + 1)), counts: CUDA int32 (B,), gt_boxes: list
         per cloud, voxels: None or dict(voxels (B, MAX_NUMBER_OF_VOXELS, MAX_POINTS_PER_VOXEL, F_out or F_out - 3 without
         use_lead_xyz), coords (B, ., 4) = (cloud, z, y, x), num_points, n_voxels (B,)), all CUDA).
+        With sample_points (NUM_POINTS k != -1) the masked rows go to SnowfallEngine.sample_points_batch, which takes the
+        shuffle after its own draws: cloud b's k rows at row b * k ('offsets' = k * arange(B + 1)), voxels None.
         """
         if not (isinstance(points, torch.Tensor) and points.is_cuda and points.dim() == 2):
             raise ValueError('forward_batch needs CUDA (N, F) rows')
@@ -150,10 +163,15 @@ class DataProcessor:
             vox = dict(voxel_size=_get(vox_cfg, 'VOXEL_SIZE'), max_points_per_voxel=_get(vox_cfg, 'MAX_POINTS_PER_VOXEL'),
                        max_voxels=_get(vox_cfg, 'MAX_NUMBER_OF_VOXELS')[self.mode])
         boxes = None if gt_boxes is None else [self._box_mask(b) for b in gt_boxes]
+        shuffle = shuffle_cfg is not None and bool(_get(shuffle_cfg, 'SHUFFLE_ENABLED')[self.mode])
+        k = self.num_points()
+        sample = k is not None and k != -1
         r = eng.processor_batch(points, off, cols, np.asarray(self.point_cloud_range), counts=counts,
                                 mask_points=self._cfg('mask_points_and_boxes_outside_range') is not None,
-                                shuffle=shuffle_cfg is not None and bool(_get(shuffle_cfg, 'SHUFFLE_ENABLED')[self.mode]),
-                                **vox)
+                                shuffle=shuffle and not sample, **vox)
+        if sample:
+            s = eng.sample_points_batch(r['points'], off, k, counts=r['counts'], shuffle=shuffle)
+            return dict(points=s['points'], offsets=s['offsets'], counts=s['counts'], gt_boxes=boxes, voxels=None)
         voxels = None
         if vox_cfg is not None:
             voxels = {k: r[k] for k in ('voxels', 'coords', 'num_points', 'n_voxels')}
