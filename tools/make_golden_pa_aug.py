@@ -3,6 +3,14 @@ Write tests/golden/pa_aug.npz: the UNMODIFIED reference's PA-AUG (lib/pa_aug/par
 PA_AUG_STRING block of DenseDataset.__getitem__) on seeded synthetic clouds.
 
     python tools/make_golden_pa_aug.py /path/to/reference
+    python tools/make_golden_pa_aug.py /path/to/reference --full
+
+--full writes tests/golden/pa_aug_full.npz instead (and leaves pa_aug.npz alone): the full-size cases of
+tests/pa_aug_scale_case.py, whose outputs are too large to store.  Per case c<k> (name, param, has_param, seed,
+n_clouds) and cloud c<k>_<i>_: in_sha (sha256 of the rows, the boxes and box_planes' result, so a test can tell changed
+inputs from a wrong kernel), counts (M, 8) int32 and n_bg (len(separated_box_points[i][j]) and len(bg_points) after the
+constructor, 0 past a box's part count), then either out_sha / out_shape / out_dtype, mask and rows (every
+ROW_STRIDE-th output row, for diagnostics) or exc, and st_* after the call.
 
 The reference is imported as written, with numba, and two shims: `np.int = int` (farthest_point_sampling allocates with
 np.int, an alias NumPy 1.24 removed; NumPy 2.x still has np.bool), and a stand-in for spconv.utils, which box_np_ops
@@ -158,6 +166,45 @@ def cases():
     return out
 
 
+def main_full(ref_root):
+    sys.path.insert(0, os.path.join(ROOT, 'tests'))
+    import pa_aug_scale_case as sc
+    PartAwareAugmentation = load_reference(ref_root)
+    d = {}
+    for k, c in enumerate(sc.cases()):
+        p = f'c{k}_'
+        d[p + 'name'] = np.array(c['name'])
+        d[p + 'param'] = np.array('' if c['param'] is None else c['param'])
+        d[p + 'has_param'] = np.array(c['param'] is not None)
+        d[p + 'seed'] = np.array(c['seed'])
+        d[p + 'n_clouds'] = np.array(len(c['clouds']))
+        np.random.seed(c['seed'])
+        for i, (pts, boxes) in enumerate(c['clouds']):
+            q = f'{p}{i}_'
+            d[q + 'in_sha'] = np.array(sc.input_digests(pts, boxes))
+            names = sc.names_of(boxes)
+            try:
+                aug = PartAwareAugmentation(pts, boxes, names, CLASS_NAMES)
+                cnt = np.zeros((len(boxes), 8), np.int32)
+                for b, parts in enumerate(aug.separated_box_points):
+                    cnt[b, :len(parts)] = [len(x) for x in parts]
+                d[q + 'counts'], d[q + 'n_bg'] = cnt, np.array(len(aug.bg_points))
+                o, m = aug.augment(pa_aug_param=c['param'])
+                d[q + 'out_sha'], d[q + 'out_shape'], d[q + 'out_dtype'] = (np.array(sc.digest(o)), np.array(o.shape),
+                                                                            np.array(o.dtype.str))
+                d[q + 'mask'], d[q + 'rows'] = np.array(m, bool).reshape(-1), o[::sc.ROW_STRIDE]
+                res = f'{o.shape} {o.dtype}, {sum(m)}/{len(m)} boxes'
+            except Exception as ex:                                # noqa: BLE001 (the reference's exception is data)
+                d[q + 'exc'] = np.array(type(ex).__name__)
+                res = f'{type(ex).__name__}: {ex}'
+            _, keys, pos, has_gauss, gauss = np.random.get_state()
+            d[q + 'st_keys'], d[q + 'st_pos'] = keys, np.array(pos)
+            d[q + 'st_gauss'] = np.array([has_gauss, gauss], np.float64)
+            print(f'{k:2d}.{i} {c["name"]:16s} {len(pts):6d} rows {len(boxes):3d} boxes -> {res}', flush=True)
+    np.savez_compressed(sc.GOLDEN, **d)
+    print(sc.GOLDEN, os.path.getsize(sc.GOLDEN), 'bytes')
+
+
 def main(ref_root):
     PartAwareAugmentation = load_reference(ref_root)
     d = {}
@@ -199,4 +246,4 @@ def main(ref_root):
 
 
 if __name__ == '__main__':
-    main(sys.argv[1])
+    main_full(sys.argv[1]) if sys.argv[2:] == ['--full'] else main(sys.argv[1])
