@@ -19,7 +19,8 @@
 //   k_gt_paste     the sampled objects' rows (db rows + box centre in double, z - mv_height in double, rounded to float32)
 //                  first, then the kept scene rows in order, each through the cloud's flip / rotation / scaling ops, and
 //                  the cloud's count.  Rotation is torch's CPU float32 matmul of (x, y, z) by the rotation matrix:
-//                  x' = fmaf(z, 0, fmaf(y, -s, x c)), y' = fmaf(z, 0, fmaf(y, c, x s)), z' = fmaf(z, 1, fmaf(y, 0, x 0)).
+//                  x' = fmaf(z, 0, fmaf(y, -s, fmaf(x, c, +0))), y' = fmaf(z, 0, fmaf(y, c, fmaf(x, s, +0))),
+//                  z' = fmaf(z, 1, fmaf(y, 0, fmaf(x, 0, +0))).  NaN results take x86's bits (fma_x86, mul_x86).
 // No allocation or synchronisation inside a call.
 #include "segments.cuh"
 
@@ -246,23 +247,42 @@ __global__ void __launch_bounds__(GT_TILE) k_gt_mark(PasteArgs a)
     seg_count<1>(cls, a.seg, b, tile);
 }
 
+// NaN results as x86 gives them (the reference's rows are computed there): the first NaN operand quieted, the
+// accumulator of an FMA first, else the default NaN 0xffc00000.  The device's own NaN is 0x7fffffff.
+__device__ __forceinline__ float quiet(float v) { return __int_as_float(__float_as_int(v) | 0x00400000); }
+
+__device__ __forceinline__ float fma_x86(float a, float b, float acc)
+{
+    const float r = __fmaf_rn(a, b, acc);
+    if (!isnan(r)) return r;
+    return isnan(acc) ? quiet(acc) : isnan(a) ? quiet(a) : isnan(b) ? quiet(b) : __int_as_float(0xffc00000);
+}
+
+__device__ __forceinline__ float mul_x86(float a, float b)
+{
+    const float r = fm(a, b);
+    if (!isnan(r)) return r;
+    return isnan(a) ? quiet(a) : isnan(b) ? quiet(b) : __int_as_float(0xffc00000);
+}
+
 __device__ __forceinline__ void apply_ops(const float *ops, int n, float &x, float &y, float &z)
 {
     for (int k = 0; k < n; k++) {
         const int code = (int)ops[k * GT_OP];
         const float p0 = ops[k * GT_OP + 1], p1 = ops[k * GT_OP + 2];
-        if (code == GT_OP_FLIP_X) {
-            y = -y;
+        if (code == GT_OP_FLIP_X) {                         // the sign bit, NaN too, as NumPy's negative flips it
+            y = __int_as_float(__float_as_int(y) ^ 0x80000000);
         } else if (code == GT_OP_FLIP_Y) {
-            x = -x;
+            x = __int_as_float(__float_as_int(x) ^ 0x80000000);
         } else if (code == GT_OP_ROT) {
             const float c = p0, s = p1;
-            const float nx = __fmaf_rn(z, 0.0f, __fmaf_rn(y, -s, fm(x, c)));
-            const float ny = __fmaf_rn(z, 0.0f, __fmaf_rn(y, c, fm(x, s)));
-            const float nz = __fmaf_rn(z, 1.0f, __fmaf_rn(y, 0.0f, fm(x, 0.0f)));
+            // each output starts from a +0 accumulator, as torch's does: x c alone would give -0 where torch gives +0
+            const float nx = fma_x86(z, 0.0f, fma_x86(y, -s, fma_x86(x, c, 0.0f)));
+            const float ny = fma_x86(z, 0.0f, fma_x86(y, c, fma_x86(x, s, 0.0f)));
+            const float nz = fma_x86(z, 1.0f, fma_x86(y, 0.0f, fma_x86(x, 0.0f, 0.0f)));
             x = nx; y = ny; z = nz;
         } else if (code == GT_OP_SCALE) {
-            x = fm(x, p0); y = fm(y, p0); z = fm(z, p0);
+            x = mul_x86(x, p0); y = mul_x86(y, p0); z = mul_x86(z, p0);
         }
     }
 }

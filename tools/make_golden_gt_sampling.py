@@ -3,6 +3,7 @@ Write tests/golden/gt_sampling.npz: the UNMODIFIED reference's DataBaseSampler a
 pcdet/datasets/augmentor) on a seeded synthetic database and seeded scenes.
 
     python tools/make_golden_gt_sampling.py /path/to/reference
+    python tools/make_golden_gt_sampling.py --full /path/to/reference     (tests/golden/gt_sampling_full.npz)
 
 The reference modules are loaded from their files under stand-in parent packages (so pcdet/__init__.py and
 pcdet/datasets/__init__.py, which import every dataset, do not run), with a SharedArray stub and the box routines
@@ -112,7 +113,77 @@ def main(ref_root):
     print(OUT, len(out), 'arrays; reference sampler on 131 072 rows (CPU):', float(out['cpu_sampler_ms_131072']), 'ms')
 
 
+def full(ref_root):
+    """tests/golden/gt_sampling_full.npz: the cases of tests/gt_sampling_scale_case.py, per cloud c<k>_<i>_*: the
+    input digest (in_sha), the output's sha256, shape and dtype, every ROW_STRIDE-th output row, the boxes' digest and
+    the names, NumPy's state and sample_groups after the call, each class's valid candidate indices (valid_<j>, in
+    sample_groups order, recorded around the sampler's add_sampled_boxes_to_scene), and the rows' sha256 after each
+    queue entry (stage_sha)."""
+    import functools
+    import gt_sampling_scale_case as S
+    DataAugmentor, Calibration = load_reference(ref_root)
+    out = {'db_sha_main': np.array(S.database_digest('main')), 'db_sha_grid': np.array(S.database_digest('grid'))}
+    with tempfile.TemporaryDirectory() as tmp:
+        roots = {kind: S.write_database(kind, os.path.join(tmp, kind)) for kind in ('main', 'grid')}
+        calib = Calibration(G.write_calib(tmp))
+        for k, case in enumerate(S.CASES):
+            p = f'c{k}_'
+            out[p + 'name'] = np.array(case['name'])
+            aug = DataAugmentor(G.Path(roots[case['db']]), S.augmentor_cfg(case), case['classes'])
+            sampler = aug.data_augmentor_queue[0]
+            rec = {}
+
+            def sample(fn, class_name, group):
+                r = fn(class_name, group)
+                rec['sampled'].append(r)
+                return r
+
+            def add(fn, data_dict, sampled_gt_boxes, total):
+                ids = {id(x) for x in total}
+                rec['valid'] = [[j for j, x in enumerate(s) if id(x) in ids] for s in rec['sampled']]
+                return fn(data_dict, sampled_gt_boxes, total)
+
+            def stage(fn, data_dict):
+                r = fn(data_dict=data_dict)
+                rec['stages'].append(S.digest(r['points']))
+                return r
+            sampler.sample_with_fixed_number = functools.partial(sample, sampler.sample_with_fixed_number)
+            sampler.add_sampled_boxes_to_scene = functools.partial(add, sampler.add_sampled_boxes_to_scene)
+            aug.data_augmentor_queue = [functools.partial(stage, fn) for fn in aug.data_augmentor_queue]
+            np.random.seed(case['seed'])
+            t0 = time.perf_counter()
+            scenes = S.scenes(k)
+            out[p + 'n_clouds'] = np.array(len(scenes))
+            for i, sc in enumerate(scenes):
+                q = f'{p}{i}_'
+                rec.update(sampled=[], valid=None, stages=[])
+                d = S.data_dict(sc, calib, case['classes'])
+                out[q + 'in_sha'] = np.array(S.input_digest(sc))
+                r = aug.forward(d)
+                pts = r['points']
+                out[q + 'out_sha'] = np.array(S.digest(pts))
+                out[q + 'out_shape'] = np.array(pts.shape, np.int64)
+                out[q + 'out_dtype'] = np.array(pts.dtype.str)
+                out[q + 'rows'] = pts[::S.ROW_STRIDE]
+                out[q + 'boxes_sha'] = np.array(S.digest(r['gt_boxes']))
+                out[q + 'names'] = r['gt_names'].astype(str)
+                out[q + 'stage_sha'] = np.array(rec['stages'])
+                valid = rec['valid'] or [[] for _ in rec['sampled']]
+                out[q + 'n_classes'] = np.array(len(valid))
+                for j, v in enumerate(valid):
+                    out[f'{q}valid_{j}'] = np.array(v, np.int32)
+                st = np.random.get_state()
+                out[q + 'st_keys'] = st[1]
+                out[q + 'st_pos'] = np.array(st[2])
+                out[q + 'st_gauss'] = np.array([st[3], st[4]], np.float64)
+                out[q + 'groups'] = np.array(S.groups_json(sampler.sample_groups))
+            print(f'{case["name"]}: {len(scenes)} clouds, {time.perf_counter() - t0:.1f} s')
+    np.savez_compressed(S.GOLDEN, **out)
+    print(S.GOLDEN, os.path.getsize(S.GOLDEN), 'bytes')
+
+
 if __name__ == '__main__':
-    if len(sys.argv) < 2 and 'REFERENCE_ROOT' not in os.environ:
+    args = [a for a in sys.argv[1:] if a != '--full']
+    if not args and 'REFERENCE_ROOT' not in os.environ:
         sys.exit(__doc__)
-    main(sys.argv[1] if len(sys.argv) > 1 else os.environ['REFERENCE_ROOT'])
+    (full if '--full' in sys.argv else main)(args[0] if args else os.environ['REFERENCE_ROOT'])
