@@ -57,15 +57,26 @@ def _cloud_offsets(offsets, name='cloud_offsets'):
     return off, B, N
 
 
+def _f32_flags(f32_distance, B):
+    """f32_distance (None, or one flag per cloud) as the int32 array of B flags the library reads"""
+    if f32_distance is None:
+        return None
+    f32 = np.ascontiguousarray(f32_distance, dtype=np.int32).reshape(-1)
+    if f32.shape[0] != B:
+        raise ValueError(f'f32_distance: expected {B} flags, got {f32.shape[0]}')
+    return f32
+
+
 def _check_tensor(name, t, device, dtype, shape=None, min_cols=0, optional=False):
     """
-    Raise ValueError unless `t` is a contiguous tensor of `dtype` on `device` (None: on any CUDA device, for mappings of
-    another rank's buffers) of shape `shape`, where None matches any size and dimension 1 has at least min_cols entries.
-    None passes for an optional argument.
+    Raise ValueError unless `t` is a contiguous tensor of `dtype` (or of one of a tuple of dtypes) on `device` (None: on
+    any CUDA device, for mappings of another rank's buffers) of shape `shape`, where None matches any size and dimension
+    1 has at least min_cols entries.  None passes for an optional argument.
     """
     if t is None and optional:
         return
-    if (isinstance(t, torch.Tensor) and (t.is_cuda if device is None else t.device == device) and t.dtype == dtype
+    dtypes = dtype if isinstance(dtype, tuple) else (dtype,)
+    if (isinstance(t, torch.Tensor) and (t.is_cuda if device is None else t.device == device) and t.dtype in dtypes
             and t.is_contiguous()
             and (shape is None or t.shape == shape
                  or (t.dim() == len(shape) and all(w is None or s == w for s, w in zip(t.shape, shape))))
@@ -74,7 +85,7 @@ def _check_tensor(name, t, device, dtype, shape=None, min_cols=0, optional=False
     dims = [] if shape is None else ['*' if w is None else str(w) for w in shape]
     if min_cols:
         dims[1] = f'n_features >= {min_cols}'
-    want = (f'a contiguous {dtype} tensor on {device or "a CUDA device"}'
+    want = (f'a contiguous {" or ".join(map(str, dtypes))} tensor on {device or "a CUDA device"}'
             + ('' if shape is None else f' of shape ({", ".join(dims)}{"," if len(dims) == 1 else ""})'))
     got = (f'a {"" if t.is_contiguous() else "non-contiguous "}{t.dtype} tensor of shape {tuple(t.shape)} on {t.device}'
            if isinstance(t, torch.Tensor) else type(t).__name__)
@@ -96,23 +107,36 @@ def _outputs(out, device, **spec):
     return out
 
 
+def _mt_words(state, name):
+    """The 625 uint32 words the library reads of an np.random.get_state() tuple: the 624 key words, then pos.  Raises
+    ValueError, naming the state `name`, for another generator or a pos outside [0, 624]."""
+    if state[0] != 'MT19937':
+        raise ValueError(f'{name} is {state[0]}, not MT19937')
+    if not 0 <= int(state[2]) <= 624:
+        raise ValueError(f'{name}: expected an MT19937 np.random.get_state() tuple with pos in [0, 624], got pos '
+                         f'{state[2]}')
+    words = np.empty(625, np.uint32)
+    words[:624] = np.asarray(state[1], dtype=np.uint32)
+    words[624] = int(state[2])
+    return words
+
+
+def _mt_tuple(words, start):
+    """The np.random.get_state() tuple of 625 words (key, pos), with the cached Gaussian (has_gauss, gauss) of the state
+    `start`: the draws that led from start to the words take no Gaussian"""
+    return ('MT19937', words[:624].copy(), int(words[624]), start[3], start[4])
+
+
 def _mt_state():
     """(words, state): NumPy's global RandomState as the 625 words the library reads (key, pos), and get_state()"""
     st = np.random.get_state()
-    if st[0] != 'MT19937':
-        raise ValueError(f'NumPy\'s global generator is {st[0]}, not MT19937')
-    words = np.empty(625, np.uint32)
-    words[:624] = st[1]
-    words[624] = int(st[2])
-    return words, st
+    return _mt_words(st, "NumPy's global generator"), st
 
 
-def _set_mt_state(state, d_words):
-    """set NumPy's global RandomState to the device's final words (one synchronising 2.5 KB copy); the cached Gaussian
-    is untouched, as the permutations draw none"""
-    w = d_words.cpu().numpy().view(np.uint32)
-    _, _, _, has_gauss, gauss = state[1]
-    np.random.set_state(('MT19937', w[:624].copy(), int(w[624]), has_gauss, gauss))
+def _set_mt_state(start, d_words):
+    """set NumPy's global RandomState to the device's final words (one synchronising 2.5 KB copy), with the cached
+    Gaussian of `start`"""
+    np.random.set_state(_mt_tuple(d_words.cpu().numpy().view(np.uint32), start))
 
 
 def _snowfall_flags(threshold_filter, camera_fov, device_prepass, assume_sorted=False):
@@ -136,7 +160,7 @@ class SnowfallEngine:
             from .calib.dense_camera import STF_HDL64_CAMERA as camera
         self.set_camera(camera)
         self._tables = {}
-        self._scratch_ws = {}                   # entry point -> its cached workspace (_scratch)
+        self._scratch_ws = {}                   # name -> its cached workspace (_scratch)
         self._pa_part_bytes = None              # the partition pa_partition_batch left at the front of the 'pa' workspace
 
     # ------------------------------------------------------------------------------------------------------------------
@@ -167,12 +191,17 @@ class SnowfallEngine:
             _lib.check(st, self.h)
         return st
 
-    def _scratch(self, name, need):
-        """The cached uint8 workspace of entry point `name`, reallocated at 1.25x + 256 bytes when it holds fewer than
-        `need`.  Calls of one entry point in flight on several streams would share it (snowfall_batch takes its own)."""
+    def _scratch(self, name, need, keep=0):
+        """The cached uint8 workspace `name`, reallocated at 1.25x + 256 bytes with its first `keep` bytes copied when
+        it holds fewer than `need` (a negative query answer counts as 0: the library then rejects the call).  The calls
+        of one name share it in stream order: no caller runs them on several streams (snowfall_batch takes its own)."""
+        need = max(int(need), 0)
         ws = self._scratch_ws.get(name)
         if ws is None or ws.numel() < need:
-            ws = self._scratch_ws[name] = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            grown = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
+            if keep:
+                grown[:keep].copy_(ws[:keep])
+            ws = self._scratch_ws[name] = grown
         return ws
 
     def set_camera(self, camera):
@@ -229,8 +258,7 @@ class SnowfallEngine:
         for attempt in range(SAMPLER_ATTEMPTS):
             # the output holds M rows per plane, as many as there are darts, so only a target not reached with M
             # darts (the stream is keyed per dart: more darts extend it, they do not change it) can fail here
-            need = self.lib.lss_sample_particles_workspace_bytes(n_planes, M)
-            ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
+            ws = self._scratch('sampler', self.lib.lss_sample_particles_workspace_bytes(n_planes, M))
             out = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device)
             counts = torch.empty((n_planes,), dtype=torch.int32, device=self.device)
             cand = torch.empty((n_planes, M, 3), dtype=torch.float64, device=self.device) if return_candidates else None
@@ -353,8 +381,7 @@ class SnowfallEngine:
         _check_tensor('points', points, self.device, torch.float32, (N, 5))
         pl = None if plane is None else np.ascontiguousarray(plane, dtype=np.float64).reshape(B, 4)
         ym = None if ymins is None else np.ascontiguousarray(ymins, dtype=np.int32).reshape(B, 50)
-        need = self.lib.lss_prepass_workspace_bytes(N, B)
-        ws = torch.empty(int(need) + 256, dtype=torch.uint8, device=self.device)
+        ws = self._scratch('prepass', self.lib.lss_prepass_workspace_bytes(N, B))
         out = _outputs(None, self.device, poly=((B, 3), torch.float64), plane=((B, 4), torch.float64),
                        fits=want_fits and ((B, 8), torch.float64), picks=want_fits and ((B, 50), torch.int32))
         self._call('lss_noise_threshold_poly', points, _ptr(off), B, float(noise_floor), _ptr(pl), _ptr(ym), out['poly'],
@@ -437,7 +464,7 @@ class SnowfallEngine:
         F = points.shape[1]
         out = _outputs(None, self.device, points=((N, F), torch.float64), fog_mask=((N,), torch.uint8),
                        info=((B, 3), torch.float64), rank=want_rank and ((N,), torch.int32))
-        ws = torch.empty(int(getattr(self.lib, ws_name)(N, B)) + 256, dtype=torch.uint8, device=self.device)
+        ws = self._scratch('fog', getattr(self.lib, ws_name)(N, B))
         self._call(name, points, F, _ptr(off), B, *params, flags, int(noise), int(noise_variant), _ptr(rs), ext_noise,
                    out['points'], out['fog_mask'], out.get('rank'), out['info'], ws, ws.numel())
         return out
@@ -464,8 +491,7 @@ class SnowfallEngine:
         steps = float(r_0_max) / float(granularity)
         rows = int(steps) + 1 if np.isfinite(steps) and 0 <= steps < 2 ** 24 else 0
         out = torch.empty((T, rows, 2), dtype=torch.float64, device=self.device)
-        need = self.lib.lss_fog_integral_tables_workspace_bytes(int(n), T)
-        ws = torch.empty(max(int(need), 0) + 256, dtype=torch.uint8, device=self.device)
+        ws = self._scratch('fog_tables', self.lib.lss_fog_integral_tables_workspace_bytes(int(n), T))
         self._call('lss_fog_integral_tables', ctypes.cast(arr, ctypes.c_void_p), T, out, ws, ws.numel())
         return out
 
@@ -484,9 +510,8 @@ class SnowfallEngine:
             diameters_nm = np.logspace(0, 7, 2000)
         d = np.ascontiguousarray(np.asarray(diameters_nm, dtype=np.float64).reshape(-1))
         T, nd = int(m.shape[0]), int(d.shape[0])
-        need = int(self.lib.lss_mie_tables_workspace_bytes(_ptr(m), _ptr(wl), T, _ptr(d), nd))
+        ws = self._scratch('mie', self.lib.lss_mie_tables_workspace_bytes(_ptr(m), _ptr(wl), T, _ptr(d), nd))
         out = torch.empty((T, nd, 2), dtype=torch.float64, device=self.device)
-        ws = torch.empty(max(need, 0) + 256, dtype=torch.uint8, device=self.device)
         self._call('lss_mie_tables', _ptr(m), _ptr(wl), T, _ptr(d), nd, out, ws, ws.numel())
         return out
 
@@ -538,18 +563,18 @@ class SnowfallEngine:
         if voxels and (T <= 0 or MV <= 0):
             raise ValueError('max_points_per_voxel > 0 and max_voxels > 0 required')
         vs = np.ascontiguousarray(voxel_size, dtype=np.float32).reshape(3) if voxels else None
-        state = _mt_state() if shuffle else None
+        words, start = _mt_state() if shuffle else (None, None)
         out = _outputs(None, self.device, points=((N, Fo), torch.float32), counts=((B,), torch.int32),
                        state=shuffle and ((625,), torch.int32), voxels=voxels and ((B, MV, T, Fo), torch.float32),
                        coords=voxels and ((B, MV, 4), torch.int32), num_points=voxels and ((B, MV), torch.int32),
                        n_voxels=voxels and ((B,), torch.int32))
         ws = self._scratch('processor', self.lib.lss_processor_workspace_bytes(N, B, Fo, T, MV))
         self._call('lss_processor_batch', points, F, _ptr(off), counts, B, _ptr(cols), Fo, _ptr(rng),
-                   1 if mask_points else 0, None if state is None else _ptr(state[0]), out.get('state'), _ptr(vs), T,
-                   MV, out['points'], out['counts'], out.get('voxels'), out.get('coords'), out.get('num_points'),
-                   out.get('n_voxels'), ws, ws.numel())
+                   1 if mask_points else 0, _ptr(words), out.get('state'), _ptr(vs), T, MV, out['points'],
+                   out['counts'], out.get('voxels'), out.get('coords'), out.get('num_points'), out.get('n_voxels'), ws,
+                   ws.numel())
         if shuffle:
-            _set_mt_state(state, out.pop('state'))
+            _set_mt_state(start, out.pop('state'))
         return out
 
     def mt19937_permutations(self, cloud_offsets, counts=None):
@@ -560,12 +585,12 @@ class SnowfallEngine:
         """
         off, B, N = _cloud_offsets(cloud_offsets)
         _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
-        state = _mt_state()
+        words, start = _mt_state()
         out = _outputs(None, self.device, perm=((N,), torch.int32), state=((625,), torch.int32))
         ws = self._scratch('processor', self.lib.lss_processor_workspace_bytes(N, B, 0, 0, 0))
-        self._call('lss_mt19937_permutations', _ptr(off), counts, B, _ptr(state[0]), out['perm'], out['state'], ws,
+        self._call('lss_mt19937_permutations', _ptr(off), counts, B, _ptr(words), out['perm'], out['state'], ws,
                    ws.numel())
-        _set_mt_state(state, out['state'])
+        _set_mt_state(start, out['state'])
         return out['perm']
 
     def sample_points_batch(self, points, cloud_offsets, num_points, counts=None, shuffle=False, run_starts=None,
@@ -585,9 +610,7 @@ class SnowfallEngine:
         state as it was before that cloud's draws.
         """
         off, B, N = _cloud_offsets(cloud_offsets)
-        if not (isinstance(points, torch.Tensor) and points.dtype in (torch.float32, torch.float64)):
-            raise ValueError('points: expected a float32 or float64 CUDA tensor')
-        _check_tensor('points', points, self.device, points.dtype, (N, None), min_cols=3)
+        _check_tensor('points', points, self.device, (torch.float32, torch.float64), (N, None), min_cols=3)
         _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
         k = int(num_points)
         if not 0 <= k < 2 ** 30:
@@ -601,18 +624,9 @@ class SnowfallEngine:
         R = starts.shape[0]
         if (len(run_states) != R or starts[0] != 0 or np.any(np.diff(starts) <= 0) or starts[-1] >= max(B, 1)):
             raise ValueError('run_starts: 0 first, increasing, below the number of clouds, one state per run')
-        words = np.empty((R, 625), np.uint32)
-        for r, st in enumerate(run_states):
-            if st[0] != 'MT19937' or not 0 <= int(st[2]) <= 624:
-                raise ValueError('run_states: MT19937 np.random.get_state() tuples with pos in [0, 624]')
-            words[r, :624] = np.asarray(st[1], dtype=np.uint32)
-            words[r, 624] = int(st[2])
+        words = np.stack([_mt_words(st, f'run_states[{r}]') for r, st in enumerate(run_states)])
         run_off = np.append(starts, B).astype(np.int32)
-        f32 = None
-        if f32_distance is not None:
-            f32 = np.ascontiguousarray(f32_distance, dtype=np.int32).reshape(-1)
-            if f32.shape[0] != B:
-                raise ValueError(f'f32_distance: expected {B} flags, got {f32.shape[0]}')
+        f32 = _f32_flags(f32_distance, B)
         F = points.shape[1]
         out = _outputs(None, self.device, points=((B * k, F), points.dtype))
         tail = torch.empty(R * 627, dtype=torch.int32, device=self.device)     # states then status: one copy back
@@ -625,8 +639,7 @@ class SnowfallEngine:
         status = h[R * 625:].reshape(R, 2)
         failed = [r for r in range(R) if status[r, 0] >= 0]
         last = min(failed, key=lambda r: status[r, 0]) if failed else R - 1
-        _, _, _, has_gauss, gauss = run_states[last]
-        np.random.set_state(('MT19937', states[last, :624].copy(), int(states[last, 624]), has_gauss, gauss))
+        np.random.set_state(_mt_tuple(states[last], run_states[last]))
         if failed:
             raise ValueError("'a' cannot be empty unless no samples are taken" if status[last, 1] == 1 else
                              "Cannot take a larger sample than population when 'replace=False'")
@@ -641,15 +654,9 @@ class SnowfallEngine:
         Returns a CUDA float64 (B,) tensor; float32 distances are exact in it.
         """
         off, B, N = _cloud_offsets(cloud_offsets)
-        if not (isinstance(points, torch.Tensor) and points.dtype in (torch.float32, torch.float64)):
-            raise ValueError('points: expected a float32 or float64 CUDA tensor')
-        _check_tensor('points', points, self.device, points.dtype, (N, None), min_cols=3)
+        _check_tensor('points', points, self.device, (torch.float32, torch.float64), (N, None), min_cols=3)
         _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
-        f32 = None
-        if f32_distance is not None:
-            f32 = np.ascontiguousarray(f32_distance, dtype=np.int32).reshape(-1)
-            if f32.shape[0] != B:
-                raise ValueError(f'f32_distance: expected {B} flags, got {f32.shape[0]}')
+        f32 = _f32_flags(f32_distance, B)
         out = torch.empty(B, dtype=torch.float64, device=self.device)
         ws = self._scratch('farthest', self.lib.lss_farthest_distance_workspace_bytes(B))
         self._call('lss_farthest_distance_batch', points, 1 if points.dtype == torch.float64 else 0, points.shape[1],
@@ -688,14 +695,7 @@ class SnowfallEngine:
             raise ValueError(f'fourier: expected an (n_components <= 16, 6) array, got shape {four.shape}')
         if not 0.0 <= fraction_random <= 0.05:
             raise ValueError(f'fraction_random must be in [0, 0.05], got {fraction_random}')
-        if state is None:
-            words, state = _mt_state()
-        else:
-            if state[0] != 'MT19937' or not 0 <= int(state[2]) <= 624:
-                raise ValueError('state: expected an MT19937 np.random.get_state() tuple with pos in [0, 624]')
-            words = np.empty(625, np.uint32)
-            words[:624] = np.asarray(state[1], dtype=np.uint32)
-            words[624] = int(state[2])
+        words, state = _mt_state() if state is None else (_mt_words(state, 'state'), state)
         F = points.shape[1]
         Fo = F + (1 if label else 0)
         n = np.diff(off)
@@ -713,9 +713,7 @@ class SnowfallEngine:
         states = h[:B * 625].view(np.uint32).reshape(B, 625)
         bad = np.flatnonzero(h[B * 625:] < 0)
         if B > 0:
-            _, _, _, has_gauss, gauss = state
-            last = int(bad[0]) if bad.size else B - 1
-            np.random.set_state(('MT19937', states[last, :624].copy(), int(states[last, 624]), has_gauss, gauss))
+            np.random.set_state(_mt_tuple(states[int(bad[0]) if bad.size else B - 1], state))
         if bad.size:
             # the reference's np.random.uniform(high=scatter_max[...]) on a NaN or infinite bound, after the lost draws
             raise OverflowError('Range exceeds valid bounds')
@@ -812,6 +810,22 @@ class SnowfallEngine:
                    out.get('mask'), ws, ws.numel())
         return out
 
+    def lisa_batch(self, points, rain_rate, alpha, seed, mode, r_min=0.9, r_max=120.0, beam_divergence=3e-3,
+                   min_diameter=0.05, range_accuracy=0.09, signal_last=False, draw_table=None):
+        """LISA.monte_carlo_augment (lib/LISA/python/lisa.py:293-341) on one device-resident cloud (lss_lisa_batch,
+        current stream, no synchronisation).  points: CUDA float64 (n, F), F >= 4, intensity in [0, 1]; seed: the
+        counter-based generator's key, or draw_table: CUDA float64 fixed-seed draw sequence (too short: raised at
+        check()); the other arguments as lisa_cloud_batch's.  Returns CUDA float64 (n, F + 2): x, y, z, intensity,
+        label, intensity_diff, zeros."""
+        _check_tensor('points', points, self.device, torch.float64, (None, None), min_cols=4)
+        _check_tensor('draw_table', draw_table, self.device, torch.float64, optional=True)
+        n, F = points.shape
+        out = torch.empty((n, F + 2), dtype=torch.float64, device=self.device)
+        self._call('lss_lisa_batch', points, F, n, float(rain_rate), int(mode), float(alpha), float(r_min),
+                   float(r_max), float(beam_divergence), float(min_diameter), float(range_accuracy),
+                   1 if signal_last else 0, draw_table, 0 if draw_table is None else draw_table.numel(), int(seed), out)
+        return out
+
     def lisa_cloud_batch(self, points, cloud_offsets, rain_rate, alpha, seed, mode, r_min=0.9, r_max=120.0,
                          beam_divergence=3e-3, min_diameter=0.05, range_accuracy=0.09, signal_last=False, counts=None,
                          apply=None, draw_table=None):
@@ -895,12 +909,8 @@ class SnowfallEngine:
                                                      int(n_fps_out))
         if need < 0:
             raise ValueError('bad PA-AUG plan sizes')
-        ws = self._scratch_ws['pa']
-        if ws.numel() < need:                                     # keep the partition: it lives at the front
-            ws = torch.empty(int(need * 1.25) + 256, dtype=torch.uint8, device=self.device)
-            ws[:self._pa_part_bytes].copy_(self._scratch_ws['pa'][:self._pa_part_bytes])
-            self._scratch_ws['pa'] = ws
-        out = torch.empty((int(n_out), 4), dtype=out_dtype, device=self.device)
+        ws = self._scratch('pa', need, keep=self._pa_part_bytes)     # the partition lives at the front
+        out =torch.empty((int(n_out), 4), dtype=out_dtype, device=self.device)
         self._call('lss_pa_apply_batch', points, points.shape[1], _ptr(off), counts, B, planes, nparts, _ptr(boff),
                    1 if boxes_f64 else 0, class_start, int(n_members), fps_segs, fps_segs.shape[0], int(n_fps_rows),
                    fps_jobs, fps_jobs.shape[0], int(n_fps_out), segs, segs.shape[0], steps, noise, normals, int(n_out),

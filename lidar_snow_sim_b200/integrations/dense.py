@@ -20,7 +20,7 @@ import random
 
 import numpy as np
 
-from ..engine import default_engine
+from ..engine import _mt_tuple, default_engine
 from ..fog.haze import SENSOR_CONSTANTS, BetaRadomization
 from ..fog.simulation import ParameterSet, simulate_fog, simulate_fog_batch_device
 from ..snowfall.precompute import SNOWFALL_RATES, TERMINAL_VELOCITIES, get_fov_flag
@@ -186,7 +186,7 @@ class OnTheFlyWeather:
         dev = points.device
         slot = np.diff(off)
         if counts is None:
-            counts = torch.from_numpy(slot.astype(np.int32)).to(dev)
+            counts = _slot_counts(off, dev)
         snow = np.zeros(B, dtype=bool)
         wet = np.zeros(B, dtype=bool)
         draws = []
@@ -198,19 +198,11 @@ class OnTheFlyWeather:
             return dict(points=points, counts=counts, intensity64=points[:, 3].double(), snow=snow, wet=wet)
         eng = self._engine()
         points, counts = points.clone(), counts.clone()
-
-        def gather(sel):                            # row indexes of the selected slots, their offsets, the cloud indexes
-            b = np.flatnonzero(sel)
-            sub = np.concatenate([[0], np.cumsum(slot[b])]).astype(np.int64)
-            shift = torch.from_numpy(off[b] - sub[:-1]).to(dev)
-            rows = torch.arange(int(sub[-1]), device=dev) + torch.repeat_interleave(
-                shift, torch.from_numpy(slot[b]).to(dev), output_size=int(sub[-1]))
-            return rows, sub, torch.from_numpy(b).to(dev)
-
         if snow.any():
             mode = draws[int(np.flatnonzero(snow)[0])]['mode']
             tid, sets = self._stack(mode)
-            rows, sub, b_dev = gather(snow)
+            rows, sub = _slot_rows(off, slot, snow, dev)
+            b_dev = torch.from_numpy(np.flatnonzero(snow)).to(dev)
             fov = eng.camera_fov_batch(points[rows], sub, counts=counts[b_dev])          # precompute.py:96-99
             order = np.stack([np.asarray(draws[k]['order'], np.int32) + 64 * sets[draws[k]['rainfall_rate']]
                               for k in np.flatnonzero(snow)])
@@ -220,7 +212,8 @@ class OnTheFlyWeather:
             counts[b_dev] = res['counts']
         intensity64 = points[:, 3].double()
         if wet.any():
-            rows, sub, b_dev = gather(wet)
+            rows, sub = _slot_rows(off, slot, wet, dev)
+            b_dev = torch.from_numpy(np.flatnonzero(wet)).to(dev)
             heights = np.array([draws[k]['water_height'] for k in np.flatnonzero(wet)])
             res = eng.wet_ground_batch(points[rows], sub, counts=counts[b_dev], water_height=heights,
                                        want_intensity64=True)
@@ -297,8 +290,7 @@ def lisa_block_batch(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, c
             if apply[b]:
                 seeds[b] = lisa.draw_seed()
     if not apply.any():
-        slot = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
-        return dict(points=points, counts=slot if counts is None else counts,
+        return dict(points=points, counts=_slot_counts(off, points.device) if counts is None else counts,
                     n_lost=torch.zeros(B, dtype=torch.int32, device=points.device))
     return lisa.augment_batch(points, off, rates, counts=counts, apply=apply, seeds=seeds)
 
@@ -344,6 +336,12 @@ def _slot_rows(off, lengths, sel, dev):
     rows = torch.arange(int(sub[-1]), device=dev) + torch.repeat_interleave(
         shift, torch.from_numpy(lengths[b]).to(dev), output_size=int(sub[-1]))
     return rows, sub
+
+
+def _slot_counts(off, dev):
+    """the counts of whole slots: the CUDA int32 (B,) slot lengths of the offsets off"""
+    import torch
+    return torch.from_numpy(np.diff(off).astype(np.int32)).to(dev)
 
 
 class FogAugmentation:
@@ -484,10 +482,9 @@ class FogAugmentation:
             return self._foggify(points, off, counts, alphas, methods, out_dtype)
         entry = np.random.get_state()                   # before BetaRadomization(seed=0) reseeds NumPy
         res, dense, haze_states = self._foggify(points, off, counts, alphas, methods, torch.float64, want_states=True)
-        gauss = np.random.get_state()[3:]               # a haze's: the reseed clears the cached Gaussian
+        reseeded = np.random.get_state()                # a haze's: the reseed clears the cached Gaussian
         starts = sorted({0} | set(np.flatnonzero(dense).tolist()))
-        states = [('MT19937', haze_states[b][:624].copy(), int(haze_states[b][624])) + gauss if dense[b] else entry
-                  for b in starts]
+        states = [_mt_tuple(haze_states[b], reseeded) if dense[b] else entry for b in starts]
         fogged = np.array([a is not None and a != '0.000' for a in alphas], dtype=bool)
         soft = bool(_cvl_options(self.cfg)[0])
         f32 = ~fogged | (~dense & (not soft))             # clear clouds; CVL clouds when only the hard fog runs
@@ -497,9 +494,8 @@ class FogAugmentation:
 
     @staticmethod
     def _passthrough(points, off, counts, out_dtype):
-        import torch
         if counts is None:
-            counts = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
+            counts = _slot_counts(off, points.device)
         return dict(points=points.to(out_dtype), offsets=off, counts=counts)
 
     def _foggify(self, points, off, counts, alphas, methods, out_dtype, want_states=False):
@@ -513,7 +509,7 @@ class FogAugmentation:
         dev, F = points.device, points.shape[1]
         slot = np.diff(off)
         if counts is None:
-            counts = torch.from_numpy(slot.astype(np.int32)).to(dev)
+            counts = _slot_counts(off, dev)
         new_slot = slot + slot // 20 + 1
         new_off = np.concatenate([[0], np.cumsum(new_slot)]).astype(np.int64)
         out = torch.zeros((int(new_off[-1]), F), dtype=out_dtype, device=dev)
@@ -654,8 +650,7 @@ def point_selection_batch(points, cloud_offsets, dataset_cfg, img_shapes=None, l
         r = engine.camera_fov_batch(res['points'], res['offsets'], counts=res['counts'], img_shapes=img_shapes)
         res = dict(points=r['points'], offsets=res['offsets'], counts=r['counts'])
     if res['counts'] is None:
-        import torch
-        res['counts'] = torch.from_numpy(np.diff(off).astype(np.int32)).to(points.device)
+        res['counts'] = _slot_counts(off, points.device)
     return res
 
 

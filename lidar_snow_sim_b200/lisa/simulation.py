@@ -28,8 +28,7 @@ from pathlib import Path
 import numpy as np
 import torch
 
-from .. import _lib
-from ..engine import default_engine, _ptr
+from ..engine import default_engine
 
 _MODES = {'rain': (0, 1.328), 'gunn': (1, 1.3031), 'sekhon': (2, 1.3031)}
 _SEED = 666                                         # lisa.py:55
@@ -161,15 +160,12 @@ class LISA:
     def augment(self, pc: np.ndarray, Rr, fixed_seed: bool = False) -> np.ndarray:
         """LISA.monte_carlo_augment (lisa.py:293-341)."""
         engine = self.engine or default_engine()
-        lib = engine.lib
         pc = np.ascontiguousarray(pc, dtype=np.float64)
-        n, F = pc.shape
-        if F < 4:
+        if pc.ndim != 2 or pc.shape[1] < 4:
             raise ValueError('pc must be (N, >= 4): x, y, z, intensity')
         Rr = float(Rr)
         a = float(self.alpha(self.Nd(self.D, Rr)))
         d_pc = torch.from_numpy(pc).to(engine.device)
-        out = torch.empty((n, F + 2), dtype=torch.float64, device=engine.device)
         seed = 0
         if not fixed_seed:
             seed = self.draw_seed()
@@ -179,12 +175,10 @@ class LISA:
         need = self._draws_bound(Rr, r_far)
         while True:
             table = self._draw_table(engine, need) if fixed_seed else None
-            with torch.cuda.device(engine.device):
-                st = lib.lss_lisa_batch(engine.h, _ptr(d_pc), F, n, Rr, _MODES[self.atm_model][0], a, float(self.r_min),
-                                        float(self.r_max), float(self.beam_divergence), float(self.min_diameter),
-                                        float(self.range_accuracy), 1 if self.signal == 'last' else 0, _ptr(table),
-                                        0 if table is None else int(table.numel()), seed, _ptr(out), engine._stream())
-            _lib.check(st, engine.h)
+            out = engine.lisa_batch(d_pc, Rr, a, seed, _MODES[self.atm_model][0], r_min=self.r_min, r_max=self.r_max,
+                                    beam_divergence=self.beam_divergence, min_diameter=self.min_diameter,
+                                    range_accuracy=self.range_accuracy, signal_last=self.signal == 'last',
+                                    draw_table=table)
             try:
                 engine.check()
                 break

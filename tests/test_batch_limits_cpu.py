@@ -6,7 +6,8 @@ import pytest
 import torch
 
 from lidar_snow_sim_b200.engine import MAX_CLOUDS
-from test_engine_args_cpu import F32, F64, I32, I64, engine, fake, prepare  # noqa: F401 (engine: the stub engine fixture)
+from test_engine_args_cpu import F32, F64, I32, I64, SETS_NUMPY_STATE, fake, prepare
+from test_engine_args_cpu import engine  # noqa: F401 (the stub engine fixture)
 
 pytestmark = pytest.mark.filterwarnings('ignore:Accessing the data pointer of FakeTensor')
 
@@ -36,6 +37,9 @@ def calls(B):
         'processor_batch': lambda e: e.processor_batch(pts, off, [0, 1, 2, 3], [0, -40, -3, 70.4, 40, 1], counts=cnt,
                                                        shuffle=False),
         'mt19937_permutations': lambda e: e.mt19937_permutations(off, counts=cnt),
+        'sample_points_batch': lambda e: e.sample_points_batch(pts, off, 0, counts=cnt),
+        'farthest_distance_batch': lambda e: e.farthest_distance_batch(pts, off, counts=cnt),
+        'haze_batch': lambda e: e.haze_batch(pts, off, np.zeros(B), np.zeros((0, 6)), counts=cnt),
         'dror_batch': lambda e: e.dror_batch(pts, off, counts=cnt),
         'strongest_last_batch': lambda e: e.strongest_last_batch(pts, off, pts, off, last_counts=cnt,
                                                                  strongest_counts=cnt),
@@ -67,7 +71,7 @@ def test_65535_clouds_pass_the_check(engine, method):
     prepare(engine, method)
     call = calls(MAX_CLOUDS)[method]
     if torch.cuda.is_available():
-        if method == 'mt19937_permutations':
+        if method in SETS_NUMPY_STATE:
             pytest.skip("it would set NumPy's generator to the stub's unwritten output state")
         call(engine)
         assert engine.lib.calls and not engine.lib.calls[-1].endswith('_workspace_bytes')

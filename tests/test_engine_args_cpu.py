@@ -10,15 +10,16 @@ import pytest
 import torch
 from torch._subclasses.fake_tensor import FakeTensorMode
 
-from lidar_snow_sim_b200.engine import SnowfallEngine
+from lidar_snow_sim_b200.engine import SnowfallEngine, _mt_tuple, _mt_words
 
 # a well-formed call that gets through to the stub library hands it the fake tensors' (meaningless) pointers
 pytestmark = pytest.mark.filterwarnings('ignore:Accessing the data pointer of FakeTensor')
 
 FAKE = FakeTensorMode()
 F32, F64, I32, I64, U8 = torch.float32, torch.float64, torch.int32, torch.int64, torch.uint8
-WRONG_DTYPE = {F32: F64, F64: F32, I32: I64, I64: I32, U8: I32}
-NP_DTYPE = {F32: np.float32, F64: np.float64, I32: np.int32, I64: np.int64, U8: np.uint8}
+F32_64 = (F32, F64)                              # rows that may be either (the well-formed call passes float32)
+WRONG_DTYPE = {F32: F64, F64: F32, I32: I64, I64: I32, U8: I32, F32_64: I32}
+NP_DTYPE = {F32: np.float32, F64: np.float64, I32: np.int32, I64: np.int64, U8: np.uint8, F32_64: np.float32}
 WS_BYTES = 4096                                  # what the stub answers to every *_workspace_bytes query
 # fake tensors on cuda:1 need either no driver or a second device (with one device torch rejects the ordinal)
 OTHER_DEVICE = not torch.cuda.is_available() or torch.cuda.device_count() > 1
@@ -55,15 +56,20 @@ def engine():
     eng.h = None
 
 
+def one(dtype):
+    """the dtype a well-formed argument of `dtype` (a dtype, or a tuple of dtypes) gets"""
+    return dtype[0] if isinstance(dtype, tuple) else dtype
+
+
 def fake(shape, dtype, device='cuda:0'):
     with FAKE:
-        return torch.empty(shape, dtype=dtype, device=device)
+        return torch.empty(shape, dtype=one(dtype), device=device)
 
 
 def non_contiguous(shape, dtype):
     k = next(i for i, s in enumerate(shape) if s > 1)
     with FAKE:
-        t = torch.empty(shape[:k] + (2 * shape[k],) + shape[k + 1:], dtype=dtype, device='cuda:0')
+        t = torch.empty(shape[:k] + (2 * shape[k],) + shape[k + 1:], dtype=one(dtype), device='cuda:0')
         return t[(slice(None),) * k + (slice(None, None, 2),)]
 
 
@@ -102,6 +108,24 @@ CASES = {
         lambda e, points, counts: e.voxelize_batch(points, OFF, [0, -40, -3, 70.4, 40, 1], [0.05, 0.05, 0.1], 5, 16,
                                                    counts=counts),
         {'points': ((N, 5), F32, [(N + 1, 5), (N, 2)]), 'counts': ((B,), I32, [(B + 1,)])}),
+    'processor_batch': (
+        lambda e, points, counts: e.processor_batch(points, OFF, [0, 1, 2, 3], [0, -40, -3, 70.4, 40, 1], counts=counts,
+                                                    shuffle=False),
+        {'points': ((N, 5), F32, [(N + 1, 5), (N, 2)]), 'counts': ((B,), I32, [(B + 1,)])}),
+    'mt19937_permutations': (
+        lambda e, counts: e.mt19937_permutations(OFF, counts=counts),
+        {'counts': ((B,), I32, [(B + 1,)])}),
+    'sample_points_batch': (
+        lambda e, points, counts: e.sample_points_batch(points, OFF, 16, counts=counts),
+        {'points': ((N, 5), F32_64, [(N + 1, 5), (N, 2)]), 'counts': ((B,), I32, [(B + 1,)])}),
+    'farthest_distance_batch': (
+        lambda e, points, counts: e.farthest_distance_batch(points, OFF, counts=counts),
+        {'points': ((N, 5), F32_64, [(N + 1, 5), (N, 2)]), 'counts': ((B,), I32, [(B + 1,)])}),
+    'haze_batch': (
+        lambda e, points, counts, angle: e.haze_batch(points, OFF, [0.05] * B, np.zeros((0, 6)), counts=counts,
+                                                      angle=angle),
+        {'points': ((N, 5), F32, [(N + 1, 5), (N, 3)]), 'counts': ((B,), I32, [(B + 1,)]),
+         'angle': ((N,), F32, [(N + 1,), (N, 1)])}),
     'dror_batch': (
         lambda e, points, counts, reuse_keep: e.dror_batch(points, OFF, counts=counts, out=dict(keep=reuse_keep)),
         {'points': ((N, 5), F32, [(N + 1, 5), (N, 2)]), 'counts': ((B,), I32, [(B + 1,)]),
@@ -114,6 +138,9 @@ CASES = {
     'camera_fov_batch': (
         lambda e, points, counts: e.camera_fov_batch(points, OFF, counts=counts),
         {'points': ((N, 5), F32, [(N + 1, 5), (N, 2)]), 'counts': ((B,), I32, [(B + 1,)])}),
+    'lisa_batch': (
+        lambda e, points, draw_table: e.lisa_batch(points, 20.0, 0.01, 0, 0, draw_table=draw_table),
+        {'points': ((N, 4), F64, [(N, 3), (N,)]), 'draw_table': ((100,), F64, [])}),
     'lisa_cloud_batch': (
         lambda e, points, counts, draw_table: e.lisa_cloud_batch(points, OFF, [20.0] * B, [0.01] * B, None, 0,
                                                                  counts=counts, draw_table=draw_table),
@@ -156,12 +183,13 @@ CASES = {
          'peer_counts_0': ((W * B,), I32, [(W * B - 1,)]), 'peer_counts_1': ((W * B,), I32, [(W * B + 1,)])}),
 }
 PEERS = {'peer_points_0', 'peer_points_1', 'peer_counts_0', 'peer_counts_1'}   # gather_push's: on any CUDA device
+SETS_NUMPY_STATE = {'mt19937_permutations', 'sample_points_batch', 'haze_batch'}  # to the state the device wrote
 
 
 def malformed(method):
     """(argument, what, value) for every way an argument of `method` is malformed"""
     for arg, (shape, dtype, bad_shapes) in CASES[method][1].items():
-        yield arg, 'cpu tensor', torch.zeros(shape, dtype=dtype)
+        yield arg, 'cpu tensor', torch.zeros(shape, dtype=one(dtype))
         yield arg, 'numpy array', np.zeros(shape, NP_DTYPE[dtype])
         yield arg, f'{WRONG_DTYPE[dtype]}', fake(shape, WRONG_DTYPE[dtype])
         yield arg, 'non-contiguous', non_contiguous(shape, dtype)
@@ -190,6 +218,8 @@ def passes_checks(engine, method, **replace):
     one, the call runs through to the stub library's entry point."""
     call = CASES[method][0]
     if torch.cuda.is_available():
+        if method in SETS_NUMPY_STATE:
+            pytest.skip("it would set NumPy's generator to the stub's unwritten output state")
         call(engine, **dict(valid(method), **replace))
         assert engine.lib.calls and not engine.lib.calls[-1].endswith('_workspace_bytes')
     else:
@@ -219,6 +249,11 @@ def test_tensors_on_another_device_than_the_engine_are_rejected(engine, method):
     with pytest.raises(ValueError, match='on cuda:1 .*, got .* on cuda:0'):
         CASES[method][0](engine, **valid(method))
     assert engine.lib.calls == []
+
+
+@pytest.mark.parametrize('method', ['farthest_distance_batch', 'sample_points_batch'])      # their points are F32_64
+def test_float64_rows_pass_every_check(engine, method):
+    passes_checks(engine, method, points=fake(CASES[method][1]['points'][0], F64))
 
 
 @pytest.mark.skipif(not OTHER_DEVICE, reason='one CUDA device: no second device to place a buffer on')
@@ -258,3 +293,21 @@ def test_cloud_offsets_must_be_one_dimensional(engine):
         with pytest.raises(ValueError, match='cloud_offsets'):
             engine.noise_threshold_poly(fake((N, 5), F32), off)
     assert engine.lib.calls == []
+
+
+def test_numpy_state_codec():
+    """np.random.get_state() tuples -> the library's 625 words -> tuples: the round trip keeps every field, the cached
+    Gaussian included, and a tuple of another generator or with pos outside [0, 624] raises ValueError naming it"""
+    rs = np.random.RandomState(7)
+    for draw in (lambda: None, rs.standard_normal, lambda: rs.random_sample(1000)):   # pos 624, has_gauss 0 and 1
+        draw()
+        st = rs.get_state()
+        got = _mt_tuple(_mt_words(st, 'state'), st)
+        assert got[0] == st[0] and got[1].dtype == st[1].dtype and np.array_equal(got[1], st[1]) and got[2:] == st[2:]
+    key = rs.get_state()[1]
+    with pytest.raises(ValueError, match="NumPy's global generator is PCG64, not MT19937"):
+        _mt_words(('PCG64', key, 0, 0, 0.0), "NumPy's global generator")
+    for pos in (-1, 625):
+        with pytest.raises(ValueError, match=re.escape(f'run_states[1]: expected an MT19937 np.random.get_state() '
+                                                       f'tuple with pos in [0, 624], got pos {pos}')):
+            _mt_words(('MT19937', key, pos, 0, 0.0), 'run_states[1]')
