@@ -414,6 +414,61 @@ LSS_API lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points, in
                                         void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_lisa_cloud_batch_workspace_bytes(int64_t n_total, int n_clouds);
 
+/* ---- LISA's fog / haze / spray modes and Goodin et al.'s rain model -----------------------------------------------------
+ * LISA.average_augment (lib/LISA/python/lisa.py:340-388: chu_hogg_fog, strong_advection_fog, moderate_advection_fog,
+ * coast_haze, continental_haze, moderate_spray, strong_spray) and LISA.goodin_augment (:391-443: 'goodin et al.') on a
+ * batch of device-resident float64 clouds.  A row is detected when p0 = (I exp((-2 alpha) r)) / (r r) > p_min, p0 taken
+ * on the rows with r > r_min (model 0, average) or r > 0 (model 1, Goodin); each detected row takes the next Gaussian of
+ * NumPy's legacy RandomState.normal, in row order, replayed from h_gauss_state.  Output rows as the reference's pc_new:
+ * x, y, z at the new range, i_new, label (2 detected, 0 not), I - i_new, zeros.
+ *   d_points        float64[n_total * n_features] (x, y, z, intensity in [0, 1], ...), n_features >= 4
+ *   h_cloud_offsets int64[n_clouds + 1] host, n_clouds <= 65535
+ *   model           0 average_augment, 1 goodin_augment
+ *   h_alpha         float64[n_clouds] host: LISA.alpha(LISA.Nd(D, Rr)) of each cloud (one value for the average modes;
+ *                   0.01 Rr^0.6 for Goodin), computed by the caller with NumPy
+ *   h_range_scale   float64[n_clouds] host, Goodin only (NULL for model 0): (1 - exp(-Rr))^2 of each cloud
+ *   p_min           0.9 r_max^-2 (average) or 0.9 r_max^-2 / pi (Goodin), computed by the caller
+ *   r_min, range_accuracy   the LISA constructor arguments (range_accuracy unused by Goodin)
+ *   shared_start    0: the clouds continue one stream in batch order (B augment calls in turn);  1: every cloud starts
+ *                   from h_gauss_state (fixed_seed: the caller passes np.random.seed(666)'s state); the final state is
+ *                   the last cloud's.  Clouds with no detected row take no Gaussian.
+ *   h_gauss_state   uint32[630] host: key [0, 624), pos [624] in [0, 624], has_gauss [625] (0 / 1), the cached Gaussian
+ *                   as a float64 at [626], 2 words unused
+ *   d_gauss_state_out  uint32[630] device: the state after the call: key, pos, kind [625] = 0 no cached Gaussian,
+ *                   2 cached Gaussian sqrt(-2 log r2 / r2) x1 with x1, r2 the float64s at [626] and [628] (for the
+ *                   caller to compute with C's libm, as NumPy does), 3 key, pos and cached Gaussian as at the start
+ *   d_out           float64[n_total * (n_features + 2)]
+ *   d_workspace     lss_lisa_average_batch_workspace_bytes(n_total, n_clouds) bytes.  No allocation, no synchronisation.
+ * The Gaussian stream's attempts are bounded by n_total (17 standard deviations above their mean): should a call need
+ * more, LSS_ERR_WORKSPACE is latched (asynchronous, lss_check_async).
+ * Parity: detected rows, labels, NaN positions, signed zeros and the final state exact; values to libm rounding. */
+LSS_API lss_status lss_lisa_average_batch(lss_engine *e, const double *d_points, int n_features,
+                                          const int64_t *h_cloud_offsets, int n_clouds, int model, const double *h_alpha,
+                                          const double *h_range_scale, double p_min, double r_min, double range_accuracy,
+                                          int shared_start, const uint32_t *h_gauss_state, double *d_out,
+                                          uint32_t *d_gauss_state_out, void *d_workspace, int64_t workspace_bytes,
+                                          void *stream);
+LSS_API int64_t lss_lisa_average_batch_workspace_bytes(int64_t n_total, int n_clouds);
+/* The dataset's LISA block (dense_dataset.py:713-746) with those models on a batch of device-resident float32 clouds:
+ * lss_lisa_cloud_batch's conversions (intensity (double)(I / 255.0f) in, round(i_new * 255) and the float32 cast out,
+ * label in column 4, columns >= 5 copied, label-0 rows dropped: only the detected rows are kept, stably compacted to the
+ * front of each slot).  A cloud's rows are bit-identical to lss_lisa_average_batch on its float64 conversion followed
+ * by those host steps.
+ *   d_points, n_features >= 5, h_cloud_offsets, d_cloud_counts, h_apply, d_out_points, d_out_counts, d_out_n_lost
+ *                   as lss_lisa_cloud_batch (clouds not applied are copied through and take no Gaussian)
+ *   model, h_alpha, h_range_scale, p_min, r_min, range_accuracy, shared_start, h_gauss_state, d_gauss_state_out
+ *                   as lss_lisa_average_batch
+ *   d_workspace     lss_lisa_average_cloud_batch_workspace_bytes(n_total, n_clouds) bytes. */
+LSS_API lss_status lss_lisa_average_cloud_batch(lss_engine *e, const float *d_points, int n_features,
+                                                const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts,
+                                                int n_clouds, const uint8_t *h_apply, int model, const double *h_alpha,
+                                                const double *h_range_scale, double p_min, double r_min,
+                                                double range_accuracy, int shared_start, const uint32_t *h_gauss_state,
+                                                float *d_out_points, int32_t *d_out_counts, int32_t *d_out_n_lost,
+                                                uint32_t *d_gauss_state_out, void *d_workspace, int64_t workspace_bytes,
+                                                void *stream);
+LSS_API int64_t lss_lisa_average_cloud_batch_workspace_bytes(int64_t n_total, int n_clouds);
+
 /* ---- point-range mask + voxelisation ("next" row, SURVEY.md 8f-4) ---------------------------------------------------------
  * The detector-input stage of the reference's data path on device-resident clouds, e.g. the slot-compacted output of
  * lss_snowfall_batch / lss_wet_ground_batch, so that the augmented batch reaches the detector without a host round trip:

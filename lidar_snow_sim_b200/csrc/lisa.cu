@@ -5,6 +5,7 @@
 //   n ~ density(Rr, D_min) * beam-cone volume particles (probabilistic rounding, :62-64), their ranges r U^(1/3) (Eq. 10,
 //   :70), diameters from the exponential size law (Eq. 12, :84), back-scattered powers (:88-90), then the strongest- /
 //   last-return logic against the attenuated hard-target power, Gaussian range noise, new intensity, label.
+// LISA's other eight modes (the fog, haze and spray modes and 'goodin et al.') are lisa_average.cu.
 //
 // One WARP per return: a return at 100 m in moderate rain draws thousands of particles, so the particle loop is what has to
 // be parallel.  Lane l handles particles l, l + 32, ...; the kept-particle rank (which fixes the diameter draw a particle

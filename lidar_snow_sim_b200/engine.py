@@ -9,6 +9,7 @@ Every public method checks all of its arguments (ValueError, like the library's 
 allocates, touches the device or calls the library: a pointer reaches a kernel only from a tensor that was checked.
 """
 import ctypes
+import math
 
 import numpy as np
 import torch
@@ -20,6 +21,7 @@ DEFAULT_MAX_DIVERGENCE_RAD = 3e-3          # callers pass beam_divergence = degr
 # sample_tables_device calls the sampler at most this often: the darts per plane start at 1.5x the expected table size
 # (+4096) and double after each call that ends short of the occupancy; the last call's failure is raised
 SAMPLER_ATTEMPTS = 4
+LISA_SEED_STATE = np.random.RandomState(666).get_state()    # np.random.seed(666): LISA's fixed_seed (lisa.py:54-55)
 MAX_CLOUDS = 65535                      # clouds per batch call: the kernels' grid y dimension (lss_batch_geometry)
 _CPU = torch.device('cpu')
 
@@ -107,35 +109,60 @@ def _outputs(out, device, **spec):
     return out
 
 
-def _mt_words(state, name):
+# the kind word [625] of a 630-word state record (gauss=True): no cached Gaussian; the cached Gaussian in the float64 at
+# [626]; the cached Gaussian sqrt(-2 log r2 / r2) x1 of the float64s x1, r2 at [626], [628]; the start state's
+_GAUSS_NONE, _GAUSS_VALUE, _GAUSS_X1_R2, _GAUSS_AS_START = 0, 1, 2, 3
+MT_GAUSS_WORDS = 630
+
+
+def _mt_words(state, name, gauss=False):
     """The 625 uint32 words the library reads of an np.random.get_state() tuple: the 624 key words, then pos.  Raises
-    ValueError, naming the state `name`, for another generator or a pos outside [0, 624]."""
+    ValueError, naming the state `name`, for another generator or a pos outside [0, 624].  With `gauss`, the 630-word
+    record of the entry points that draw Gaussians: then has_gauss (0 or 1) and the cached Gaussian as a float64 follow."""
     if state[0] != 'MT19937':
         raise ValueError(f'{name} is {state[0]}, not MT19937')
     if not 0 <= int(state[2]) <= 624:
         raise ValueError(f'{name}: expected an MT19937 np.random.get_state() tuple with pos in [0, 624], got pos '
                          f'{state[2]}')
-    words = np.empty(625, np.uint32)
+    words = np.zeros(MT_GAUSS_WORDS if gauss else 625, np.uint32)
     words[:624] = np.asarray(state[1], dtype=np.uint32)
     words[624] = int(state[2])
+    if gauss:
+        if int(state[3]) not in (0, 1):
+            raise ValueError(f'{name}: has_gauss must be 0 or 1, got {state[3]}')
+        words[625] = int(state[3])
+        words[626:628] = np.array([float(state[4])], np.float64).view(np.uint32)
     return words
 
 
 def _mt_tuple(words, start):
     """The np.random.get_state() tuple of 625 words (key, pos), with the cached Gaussian (has_gauss, gauss) of the state
-    `start`: the draws that led from start to the words take no Gaussian"""
-    return ('MT19937', words[:624].copy(), int(words[624]), start[3], start[4])
+    `start`: the draws that led from start to the words take no Gaussian.  A 630-word record carries its own cached
+    Gaussian (see _GAUSS_*); a device-drawn one is computed here as NumPy's legacy_gauss does, with C's libm."""
+    if words.shape[0] < MT_GAUSS_WORDS:
+        return ('MT19937', words[:624].copy(), int(words[624]), start[3], start[4])
+    kind = int(words[625])
+    v = np.ascontiguousarray(words[626:630]).view(np.float64)
+    if kind == _GAUSS_AS_START:
+        has, g = start[3], start[4]
+    elif kind == _GAUSS_X1_R2:
+        has, g = 1, math.sqrt(-2.0 * math.log(float(v[1])) / float(v[1])) * float(v[0])
+    elif kind == _GAUSS_VALUE:
+        has, g = 1, float(v[0])
+    else:
+        has, g = 0, 0.0
+    return ('MT19937', words[:624].copy(), int(words[624]), has, g)
 
 
-def _mt_state():
-    """(words, state): NumPy's global RandomState as the 625 words the library reads (key, pos), and get_state()"""
+def _mt_state(gauss=False):
+    """(words, state): NumPy's global RandomState as the words the library reads (_mt_words), and get_state()"""
     st = np.random.get_state()
-    return _mt_words(st, "NumPy's global generator"), st
+    return _mt_words(st, "NumPy's global generator", gauss), st
 
 
 def _set_mt_state(start, d_words):
     """set NumPy's global RandomState to the device's final words (one synchronising 2.5 KB copy), with the cached
-    Gaussian of `start`"""
+    Gaussian of `start` or, for a 630-word record, its own"""
     np.random.set_state(_mt_tuple(d_words.cpu().numpy().view(np.uint32), start))
 
 
@@ -853,6 +880,72 @@ class SnowfallEngine:
                    float(range_accuracy), 1 if signal_last else 0, draw_table,
                    0 if draw_table is None else draw_table.numel(), out['points'], out['counts'], out['n_lost'], ws,
                    ws.numel())
+        return out
+
+    def _lisa_average_params(self, B, model, alpha, range_scale, fixed_seed):
+        """(alpha, range_scale, start state, its 630 words) of lisa_average_batch / lisa_average_cloud_batch, checked"""
+        if model not in (0, 1):
+            raise ValueError(f'model: expected 0 (average_augment) or 1 (goodin_augment), got {model}')
+        al = np.ascontiguousarray(np.broadcast_to(np.asarray(alpha, dtype=np.float64), (B,)))
+        sc = None
+        if model == 1:
+            if range_scale is None:
+                raise ValueError('range_scale: Goodin needs (1 - exp(-Rr))**2 per cloud')
+            sc = np.ascontiguousarray(np.broadcast_to(np.asarray(range_scale, dtype=np.float64), (B,)))
+        start = LISA_SEED_STATE if fixed_seed else np.random.get_state()
+        return al, sc, start, _mt_words(start, 'fixed_seed state' if fixed_seed else "NumPy's global generator", True)
+
+    def lisa_average_batch(self, points, cloud_offsets, model, alpha, p_min, r_min=0.9, range_accuracy=0.09,
+                           range_scale=None, fixed_seed=False):
+        """
+        LISA.average_augment (model 0: the fog, haze and spray modes, lisa.py:340-388) or LISA.goodin_augment (model 1,
+        :391-443) on a batch of device-resident float64 clouds (lss_lisa_average_batch, current stream).  points: CUDA
+        float64 (N, F), F >= 4, intensity in [0, 1]; alpha: per cloud (or one for all), LISA.alpha(LISA.Nd(D, Rr));
+        p_min: 0.9 r_max^-2 (average) or that / pi (Goodin); range_scale: Goodin's (1 - exp(-Rr))**2 per cloud.  The
+        detected rows draw NumPy's legacy Gaussians: without fixed_seed from the global generator, cloud after cloud (B
+        augment calls in turn); with it, every cloud from np.random.seed(666).  The call synchronises once, for the copy
+        of the final state, and sets NumPy's global state to it (as the last augment call leaves it).  Returns CUDA
+        float64 (N, F + 2), the reference's pc_new of every cloud at its rows.
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float64, (N, None), min_cols=4)
+        al, sc, start, words = self._lisa_average_params(B, model, alpha, range_scale, fixed_seed)
+        F = points.shape[1]
+        out = _outputs(None, self.device, points=((N, F + 2), torch.float64), state=((MT_GAUSS_WORDS,), torch.int32))
+        ws = self._scratch('lisa_average', self.lib.lss_lisa_average_batch_workspace_bytes(N, B))
+        self._call('lss_lisa_average_batch', points, F, _ptr(off), B, int(model), _ptr(al), _ptr(sc), float(p_min),
+                   float(r_min), float(range_accuracy), 1 if fixed_seed else 0, _ptr(words), out['points'],
+                   out['state'], ws, ws.numel())
+        if B > 0:
+            _set_mt_state(start, out['state'])
+        return out['points']
+
+    def lisa_average_cloud_batch(self, points, cloud_offsets, model, alpha, p_min, r_min=0.9, range_accuracy=0.09,
+                                 range_scale=None, counts=None, apply=None, fixed_seed=False):
+        """
+        The dataset's LISA block (dense_dataset.py:713-746) with average_augment or goodin_augment on a batch of
+        device-resident float32 clouds (lss_lisa_average_cloud_batch, current stream): lisa_cloud_batch's conversions and
+        layout, lisa_average_batch's models and Gaussians.  points: CUDA float32 (N, F), F >= 5, intensity in [0, 255];
+        counts: optional CUDA int32 (B,) valid rows per slot; apply: optional length-B booleans (clouds with False are
+        copied through and draw nothing).  Synchronises once and sets NumPy's global state as B augment calls on the
+        applied clouds leave it.  Returns dict(points (N, F) float32: each cloud's detected rows at the front of its slot,
+        label 2 in column 4; counts (B,) int32; n_lost (B,) int32).
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=5)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        al, sc, start, words = self._lisa_average_params(B, model, alpha, range_scale, fixed_seed)
+        ap = None if apply is None else np.ascontiguousarray(np.asarray(apply, dtype=bool).reshape(B), dtype=np.uint8)
+        F = points.shape[1]
+        out = _outputs(None, self.device, points=((N, F), torch.float32), counts=((B,), torch.int32),
+                       n_lost=((B,), torch.int32), state=((MT_GAUSS_WORDS,), torch.int32))
+        ws = self._scratch('lisa_average', self.lib.lss_lisa_average_cloud_batch_workspace_bytes(N, B))
+        self._call('lss_lisa_average_cloud_batch', points, F, _ptr(off), counts, B, _ptr(ap), int(model), _ptr(al),
+                   _ptr(sc), float(p_min), float(r_min), float(range_accuracy), 1 if fixed_seed else 0, _ptr(words),
+                   out['points'], out['counts'], out['n_lost'], out['state'], ws, ws.numel())
+        state = out.pop('state')
+        if B > 0 and (ap is None or ap.any()):
+            _set_mt_state(start, state)
         return out
 
     def _pa_args(self, points, cloud_offsets, planes, nparts, box_offsets, counts):

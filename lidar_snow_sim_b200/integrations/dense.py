@@ -275,8 +275,13 @@ def lisa_block_batch(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, c
     F >= 5; cloud b = rows cloud_offsets[b]:cloud_offsets[b+1] (the first counts[b] with `counts`).  The draws are taken
     sample by sample in batch order -- coin flip, rain rate, and for an applied sample the generator key augment would
     draw -- so every cloud's rows and NumPy's global state afterwards equal B lisa_block calls in turn.  Returns
-    dict(points (N, F) float32, each cloud's rows at the front of its slot; counts (B,) int32; n_lost (B,) int32)."""
+    dict(points (N, F) float32, each cloud's rows at the front of its slot; counts (B,) int32; n_lost (B,) int32).
+    Only LISA's Monte-Carlo modes: the others draw NumPy's Gaussians on the device, which the per-sample host draws
+    (coin flip, rain rate) would have to interleave with; lisa_block takes them one sample at a time."""
     import torch
+    if not getattr(lisa, 'monte_carlo', True):
+        raise NotImplementedError(f"lisa_block_batch runs LISA's Monte-Carlo modes only, not '{lisa.atm_model}': their "
+                                  f"Gaussians interleave with the per-sample host draws; use lisa_block per sample")
     off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
     B = off.shape[0] - 1
     if points.dim() != 2 or points.shape[1] < 5:

@@ -19,8 +19,18 @@ NumPy's own draw sequence and reproduces the reference up to libm rounding.  Wit
 reproducible itself (a thread pool shares the global generator, :333-339); the device then uses a counter-based
 generator seeded from NumPy's global state (so np.random.seed() still controls it): same distribution, different draws.
 
-The fog / haze / spray modes of the reference (`average_augment`, `goodin_augment`) are not part of this path.
+The reference's other eight modes -- the fog, haze and spray modes ('chu_hogg_fog', 'strong_advection_fog',
+'moderate_advection_fog', 'coast_haze', 'continental_haze', 'moderate_spray', 'strong_spray': average_augment,
+lisa.py:340-388) and 'goodin et al.' (goodin_augment, :391-443) -- run on the engine with `all_modes=True`:
+
+    out = LISA(mode='strong_advection_fog', all_modes=True).augment(pc)              # (N, F + 2), Rr not used
+    out = LISA(mode='goodin et al.', all_modes=True).augment(pc, Rr=20.0, fixed_seed=True)
+
+Their detected rows draw NumPy's legacy Gaussians (np.random.normal) from its global generator, replayed on the device
+in the reference's order, so rows and NumPy's state afterwards are the reference's (values up to libm rounding).
+Without `all_modes` those modes raise NotImplementedError as before; making it the default is left to a later change.
 """
+import math
 import os
 import weakref
 from pathlib import Path
@@ -31,6 +41,12 @@ import torch
 from ..engine import default_engine
 
 _MODES = {'rain': (0, 1.328), 'gunn': (1, 1.3031), 'sekhon': (2, 1.3031)}
+# average_augment's modes: the gamma size law's (rho, alpha, g, Rc) (lisa.py:686-723); every one is water (1.328)
+_GAMMA_MODES = {'chu_hogg_fog': (20, 2, 0.5, 1), 'strong_advection_fog': (20, 3, 1., 10),
+                'moderate_advection_fog': (20, 3, 1., 8), 'coast_haze': (100, 1, 0.5, 0.05e-3),
+                'continental_haze': (100, 2, 0.5, 0.07), 'moderate_spray': (100, 6, 1., 2),
+                'strong_spray': (100, 6, 1., 4)}
+_GOODIN = 'goodin et al.'
 _SEED = 666                                         # lisa.py:55
 _DEVICE_MIE = weakref.WeakKeyDictionary()           # engine -> {(m, wavelength, nd, diameter_range): (D, qext, qback)}
 
@@ -72,6 +88,12 @@ def generate_mie_tables(pairs, save_path, engine=None):
     return paths
 
 
+def gamma_distribution_Nd(D, rho, alpha, g, Rc):
+    """The gamma size law (lisa.py:669-686), operation for operation: D in um, N(D) in cm^-3 um^-1"""
+    b = alpha / (g * Rc ** g)
+    return g * rho * b ** ((alpha + 1) / g) * (D / 2) ** alpha * np.exp(-b * (D / 2) ** g) / math.gamma((alpha + 1) / g)
+
+
 def _size_law(mode, Rr):
     """N0, Lambda of the exponential size distribution N(D) = N0 exp(-Lambda D) (lisa.py:497-664)."""
     if mode == 'rain':
@@ -84,16 +106,19 @@ def _size_law(mode, Rr):
 class LISA:
     def __init__(self, wavelength: float = 905, r_min: float = 0.9, r_max: float = 120, beam_divergence: float = 3e-3,
                  min_diameter: float = 0.05, range_accuracy: float = 0.09, signal: str = 'strongest', mode: str = 'rain',
-                 show_progressbar: bool = False, *, mie_table=None, engine=None) -> None:
-        if mode not in _MODES:
-            raise NotImplementedError(f"mode '{mode}': only the Monte-Carlo modes 'rain', 'gunn', 'sekhon' run on the engine")
+                 show_progressbar: bool = False, *, mie_table=None, engine=None, all_modes: bool = False) -> None:
+        """The reference's constructor.  all_modes (keyword only, default False): also accept the fog, haze and spray
+        modes and 'goodin et al.'; without it they raise NotImplementedError, as before it existed."""
+        if mode not in _MODES and not (all_modes and (mode in _GAMMA_MODES or mode == _GOODIN)):
+            raise NotImplementedError(f"mode '{mode}': only the Monte-Carlo modes 'rain', 'gunn', 'sekhon' run on the engine"
+                                      + ('' if all_modes else ' (pass all_modes=True for the other eight)'))
         if signal not in ('strongest', 'last'):
             raise ValueError('Invalid lidar return mode')
         self.r_min, self.r_max, self.signal, self.atm_model = r_min, r_max, signal, mode
         self.wavelength, self.min_diameter = wavelength, min_diameter
         self.range_accuracy, self.beam_divergence = range_accuracy, beam_divergence
         self.show_progressbar = show_progressbar
-        self.refractive_index = _MODES[mode][1]
+        self.refractive_index = _MODES[mode][1] if mode in _MODES else 1.328
         self.engine = engine
         self.D, self.qext = self._load_mie(mie_table)
         self._tables = {}
@@ -120,7 +145,18 @@ class LISA:
                                 f"it in lib/LISA/python/)")
 
     # ---- the reference's helpers the callers use (pointcloud_viewer.py:2794-2796) ------------------------------------
-    def Nd(self, D, Rr):
+    @property
+    def monte_carlo(self):
+        """whether the mode is one of the Monte-Carlo modes 'rain', 'gunn', 'sekhon' (monte_carlo_augment)"""
+        return self.atm_model in _MODES
+
+    def Nd(self, D, Rr=None):
+        """The mode's size distribution N(D) [m^-3 mm^-1] (lisa.py:497-723); Rr is not used by the gamma laws, and
+        Goodin's 'distribution' is np.array(Rr) (:485-487)"""
+        if self.atm_model == _GOODIN:
+            return np.array(Rr)
+        if self.atm_model in _GAMMA_MODES:
+            return 1e9 * gamma_distribution_Nd(D * 1e3, *_GAMMA_MODES[self.atm_model])
         n0, lam = _size_law(self.atm_model, Rr)
         return n0 * np.exp(-lam * D)
 
@@ -157,8 +193,21 @@ class LISA:
         n_max = self.density(Rr, self.min_diameter) * (np.pi / 3) * max(r_far, 1.0) * (half * max(r_far, 1.0) / self.r_max) ** 2
         return int(2 * (n_max + 2) + 128)
 
-    def augment(self, pc: np.ndarray, Rr, fixed_seed: bool = False) -> np.ndarray:
-        """LISA.monte_carlo_augment (lisa.py:293-341)."""
+    def _average_params(self, Rr):
+        """(model, alpha, range scale, p_min) of average_augment (model 0) or goodin_augment (model 1), computed with
+        NumPy as the reference does (lisa.py:355-361, 409-416, 421).  Goodin with Rr=None raises TypeError, as there."""
+        if self.atm_model == _GOODIN:
+            alpha = float(self.alpha(np.array(Rr)))
+            return 1, alpha, float((1 - np.exp(-Rr)) ** 2), 0.9 * self.r_max ** (-2) / np.pi
+        return 0, float(self.alpha(self.Nd(self.D, Rr=Rr))), 0.0, 0.9 * self.r_max ** (-2)
+
+    def augment(self, pc: np.ndarray, Rr=None, fixed_seed: bool = False) -> np.ndarray:
+        """LISA.monte_carlo_augment (lisa.py:293-341), or with all_modes LISA.average_augment (:340-388, Rr not used) /
+        LISA.goodin_augment (:391-443).  The Monte-Carlo modes and Goodin need Rr."""
+        if not self.monte_carlo:
+            return self._average_augment(pc, Rr, fixed_seed)
+        if Rr is None:
+            raise TypeError("augment() missing the rain rate Rr of the Monte-Carlo modes")
         engine = self.engine or default_engine()
         pc = np.ascontiguousarray(pc, dtype=np.float64)
         if pc.ndim != 2 or pc.shape[1] < 4:
@@ -188,6 +237,42 @@ class LISA:
                 need *= 4                                              # the draw table was too short for some return
         return out.cpu().numpy()
 
+    def _average_augment(self, pc, Rr, fixed_seed):
+        """average_augment / goodin_augment of one cloud: lss_lisa_average_batch with one cloud"""
+        model, alpha, scale, p_min = self._average_params(Rr)
+        engine = self.engine or default_engine()
+        pc = np.ascontiguousarray(pc, dtype=np.float64)
+        if pc.ndim != 2 or pc.shape[1] < 4:
+            raise ValueError('pc must be (N, >= 4): x, y, z, intensity')
+        d_pc = torch.from_numpy(pc).to(engine.device)
+        out = engine.lisa_average_batch(d_pc, [0, pc.shape[0]], model, alpha, p_min, r_min=float(self.r_min),
+                                        range_accuracy=float(self.range_accuracy), range_scale=scale,
+                                        fixed_seed=fixed_seed)
+        engine.check()
+        return out.cpu().numpy()
+
+    def _average_augment_batch(self, points, off, Rr, counts, apply, fixed_seed):
+        """augment_batch of the fog / haze / spray modes and Goodin: lss_lisa_average_cloud_batch"""
+        B = off.shape[0] - 1
+        ap = np.ones(B, dtype=bool) if apply is None else np.asarray(apply, dtype=bool).reshape(B)
+        alpha, scale = np.zeros(B), np.zeros(B)
+        model, p_min = (1, 0.9 * self.r_max ** (-2) / np.pi) if self.atm_model == _GOODIN else (0, 0.9 * self.r_max ** (-2))
+        if model == 0:
+            alpha[:] = self._average_params(None)[1]
+        else:
+            rr = Rr if np.ndim(Rr) else [Rr] * B
+            if len(rr) != B:
+                raise ValueError(f'Rr: {len(rr)} rain rates for {B} clouds')
+            for b in np.flatnonzero(ap):
+                _, alpha[b], scale[b], _ = self._average_params(rr[b])
+        engine = self.engine or default_engine()
+        out = engine.lisa_average_cloud_batch(points, off, model, alpha, p_min, r_min=float(self.r_min),
+                                              range_accuracy=float(self.range_accuracy),
+                                              range_scale=scale if model == 1 else None, counts=counts, apply=ap,
+                                              fixed_seed=fixed_seed)
+        engine.check()
+        return out
+
     def augment_batch(self, points, cloud_offsets, Rr, counts=None, apply=None, fixed_seed=False, seeds=None):
         """The dataset's LISA block (dense_dataset.py:732-746) on a batch of device-resident clouds, one call.
 
@@ -199,9 +284,17 @@ class LISA:
         augment's two np.random.randint calls (`seeds` passes keys drawn elsewhere instead, one per cloud), so each
         sees the NumPy state a loop of augment calls would give it.  Runs on the current stream without synchronising,
         except with fixed_seed, which checks (and grows) the draw table like augment.
+        With all_modes' fog, haze and spray modes (Rr not used) and 'goodin et al.' (Rr per cloud), the applied clouds'
+        detected rows draw NumPy's legacy Gaussians in batch order (with fixed_seed each from np.random.seed(666)); the
+        call synchronises once and leaves NumPy's state as B augment calls would; `seeds` is rejected.
         Returns dict(points (N, F) float32: kept rows at the front of each slot; counts (B,) int32; n_lost (B,) int32)."""
-        engine = self.engine or default_engine()
         off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+        if not self.monte_carlo:
+            if seeds is not None:
+                raise ValueError(f"seeds: mode '{self.atm_model}' draws NumPy's Gaussians itself; seeds are for the "
+                                 f"Monte-Carlo modes")
+            return self._average_augment_batch(points, off, Rr, counts, apply, fixed_seed)
+        engine = self.engine or default_engine()
         B = off.shape[0] - 1
         rr = np.broadcast_to(np.asarray(Rr, dtype=np.float64), (B,))
         ap = np.ones(B, dtype=bool) if apply is None else np.asarray(apply, dtype=bool).reshape(B)
