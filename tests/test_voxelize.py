@@ -29,11 +29,11 @@ def literal_rule(points, rng, vsize, max_points, max_voxels):
         coor = [0, 0, 0]
         failed = False
         for j in range(3):
-            c = int(np.floor((np.float32(points[i, j]) - rng[j]) / vsize[j]))
-            if c < 0 or c >= gs[j]:
+            c = np.floor((np.float32(points[i, j]) - rng[j]) / vsize[j])
+            if not (c >= 0 and c < gs[j]):          # (a NaN or infinite quotient casts to INT_MIN in C++: skipped)
                 failed = True
                 break
-            coor[2 - j] = c
+            coor[2 - j] = int(c)
         if failed:
             continue
         vid = lut[coor[0], coor[1], coor[2]]
