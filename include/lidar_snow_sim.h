@@ -262,6 +262,27 @@ LSS_API lss_status lss_wet_ground_batch_params(lss_engine *e, const float *d_poi
                                                int32_t *d_out_ymins, void *d_workspace, int64_t workspace_bytes,
                                                void *stream);
 LSS_API int64_t lss_wet_ground_workspace_bytes(int64_t n_total, int n_clouds);
+/* lss_wet_ground_batch_params with estimation_method='poly' (augmentation.py:171-192, 223-228, 243-246): the laser power
+ * is np.polyfit(d, I/cos, 2) over the ground points and the noise floor ransac_polyfit(x, min_vals, order=2) over the
+ * minima points of the linear path, its 100 trials drawn from NumPy's legacy RandomState (np.random.randint(m, size=15)
+ * each), the clouds in batch order as B sequential calls draw them.
+ *   h_mt_state        uint32[625] host: the state before the batch, the 624 key words then pos (np.random.get_state())
+ *   d_mt_state_out    uint32[625] device: the state after the batch, in the same layout
+ *   d_out_poly_fit    float64[n_clouds*8] or NULL: p0, p1, p2, pmin0, pmin1, pmin2 (highest power first), the chosen
+ *                     trial (-1: the fit on all minima points) and m, the number of minima points
+ * d_out_passthrough adds code 3: no minima point (m == 0), where the reference raises TypeError before any draw; the cloud
+ * is returned unchanged and nothing is latched.  A cloud with passthrough 1, 2 or 3 draws nothing.  Everything else as
+ * lss_wet_ground_batch_params.                                                                                         */
+LSS_API lss_status lss_wet_ground_batch_poly(lss_engine *e, const float *d_points, const int64_t *h_cloud_offsets,
+                                             const int32_t *d_cloud_counts, int n_clouds, const double *h_water_height,
+                                             double pavement_depth, double noise_floor, double power_factor,
+                                             int flat_earth, double delta, int replace, const double *h_plane_in,
+                                             const int32_t *h_ymins_in, const uint32_t *h_mt_state,
+                                             float *d_out_points, double *d_out_intensity64, int32_t *d_out_counts,
+                                             int32_t *d_out_passthrough, double *d_out_plane, double *d_out_fit,
+                                             int32_t *d_out_ymins, uint32_t *d_mt_state_out, double *d_out_poly_fit,
+                                             void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_wet_ground_poly_workspace_bytes(int64_t n_total, int n_clouds);
 
 /* ---- fog simulation ("next" row, SURVEY.md 8f-3) -----------------------------------------------------------------------
  * Batched simulate_fog() (lib/LiDAR_fog_sim/fog_simulation.py:299-316: P_R_fog_hard :183-189, P_R_fog_soft :192-296) on

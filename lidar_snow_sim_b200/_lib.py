@@ -95,6 +95,10 @@ SIGNATURES = [
                                                _c.c_int, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P,
                                                _P, _c.c_int64, _P]),
     ('lss_wet_ground_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_wet_ground_batch_poly', _c.c_int, [_P, _P, _P, _P, _c.c_int, _P, _c.c_double, _c.c_double, _c.c_double,
+                                             _c.c_int, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P,
+                                             _P, _P, _P, _c.c_int64, _P]),
+    ('lss_wet_ground_poly_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_fog_batch', _c.c_int, [_P, _P, _c.c_int, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _P, _c.c_uint32,
                                  _c.c_int, _c.c_int, _P, _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_fog_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),

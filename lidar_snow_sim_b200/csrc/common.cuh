@@ -443,7 +443,31 @@ __device__ __forceinline__ double lss_plane_dot(double x, double y, double z, co
 {
     return __dadd_rn(__dadd_rn(__dmul_rn(x, w[0]), __dmul_rn(y, w[1])), __dmul_rn(z, w[2]));
 }
-int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds);
+// poly: the workspace of a pre-pass with PrepassIO::d_wet_poly (wet ground's estimation_method='poly')
+int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds, bool poly = false);
+// Least squares c0 + c1 t + c2 t^2 from the sums s0..s4 = S t^0..4 and r0..r2 = S y t^0..2: the normal equations by
+// Gaussian elimination with partial pivoting; c = 0 when a pivot vanishes
+__device__ __forceinline__ void lss_solve3(double s0, double s1, double s2, double s3, double s4, double r0, double r1,
+                                           double r2, double (&c)[3])
+{
+    double A[3][4] = {{s0, s1, s2, r0}, {s1, s2, s3, r1}, {s2, s3, s4, r2}};
+    for (int q = 0; q < 3; q++) {
+        int piv = q;
+        for (int r = q + 1; r < 3; r++) if (fabs(A[r][q]) > fabs(A[piv][q])) piv = r;
+        if (!(fabs(A[piv][q]) >= 1e-300)) { c[0] = c[1] = c[2] = 0.0; return; }
+        for (int k = 0; k < 4; k++) { const double t = A[q][k]; A[q][k] = A[piv][k]; A[piv][k] = t; }
+        for (int r = q + 1; r < 3; r++) {
+            const double f = A[r][q] / A[q][q];
+            for (int k = q; k < 4; k++) A[r][k] -= f * A[q][k];
+        }
+    }
+    c[2] = A[2][3] / A[2][2];
+    c[1] = (A[1][3] - A[1][2] * c[2]) / A[1][1];
+    c[0] = (A[0][3] - A[0][1] * c[1] - A[0][2] * c[2]) / A[0][0];
+}
+// wet ground, estimation_method='poly': the pre-pass's record per cloud (k_wet_poly_prep): p0, p1, p2 of
+// np.polyfit(d, I/cos, 2), m, then the m minima points' x and y (augmentation.py:232-241) in slots of 50
+constexpr int LSS_WET_POLY_REC = 104;
 // Optional inputs / outputs of the pre-pass.  The two host inputs replay what the reference host drew / picked
 // (sklearn RANSAC plane, np.argpartition's pick among the least populated bins) so that everything downstream can be
 // compared with reference-generated fixtures; NULL = the device's own deterministic choice.
@@ -459,6 +483,9 @@ struct PrepassIO {
     // a cloud with at least this many ground points latches LSS_ERR_INTENSITY_RANGE when its I/cos range is degenerate
     // (the snowfall path fits from 3 ground points on; wet ground returns below 1000 first, augmentation.py:51-52)
     int range_min_ground = 3;
+    // device [B * LSS_WET_POLY_REC]: wet ground's estimation_method='poly' (k_wet_poly_prep); non-null selects the
+    // pre-pass's poly workspace (lss_prepass_ws_bytes(.., true)) and adds the sums the fit needs to the ground pass
+    double *d_wet_poly = nullptr;
 };
 // Adds the pre-pass's staging to a caller's StageList: the zero fill of its per-cloud records and the upload of io's host
 // inputs.  The pre-pass enqueues no staging of its own: every caller of lss_prepass_run must have added this to its own

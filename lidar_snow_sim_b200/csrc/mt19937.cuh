@@ -62,6 +62,7 @@ __device__ __forceinline__ int smear(int i)
     return (int)m;
 }
 
+#ifndef LSS_MT_WORDS_ONLY
 struct Chain { int b, i, pos, cur, done; };
 
 // The chain of one CTA of MT_TPB threads over the clouds of `cl`, from the key block key_at(0 .. 623) at position pos0
@@ -229,5 +230,7 @@ __global__ void __launch_bounds__(SHUF_TPB) k_shuffle(ShufArgs a)
         if (!__syncthreads_or(left)) break;
     }
 }
+
+#endif  // LSS_MT_WORDS_ONLY
 
 }  // namespace

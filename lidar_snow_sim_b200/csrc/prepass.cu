@@ -445,9 +445,13 @@ __device__ __forceinline__ int ground_blocks(int n, int launched)
     return min(launched, max(1, (n + PP_TPB * 8 - 1) / (PP_TPB * 8)));
 }
 
+// POLY (wet ground, estimation_method='poly'): also S y, S y t, S y t^2 with y = I/cos, for np.polyfit(d, I/cos, 2)
+// (augmentation.py:225-226); the block's record is then 19 doubles, the three sums after vmax.
+template <bool POLY>
 __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
 {
-    __shared__ double red[15 * (PP_TPB / 32)];
+    constexpr int NV = POLY ? 18 : 15;
+    __shared__ double red[NV * (PP_TPB / 32)];
     __shared__ double mx[PP_TPB / 32];
     const int b = blockIdx.y;
     const CloudPre cp = a.cp[b];
@@ -457,7 +461,7 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
     if ((int)blockIdx.x >= nb) return;
     const int lane = threadIdx.x & 31;
     // 0 n, 1-4 first regression (shifted), 5-8 S t .. S t^4, 9-11 S cos t^k, 12-14 S d cos t^k
-    double v[15] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    double v[NV] = {};
     double vmax = -1e300;
     // every thread sums its own rows in ascending order (the bits of the polynomial depend on it); the loop runs per warp
     // so that the warp can append its records together
@@ -480,6 +484,7 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
             v[5] += t; v[6] += t2; v[7] += t2 * t; v[8] += t2 * t2;
             v[9] += c; v[10] += c * t; v[11] += c * t2;
             v[12] += dc; v[13] += dc * t; v[14] += dc * t2;
+            if constexpr (POLY) { const double y = g.norm_i; v[15] += y; v[16] += y * t; v[17] += y * t2; }
             if (g.norm_i >= 4.5) bx = edge_bin(g.d, 10.0, 70.0, HIST_NX);
         }
         const unsigned m = __ballot_sync(0xffffffffu, bx >= 0);
@@ -497,17 +502,18 @@ __global__ void __launch_bounds__(PP_TPB) k_ground_stats(PreArgs a)
 #pragma unroll
     for (int s = 16; s > 0; s >>= 1) vmax = nan_max(vmax, __shfl_down_sync(0xffffffffu, vmax, s));
     if ((threadIdx.x & 31) == 0) mx[threadIdx.x >> 5] = vmax;
-    block_sum<15>(v, red);
+    block_sum<NV>(v, red);
     if (threadIdx.x == 0) {
         for (int q = 0; q < PP_TPB / 32; q++) vmax = nan_max(vmax, mx[q]);
-        double *p = a.partial + ((size_t)b * a.max_blocks + blockIdx.x) * 16;
+        double *p = a.partial + ((size_t)b * a.max_blocks + blockIdx.x) * (POLY ? 19 : 16);
         for (int k = 0; k < 15; k++) p[k] = v[k];
         p[15] = vmax;
+        if constexpr (POLY) { p[16] = v[15]; p[17] = v[16]; p[18] = v[17]; }
     }
 }
 
 // fixed-order reduction of the per-block partials: one warp per cloud, lane q owns partials q, q+32, ...
-template <int NV>
+template <int NV, int STRIDE = 16>
 __device__ __forceinline__ void warp_reduce_partials(const double *partial, int n_blocks, double (&v)[NV], double *vmax)
 {
     const int lane = threadIdx.x & 31;
@@ -515,7 +521,7 @@ __device__ __forceinline__ void warp_reduce_partials(const double *partial, int 
     for (int k = 0; k < NV; k++) v[k] = 0.0;
     double m = -1e300;
     for (int q = lane; q < n_blocks; q += 32) {
-        const double *p = partial + (size_t)q * 16;
+        const double *p = partial + (size_t)q * STRIDE;
 #pragma unroll
         for (int k = 0; k < NV; k++) v[k] += p[k];
         if (vmax) m = nan_max(m, p[NV]);
@@ -539,6 +545,8 @@ __device__ __forceinline__ void warp_reduce_partials(const double *partial, int 
 #endif
 constexpr int HIST_SLAB = LSS_HIST_SLAB, HIST_SLABS = (HIST_NX + HIST_SLAB - 1) / HIST_SLAB, HIST_TPB = 512;
 
+// STRIDE: doubles per block record of the ground pass (16, or 19 for k_ground_stats<true>)
+template <int STRIDE>
 __global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_blocks)
 {
     extern __shared__ unsigned hist[];         // [HIST_SLAB * HIST_NY]
@@ -549,7 +557,8 @@ __global__ void __launch_bounds__(HIST_TPB) k_ground_hist(PreArgs a, int n_block
     if (warp == 0) {
         double v[15], vmax;
         const int n = a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - a.cloud_off[b]);
-        warp_reduce_partials<15>(a.partial + (size_t)b * a.max_blocks * 16, ground_blocks(n, n_blocks), v, &vmax);
+        warp_reduce_partials<15, STRIDE>(a.partial + (size_t)b * a.max_blocks * STRIDE, ground_blocks(n, n_blocks), v,
+                                         &vmax);
         if (lane == 0) {
             stat[0] = v[0];
             stat[1] = fabs(vmax);
@@ -710,11 +719,51 @@ __global__ void k_poly_solve(PreArgs a, double *poly_out /* [B*3] or null */, do
     if (ymins_out) for (int k = 0; k < HIST_NX; k++) ymins_out[b * HIST_NX + k] = picked ? a.ymins[b * HIST_NX + k] : -1;
 }
 
+// ---- 8. estimation_method='poly' of wet ground (augmentation.py:223-241): one warp per cloud ------------------------------
+// p = np.polyfit(d, I/cos, 2) over the ground points from the ground pass's sums S t^k and S y t^k, t = (d - 40) / 30,
+// solved as k_poly_solve solves its fit; and the minima points (x, min_vals) of the linear path, in range-bin order.
+// rec [B * LSS_WET_POLY_REC]: p0, p1, p2, m, x[50], y[50] (common.cuh).
+__global__ void k_wet_poly_prep(PreArgs a, int n_blocks, double *rec)
+{
+    const int b = blockIdx.x, lane = threadIdx.x & 31;
+    const CloudPre &cp = a.cp[b];
+    const int n = a.cloud_cnt ? a.cloud_cnt[b] : (int)(a.cloud_off[b + 1] - a.cloud_off[b]);
+    const double *part = a.partial + (size_t)b * a.max_blocks * 19;
+    double v[3] = {0, 0, 0};                          // the order of warp_reduce_partials
+    for (int q = lane; q < ground_blocks(n, n_blocks); q += 32)
+        for (int k = 0; k < 3; k++) v[k] += part[(size_t)q * 19 + 16 + k];
+    for (int s = 16; s > 0; s >>= 1)
+        for (int k = 0; k < 3; k++) v[k] += __shfl_xor_sync(0xffffffffu, v[k], s);
+    if (lane != 0) return;
+    double *r = rec + (size_t)b * LSS_WET_POLY_REC;
+    double c[3] = {0, 0, 0};
+    if (cp.n_ground >= 3) lss_solve3(cp.mom[0], cp.mom[1], cp.mom[2], cp.mom[3], cp.mom[4], v[0], v[1], v[2], c);
+    const double m = 40.0, sc = 30.0;                 // t = (d - m) / sc
+    r[0] = c[2] / (sc * sc);
+    r[1] = c[1] / sc - 2.0 * c[2] * m / (sc * sc);
+    r[2] = c[0] - c[1] * m / sc + c[2] * m * m / (sc * sc);
+    int k_out = 0;
+    if (cp.n_ground >= 3 && lss_intensity_range_ok(cp.ymax)) {
+        double ylo, yhi, x, y;
+        intensity_edges(cp.ymax, ylo, yhi);
+        const double ystep = (yhi - ylo) / HIST_NY;
+        for (int k = 0; k < HIST_NX; k++)
+            if (minima_point(k, a.ymins[b * HIST_NX + k], ylo, yhi, ystep, x, y)) {
+                r[4 + k_out] = x;
+                r[4 + HIST_NX + k_out] = y;
+                k_out++;
+            }
+    }
+    r[3] = k_out;
+}
+
 }  // namespace
 
 // The workspace, region by region.  The staging region is reused for the histogram records (8 + 1 bytes per row).
 // plane_in / ymins_in: where a caller's planes [B * 4] and bin picks [B * HIST_NX] are uploaded.
-static void prepass_carve(WsCarve &c, PreArgs &a, double *&plane_in, int32_t *&ymins_in, int64_t n_total, int n_clouds)
+// poly: the ground pass's block records carry the three sums of k_ground_stats<true>
+static void prepass_carve(WsCarve &c, PreArgs &a, double *&plane_in, int32_t *&ymins_in, int64_t n_total, int n_clouds,
+                          bool poly)
 {
     a.max_blocks = 64;
     a.cp = c.take<CloudPre>(n_clouds);
@@ -726,19 +775,19 @@ static void prepass_carve(WsCarve &c, PreArgs &a, double *&plane_in, int32_t *&y
     a.tile_cnt = c.take<int>(n_total / 32 + n_clouds + 2);
     a.tile_base = c.take<int32_t>(n_clouds + 1);
     a.trial = c.take<double>((int64_t)n_clouds * RANSAC_T * 8);
-    a.partial = c.take<double>((int64_t)n_clouds * a.max_blocks * 16);
+    a.partial = c.take<double>((int64_t)n_clouds * a.max_blocks * (poly ? 19 : 16));
     plane_in = c.take<double>((int64_t)n_clouds * 4);
     a.ymins = c.take<int32_t>((int64_t)n_clouds * HIST_NX);
     ymins_in = c.take<int32_t>((int64_t)n_clouds * HIST_NX);
 }
 
-int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds)
+int64_t lss_prepass_ws_bytes(int64_t n_total, int n_clouds, bool poly)
 {
     WsCarve c;
     PreArgs a;
     double *plane_in;
     int32_t *ymins_in;
-    prepass_carve(c, a, plane_in, ymins_in, n_total, n_clouds);
+    prepass_carve(c, a, plane_in, ymins_in, n_total, n_clouds, poly);
     return c.used;
 }
 
@@ -748,7 +797,7 @@ void lss_prepass_stage(StageList &l, const PrepassIO &io, void *d_ws, int64_t n_
     PreArgs a;
     double *d_plane;
     int32_t *d_ymins_in;
-    prepass_carve(c, a, d_plane, d_ymins_in, n_total, n_clouds);
+    prepass_carve(c, a, d_plane, d_ymins_in, n_total, n_clouds, io.d_wet_poly != nullptr);
     l.zero(a.cp,(size_t)((char *)a.rec_cnt - (char *)a.cp) + sizeof(int) * n_clouds);   // records and record cursors
     if (io.h_ymins_in) l.upload(d_ymins_in, io.h_ymins_in, sizeof(int32_t) * HIST_NX * n_clouds);
     if (io.h_plane_in) l.upload(d_plane, io.h_plane_in, sizeof(double) * 4 * n_clouds);
@@ -808,7 +857,8 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
     WsCarve c{(char *)d_ws};
     double *d_plane;
     int32_t *d_ymins_in;
-    prepass_carve(c, a, d_plane, d_ymins_in, N, B);
+    const bool poly = io.d_wet_poly != nullptr;
+    prepass_carve(c, a, d_plane, d_ymins_in, N, B, poly);
     if (lss_status rc = lss_prepass_check(e, h_cloud_off, B, h_plane_in != nullptr)) return rc;
     if (ws_bytes < c.used) return lss_fail(e, LSS_ERR_WORKSPACE, "pre-pass workspace too small");
     a.pts = d_pts;
@@ -847,13 +897,23 @@ lss_status lss_prepass_run(lss_engine *e, const float *d_pts, const int64_t *d_c
             LSS_CUDA_CHECK(e, lss_launch(e, k_ransac_trials, dim3(RANSAC_T, B), PP_TPB, 0, stream, a));
             LSS_CUDA_CHECK(e, lss_launch(e, k_ransac_refit, B, PP_TPB, 0, stream, a));
         }
-        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats, dim3(nblk, B), PP_TPB, 0, stream, a));
         const size_t hist_smem = sizeof(unsigned) * HIST_SLAB * HIST_NY;
-        if (hist_smem > 48 * 1024)
-            LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_ground_hist, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)hist_smem));
-        LSS_CUDA_CHECK(e, lss_launch(e, k_ground_hist, dim3(HIST_SLABS, B), HIST_TPB, hist_smem, stream, a, nblk));
+        if (poly) {
+            LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats<true>, dim3(nblk, B), PP_TPB, 0, stream, a));
+            if (hist_smem > 48 * 1024)
+                LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_ground_hist<19>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       (int)hist_smem));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_ground_hist<19>, dim3(HIST_SLABS, B), HIST_TPB, hist_smem, stream, a, nblk));
+        } else {
+            LSS_CUDA_CHECK(e, lss_launch(e, k_ground_stats<false>, dim3(nblk, B), PP_TPB, 0, stream, a));
+            if (hist_smem > 48 * 1024)
+                LSS_CUDA_CHECK(e, cudaFuncSetAttribute(k_ground_hist<16>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                       (int)hist_smem));
+            LSS_CUDA_CHECK(e, lss_launch(e, k_ground_hist<16>, dim3(HIST_SLABS, B), HIST_TPB, hist_smem, stream, a, nblk));
+        }
         LSS_CUDA_CHECK(e, lss_launch(e, k_poly_solve, B, 32, 0, stream, a, d_poly_out, d_plane_out, io.d_fit_out,
                                      io.d_ymins_out));
+        if (poly) LSS_CUDA_CHECK(e, lss_launch(e, k_wet_poly_prep, B, 32, 0, stream, a, nblk, io.d_wet_poly));
     }
     return LSS_OK;
 }

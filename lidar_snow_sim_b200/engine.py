@@ -417,7 +417,7 @@ class SnowfallEngine:
 
     def wet_ground_batch(self, points, cloud_offsets, counts=None, water_height=0.001, pavement_depth=0.0012,
                          noise_floor=0.7, power_factor=15, flat_earth=False, delta=0.5, replace=True, plane=None,
-                         want_intensity64=False, ymins=None, out=None, want_fits=False):
+                         want_intensity64=False, ymins=None, out=None, want_fits=False, estimation_method='linear'):
         """
         Batched ground_water_augmentation() on device-resident clouds (current stream, no synchronisation).
         counts: optional CUDA int32 (B,) valid rows per cloud slot (fused snow -> wet path).
@@ -426,22 +426,43 @@ class SnowfallEngine:
         Returns dict(points (N,5) float32 slot-compacted, counts (B,), passthrough (B,), plane (B,4) [, intensity64]
         [, fits (B,8) float64, picks (B,50) int32 with want_fits, laid out as in noise_threshold_poly]).
         passthrough: 0 augmented, 1 fewer than 1000 ground points, 2 degenerate I/cos range (check() raises ValueError).
+        estimation_method='poly' (lss_wet_ground_batch_poly): the quadratic laser power and the RANSAC noise floor of
+        augmentation.py:171-192,223-246, drawn on NumPy's global RandomState, whose state is then set as B sequential
+        calls leave it (the call synchronises once to copy it back).  water_height is forwarded once per cloud, check()
+        raises for no cloud, and passthrough adds 3: no minima point, where the reference raises TypeError.  want_fits
+        adds poly_fits (B,8) float64: p0, p1, p2, pmin0, pmin1, pmin2, the chosen trial (-1: the full fit), m.
         """
+        if estimation_method not in ('linear', 'poly'):
+            raise ValueError(f"estimation_method: 'linear' or 'poly', got {estimation_method!r}")
+        poly = estimation_method == 'poly'
         off, B, N = _cloud_offsets(cloud_offsets)
         _check_tensor('points', points, self.device, torch.float32, (N, 5))
         _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
         pl = None if plane is None else np.ascontiguousarray(plane, dtype=np.float64).reshape(B, 4)
         ym = None if ymins is None else np.ascontiguousarray(ymins, dtype=np.int32).reshape(B, 50)
-        per_cloud = np.ndim(water_height) > 0
+        per_cloud = np.ndim(water_height) > 0 or poly
         if per_cloud:
-            heights = np.ascontiguousarray(water_height, dtype=np.float64).reshape(-1)
+            heights = np.ascontiguousarray(np.broadcast_to(np.asarray(water_height, dtype=np.float64),
+                                                           (B,) if np.ndim(water_height) == 0 else np.shape(water_height)))
+            heights = heights.reshape(-1)
             if heights.shape[0] != B:
                 raise ValueError(f'water_height: {heights.shape[0]} heights for {B} clouds')
         # (pass the returned dict back in as `out` to reuse the buffers)
         out = _outputs(out, self.device, points=((N, 5), torch.float32), counts=((B,), torch.int32),
                        passthrough=((B,), torch.int32), plane=((B, 4), torch.float64),
                        intensity64=want_intensity64 and ((N,), torch.float64), fits=want_fits and ((B, 8), torch.float64),
-                       picks=want_fits and ((B, 50), torch.int32))
+                       picks=want_fits and ((B, 50), torch.int32),
+                       poly_fits=poly and want_fits and ((B, 8), torch.float64), state=poly and ((625,), torch.int32))
+        if poly:
+            words, start = _mt_state()
+            ws = self._scratch('wet', self.lib.lss_wet_ground_poly_workspace_bytes(N, B))
+            self._call('lss_wet_ground_batch_poly', points, _ptr(off), counts, B, _ptr(heights), float(pavement_depth),
+                       float(noise_floor), float(power_factor), 1 if flat_earth else 0, float(delta), 1 if replace else 0,
+                       _ptr(pl), _ptr(ym), _ptr(words), out['points'], out.get('intensity64') if want_intensity64 else None,
+                       out['counts'], out['passthrough'], out['plane'], out.get('fits') if want_fits else None,
+                       out.get('picks') if want_fits else None, out['state'], out.get('poly_fits'), ws, ws.numel())
+            _set_mt_state(start, out.pop('state'))
+            return out
         ws = self._scratch('wet', self.lib.lss_wet_ground_workspace_bytes(N, B))
         self._call('lss_wet_ground_batch_params' if per_cloud else 'lss_wet_ground_batch', points, _ptr(off), counts, B,
                    _ptr(heights) if per_cloud else float(water_height), float(pavement_depth), float(noise_floor),
