@@ -812,6 +812,52 @@ LSS_API lss_status lss_pa_apply_batch(lss_engine *e, const float *d_points, int 
                                       const double *d_normals, int64_t n_out, void *d_out, int out_f64,
                                       void *d_workspace, int64_t workspace_bytes, void *stream);
 
+/* PA-AUG's robustness test sets (PartAwareAugmentation.create_robusteness_test_data) on a batch of device-resident
+ * clouds.  KITTI-D runs on lss_pa_partition_batch / lss_pa_apply_batch with a host plan; these are KITTI-S and KITTI-J.
+ * lss_pa_fps_cloud_batch: farthest_point_sampling over every whole cloud (KITTI-S, sparse_robustness_test): K_b picks from
+ *   row h_start[b] (the caller's np.random.randint(n_b)), distances in float64 ((dx^2 + dy^2) + dz^2), the running
+ *   minimum propagating NaN, each pick np.argmax's (a NaN first, then the first maximum).  A float32 cloud of at most the
+ *   on-chip capacity runs on one thread-block cluster with its rows in shared memory; a larger cloud, and every cloud of
+ *   float64 rows, runs on one CTA over float64 rows in the workspace.
+ *   d_points        float32 (points_f64 == 0) or float64 (N, n_features), n_features >= 3; cloud b at rows
+ *                   h_cloud_offsets[b].., its first h_cloud_counts[b] rows (host int32 [B], or NULL: the slot)
+ *   h_k, h_start    host int32 [B]: picks (>= 1 for a cloud with rows) and the first pick (< the cloud's rows)
+ *   d_out           (sum K_b, n_features) of the input's dtype: cloud b's picked rows in pick order from the exclusive
+ *                   prefix of h_k;  d_out_index int32 [sum K_b]: the picks, row indices inside the cloud
+ * lss_pa_fps_cloud_config: on `device`, the cluster size a call whose largest on-chip cloud has n_rows rows launches
+ *   with (0 when n_rows is above the capacity), and the capacity: the most rows a cloud may have to run on-chip.
+ * lss_pa_noise_test_batch: KITTI-N (generate_noise_robustness_test): per cloud np.random.choice(range(n_b), k_b,
+ *   replace=False) (np.random.permutation(n_b)[:k_b]) then 4 k_b uniforms, clouds in turn on NumPy's MT19937 stream from
+ *   h_mt_state (625 words); the kept rows in order, widened to float64, then the noise rows low + (high - low) u of
+ *   columns 0..3.  d_out float64 (sum n_b, 4), cloud b at the prefix of n_b; h_cloud_counts host int32 [B] or NULL; h_k
+ *   host int32 [B].  Only clouds below n_draw_clouds draw; the draws stop after the first cloud with a non-finite range,
+ *   whose columns drawn (< 4) d_out_columns (int32 [B]) reports; d_mt_state_out the state after the last draw.
+ * lss_pa_jitter_test_batch: KITTI-J (jitter_robustness_test): np.random.normal(0, sigma, (n_b, 3)) per cloud from the
+ *   legacy Gaussian stream, clouds chained in batch order; x = x + noise in float64, stored in the rows' dtype; the other
+ *   columns copied.  h_out_offsets: int64 [B + 1] exact-size output slots of n_b rows; h_gauss_state / d_gauss_state_out
+ *   the 630-word state records of lss_lisa_average_batch.                                                             */
+LSS_API lss_status lss_pa_fps_cloud_config(int device, int64_t n_rows, int *cluster_size, int64_t *capacity);
+LSS_API int64_t lss_pa_fps_cloud_workspace_bytes(const int64_t *h_cloud_offsets, const int32_t *h_cloud_counts,
+                                                 const int32_t *h_k, int n_clouds, int points_f64);
+LSS_API lss_status lss_pa_fps_cloud_batch(lss_engine *e, const void *d_points, int points_f64, int n_features,
+                                          const int64_t *h_cloud_offsets, const int32_t *h_cloud_counts, int n_clouds,
+                                          const int32_t *h_k, const int32_t *h_start, void *d_out,
+                                          int32_t *d_out_index, void *d_workspace, int64_t workspace_bytes,
+                                          void *stream);
+LSS_API int64_t lss_pa_noise_test_workspace_bytes(const int64_t *h_cloud_offsets, const int32_t *h_cloud_counts,
+                                                  const int32_t *h_k, int n_clouds);
+LSS_API lss_status lss_pa_noise_test_batch(lss_engine *e, const void *d_points, int points_f64, int n_features,
+                                           const int64_t *h_cloud_offsets, const int32_t *h_cloud_counts, int n_clouds,
+                                           const int32_t *h_k, int n_draw_clouds, const uint32_t *h_mt_state,
+                                           double *d_out, int32_t *d_out_columns, uint32_t *d_mt_state_out,
+                                           void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_pa_jitter_test_workspace_bytes(int64_t n_total, int n_clouds);
+LSS_API lss_status lss_pa_jitter_test_batch(lss_engine *e, const void *d_points, int points_f64, int n_features,
+                                            const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts,
+                                            int n_clouds, const int64_t *h_out_offsets, double sigma,
+                                            const uint32_t *h_gauss_state, void *d_out, uint32_t *d_gauss_state_out,
+                                            void *d_workspace, int64_t workspace_bytes, void *stream);
+
 /* OpenPCDet's DATA_AUGMENTOR point path (gt_sampling, random_world_flip / rotation / scaling) on a batch of device-
  * resident clouds, in two calls around the host planner (lidar_snow_sim_b200/augmentor/plan.py), which replays the
  * reference's random draws and does the box-level work.

@@ -149,6 +149,16 @@ SIGNATURES = [
     ('lss_camera_fov_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
     ('lss_pa_partition_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int]),
     ('lss_pa_partition_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _c.c_int, _P, _P, _c.c_int64, _P]),
+    ('lss_pa_fps_cloud_config', _c.c_int, [_c.c_int, _c.c_int64, _P, _P]),
+    ('lss_pa_fps_cloud_workspace_bytes', _c.c_int64, [_P, _P, _P, _c.c_int, _c.c_int]),
+    ('lss_pa_fps_cloud_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _P, _P, _c.c_int64,
+                                          _P]),
+    ('lss_pa_noise_test_workspace_bytes', _c.c_int64, [_P, _P, _P, _c.c_int]),
+    ('lss_pa_noise_test_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _c.c_int, _P, _P, _P, _P, _P,
+                                           _c.c_int64, _P]),
+    ('lss_pa_jitter_test_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_pa_jitter_test_batch', _c.c_int, [_P, _P, _c.c_int, _c.c_int, _P, _P, _c.c_int, _P, _c.c_double, _P, _P, _P,
+                                            _P, _c.c_int64, _P]),
     ('lss_pa_apply_workspace_bytes', _c.c_int64, [_P, _P, _c.c_int, _c.c_int64, _c.c_int64, _c.c_int64]),
     ('lss_pa_apply_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _P, _c.c_int, _P, _c.c_int64, _P,
                                       _c.c_int, _c.c_int64, _P, _c.c_int, _c.c_int64, _P, _c.c_int, _P, _P, _P,

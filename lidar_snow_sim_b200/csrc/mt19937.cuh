@@ -16,6 +16,7 @@
 // tests/shuffle_model.py restates the word generation, the chunk rule and the reservation shuffle in NumPy.
 #pragma once
 #include "segments.cuh"
+#include <type_traits>
 
 namespace {
 
@@ -63,7 +64,24 @@ __device__ __forceinline__ int smear(int i)
 }
 
 #ifndef LSS_MT_WORDS_ONLY
-struct Chain { int b, i, pos, cur, done; };
+struct Chain { int b, i, pos, cur, done; long long skip, t; };
+
+// A cloud list may give each cloud a tail: cl.tail(b) raw words drawn right after the cloud's chain, handed to
+// cl.word(b, t, tempered word t of the tail) (the uniform doubles of KITTI-N's noise rows, pa_aug.cu)
+template <class T, class = void> struct mt_has_tail : std::false_type {};
+template <class T> struct mt_has_tail<T, std::void_t<decltype(&T::tail)>> : std::true_type {};
+
+// the end of cloud b's chain: its tail, if any, else the next cloud
+template <class Cl>
+__device__ __forceinline__ void mt_cloud_done(const Cl &cl, int &b, int &i, int &done, long long &skip, long long &t)
+{
+    if constexpr (mt_has_tail<Cl>::value) {
+        skip = cl.tail(b);
+        t = 0;
+        if (skip > 0) return;
+    }
+    cl.next(b, i, done);
+}
 
 // The chain of one CTA of MT_TPB threads over the clouds of `cl`, from the key block key_at(0 .. 623) at position pos0
 // (0 .. 624).  cl.next(b, i, done) moves b to the next cloud with at least two rows (fewer draw nothing) and sets
@@ -80,7 +98,7 @@ __device__ __forceinline__ void mt_chain(const Cl &cl, Key key_at, int pos0, int
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     for (int t = tid; t < MT_N; t += MT_TPB) key[0][t] = key_at(t);
     if (tid == 0) {
-        s.b = -1; s.i = 0; s.pos = pos0; s.cur = 0; s.done = 0;
+        s.b = -1; s.i = 0; s.pos = pos0; s.cur = 0; s.done = 0; s.skip = 0; s.t = 0;
         cl.next(s.b, s.i, s.done);
     }
     for (;;) {
@@ -90,6 +108,20 @@ __device__ __forceinline__ void mt_chain(const Cl &cl, Key key_at, int pos0, int
             mt_gen_block(key[s.cur], key[s.cur ^ 1], tid);
             if (tid == 0) { s.cur ^= 1; s.pos = 0; }
             continue;
+        }
+        if constexpr (mt_has_tail<Cl>::value) {
+            if (s.skip > 0) {                                   // the cloud's tail words in this block
+                const int p = s.pos, b = s.b;
+                const long long sk = s.skip, t0 = s.t;
+                const int n = (int)min((long long)(MT_N - p), sk);
+                if (tid < n) cl.word(b, t0 + tid, mt_temper(key[s.cur][p + tid]));
+                __syncthreads();
+                if (tid == 0) {
+                    s.pos = p + n; s.t = t0 + n; s.skip = sk - n;
+                    if (s.skip == 0) cl.next(s.b, s.i, s.done);
+                }
+                continue;
+            }
         }
         const uint32_t *w = key[s.cur];
         const int p = s.pos, i = s.i, C = MT_N - p;
@@ -136,11 +168,12 @@ __device__ __forceinline__ void mt_chain(const Cl &cl, Key key_at, int pos0, int
             if (tid == 0) {
                 s.i = i - (nS + cum[nA]);
                 s.pos = MT_N;
-                if (s.i == 0) cl.next(s.b, s.i, s.done);
+                if (s.i == 0) mt_cloud_done(cl, s.b, s.i, s.done, s.skip, s.t);
             }
         } else if (warp == 0) {
             // 32 words at a time: the same rule when one mask covers the group, else word by word
             int q = p, ci = i, b = b0, done = 0;
+            long long skip = 0, tt = 0;
             int64_t cb = base;
             while (q < MT_N) {
                 const int g = min(32, MT_N - q);
@@ -160,8 +193,8 @@ __device__ __forceinline__ void mt_chain(const Cl &cl, Key key_at, int pos0, int
                     ci -= __popc(acc);
                     q += g;
                     if (ci == 0) {
-                        cl.next(b, ci, done);
-                        if (done) break;
+                        mt_cloud_done(cl, b, ci, done, skip, tt);
+                        if (done || skip) break;
                         cb = cl.base(b);
                     }
                 } else {
@@ -171,16 +204,16 @@ __device__ __forceinline__ void mt_chain(const Cl &cl, Key key_at, int pos0, int
                         if (v > ci) continue;
                         if (lane == 0) J[cb + ci] = v;
                         if (--ci == 0) {
-                            cl.next(b, ci, done);
-                            if (done) { k++; break; }
+                            mt_cloud_done(cl, b, ci, done, skip, tt);
+                            if (done || skip) { k++; break; }
                             cb = cl.base(b);
                         }
                     }
                     q += k;
-                    if (done) break;
+                    if (done || skip) break;
                 }
             }
-            if (lane == 0) { s.pos = q; s.i = ci; s.b = b; s.done = done; }
+            if (lane == 0) { s.pos = q; s.i = ci; s.b = b; s.done = done; s.skip = skip; s.t = tt; }
         }
     }
     for (int t = tid; t < MT_N; t += MT_TPB) state_out[t] = key[s.cur][t];

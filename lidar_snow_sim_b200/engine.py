@@ -1031,6 +1031,99 @@ class SnowfallEngine:
                    out, 1 if out_dtype == torch.float64 else 0, ws, ws.numel())
         return out
 
+    def pa_fps_cloud_config(self, n_rows):
+        """(cluster size, capacity) of lss_pa_fps_cloud_config on this engine's device: the cluster size a call whose
+        largest on-chip cloud has n_rows rows uses (0 above the capacity), and the most rows an on-chip cloud may have"""
+        cs, cap = ctypes.c_int(), ctypes.c_int64()
+        _lib.check(self.lib.lss_pa_fps_cloud_config(self.device.index, int(n_rows), ctypes.byref(cs), ctypes.byref(cap)))
+        return cs.value, cap.value
+
+    def pa_fps_cloud_batch(self, points, cloud_offsets, k, start, counts=None):
+        """
+        farthest_point_sampling (part_aware_augmentation.py:197-209) over every whole cloud (lss_pa_fps_cloud_batch,
+        current stream, no synchronisation).  points: CUDA float32 or float64 (N, F >= 3); counts: optional HOST int32
+        (B,) rows per slot; k, start: host (B,) picks and first picks (the caller's np.random.randint(n_b)).  Returns
+        dict(points (sum k, F) of points' dtype, cloud b's picked rows at the exclusive prefix of k; index CUDA int32
+        (sum k,) the picks inside each cloud).
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, (torch.float32, torch.float64), (N, None), min_cols=3)
+        cnt = None if counts is None else np.ascontiguousarray(counts, dtype=np.int32).reshape(-1)
+        kk = np.ascontiguousarray(k, dtype=np.int32).reshape(-1)
+        s0 = np.ascontiguousarray(start, dtype=np.int32).reshape(-1)
+        for name, a in (('counts', cnt), ('k', kk), ('start', s0)):
+            if a is not None and a.shape[0] != B:
+                raise ValueError(f'{name}: expected {B} entries, got {a.shape[0]}')
+        f64 = 1 if points.dtype == torch.float64 else 0
+        F = points.shape[1]
+        K = int(kk.astype(np.int64).sum())
+        out = _outputs(None, self.device, points=((K, F), points.dtype), index=((K,), torch.int32))
+        with torch.cuda.device(self.device):
+            need = self.lib.lss_pa_fps_cloud_workspace_bytes(_ptr(off), _ptr(cnt), _ptr(kk), B, f64)
+        if need < 0:
+            raise ValueError('bad cloud_offsets / counts / k (counts within the slots, k >= 1 for a cloud with rows)')
+        ws = self._scratch('pa_fps', need)
+        self._call('lss_pa_fps_cloud_batch', points, f64, F, _ptr(off), _ptr(cnt), B, _ptr(kk), _ptr(s0), out['points'],
+                   out['index'], ws, ws.numel())
+        return out
+
+    def pa_noise_test_batch(self, points, cloud_offsets, k, n_draw_clouds=None, counts=None):
+        """
+        generate_noise_robustness_test (part_aware_augmentation.py:749-767) on B clouds in turn
+        (lss_pa_noise_test_batch, current stream): per cloud np.random.choice(range(n_b), k_b, replace=False) and 4 k_b
+        uniforms on NumPy's global RandomState, the kept rows in order then the noise rows.  points: CUDA float32 or
+        float64 (N, F >= 4); counts: optional HOST int32 (B,) rows per slot; k: host (B,); only the first n_draw_clouds
+        clouds (default B) draw.  Synchronises once and sets NumPy's global state (the cached Gaussian kept) as the
+        draws leave it.  Returns dict(points CUDA float64 (sum n_b, 4), cloud b at the exclusive prefix of n_b;
+        columns host int32 (B,): 4, or the first column whose range is not finite, after which nothing was drawn).
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, (torch.float32, torch.float64), (N, None), min_cols=4)
+        cnt = None if counts is None else np.ascontiguousarray(counts, dtype=np.int32).reshape(-1)
+        kk = np.ascontiguousarray(k, dtype=np.int32).reshape(-1)
+        for name, a in (('counts', cnt), ('k', kk)):
+            if a is not None and a.shape[0] != B:
+                raise ValueError(f'{name}: expected {B} entries, got {a.shape[0]}')
+        D = B if n_draw_clouds is None else int(n_draw_clouds)
+        n = np.diff(off) if cnt is None else cnt.astype(np.int64)
+        words, start = _mt_state()
+        tail = torch.empty(625 + B, dtype=torch.int32, device=self.device)      # state, columns: one copy back
+        out = torch.empty((int(n.sum()), 4), dtype=torch.float64, device=self.device)
+        need = self.lib.lss_pa_noise_test_workspace_bytes(_ptr(off), _ptr(cnt), _ptr(kk), B)
+        if need < 0:
+            raise ValueError('bad cloud_offsets / counts / k (counts within the slots, k in [0, count])')
+        ws = self._scratch('pa_noise', need)
+        self._call('lss_pa_noise_test_batch', points, 1 if points.dtype == torch.float64 else 0, points.shape[1],
+                   _ptr(off), _ptr(cnt), B, _ptr(kk), D, _ptr(words), out, tail[625:], tail[:625], ws, ws.numel())
+        h = tail.cpu().numpy()
+        if B > 0:
+            np.random.set_state(_mt_tuple(h[:625].view(np.uint32), start))
+        return {'points': out, 'columns': h[625:].copy()}
+
+    def pa_jitter_test_batch(self, points, cloud_offsets, out_offsets, sigma, counts=None):
+        """
+        jitter_robustness_test (part_aware_augmentation.py:775-778) on B clouds in turn (lss_pa_jitter_test_batch,
+        current stream): np.random.normal(0, sigma, (n_b, 3)) from NumPy's global RandomState, cloud after cloud, added
+        to x, y, z in float64 and stored in the rows' dtype.  points: CUDA float32 or float64 (N, F >= 3); counts:
+        optional CUDA int32 (B,); out_offsets: host (B + 1) exact-size slots of n_b rows.  Synchronises once, for the
+        final state, and sets NumPy's global state to it.  Returns (out_offsets[-1], F) of points' dtype.
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, (torch.float32, torch.float64), (N, None), min_cols=3)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        ooff, B_out, n_out = _row_offsets(out_offsets, 'out_offsets')
+        if B_out != B:
+            raise ValueError(f'out_offsets: {B_out + 1} entries for {B} clouds')
+        words, start = _mt_state(gauss=True)
+        F = points.shape[1]
+        out = _outputs(None, self.device, points=((n_out, F), points.dtype), state=((MT_GAUSS_WORDS,), torch.int32))
+        ws = self._scratch('pa_jitter', self.lib.lss_pa_jitter_test_workspace_bytes(N, B))
+        self._call('lss_pa_jitter_test_batch', points, 1 if points.dtype == torch.float64 else 0, F, _ptr(off), counts, B,
+                   _ptr(ooff), float(sigma), _ptr(words), out['points'], out['state'], ws, ws.numel())
+        if B > 0:
+            _set_mt_state(start, out['state'])
+        return out['points']
+
     def gt_collide_batch(self, boxes, box_offsets, n_gt, class_offsets, bits_offsets, max_pairs, n_pairs, n_classes):
         """
         GT sampling's collision test (lss_gt_collide_batch, current stream, no synchronisation).  boxes: CUDA float32

@@ -342,3 +342,68 @@ def plan_cloud(counts, n_bg, gt_boxes, gt_names, num_classes, param, n_features=
     return dict(parts=out_parts, bg=['bg', None, int(n_bg), []], fps=fps,
                 noise=np.concatenate(noise) if noise else np.zeros((0, 4)),
                 normals=np.concatenate(normals) if normals else np.zeros((0, 4)), mask=mask, n_out=n_out)
+
+
+# ------------------------------------------------------------------------------------------------ robustness test sets
+def partition_corners_list(gt_boxes, gt_names):
+    """the constructor's partition_corners: per box a float64 (parts, 8, 3) array, the parts' corners in the boxes'
+    dtype (assign_box_points_partition)"""
+    corners = box_corners(gt_boxes) if gt_boxes.shape[0] else np.zeros((0, 8, 3))
+    out = []
+    for i, name in enumerate(np.asarray(gt_names)):
+        pc = np.zeros((NUM_PARTITION[name], 8, 3))
+        for j in range(NUM_PARTITION[name]):
+            pc[j] = partition_corners(corners[i], name, j)
+        out.append(pc)
+    return out
+
+
+class RobustState:
+    """The state create_robusteness_test_data('KITTI-D') reads and changes, on member counts: the boxes and names left,
+    gt_boxes_mask, aug_flag and, per box left, its parts as [input box, part, rows, dropped]."""
+
+    def __init__(self, gt_boxes, gt_names):
+        self.gt_boxes = gt_boxes
+        self.gt_names = np.asarray(gt_names)
+        self.num_gt_boxes = gt_boxes.shape[0]
+        self.gt_boxes_mask = [True] * self.num_gt_boxes
+        self.aug_flag = np.zeros((self.num_gt_boxes, 8, 6), dtype=bool)
+        self.parts = None
+
+    def dropout_test(self, counts, n_features):
+        """dropout_partitions(num_dropout_partition=1, p=1.0, robustness_test=True), stack_fg_points and the vstack with
+        the background: per box within distance one rand(1) draw, the last fullest part dropped and its count printed,
+        then remove_empty_gt_boxes.  Returns the output's member segments [(input box, part, rows)] before the
+        background; raises the reference's ValueError for rows of other than four columns after the draws.
+        counts: (M, MAX_PARTS) member counts of the constructor's boxes, read by the first call only."""
+        if self.parts is None:
+            self.parts = [[[i, j, int(counts[i][j]), False] for j in range(NUM_PARTITION[n])]
+                          for i, n in enumerate(self.gt_names)]
+        for i in range(self.num_gt_boxes):
+            if self.gt_boxes[i][0] > 100:
+                continue
+            if np.random.rand(1) > 1.0:
+                continue
+            max_num_points = 0
+            for j, q in enumerate(self.parts[i]):
+                n = 0 if q[3] else q[2]
+                if n >= max_num_points:
+                    max_num_points = n
+                    idx = j
+            print(max_num_points)
+            self.parts[i][idx][3] = True
+            self.aug_flag[i, idx, 0] = True
+        for i in range(self.num_gt_boxes):                        # remove_empty_gt_boxes, statement for statement
+            if all(q[3] or q[2] == 0 for q in self.parts[i]):
+                self.gt_boxes_mask[i] = False
+        self.gt_boxes = self.gt_boxes[self.gt_boxes_mask]
+        self.gt_names = self.gt_names[self.gt_boxes_mask]
+        self.num_gt_boxes = self.gt_boxes.shape[0]
+        self.parts = [d for d, s in zip(self.parts, self.gt_boxes_mask) if s]
+        self.aug_flag = self.aug_flag[self.gt_boxes_mask]
+        for box in self.parts:                                     # np.vstack onto np.zeros((0, 4))
+            for q in box:
+                if not q[3]:
+                    _concat_cols(4, n_features)
+        _concat_cols(4, n_features)                                # np.vstack((fg_points, bg_points))
+        return [(q[0], q[1], q[2]) for box in self.parts for q in box if not q[3] and q[2] > 0]
