@@ -1,13 +1,13 @@
 """Diagnostic: device step time vs clouds per call (fixed per-call cost of the kernel chain)."""
 import json
 import sys
-import time
 
 import numpy as np
 import torch
 
 sys.path.insert(0, '.')
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 from lidar_snow_sim_b200.snowfall.sampling import sample_table_set               # noqa: E402
 
@@ -23,16 +23,8 @@ def main():
         for pre in (True, False):
             out = {}
             kw = dict(device_prepass=True) if pre else dict(thresh_poly=np.tile(np.array(bench.FIXED_POLY), (B, 1)))
-            for _ in range(3):
-                eng.snowfall_batch(tid, d, off, orders[:B], bench.DIV_DEG, out=out, **kw)
-            torch.cuda.synchronize()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(10):
-                eng.snowfall_batch(tid, d, off, orders[:B], bench.DIV_DEG, out=out, **kw)
-            e1.record()
-            torch.cuda.synchronize()
-            ms = e0.elapsed_time(e1) / 10
+            ms = float(np.mean(measure.time_calls(
+                lambda: eng.snowfall_batch(tid, d, off, orders[:B], bench.DIV_DEG, out=out, **kw), 10, 3)))
             eng.set_profiling(True)
             for _ in range(3):
                 eng.snowfall_batch(tid, d, off, orders[:B], bench.DIV_DEG, out=out, **kw)

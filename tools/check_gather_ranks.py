@@ -18,15 +18,11 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure                                                                  # noqa: E402
 
 
 def main():
-    world = int(os.environ.get('WORLD_SIZE', '1'))
-    rank = int(os.environ.get('RANK', '0'))
-    lr = int(os.environ.get('LOCAL_RANK', '0'))
-    torch.cuda.set_device(lr)
-    dev = torch.device('cuda', lr)
-    dist.init_process_group('nccl', device_id=dev)
+    world, rank, lr, dev = measure.init_ranks()
     from lidar_snow_sim_b200.distributed import BatchGather
     from lidar_snow_sim_b200.engine import SnowfallEngine
     eng = SnowfallEngine(lr)
@@ -45,11 +41,8 @@ def main():
     ok_all = True
     for name, kind, env in (('push', 'push', {}), ('push_unicast', 'push', {'LSS_GATHER_MULTICAST': '0'}), ('ce', 'ce', {}),
                             ('nccl', 'nccl', {})):
-        for k, v in env.items():
-            os.environ[k] = v
-        g = BatchGather(n_rows, B, dev, depth=2, kind=kind, engine=eng, cloud_offsets=off)
-        for k in env:
-            del os.environ[k]
+        with measure.env(**env):
+            g = BatchGather(n_rows, B, dev, depth=2, kind=kind, engine=eng, cloud_offsets=off)
         ok = True
         for step in range(4):
             j = step & 1

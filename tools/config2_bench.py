@@ -1,6 +1,7 @@
 """BASELINE.json configs[2]: batch = 32 clouds, snowfall + wet ground fused on the device (water_height = 1 mm): the
 snowfall stage's slot-compacted output and per-cloud counts feed `wet_ground_batch` directly, no host round trip.
 Prints one JSON object; needs a GPU."""
+import itertools
 import json
 import os
 import sys
@@ -11,6 +12,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 from lidar_snow_sim_b200.snowfall.sampling import sample_table_set               # noqa: E402
 
@@ -37,24 +39,17 @@ def main():
 
     res = {}
     for name, fn in (('snowfall', snow), ('snowfall + wet ground (fused on device)', fused), ('wet ground alone', wet_only)):
-        for k in range(3):
-            fn(k)
+        k = itertools.count()
+        ms = float(np.mean(measure.time_calls(lambda: fn(next(k)), 20, 3)))
         eng.check()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        steps = 20
-        e0.record()
-        for k in range(steps):
-            fn(k)
-        e1.record()
-        torch.cuda.synchronize()
-        eng.check()
-        ms = e0.elapsed_time(e1) / steps
         res[name] = {'ms_per_step': ms, 'points_per_s': N / (ms * 1e-3), 'clouds_per_s': B / (ms * 1e-3)}
     r = fused(0)
     torch.cuda.synchronize()
     res['kept_fraction_after_both'] = float(r['counts'].sum().item()) / N
+    gpu = measure.card()
     print(json.dumps({'config': 'BASELINE.json configs[2]: batch=32 synthetic 64x2048 clouds, 2.5 mm/h gunn, '
-                                'water_height=1 mm, 1 x ' + torch.cuda.get_device_name() + ', device-resident', 'results': res}))
+                                f'water_height=1 mm, 1 x {gpu["name"]} ({gpu["power_limit_w"]} W power limit), '
+                                'device-resident', 'results': res}))
 
 
 if __name__ == '__main__':

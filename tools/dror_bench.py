@@ -2,15 +2,15 @@
 points from bench.make_workload, 3 300 rows of every cloud replaced by seeded snow (isolated points and pairs), beta 3,
 k_min 3, sr_min 0.04, alpha 0.16 and 0.45, compacted rows written.  Prints one JSON object:
   - the device and its power limit;
-  - per alpha: median ms and points/s of 20 timed calls after warm-up (two inputs alternated, CUDA events per call),
+  - per alpha: median ms and points/s of 20 timed calls after warm-up (two inputs alternated, each call synchronised),
     kernel time from the `dror` profiling id (a separate run), and from a further debug run the mean cells visited and
     candidates tested per query and the share of queries that exited early (reached k_min + 1);
   - the oracle port (oracle/dror.py, scipy cKDTree + exact re-test, one host process) on one cloud, labelled as such.
 Needs a GPU."""
+import itertools
 import json
 import os
 import sys
-import time
 
 import numpy as np
 import torch
@@ -18,6 +18,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 
 
@@ -50,18 +51,8 @@ def main():
         def call(k):
             outs[k & 1] = eng.dror_batch(inputs[k & 1], off, alpha=alpha, out=outs[k & 1])
             return outs[k & 1]
-        for k in range(4):
-            call(k)
-        torch.cuda.synchronize()
-        times = []
-        for k in range(20):
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            call(k)
-            e1.record()
-            torch.cuda.synchronize()
-            times.append(e0.elapsed_time(e1))
-        ms = float(np.median(times))
+        k = itertools.count()
+        ms, lo, hi = measure.median_min_max(measure.time_calls(lambda: call(next(k)), 20, 4))
         eng.set_profiling(True)
         eng.kernel_times(reset=True)
         for k in range(10):
@@ -73,17 +64,16 @@ def main():
         torch.cuda.synchronize()
         q, cells, cand, early = [int(v) for v in dbg['work'].cpu().numpy()]
         snow = int(call(0)['n_snow'].sum().item())
-        res[f'alpha {alpha}'] = {'median_ms': ms, 'min_ms': float(np.min(times)), 'max_ms': float(np.max(times)),
+        res[f'alpha {alpha}'] = {'median_ms': ms, 'min_ms': lo, 'max_ms': hi,
                                  'points_per_s': N / (ms * 1e-3), 'kernel_ms': k_ms, 'snow_fraction': snow / N,
                                  'cells_per_query': cells / q, 'candidates_per_query': cand / q,
                                  'early_exit_share': early / q}
     from oracle import dror as od
-    t0 = time.perf_counter()
-    od.keep_mask(host, alpha=0.16)
-    t_or = time.perf_counter() - t0
+    t_or = measure.time_calls(lambda: od.keep_mask(host, alpha=0.16), 1, 0)[0] * 1e-3
+    gpu = measure.card()
     out = {'metric': 'DROR-filtered LiDAR points/sec',
            'workload': f'{B} clouds x 131072 points (bench.make_workload + seeded snow), beta 3, k_min 3, sr_min 0.04',
-           'gpu': torch.cuda.get_device_name(0), 'gpu_power_limit_w': bench.power_limit_w(0), 'cases': res,
+           'gpu': gpu['name'], 'gpu_power_limit_w': gpu['power_limit_w'], 'cases': res,
            'oracle_port_host': {'what': 'oracle/dror.py (scipy cKDTree ball query + exact re-test), one process, one '
                                         'cloud, alpha 0.16 -- the oracle, not the reference (which needs python-pcl)',
                                 'points_per_s': host.shape[0] / t_or, 'cpu_count': os.cpu_count()}}

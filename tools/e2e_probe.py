@@ -2,13 +2,13 @@
 SnowfallEngine.snowfall_batch_host over chunk/slot settings.  Needs a GPU; prints one JSON object."""
 import json
 import sys
-import time
 
 import numpy as np
 import torch
 
 sys.path.insert(0, '.')
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 from lidar_snow_sim_b200.snowfall.sampling import sample_table_set               # noqa: E402
 
@@ -27,18 +27,11 @@ def main():
     d2 = torch.empty_like(d)
     res = {'bytes': N * 20}
 
-    def timed(fn, reps=10):
-        for _ in range(3):
-            fn()
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        for _ in range(reps):
-            fn()
-        torch.cuda.synchronize()
-        return (time.perf_counter() - t0) / reps * 1e3
+    def mean_ms(fn, runs=10):
+        return float(np.mean(measure.time_calls(fn, runs, 3)))
 
-    res['h2d_ms'] = timed(lambda: d.copy_(host, non_blocking=True))
-    res['d2h_ms'] = timed(lambda: host2.copy_(d2, non_blocking=True))
+    res['h2d_ms'] = mean_ms(lambda: d.copy_(host, non_blocking=True))
+    res['d2h_ms'] = mean_ms(lambda: host2.copy_(d2, non_blocking=True))
     s1, s2 = torch.cuda.Stream(), torch.cuda.Stream()
 
     def both():
@@ -46,17 +39,19 @@ def main():
             d.copy_(host, non_blocking=True)
         with torch.cuda.stream(s2):
             host2.copy_(d2, non_blocking=True)
-    res['duplex_ms'] = timed(both)
+    res['duplex_ms'] = mean_ms(both)
     out = {}
-    res['device_ms'] = timed(lambda: eng.snowfall_batch(tid, d, off, orders, bench.DIV_DEG, device_prepass=True, out=out))
+    res['device_ms'] = mean_ms(lambda: eng.snowfall_batch(tid, d, off, orders, bench.DIV_DEG, device_prepass=True,
+                                                          out=out))
     res['host'] = {}
     res['inflight2'] = {}
     res['inflight3'] = {}
     hos = [{}, {}, {}]
     for chunks in (1, 2, 3, 4):
         ho = hos[0]
-        res['host'][str(chunks)] = timed(lambda: eng.snowfall_batch_host(tid, host, off, orders, bench.DIV_DEG, host_out=ho,
-                                                                        device_prepass=True, n_chunks=chunks), reps=8)
+        res['host'][str(chunks)] = mean_ms(lambda: eng.snowfall_batch_host(tid, host, off, orders, bench.DIV_DEG,
+                                                                          host_out=ho, device_prepass=True,
+                                                                          n_chunks=chunks), 8)
         for depth in (2, 3):
             def run(steps):
                 ts = []
@@ -68,9 +63,7 @@ def main():
                 for t in ts:
                     eng.snowfall_batch_host_wait(t)
             run(4)
-            t0 = time.perf_counter()
-            run(12)
-            res[f'inflight{depth}'][str(chunks)] = (time.perf_counter() - t0) / 12 * 1e3
+            res[f'inflight{depth}'][str(chunks)] = measure.time_calls(lambda: run(12), 1, 0)[0] / 12
     res['trace'] = {}
     for chunks in (4, 8):
         eng.snowfall_batch_host(tid, host, off, orders, bench.DIV_DEG, host_out=ho, device_prepass=True, n_chunks=chunks)

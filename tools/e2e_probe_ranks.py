@@ -14,7 +14,6 @@ import argparse
 import json
 import os
 import sys
-import time
 
 import numpy as np
 import torch
@@ -22,6 +21,7 @@ import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 
 
 def main():
@@ -30,13 +30,7 @@ def main():
     ap.add_argument('--engine', type=int, default=1)
     ap.add_argument('--trace', type=int, default=0, help='device timeline of synchronous host calls on every rank')
     args = ap.parse_args()
-    world = int(os.environ.get('WORLD_SIZE', '1'))
-    rank = int(os.environ.get('RANK', '0'))
-    lr = int(os.environ.get('LOCAL_RANK', '0'))
-    torch.cuda.set_device(lr)
-    dev = torch.device('cuda', lr)
-    if world > 1:
-        dist.init_process_group('nccl', device_id=dev)
+    world, rank, lr, dev = measure.init_ranks()
     cpus = None
     if args.bind:
         from lidar_snow_sim_b200.distributed import bind_host_to_gpu
@@ -55,21 +49,21 @@ def main():
             dist.barrier()
             torch.cuda.synchronize(dev)
 
-    def timed(fn, reps=20):
-        for _ in range(3):
+    def every_rank(t):
+        """this rank's tensor t gathered from every rank"""
+        if world == 1:
+            return [t]
+        g = [torch.zeros_like(t) for _ in range(world)]
+        dist.all_gather(g, t)
+        return g
+
+    def ranks_ms(fn, reps=20, warmup=3):
+        """every rank's mean ms per call of fn(), all ranks starting together after the warm-up calls"""
+        for _ in range(warmup):
             fn()
         sync()
-        t0 = time.perf_counter()
-        for _ in range(reps):
-            fn()
-        torch.cuda.synchronize(dev)
-        dt = (time.perf_counter() - t0) / reps * 1e3
-        t = torch.tensor([dt], dtype=torch.float64, device=dev)
-        if world > 1:
-            g = [torch.zeros_like(t) for _ in range(world)]
-            dist.all_gather(g, t)
-            return [float(x.item()) for x in g]
-        return [dt]
+        ms = float(np.mean(measure.time_calls(fn, reps, 0)))
+        return [float(x.item()) for x in every_rank(torch.tensor([ms], dtype=torch.float64, device=dev))]
 
     def duplex():
         with torch.cuda.stream(s1):
@@ -78,9 +72,9 @@ def main():
             host_out.copy_(d_out, non_blocking=True)
 
     res = {'world': world, 'bytes_each_way': N * 20, 'bound_cpus': None if cpus is None else len(cpus)}
-    res['h2d_ms'] = timed(lambda: d_in.copy_(host_in, non_blocking=True))
-    res['d2h_ms'] = timed(lambda: host_out.copy_(d_out, non_blocking=True))
-    res['duplex_ms'] = timed(duplex)
+    res['h2d_ms'] = ranks_ms(lambda: d_in.copy_(host_in, non_blocking=True))
+    res['d2h_ms'] = ranks_ms(lambda: host_out.copy_(d_out, non_blocking=True))
+    res['duplex_ms'] = ranks_ms(duplex)
     gb = N * 20 / 1e9
     res['aggregate_GBs'] = {'h2d': sum(gb / (m * 1e-3) for m in res['h2d_ms']),
                             'd2h': sum(gb / (m * 1e-3) for m in res['d2h_ms']),
@@ -96,8 +90,8 @@ def main():
         outs = [{}, {}, {}]
         d_res = {}
         d_pts = hp.to(dev)
-        res['device_step_ms'] = timed(lambda: eng.snowfall_batch(tid, d_pts, off, orders, bench.DIV_DEG, device_prepass=True,
-                                                                 out=d_res))
+        res['device_step_ms'] = ranks_ms(lambda: eng.snowfall_batch(tid, d_pts, off, orders, bench.DIV_DEG,
+                                                                    device_prepass=True, out=d_res))
         for depth in (1, 3):
             def run(steps=12):
                 tickets = []
@@ -109,43 +103,25 @@ def main():
                 for t in tickets:
                     eng.snowfall_batch_host_wait(t)
             run(3)
-            sync()
-            t0 = time.perf_counter()
-            run(12)
-            torch.cuda.synchronize(dev)
-            dt = (time.perf_counter() - t0) / 12 * 1e3
-            t = torch.tensor([dt], dtype=torch.float64, device=dev)
-            if world > 1:
-                g = [torch.zeros_like(t) for _ in range(world)]
-                dist.all_gather(g, t)
-                res[f'pipeline_inflight{depth}_ms'] = [float(x.item()) for x in g]
-            else:
-                res[f'pipeline_inflight{depth}_ms'] = [dt]
+            res[f'pipeline_inflight{depth}_ms'] = [x / 12 for x in ranks_ms(lambda: run(12), 1, 0)]
         if args.trace:
             # where does a synchronous call spend its time when all ranks run at once?  Device timeline of the last of 6
             # calls (ms since the call's first enqueued operation): rows landed, polynomial ready, beam stage done, on host
             for nch in (1, 2, 4):
                 sync()
-                walls = []
-                for _ in range(6):
-                    t0 = time.perf_counter()
-                    eng.snowfall_batch_host(tid, hp, off, orders, bench.DIV_DEG, host_out=outs[0], device_prepass=True,
-                                            n_chunks=nch)
-                    walls.append((time.perf_counter() - t0) * 1e3)
+                walls = measure.time_calls(lambda: eng.snowfall_batch_host(tid, hp, off, orders, bench.DIV_DEG,
+                                                                           host_out=outs[0], device_prepass=True,
+                                                                           n_chunks=nch), 5, 1)
                 tr = eng.host_pipeline_trace().astype(np.float64).reshape(-1)
                 t = torch.zeros(1 + 16, dtype=torch.float64, device=dev)
-                t[0] = float(np.median(walls[1:]))
+                t[0] = float(np.median(walls))
                 t[1:1 + tr.size] = torch.from_numpy(tr).to(dev)
-                if world > 1:
-                    g = [torch.zeros_like(t) for _ in range(world)]
-                    dist.all_gather(g, t)
-                else:
-                    g = [t]
                 res[f'sync_chunks{nch}'] = [{'wall_ms': round(float(x[0]), 3),
-                                             'timeline_ms': [round(float(v), 3) for v in x[1:1 + 4 * nch]]} for x in g]
+                                             'timeline_ms': [round(float(v), 3) for v in x[1:1 + 4 * nch]]}
+                                            for x in every_rank(t)]
     if rank == 0:
         print(json.dumps(res))
-    if world > 1:
+    if dist.is_initialized():
         dist.destroy_process_group()
 
 

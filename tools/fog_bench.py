@@ -1,6 +1,7 @@
 """Throughput of the fog path (next row, SURVEY 8f-3) on the snowfall bench's cloud shape: 32 clouds x 131 072 points,
 alpha = 0.06, noise variant v1 from per-cloud generator states.  Prints one JSON object (points/s, HBM roofline of the
 60 B/point the path has to move: 20 B in, 40 B out) -- needs a GPU; the LUT comes from tests/golden/fog.npz."""
+import itertools
 import json
 import os
 import sys
@@ -11,6 +12,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 from lidar_snow_sim_b200.fog import ParameterSet                                 # noqa: E402
 from lidar_snow_sim_b200.fog.simulation import _pcg64_state                      # noqa: E402
@@ -33,17 +35,8 @@ def main():
                      ('hard+soft no noise', dict(noise=0)), ('hard only', dict(soft=False))):
         def step(k):
             return eng.fog_batch(pts[k & 1], off, lut, p.alpha, p.beta, p.beta_0, **kw)
-        for k in range(3):
-            step(k)
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        steps = 20
-        e0.record()
-        for k in range(steps):
-            step(k)
-        e1.record()
-        torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / steps
+        k = itertools.count()
+        ms = float(np.mean(measure.time_calls(lambda: step(next(k)), 20, 3)))
         eng.set_profiling(True)
         for k in range(4):
             step(k)

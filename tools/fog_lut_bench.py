@@ -12,31 +12,23 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 from lidar_snow_sim_b200.fog import ParameterSet                                 # noqa: E402
 from lidar_snow_sim_b200.fog.simulation import _pcg64_state                      # noqa: E402
 
 
-def timed(fn, steps=20, warmup=3):
-    for k in range(warmup):
-        fn(k)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for k in range(steps):
-        fn(k)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / steps
+def mean_ms(fn, runs=20):
+    return float(np.mean(measure.time_calls(fn, runs, 3)))
 
 
 def main():
     eng = SnowfallEngine(0)
-    res = {'device': torch.cuda.get_device_name(0)}
+    res = {'device': measure.card()}
     tables = {}
     for T in (1, 9, 32):
         ps = [ParameterSet(alpha=0.005 + 0.2 * k / 32, gamma=0.000001) for k in range(T)]
-        ms = timed(lambda k: eng.fog_integral_tables(ps), steps=10)
+        ms = mean_ms(lambda: eng.fog_integral_tables(ps), 10)
         eng.set_profiling(True)
         eng.fog_integral_tables(ps)
         kt = eng.kernel_times()['fog_lut']
@@ -59,10 +51,10 @@ def main():
     p06 = ParameterSet(alpha=0.06, gamma=0.000001)
     lut06 = eng.fog_integral_tables([p06])[0]
     kw = dict(noise=10, noise_variant=1, rng_states=states)
-    one = timed(lambda k: eng.fog_batch(pts, off, lut06, p06.alpha, p06.beta, p06.beta_0, **kw))
-    per = timed(lambda k: eng.fog_batch_params(pts, off, luts, alpha, beta, beta_0, idx, **kw))
-    with_tables = timed(lambda k: eng.fog_batch_params(pts, off, eng.fog_integral_tables(ps), alpha, beta, beta_0, idx,
-                                                       **kw))
+    one = mean_ms(lambda: eng.fog_batch(pts, off, lut06, p06.alpha, p06.beta, p06.beta_0, **kw))
+    per = mean_ms(lambda: eng.fog_batch_params(pts, off, luts, alpha, beta, beta_0, idx, **kw))
+    with_tables = mean_ms(lambda: eng.fog_batch_params(pts, off, eng.fog_integral_tables(ps), alpha, beta, beta_0, idx,
+                                                         **kw))
     res['batch'] = {'workload': f'{B} clouds x 131072 points, 5 features, noise v1',
                     'fog_batch_one_alpha': {'ms': one, 'points_per_s': N / (one * 1e-3)},
                     'fog_batch_params_32_alphas': {'ms': per, 'points_per_s': N / (per * 1e-3)},

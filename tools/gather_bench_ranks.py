@@ -6,8 +6,8 @@ gather kind deliver for the bench's batch (32 x 131072 rows per rank, ~75 % of t
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port 29513 \
         tools/gather_bench_ranks.py
 
-Per variant: ms per exchange (CUDA events on the launching rank, max over ranks, 20 exchanges back to back, double
-buffered) and the bytes that landed on one rank from its peers.  Rank 0 prints one JSON object.
+Per variant: ms per exchange (host clock around 20 exchanges back to back, double buffered, and a device synchronise;
+max over ranks) and the bytes that landed on one rank from its peers.  Rank 0 prints one JSON object.
 """
 import json
 import os
@@ -18,15 +18,11 @@ import torch
 import torch.distributed as dist
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure                                                                  # noqa: E402
 
 
 def main():
-    world = int(os.environ.get('WORLD_SIZE', '1'))
-    rank = int(os.environ.get('RANK', '0'))
-    lr = int(os.environ.get('LOCAL_RANK', '0'))
-    torch.cuda.set_device(lr)
-    dev = torch.device('cuda', lr)
-    dist.init_process_group('nccl', device_id=dev)
+    world, rank, lr, dev = measure.init_ranks()
     from lidar_snow_sim_b200.distributed import BatchGather
     from lidar_snow_sim_b200.engine import SnowfallEngine
     eng = SnowfallEngine(lr)
@@ -45,11 +41,8 @@ def main():
                 ('push_uni_b132', 'push', {'LSS_GATHER_MULTICAST': '0', 'LSS_GATHER_BLOCKS': '132'}),
                 ('ce', 'ce', {}), ('nccl', 'nccl', {})]
     for name, kind, env in variants:
-        for k, v in env.items():
-            os.environ[k] = v
-        g = BatchGather(n_rows, B, dev, depth=2, kind=kind, engine=eng, cloud_offsets=off)
-        for k in env:
-            del os.environ[k]
+        with measure.env(**env):
+            g = BatchGather(n_rows, B, dev, depth=2, kind=kind, engine=eng, cloud_offsets=off)
 
         def run(n):
             for s in range(n):
@@ -60,12 +53,7 @@ def main():
         torch.cuda.synchronize(dev)
         dist.barrier()
         torch.cuda.synchronize(dev)
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        run(20)
-        e1.record()
-        torch.cuda.synchronize(dev)
-        t = torch.tensor([e0.elapsed_time(e1) / 20], dtype=torch.float64, device=dev)
+        t = torch.tensor([measure.time_calls(lambda: run(20), 1, 0)[0] / 20], dtype=torch.float64, device=dev)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         moved = (cnt.sum() if g.kind == 'push' else n_rows) * 20.0 * (world - 1)
         res[name] = {'kind_used': g.kind, 'multicast': bool(getattr(g, 'multicast', False)), 'ms': round(float(t.item()), 4),

@@ -13,16 +13,15 @@ import argparse
 import json
 import os
 import pickle
-import subprocess
 import sys
 import tempfile
-import time
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import measure  # noqa: E402
 from lidar_snow_sim_b200.augmentor import DataAugmentor  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine  # noqa: E402
 
@@ -64,15 +63,6 @@ def config():
         Cfg(NAME='random_world_scaling', WORLD_SCALE_RANGE=[0.95, 1.05])])
 
 
-def card():
-    try:
-        q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-        return q
-    except Exception as e:                                      # noqa: BLE001
-        return f'unknown ({e})'
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--clouds', type=int, default=32)
@@ -81,7 +71,6 @@ def main():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--out', default=None, help='also write the JSON result to this file')
     a = ap.parse_args()
-    assert torch.cuda.is_available(), 'needs the GPU'
     rng = np.random.default_rng(0)
     B, N = a.clouds, a.rows
     names_pool = np.array(['Car', 'Pedestrian', 'Cyclist', 'Van'])
@@ -105,48 +94,37 @@ def main():
         boxes = np.concatenate([s[1] for s in scenes])
         names = np.concatenate([s[2] for s in scenes])
         boff = np.arange(B + 1) * 10
-        ev = {}
-        orig_c, orig_p = eng.gt_collide_batch, eng.gt_paste_batch
+        calls = []                                          # per call: the events around its two engine calls
 
-        def timed(fn, key):
+        def with_events(fn):
             def w(*args, **kw):
                 s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
                 s.record()
                 r = fn(*args, **kw)
                 e.record()
-                ev.setdefault(key, []).append((s, e))
+                calls[-1].append((s, e))
                 return r
             return w
-        eng.gt_collide_batch, eng.gt_paste_batch = timed(orig_c, 'collide'), timed(orig_p, 'paste')
-        np.random.seed(0)
-        times = []
-        for it in range(a.warmup + a.iters):
-            ev.clear()
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            r = aug.forward_batch(pts, offs, boxes, boff, names, engine=eng)
-            torch.cuda.synchronize()
-            dt = (time.perf_counter() - t0) * 1e3
-            if it >= a.warmup:
-                kern = sum(s.elapsed_time(e) for v in ev.values() for s, e in v)
-                times.append((dt, kern))
-        rows_out = int(r['counts'].sum())
-        seq = []
-        calib = None
-        for it in range(max(2, a.iters // 5)):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
+        eng.gt_collide_batch, eng.gt_paste_batch = with_events(eng.gt_collide_batch), with_events(eng.gt_paste_batch)
+
+        def batch():
+            calls.append([])
+            return aug.forward_batch(pts, offs, boxes, boff, names, engine=eng)
+
+        def sequential():
             for p, bx, nm in scenes:
-                d = {'points': p, 'gt_boxes': bx.copy(), 'gt_names': nm, 'calib': calib,
-                     'gt_boxes_mask': np.array([n in aug.class_names for n in nm])}
-                aug.forward(d)
-            torch.cuda.synchronize()
-            seq.append((time.perf_counter() - t0) * 1e3)
-    t = np.array(times)
-    res = {'card': card(), 'clouds': B, 'rows_per_cloud': N, 'db_objects': 3600,
-           'batch_ms_median': float(np.median(t[:, 0])), 'kernel_ms_median': float(np.median(t[:, 1])),
-           'host_ms_median': float(np.median(t[:, 0] - t[:, 1])), 'sequential_forward_ms_median': float(np.median(seq)),
-           'rows_out': rows_out}
+                aug.forward({'points': p, 'gt_boxes': bx.copy(), 'gt_names': nm, 'calib': None,
+                             'gt_boxes_mask': np.array([n in aug.class_names for n in nm])})
+
+        np.random.seed(0)
+        batch_ms = np.array(measure.time_calls(batch, a.iters, a.warmup))
+        kernel_ms = np.array([sum(s.elapsed_time(e) for s, e in c) for c in calls[a.warmup:]])
+        rows_out = int(batch()['counts'].sum())
+        seq = measure.time_calls(sequential, max(2, a.iters // 5), 0)
+    res = {'card': measure.card(), 'clouds': B, 'rows_per_cloud': N, 'db_objects': 3600,
+           'batch_ms_median': float(np.median(batch_ms)), 'kernel_ms_median': float(np.median(kernel_ms)),
+           'host_ms_median': float(np.median(batch_ms - kernel_ms)),
+           'sequential_forward_ms_median': float(np.median(seq)), 'rows_out': rows_out}
     print(json.dumps(res))
     if a.out:
         os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)

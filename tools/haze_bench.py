@@ -6,7 +6,7 @@ Time DENSE haze on the device against the host's per-sample work.
 Device: SnowfallEngine.haze_batch on B slots of N synthetic rows (ranges 1 - 80 m, integer intensities), each cloud's
 beta drawn uniformly from the dataset's default FOG_ALPHAS without '0.000' (the samples that fog), float32 rows out as the
 dataset block keeps them; the median of `calls` calls, each ending in the synchronising copy of the final states.  The
-kernel split comes from torch.profiler over one call.  The dataset block, FogAugmentation.batch under DENSE_uniform
+kernel split comes from measure.kernel_ms over one call.  The dataset block, FogAugmentation.batch under DENSE_uniform
 and CVL_uniform (the default alphas, '0.000' included), on the same batch: median of `calls` synchronised calls.
 Host: B sequential calls of oracle/haze.py (NumPy, the same float64 algorithm as the reference's haze_point_cloud) on
 the same clouds.  Prints one JSON line with the device name and power limit.
@@ -14,27 +14,18 @@ the same clouds.  Prints one JSON line with the device name and power limit.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import measure  # noqa: E402
 from lidar_snow_sim_b200.engine import default_engine  # noqa: E402
 from oracle import haze as oh  # noqa: E402
 
 ALPHAS = [0.005, 0.010, 0.020, 0.030, 0.060]
-
-
-def gpu_info():
-    try:
-        return subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception:
-        return torch.cuda.get_device_name(0)
 
 
 def clouds(B, N, seed=0):
@@ -66,53 +57,20 @@ def main():
     def call():
         return eng.haze_batch(dev, off, betas, four, state=st)
 
-    for _ in range(3):
-        call()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(args.calls):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        r = call()
-        times.append((time.perf_counter() - t0) * 1e3)
-    rows_out = int(r['counts'].sum())
-
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA], acc_events=True) as prof:
-        call()
-        torch.cuda.synchronize()
-    split = {}
-    for ev in prof.key_averages():
-        if ev.device_type.name != 'CUDA' or 'emcpy' in ev.key or 'emset' in ev.key:
-            continue
-        name = ev.key.replace('void ', '').replace('(anonymous namespace)::', '').split('(')[0].split('<')[0]
-        us = getattr(ev, 'device_time_total', None)
-        if us is None:
-            us = ev.cuda_time_total
-        split[name] = round(split.get(name, 0.0) + us / 1e3, 4)
+    times = measure.time_calls(call, args.calls, 3)
+    rows_out = int(call()['counts'].sum())
+    split = measure.kernel_ms(call)
 
     from lidar_snow_sim_b200.integrations.dense import FogAugmentation
     block = {}
     for key in ('DENSE_uniform', 'CVL_uniform'):
         fog = FogAugmentation({'FOG_AUGMENTATION': key}, random_generator=np.random.default_rng(1), engine=eng)
-        for _ in range(2):
-            fog.batch(dev, off)
-        bt = []
-        for _ in range(args.calls):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fog.batch(dev, off)
-            torch.cuda.synchronize()
-            bt.append((time.perf_counter() - t0) * 1e3)
-        block[key] = round(float(np.median(bt)), 3)
+        block[key] = round(float(np.median(measure.time_calls(lambda: fog.batch(dev, off), args.calls, 2))), 3)
 
-    host = []
-    for b in range(min(args.host_clouds, B)):
-        t0 = time.perf_counter()
-        oh.haze(pts[b], float(betas[b]), four, st)
-        host.append((time.perf_counter() - t0) * 1e3)
+    host = [measure.time_calls(lambda: oh.haze(pts[b], float(betas[b]), four, st), 1, 0)[0]
+            for b in range(min(args.host_clouds, B))]
     host_ms = float(np.mean(host)) * B
-    print(json.dumps({'bench': 'haze', 'gpu': gpu_info(), 'clouds': B, 'rows_per_cloud': N, 'rows_out': rows_out,
+    print(json.dumps({'bench': 'haze', 'gpu': measure.card(), 'clouds': B, 'rows_per_cloud': N, 'rows_out': rows_out,
                       'device_ms_median': round(float(np.median(times)), 3),
                       'device_ms_min': round(float(np.min(times)), 3), 'kernel_ms': split, 'block_ms_median': block,
                       'host_ms_per_cloud': round(float(np.mean(host)), 2), 'host_ms_batch_estimate': round(host_ms, 1),

@@ -4,19 +4,15 @@ drawn (seeded) from the dataset's eight rates, modes 'rain' and 'gunn', stronges
 Prints one JSON object:
   - the device and its power limit;
   - per mode: median ms of `augment_batch` (inputs on the device, each call synchronised) over 10 timed calls after
-    warm-up, points/s, the per-kernel times of one call (torch.profiler, a separate run), and the expected particles
+    warm-up, points/s, the per-kernel times of one call (measure.kernel_ms, a separate run), and the expected particles
     drawn per batch (sum over the returns beyond r_min of density x beam-cone volume, lisa.py:62-64);
   - per mode: median ms of the current way, B sequential LISA.augment calls on the dataset's float64 conversion plus the
     host post-processing (round(i * 255), the float32 cast, the label-0 filter), over 3 timed runs;
-  - registers and spills of the kernels (-Xptxas -v on csrc/lisa.cu, compiled into a temporary directory).
+  - registers and spills of the kernels (measure.ptxas on csrc/lisa.cu).
 Needs a GPU."""
 import json
 import os
-import re
-import subprocess
 import sys
-import tempfile
-import time
 
 import numpy as np
 import torch
@@ -24,7 +20,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench                                                                    # noqa: E402
-from lidar_snow_sim_b200 import build                                           # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                           # noqa: E402
 from lidar_snow_sim_b200.integrations.dense import DATASET_SNOWFALL_RATES, DATASET_TERMINAL_VELOCITIES  # noqa: E402
 from lidar_snow_sim_b200.lisa import LISA                                       # noqa: E402
@@ -32,28 +28,6 @@ from lidar_snow_sim_b200.snowfall.sampling import snowfall_rate_to_rainfall_rate
 
 B = 32
 RATES = [snowfall_rate_to_rainfall_rate(rs, tv) for rs, tv in zip(DATASET_SNOWFALL_RATES, DATASET_TERMINAL_VELOCITIES)]
-
-
-def ptxas_resources():
-    """{kernel: (registers, spill stores + loads)} of csrc/lisa.cu for sm_90a."""
-    with tempfile.TemporaryDirectory() as tmp:
-        flags = [f for f in build.NVCC_FLAGS if f not in ('--shared',)]
-        cmd = [build.find_nvcc()] + flags + ['-Xptxas', '-v', '-c', '-o', os.path.join(tmp, 'lisa.o'),
-                                             os.path.join(build.CSRC, 'lisa.cu')]
-        log = subprocess.run(cmd, capture_output=True, text=True, check=True).stderr
-    res, name = {}, None
-    for line in log.splitlines():
-        m = re.search(r"Compiling entry function '(\w+)'", line)
-        if m:
-            name = next((k for k in ('k_lisa_cloud', 'k_lisa_scatter', 'k_seg_count_codes', 'k_seg_scan', 'k_lisa')
-                         if k in m.group(1)), None)
-        m = re.search(r'(\d+) bytes spill stores, (\d+) bytes spill loads', line)
-        if m and name:
-            res.setdefault(name, {})['spill_bytes'] = int(m.group(1)) + int(m.group(2))
-        m = re.search(r'Used (\d+) registers', line)
-        if m and name:
-            res.setdefault(name, {})['registers'] = int(m.group(1))
-    return res
 
 
 def expected_particles(lisa, clouds, rr):
@@ -92,47 +66,23 @@ def main():
     res = {}
     for mode in ('rain', 'gunn'):
         lisa = LISA(mode=mode, mie_table=(g['D'], g['qext_water'] if mode == 'rain' else g['qext_ice']), engine=eng)
-        for _ in range(3):
-            out = lisa.augment_batch(pts, off, rr)
+        kept = int(lisa.augment_batch(pts, off, rr)['counts'].sum())
         eng.check()
-        times = []
-        for _ in range(10):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            out = lisa.augment_batch(pts, off, rr)
-            torch.cuda.synchronize()
-            times.append((time.perf_counter() - t0) * 1e3)
-        ms = float(np.median(times))
-        kept = int(out['counts'].sum())
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
-            lisa.augment_batch(pts, off, rr)
-            torch.cuda.synchronize()
-        kernels = {}
-        for e in prof.key_averages():
-            if e.device_type == torch.autograd.DeviceType.CUDA and not e.key.startswith(('Memcpy', 'Memset')):
-                name = re.sub(r'^.*?(k_\w+).*$', r'\1', e.key)
-                kernels[name] = kernels.get(name, 0.0) + e.device_time_total / 1e3
+        ms, lo, hi = measure.median_min_max(measure.time_calls(lambda: lisa.augment_batch(pts, off, rr), 10, 2))
+        kernels = measure.kernel_ms(lambda: lisa.augment_batch(pts, off, rr))
         sequential(lisa, clouds[:2], rr[:2])
-        seq = []
-        for _ in range(3):
-            t0 = time.perf_counter()
-            sequential(lisa, clouds, rr)
-            seq.append((time.perf_counter() - t0) * 1e3)
-        seq_ms = float(np.median(seq))
-        res[mode] = {'batch_median_ms': ms, 'batch_min_ms': float(np.min(times)), 'batch_max_ms': float(np.max(times)),
+        seq_ms = float(np.median(measure.time_calls(lambda: sequential(lisa, clouds, rr), 3, 0)))
+        res[mode] = {'batch_median_ms': ms, 'batch_min_ms': lo, 'batch_max_ms': hi,
                      'points_per_s': N / (ms * 1e-3), 'kernel_ms': kernels, 'kept_rows': kept,
                      'expected_particles_per_batch': expected_particles(lisa, clouds, rr),
                      'sequential_median_ms': seq_ms, 'sequential_points_per_s': N / (seq_ms * 1e-3),
                      'speedup': seq_ms / ms}
-    try:
-        ptx = ptxas_resources()
-    except (RuntimeError, OSError, subprocess.CalledProcessError) as exc:
-        ptx = f'not available: {exc}'
+    gpu = measure.card()
     out = {'metric': 'LISA-augmented LiDAR points/sec',
            'workload': f'{B} clouds x 131072 points (bench.make_workload), rain rate per cloud from the dataset\'s eight '
                        f'(seeded): {[round(float(r), 2) for r in rr]}; strongest return, counter-based generator',
-           'gpu': torch.cuda.get_device_name(0), 'gpu_power_limit_w': bench.power_limit_w(0), 'modes': res,
-           'ptxas': ptx}
+           'gpu': gpu['name'], 'gpu_power_limit_w': gpu['power_limit_w'], 'modes': res,
+           'ptxas': measure.ptxas('lisa.cu', ('k_lisa', 'k_seg_'))}
     print(json.dumps(out))
 
 

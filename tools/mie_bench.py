@@ -5,58 +5,21 @@
     shipped pairs in one call, with the kernel time of one call (CUDA events around k_mie);
   - the dependent chain of the longest row (downward + upward steps) and the total steps of each call;
   - the NumPy oracle's seconds per table on the host (oracle/mie.py, one run);
-  - registers and spills of k_mie (-Xptxas -v on csrc/mie.cu, compiled into a temporary directory).
+  - registers and spills of k_mie (measure.ptxas on csrc/mie.cu).
 Needs a GPU."""
 import json
 import os
-import re
-import subprocess
 import sys
-import tempfile
-import time
 
 import numpy as np
-import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-import bench                                                                    # noqa: E402
-from lidar_snow_sim_b200 import build                                           # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                           # noqa: E402
 from oracle import mie                                                          # noqa: E402
 
 SHIPPED = ((1.328, 905), (1.3031, 905), (1.328, 1550), (1.3031, 1550))
-
-
-def ptxas_resources():
-    with tempfile.TemporaryDirectory() as tmp:
-        flags = [f for f in build.NVCC_FLAGS if f not in ('--shared',)]
-        cmd = [build.find_nvcc()] + flags + ['-Xptxas', '-v', '-c', '-o', os.path.join(tmp, 'mie.o'),
-                                             os.path.join(build.CSRC, 'mie.cu')]
-        log = subprocess.run(cmd, capture_output=True, text=True, check=True).stderr
-    res = {}
-    m = re.search(r'(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads', log)
-    if m:
-        res['stack_bytes'], res['spill_bytes'] = int(m.group(1)), int(m.group(2)) + int(m.group(3))
-    m = re.search(r'Used (\d+) registers', log)
-    if m:
-        res['registers'] = int(m.group(1))
-    return res
-
-
-def median_ms(fn, steps=10, warmup=3):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(steps):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        fn()
-        e1.record()
-        torch.cuda.synchronize()
-        ts.append(e0.elapsed_time(e1))
-    return float(np.median(ts)), float(min(ts)), float(max(ts))
 
 
 def steps(pairs, d):
@@ -74,12 +37,13 @@ def steps(pairs, d):
 def main():
     eng = SnowfallEngine(0)
     d = mie.diameters_nm()
-    res = {'gpu': torch.cuda.get_device_name(0), 'gpu_power_limit_w': bench.power_limit_w(0),
+    gpu = measure.card()
+    res = {'gpu': gpu['name'], 'gpu_power_limit_w': gpu['power_limit_w'],
            'grid': '2000 diameters, logspace 1 nm .. 1 cm'}
     for name, pairs in (('one_table_water_905', SHIPPED[:1]), ('four_shipped_pairs', SHIPPED)):
         ms = [m for m, _ in pairs]
         wls = [w for _, w in pairs]
-        med, lo, hi = median_ms(lambda: eng.mie_tables(ms, wls, d))
+        med, lo, hi = measure.median_min_max(measure.time_calls(lambda: eng.mie_tables(ms, wls, d), 10, 3))
         eng.set_profiling(True)
         kts = []
         for _ in range(5):
@@ -91,13 +55,9 @@ def main():
         res[name] = {'ms_median': med, 'ms_min': lo, 'ms_max': hi, 'kernel_ms_median': float(np.median(kts)),
                      'longest_chain_steps': chain, 'total_steps': total,
                      'ns_per_chain_step': 1e6 * float(np.median(kts)) / chain}
-    host = []
-    for m, wl in SHIPPED:
-        t0 = time.perf_counter()
-        mie.mie_q(m, wl, d)
-        host.append(time.perf_counter() - t0)
+    host = [measure.time_calls(lambda: mie.mie_q(m, wl, d), 1, 0)[0] * 1e-3 for m, wl in SHIPPED]
     res['numpy_oracle_s_per_table'] = {f'{m}_{wl}': t for (m, wl), t in zip(SHIPPED, host)}
-    res['k_mie'] = ptxas_resources()
+    res['k_mie'] = measure.ptxas('mie.cu', ['k_mie'])['k_mie']
     print(json.dumps(res))
     eng.close()
 

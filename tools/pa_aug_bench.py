@@ -11,7 +11,6 @@ reference (numba) on the host, per sample, on the same clouds (needs tools/make_
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -44,14 +43,6 @@ def workload(B, n_boxes):
     return clouds, boxes
 
 
-def card():
-    try:
-        return subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception:                                              # noqa: BLE001
-        return 'unknown'
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--clouds', type=int, default=32)
@@ -75,6 +66,7 @@ def main():
             t.append(time.perf_counter() - t0)
         res.update(reference_ms_per_sample=float(np.median(t) * 1e3), host_cores=os.cpu_count())
     else:
+        import measure
         import torch
         from lidar_snow_sim_b200.engine import SnowfallEngine
         from lidar_snow_sim_b200.pa_aug import pa_aug_batch
@@ -83,29 +75,22 @@ def main():
         offs = np.concatenate([[0], np.cumsum([len(c) for c in clouds])])
         bx = np.concatenate(boxes)
         boff = np.concatenate([[0], np.cumsum([len(b) for b in boxes])])
+
+        def call():
+            return pa_aug_batch(pts, offs, bx, boff, PARAM, engine=eng)
+
         np.random.seed(0)
         for _ in range(2):
-            pa_aug_batch(pts, offs, bx, boff, PARAM, engine=eng)
-        torch.cuda.synchronize()
+            call()
         eng.set_profiling(True)
         eng.kernel_times(reset=True)
-        t = []
         for _ in range(a.iters):
-            t0 = time.perf_counter()
-            r = pa_aug_batch(pts, offs, bx, boff, PARAM, engine=eng)
-            torch.cuda.synchronize()
-            t.append(time.perf_counter() - t0)
+            r = call()
         kt = eng.kernel_times(reset=True).get('pa_aug', (0.0, 0))
         eng.set_profiling(False)
-        t = []
-        for _ in range(a.iters):                                   # timed without the profiling events
-            t0 = time.perf_counter()
-            r = pa_aug_batch(pts, offs, bx, boff, PARAM, engine=eng)
-            torch.cuda.synchronize()
-            t.append(time.perf_counter() - t0)
-        ms = float(np.median(t) * 1e3)
+        ms = float(np.median(measure.time_calls(call, a.iters, 0)))         # timed without the profiling events
         res.update(ms_per_batch=ms, kernel_ms_per_batch=kt[0] / a.iters, host_ms_per_batch=ms - kt[0] / a.iters,
-                   out_rows=int(r['offsets'][-1]), card=card())
+                   out_rows=int(r['offsets'][-1]), card=measure.card())
     print(json.dumps(res))
 
 

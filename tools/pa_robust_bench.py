@@ -11,15 +11,14 @@ import contextlib
 import io
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+import measure                                                              # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                       # noqa: E402
 from lidar_snow_sim_b200.pa_aug.augmentation import pa_robustness_batch     # noqa: E402
 from lidar_snow_sim_b200.synthetic import synthetic_cloud                  # noqa: E402
@@ -42,16 +41,9 @@ def batch(B, n, m, seed=0):
     return np.concatenate(pts), np.arange(B + 1) * n, np.concatenate(boxes), np.arange(B + 1) * m
 
 
-def timed(fn, reps):
-    ts = []
-    for _ in range(reps):
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        with contextlib.redirect_stdout(io.StringIO()):
-            fn()
-        torch.cuda.synchronize()
-        ts.append(time.perf_counter() - t0)
-    return float(np.median(ts))
+def median_s(fn, reps, warmup=1):
+    with contextlib.redirect_stdout(io.StringIO()):            # the reference prints as it goes
+        return float(np.median(measure.time_calls(fn, reps, warmup))) * 1e-3
 
 
 def main():
@@ -60,31 +52,26 @@ def main():
     ap.add_argument('--reference', default=None)
     a = ap.parse_args()
     eng = SnowfallEngine(0)
-    smi = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True,
-                         text=True).stdout.strip().splitlines()
     N, B, M = 131072, 32, 30
     pts, off, boxes, boff = batch(B, N, M)
     assert pts.shape[0] == B * N
     d = torch.from_numpy(pts).cuda()
-    res = {'card': smi[0] if smi else None, 'batch': f'{B} x {N} rows, {M} boxes'}
+    res = {'card': measure.card(), 'batch': f'{B} x {N} rows, {M} boxes'}
     cs, cap = eng.pa_fps_cloud_config(N)
     res['fps_cluster_size'], res['fps_capacity_rows'] = cs, cap
     for test in ('KITTI-D', 'KITTI-N', 'KITTI-J', 'KITTI-S'):
         fn = lambda: pa_robustness_batch(d, off, boxes, boff, test, engine=eng)      # noqa: E731
-        timed(fn, 1)
-        res[f'{test}_s'] = timed(fn, a.reps if test != 'KITTI-S' else max(1, a.reps // 2))
+        res[f'{test}_s'] = median_s(fn, a.reps if test != 'KITTI-S' else max(1, a.reps // 2))
     one = d[:N]
     K1 = int(N * 0.3)
     fn = lambda: eng.pa_fps_cloud_batch(one, [0, N], [K1], [0])      # noqa: E731
-    timed(fn, 1)
-    t1 = timed(fn, 3)
+    t1 = median_s(fn, 3)
     res['KITTI-S_one_cloud_s'] = t1
     res['KITTI-S_one_cloud_per_round_us'] = 1e6 * t1 / (K1 - 1)
     big = torch.from_numpy(np.concatenate([pts] * 2)[:cap + 1024]).cuda()
     n_big = big.shape[0]
     fn = lambda: eng.pa_fps_cloud_batch(big, [0, n_big], [int(n_big * 0.3)], [0])      # noqa: E731
-    timed(fn, 1)
-    res['KITTI-S_fallback_one_cloud_s'] = timed(fn, 1)
+    res['KITTI-S_fallback_one_cloud_s'] = median_s(fn, 1)
     res['KITTI-S_fallback_rows'] = n_big
     if a.reference:
         sys.path.insert(0, os.path.join(ROOT, 'tools'))
@@ -94,12 +81,12 @@ def main():
         names = np.array(['Car'] * M)
         for test in ('KITTI-D', 'KITTI-J'):
             fn = lambda: PAA(pts[:N].copy(), boxes[:M], names, ['Car', 'Pedestrian', 'Cyclist']).create_robusteness_test_data(test)  # noqa: E501,E731
-            res[f'reference_{test}_per_cloud_s'] = timed(fn, 3)
+            res[f'reference_{test}_per_cloud_s'] = median_s(fn, 3, warmup=0)
         xyz = pts[:N, :3]
-        t0 = time.perf_counter()
-        for _ in range(20):
+
+        def fps_round():
             np.minimum(ref.calc_distances(xyz[0].astype(np.float64), xyz), ref.calc_distances(xyz[1], xyz)).argmax()
-        per_round = (time.perf_counter() - t0) / 20
+        per_round = float(np.mean(measure.time_calls(fps_round, 20, 0))) * 1e-3
         res['reference_fps_round_s'] = per_round
         res['reference_KITTI-S_per_cloud_s_extrapolated'] = per_round * int(N * 0.3)
     print(json.dumps(res))

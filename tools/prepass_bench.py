@@ -1,13 +1,15 @@
 """The device pre-pass alone (ground plane, laser-parameter regressions, noise-threshold polynomial) on the snowfall
 bench's batch: 32 clouds x 131 072 points from bench.make_workload, two input batches alternating so the rows do not
-sit in L2 from one call to the next.  Prints one JSON object: the median call time (CUDA events), the per-kernel times
-(torch.profiler, in a run of its own), the bytes a call moves (from the shapes) and the card with its power limit.
+sit in L2 from one call to the next.  Prints one JSON object: the median call time (each call synchronised), the
+per-kernel times per call (measure.kernel_ms, in a run of its own), the kernel launches per call (the engine's launch
+count), the bytes a call moves (from the shapes) and the card with its power limit.
 
     python tools/prepass_bench.py [--calls 50] [--dump DIR]
 
 --dump DIR writes poly, plane, fits and picks of both batches as DIR/<name>_<batch>.npy (for bit-for-bit comparisons
 between builds).  Needs a GPU."""
 import argparse
+import itertools
 import json
 import os
 import sys
@@ -18,6 +20,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench                                                                    # noqa: E402
+import measure                                                                  # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                            # noqa: E402
 
 B = 32
@@ -39,7 +42,6 @@ def main():
     ap.add_argument('--calls', type=int, default=50)
     ap.add_argument('--dump', metavar='DIR', default=None)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), 'prepass_bench needs a GPU'
     eng = SnowfallEngine(0)
     batches = [bench.make_workload(0, B)[0], bench.make_workload(0, B, seed0=500000)[0]]
     off = np.concatenate([[0], np.cumsum([c.shape[0] for c in batches[0]])]).astype(np.int64)
@@ -49,26 +51,15 @@ def main():
     def call(k, fits=False):
         return eng.noise_threshold_poly(pts[k & 1], off, 0.7, want_fits=fits)
 
-    for k in range(5):
-        call(k)
-    torch.cuda.synchronize()
-    ms = []
-    for k in range(args.calls):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        call(k)
-        e1.record()
-        torch.cuda.synchronize()
-        ms.append(e0.elapsed_time(e1))
+    k = itertools.count()
+    ms = measure.time_calls(lambda: call(next(k)), args.calls, 5)
 
-    kernels = {}
-    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+    def ten_calls():
         for k in range(10):
             call(k)
-        torch.cuda.synchronize()
-    for ev in prof.key_averages():
-        if ev.device_type == torch.autograd.DeviceType.CUDA and ev.count:
-            kernels[ev.key] = {'ms': ev.device_time_total / ev.count / 1e3, 'calls_per_prepass': ev.count / 10}
+    launches = eng.launch_count()
+    kernels = {name: t / 10 for name, t in measure.kernel_ms(ten_calls).items()}
+    launches = (eng.launch_count() - launches) / 10
 
     fits = [call(k, fits=True) for k in range(2)]
     n_ground = float(fits[0][2][:, 5].sum())
@@ -78,13 +69,14 @@ def main():
             for name, t in zip(('poly', 'plane', 'fits', 'picks'), res):
                 np.save(os.path.join(args.dump, f'{name}_{k}.npy'), t.cpu().numpy())
     # the histogram records are the ground points inside 10 <= d <= 70, 5 <= I/cos: the ground count bounds them
+    gpu = measure.card()
     out = {'metric': 'device pre-pass call', 'workload': f'{B} clouds x {N // B} points (bench.make_workload), 2 batches '
                                                           'alternating',
            'median_ms': float(np.median(ms)), 'min_ms': float(np.min(ms)), 'calls': args.calls,
-           'kernels': kernels, 'launches_per_call': sum(v['calls_per_prepass'] for v in kernels.values()),
+           'kernels': kernels, 'launches_per_call': launches,
            'n_ground_batch0': n_ground,
            'bytes_per_call_upper_bound': traffic_bytes(N, int(n_ground)),
-           'gpu': torch.cuda.get_device_name(0), 'gpu_power_limit_w': bench.power_limit_w(0)}
+           'gpu': gpu['name'], 'gpu_power_limit_w': gpu['power_limit_w']}
     print(json.dumps(out))
     eng.close()
 

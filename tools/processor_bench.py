@@ -7,21 +7,20 @@ Device: DataProcessor.forward_batch with dense_dataset.yaml's processor (range m
 0.05 x 0.1 m, 5 points, 16 000 voxels) and its encoder (x, y, z, intensity of 5 columns), over B slots of N rows
 (synthetic clouds spread over and beyond the range); the median of `calls` calls, each ending in the synchronising copy
 of the generator state.  The shares: lss_mt19937_permutations alone (word generation + rejection chain + swaps) and
-lss_voxelize_batch alone on the same rows, timed with CUDA events.
+lss_voxelize_batch alone on the same rows, the median of `calls` synchronised calls.
 Host: B sequential mask_points_by_range + np.random.permutation + gather (the voxels need spconv, which is not part of
 this comparison).  Prints one JSON line with the device name and power limit.
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 from lidar_snow_sim_b200.engine import default_engine  # noqa: E402
 from lidar_snow_sim_b200.processor import DataProcessor, PointFeatureEncoder  # noqa: E402
 
@@ -32,26 +31,6 @@ CFGS = [{'NAME': 'mask_points_and_boxes_outside_range', 'REMOVE_OUTSIDE_BOXES': 
         {'NAME': 'shuffle_points', 'SHUFFLE_ENABLED': {'train': True, 'test': False}},
         {'NAME': 'transform_points_to_voxels', 'VOXEL_SIZE': [0.05, 0.05, 0.1], 'MAX_POINTS_PER_VOXEL': 5,
          'MAX_NUMBER_OF_VOXELS': {'train': 16000, 'test': 40000}}]
-
-
-def gpu_info():
-    try:
-        return subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception:
-        return torch.cuda.get_device_name(0)
-
-
-def events_ms(fn, calls):
-    out = []
-    for _ in range(calls):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        out.append(a.elapsed_time(b))
-    return float(np.median(out))
 
 
 def main():
@@ -74,33 +53,27 @@ def main():
     def device_call():
         return proc.forward_batch(pts, off, columns=enc.columns(), engine=eng)
 
+    def median_of(fn, runs=args.calls, warmup=0):
+        return round(float(np.median(measure.time_calls(fn, runs, warmup))), 3)
+
     r = device_call()
-    for _ in range(2):
-        device_call()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(args.calls):
-        t = time.perf_counter()
-        device_call()
-        torch.cuda.synchronize()
-        times.append((time.perf_counter() - t) * 1e3)
+    device_ms = median_of(device_call, warmup=2)
     counts = r['counts']
-    vox_ms = events_ms(lambda: eng.voxelize_batch(r['points'], off, RANGE, [0.05, 0.05, 0.1], 5, 16000, counts=counts,
-                                                  mask_xy_range=False), args.calls)
-    perm_ms = events_ms(lambda: eng.mt19937_permutations(off, counts=counts), args.calls)
-    host_times = []
-    for _ in range(max(3, args.calls // 3)):
-        t = time.perf_counter()
+    vox_ms = median_of(lambda: eng.voxelize_batch(r['points'], off, RANGE, [0.05, 0.05, 0.1], 5, 16000, counts=counts,
+                                                  mask_xy_range=False))
+    perm_ms = median_of(lambda: eng.mt19937_permutations(off, counts=counts))
+
+    def host_call():
         for b in range(B):
             p = host[off[b]:off[b + 1]][:, [0, 1, 2, 3]]
             m = (p[:, 0] >= RANGE[0]) & (p[:, 0] <= RANGE[3]) & (p[:, 1] >= RANGE[1]) & (p[:, 1] <= RANGE[4])
             p = p[m]
             p = p[np.random.permutation(p.shape[0])]
-        host_times.append((time.perf_counter() - t) * 1e3)
-    print(json.dumps({'bench': 'processor', 'gpu': gpu_info(), 'clouds': B, 'rows_per_cloud': N,
-                      'kept_rows': int(counts.sum()), 'device_call_ms': round(float(np.median(times)), 3),
-                      'permutation_ms': round(perm_ms, 3), 'voxelize_ms': round(vox_ms, 3),
-                      'host_mask_permutation_gather_ms': round(float(np.median(host_times)), 3)}))
+
+    print(json.dumps({'bench': 'processor', 'gpu': measure.card(), 'clouds': B, 'rows_per_cloud': N,
+                      'kept_rows': int(counts.sum()), 'device_call_ms': device_ms,
+                      'permutation_ms': perm_ms, 'voxelize_ms': vox_ms,
+                      'host_mask_permutation_gather_ms': median_of(host_call, max(3, args.calls // 3))}))
 
 
 if __name__ == '__main__':

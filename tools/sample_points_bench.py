@@ -17,14 +17,13 @@ power limit.
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+import measure  # noqa: E402
 from lidar_snow_sim_b200.engine import default_engine  # noqa: E402
 from lidar_snow_sim_b200.integrations.dense import FOG_ALPHAS, FogAugmentation  # noqa: E402
 from lidar_snow_sim_b200.processor import DataProcessor  # noqa: E402
@@ -33,27 +32,6 @@ RANGE = np.array([0, -40, -3, 70.4, 40, 1], np.float32)
 CFGS = [{'NAME': 'mask_points_and_boxes_outside_range', 'REMOVE_OUTSIDE_BOXES': True},
         {'NAME': 'sample_points', 'NUM_POINTS': {'train': 16384, 'test': 16384}},
         {'NAME': 'shuffle_points', 'SHUFFLE_ENABLED': {'train': True, 'test': False}}]
-
-
-def gpu_info():
-    try:
-        return subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception:
-        return torch.cuda.get_device_name(0)
-
-
-def median_ms(fn, calls, warmup=2):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(calls):
-        t = time.perf_counter()
-        fn()
-        torch.cuda.synchronize()
-        times.append((time.perf_counter() - t) * 1e3)
-    return round(float(np.median(times)), 3)
 
 
 def host_sample(p, k):
@@ -84,31 +62,32 @@ def main():
     np.random.seed(0)
     cols = [0, 1, 2, 3]
 
-    processor_ms = median_ms(lambda: proc.forward_batch(pts, off, columns=cols, engine=eng), args.calls)
+    def median_of(fn, runs=args.calls, warmup=2):
+        return round(float(np.median(measure.time_calls(fn, runs, warmup))), 3)
+
+    processor_ms = median_of(lambda: proc.forward_batch(pts, off, columns=cols, engine=eng))
     masked = eng.processor_batch(pts, off, cols, RANGE.astype(np.float64), shuffle=False)
-    sample_ms = median_ms(lambda: eng.sample_points_batch(masked['points'], off, k, counts=masked['counts'],
-                                                          shuffle=True), args.calls)
+    sample_ms = median_of(lambda: eng.sample_points_batch(masked['points'], off, k, counts=masked['counts'],
+                                                          shuffle=True))
 
     fog = FogAugmentation({'FOG_AUGMENTATION_AFTER': 'DENSE_uniform'}, engine=eng)
     alphas = [FOG_ALPHAS[int(i)] for i in np.random.default_rng(1).integers(0, len(FOG_ALPHAS), B)]
     fog._last = (alphas, ['DENSE'] * B)
-    fog_ms = median_ms(lambda: fog.after_batch(masked['points'], off, masked['counts']), args.calls)
-    after_ms = median_ms(lambda: fog.after_batch(masked['points'], off, masked['counts'], processor=proc), args.calls)
+    fog_ms = median_of(lambda: fog.after_batch(masked['points'], off, masked['counts']))
+    after_ms = median_of(lambda: fog.after_batch(masked['points'], off, masked['counts'], processor=proc))
 
-    host_times = []
-    for _ in range(max(3, args.calls // 3)):
-        t = time.perf_counter()
+    def host_call():
         for b in range(B):
             p = host[off[b]:off[b + 1]][:, cols]
             m = (p[:, 0] >= RANGE[0]) & (p[:, 0] <= RANGE[3]) & (p[:, 1] >= RANGE[1]) & (p[:, 1] <= RANGE[4])
             p = host_sample(p[m], k)
             p = p[np.random.permutation(p.shape[0])]
-        host_times.append((time.perf_counter() - t) * 1e3)
-    print(json.dumps({'bench': 'sample_points', 'gpu': gpu_info(), 'clouds': B, 'rows_per_cloud': N, 'num_points': k,
-                      'kept_rows': int(masked['counts'].sum()), 'processor_call_ms': processor_ms,
+
+    print(json.dumps({'bench': 'sample_points', 'gpu': measure.card(), 'clouds': B, 'rows_per_cloud': N,
+                      'num_points': k, 'kept_rows': int(masked['counts'].sum()), 'processor_call_ms': processor_ms,
                       'sample_points_call_ms': sample_ms, 'after_fog_dense_ms': fog_ms,
                       'after_fog_dense_resample_ms': after_ms,
-                      'host_mask_sample_shuffle_ms': round(float(np.median(host_times)), 3)}))
+                      'host_mask_sample_shuffle_ms': median_of(host_call, max(3, args.calls // 3), 0)}))
 
 
 if __name__ == '__main__':

@@ -46,10 +46,10 @@ def run(steps):
     import torch
     sys.path.insert(0, ROOT)
     import bench
+    import measure
     from lidar_snow_sim_b200 import _lib
     from lidar_snow_sim_b200.engine import SnowfallEngine
     from lidar_snow_sim_b200.snowfall.sampling import sample_table_set
-    assert torch.cuda.is_available(), 'solve_phases needs a GPU'
     dev = torch.device('cuda', 0)
     eng = SnowfallEngine(0)
     tid = eng.upload_tables(sample_table_set(bench.MODE, bench.SNOWFALL_RATE, bench.TERMINAL_VELOCITY,
@@ -74,6 +74,7 @@ def run(steps):
     tiles, warps = v[len(PHASES)], v[len(PHASES) + 1]
     cls = v[len(PHASES) + 2:]
     total = sum(cyc)
+    gpu = measure.card()
     out = {'metric': 'k_solve phase shares of the summed warp cycles (clock64 stamps, -DLSS_SOLVE_PHASE_CLOCKS build)',
            'workload': f'bench.make_workload: {bench.BATCH_PER_GPU} clouds x {int(off[-1]) // bench.BATCH_PER_GPU} points, '
                        f'2 batches alternating, {steps} steps',
@@ -83,7 +84,7 @@ def run(steps):
            'tiles_per_step': tiles / steps, 'warps_per_launch': warps / steps, 'tiles_per_warp': tiles / warps,
            'listed_beams_per_step': sum(cls) / steps,
            'listed_beams_per_class_per_step': {class_name(c): n / steps for c, n in enumerate(cls) if n},
-           'gpu': torch.cuda.get_device_name(0), 'gpu_power_limit_w': bench.power_limit_w(0)}
+           'gpu': gpu['name'], 'gpu_power_limit_w': gpu['power_limit_w']}
     print(json.dumps(out))
     eng.close()
 

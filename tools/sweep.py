@@ -6,7 +6,7 @@ BASELINE.json configs[4]: snowfall-rate x terminal-velocity sweep -- throughput 
 
 For every (snowfall_rate, terminal_velocity) the 64 snowflake planes are drawn ON THE DEVICE by the engine's sampler,
 indexed, and a batch of synthetic 64 x 2048 clouds is augmented (full pipeline, device pre-pass); the line reports
-particles per plane, occluders per beam, label fractions and points/s (CUDA events, max over ranks).
+particles per plane, occluders per beam, label fractions and points/s (mean of synchronised steps, max over ranks).
 """
 import argparse
 import json
@@ -20,6 +20,7 @@ import torch.distributed as dist
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+import measure                                                           # noqa: E402
 from lidar_snow_sim_b200.engine import SnowfallEngine                    # noqa: E402
 from lidar_snow_sim_b200.synthetic import synthetic_cloud                # noqa: E402
 
@@ -33,13 +34,7 @@ def main():
     ap.add_argument('--steps', type=int, default=5)
     ap.add_argument('--out', default=None)
     args = ap.parse_args()
-    world = int(os.environ.get('WORLD_SIZE', '1'))
-    rank = int(os.environ.get('RANK', '0'))
-    local = int(os.environ.get('LOCAL_RANK', '0'))
-    torch.cuda.set_device(local)
-    dev = torch.device('cuda', local)
-    if world > 1:
-        dist.init_process_group('nccl', device_id=dev)
+    world, rank, local, dev = measure.init_ranks()
     eng = SnowfallEngine(local)
     clouds = [synthetic_cloud(seed=7000 + rank * 1000 + b) for b in range(args.batch)]
     off = np.concatenate([[0], np.cumsum([c.shape[0] for c in clouds])]).astype(np.int64)
@@ -64,15 +59,10 @@ def main():
                 frac = [float((full[:, 4] == l).float().mean()) for l in (0, 1, 2)]
                 nocc = float(r['nocc'].float().mean())
                 out2 = {}
-                evs = []
-                for _ in range(args.steps):
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                    eng.snowfall_batch(tid, pts, off, orders, div, device_prepass=True, out=out2)
-                    e1.record()
-                    evs.append((e0, e1))
+                ms = float(np.mean(measure.time_calls(
+                    lambda: eng.snowfall_batch(tid, pts, off, orders, div, device_prepass=True, out=out2),
+                    args.steps, 0)))
                 eng.check()
-                ms = float(np.mean([a.elapsed_time(b) for a, b in evs]))
                 t = torch.tensor([ms], dtype=torch.float64, device=dev)
                 if world > 1:
                     dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -89,9 +79,9 @@ def main():
                 print(json.dumps(rows[-1]), flush=True)
     if rank == 0 and args.out:
         json.dump({'workload': f'batch={args.batch} synthetic 64x2048 clouds per GPU, gunn DSD, device sampler seed 1000, '
-                               f'device pre-pass, CUDA-event ms per step (mean of {args.steps})', 'rows': rows},
+                               f'device pre-pass, ms per synchronised step (mean of {args.steps})', 'rows': rows},
                   open(args.out, 'w'), indent=1)
-    if world > 1:
+    if dist.is_initialized():
         dist.destroy_process_group()
 
 

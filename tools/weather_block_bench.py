@@ -15,37 +15,17 @@ LSS_NVCC_FLAGS=-DLSS_SCHED_PLANES=512 and run --only-stack on the second build. 
 and its power limit.
 """
 import argparse
+import itertools
 import json
 import os
 import random
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-
-
-def card():
-    try:
-        return subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'],
-                              capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
-    except Exception:                                              # noqa: BLE001
-        return 'unknown'
-
-
-def median_ms(fn, iters, sync):
-    fn(0)
-    sync()
-    t = []
-    for i in range(iters):
-        t0 = time.perf_counter()
-        fn(i)
-        sync()
-        t.append(time.perf_counter() - t0)
-    return float(np.median(t) * 1e3)
+import measure                                                     # noqa: E402
 
 
 def main():
@@ -59,12 +39,16 @@ def main():
     from lidar_snow_sim_b200.engine import SnowfallEngine
     from lidar_snow_sim_b200.integrations.dense import OnTheFlyWeather
     eng = SnowfallEngine(0)
-    sync = torch.cuda.synchronize
+
+    def median_of(fn):
+        i = itertools.chain([0], range(a.iters))          # fn(0) warms up, then fn(0) .. fn(iters - 1) are timed
+        return float(np.median(measure.time_calls(lambda: fn(next(i)), a.iters, 1)))
+
     clouds, _ = make_workload(0, a.clouds)
     off = np.concatenate([[0], np.cumsum([c.shape[0] for c in clouds])]).astype(np.int64)
     pts = torch.from_numpy(np.concatenate(clouds)).cuda()
     div = float(np.degrees(3e-3))
-    res = dict(clouds=a.clouds, rows_per_cloud=int(clouds[0].shape[0]), iters=a.iters, card=card(),
+    res = dict(clouds=a.clouds, rows_per_cloud=int(clouds[0].shape[0]), iters=a.iters, card=measure.card(),
                build_flags=os.environ.get('LSS_NVCC_FLAGS', ''))
 
     base = OnTheFlyWeather({'SNOW': 'uniform_gunn_8in9'}, engine=eng)
@@ -82,7 +66,7 @@ def main():
     orders = np.stack([rng.permutation(64) for _ in range(a.clouds)]).astype(np.int32)
     stack_orders = orders + 64 * rng.integers(0, len(sets), a.clouds, dtype=np.int32)[:, None]
     kw = dict(threshold_filter=True, camera_fov=True, device_prepass=True)
-    res['stack_ms'] = median_ms(lambda i: eng.snowfall_batch(tid, pts, off, stack_orders, div, **kw), a.iters, sync)
+    res['stack_ms'] = median_of(lambda i: eng.snowfall_batch(tid, pts, off, stack_orders, div, **kw))
     eng.check()
     if a.only_stack:
         print(json.dumps(res))
@@ -97,9 +81,9 @@ def main():
     one = base.pairs[34]
     t34 = eng.sample_tables_device('gunn', one[0], one[1], seed=base.table_seed)
     res['fov_rows'] = int(cnt.sum())
-    res['dense_ms'] = median_ms(lambda i: eng.snowfall_batch(t34, dense, off_d, orders, div, **kw), a.iters, sync)
-    res['slots_ms'] = median_ms(lambda i: eng.snowfall_batch(t34, fov['points'], off, orders, div,
-                                                            counts=fov['counts'], **kw), a.iters, sync)
+    res['dense_ms'] = median_of(lambda i: eng.snowfall_batch(t34, dense, off_d, orders, div, **kw))
+    res['slots_ms'] = median_of(lambda i: eng.snowfall_batch(t34, fov['points'], off, orders, div,
+                                                            counts=fov['counts'], **kw))
     eng.check()
     eng.free_tables(t34)
 
@@ -112,7 +96,7 @@ def main():
         out = pts.clone()
         out[rows] = sub
 
-    res['gather_scatter_ms'] = median_ms(gather_scatter, a.iters, sync)
+    res['gather_scatter_ms'] = median_of(gather_scatter)
 
     for name, cfg in (('uncoupled', {'SNOW': 'uniform_gunn_8in9', 'WET_SURFACE': '1in2'}),
                       ('coupled', {'SNOW': 'uniform_gunn_8in9', 'WET_SURFACE': '1in2', 'COUPLED': True})):
@@ -132,16 +116,16 @@ def main():
             for c in clouds:
                 aug(c)
 
-        ms_block = median_ms(block, a.iters, sync)
+        ms_block = median_of(block)
         eng.check()
         eng.set_profiling(True)                     # the engine's kernels inside the block; the rest is torch + host
         eng.kernel_times(reset=True)
         for i in range(a.iters):
             block(i)
-        sync()
+        torch.cuda.synchronize()
         kernel_ms = {k: v[0] / a.iters for k, v in eng.kernel_times(reset=True).items() if v[1]}   # (timers nest)
         eng.set_profiling(False)
-        ms_seq = median_ms(sequential, a.iters, sync)
+        ms_seq = median_of(sequential)
         seeded(0)
         r = aug.batch(pts, off)
         res[name] = dict(block_ms=ms_block, block_kernel_ms=kernel_ms, sequential_ms=ms_seq, snow=int(r['snow'].sum()),
