@@ -489,6 +489,37 @@ LSS_API lss_status lss_lisa_average_cloud_batch(lss_engine *e, const float *d_po
                                                 uint32_t *d_gauss_state_out, void *d_workspace, int64_t workspace_bytes,
                                                 void *stream);
 LSS_API int64_t lss_lisa_average_cloud_batch_workspace_bytes(int64_t n_total, int n_clouds);
+/* The whole LISA block of DenseDataset.__getitem__ (dense_dataset.py:713-746) with those models, the per-sample draws
+ * included: for each cloud in batch order, the coin flip np.random.choice(choices), if it comes up true and n_rates > 0
+ * the rain rate np.random.choice(rainfall_rates), then one legacy Gaussian per row detected under that rate, all on one
+ * NumPy legacy stream replayed from h_gauss_state.  The rows, counts and final state equal B calls of the block in turn
+ * (lss_lisa_average_cloud_batch with the decisions those calls draw).
+ *   d_points, n_features >= 5, h_cloud_offsets, d_cloud_counts, d_out_points, d_out_counts, d_out_n_lost
+ *                   as lss_lisa_average_cloud_batch (clouds not applied are copied through); fewer than 2^29 rows in all
+ *   h_choices       uint8[n_choices] host, 1 <= n_choices <= 64: the coin flip's list (nonzero = applied)
+ *   h_rate_candidate int32[n_rates] host: the candidate (< n_candidates) of each entry of the rain-rate list; n_rates 0:
+ *                   no rate is drawn and every applied cloud takes candidate 0 (sampling other than 'uniform')
+ *   model, p_min, r_min, range_accuracy, h_gauss_state, d_gauss_state_out   as lss_lisa_average_batch
+ *   h_alpha, h_range_scale  float64[n_candidates] host, 1 <= n_candidates <= 64: each candidate's alpha (and Goodin's
+ *                   (1 - exp(-Rr))^2), computed by the caller with NumPy
+ *   d_out_draws     int64[n_clouds * 4]: per cloud the rate index drawn (0 without a rate draw; -1 not applied), the raw
+ *                   word its Gaussians start at (counted from word 0 of the start key), whether a cached Gaussian
+ *                   was waiting there (0 / 1), and the Gaussians it took
+ *   d_workspace     lss_lisa_average_block_batch_workspace_bytes(n_total, n_clouds, n_candidates, n_rates) bytes.
+ * Launches per call do not depend on n_clouds.  The stream is bounded as lss_lisa_average_batch's, plus the coin and rate
+ * words (17 standard deviations); a call that needs more latches LSS_ERR_WORKSPACE and never returns a wrong row. */
+LSS_API lss_status lss_lisa_average_block_batch(lss_engine *e, const float *d_points, int n_features,
+                                                const int64_t *h_cloud_offsets, const int32_t *d_cloud_counts,
+                                                int n_clouds, const uint8_t *h_choices, int n_choices,
+                                                const int32_t *h_rate_candidate, int n_rates, int model,
+                                                const double *h_alpha, const double *h_range_scale, int n_candidates,
+                                                double p_min, double r_min, double range_accuracy,
+                                                const uint32_t *h_gauss_state, float *d_out_points,
+                                                int32_t *d_out_counts, int32_t *d_out_n_lost, int64_t *d_out_draws,
+                                                uint32_t *d_gauss_state_out, void *d_workspace,
+                                                int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_lisa_average_block_batch_workspace_bytes(int64_t n_total, int n_clouds, int n_candidates,
+                                                             int n_rates);
 
 /* ---- point-range mask + voxelisation ("next" row, SURVEY.md 8f-4) ---------------------------------------------------------
  * The detector-input stage of the reference's data path on device-resident clouds, e.g. the slot-compacted output of

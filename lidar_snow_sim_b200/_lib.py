@@ -122,6 +122,10 @@ SIGNATURES = [
                                                 _c.c_double, _c.c_double, _c.c_int, _P, _P, _P, _P, _P, _P, _c.c_int64,
                                                 _P]),
     ('lss_lisa_average_cloud_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_lisa_average_block_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _c.c_int, _P, _c.c_int,
+                                                _c.c_int, _P, _P, _c.c_int, _c.c_double, _c.c_double, _c.c_double, _P,
+                                                _P, _P, _P, _P, _P, _P, _c.c_int64, _P]),
+    ('lss_lisa_average_block_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int]),
     ('lss_voxelize_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_int, _c.c_int, _P, _P, _P,
                                       _P, _P, _c.c_int64, _P]),
     ('lss_voxelize_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int, _c.c_int, _c.c_int]),

@@ -62,12 +62,26 @@ struct GaussArgs {
     int *status;
 };
 
+// The raw key blocks 0 .. n_blocks - 1 from the start key, block after block, by every thread of a CTA of MT_TPB threads
+__device__ __forceinline__ void lg_key_blocks(const uint32_t *key0, uint32_t *stream, int n_blocks)
+{
+    __shared__ uint32_t key[2][MT_N];
+    const int tid = threadIdx.x;
+    for (int t = tid; t < MT_N; t += MT_TPB) key[0][t] = stream[t] = key0[t];
+    __syncthreads();
+    for (int k = 1; k < n_blocks; k++) {
+        const uint32_t *o = key[(k - 1) & 1];
+        uint32_t *nw = key[k & 1];
+        mt_gen_block(o, nw, tid);
+        for (int t = tid; t < MT_N; t += MT_TPB) stream[(int64_t)k * MT_N + t] = nw[t];
+    }
+}
+
 // The plan's tail, by every thread of a CTA of MT_TPB threads: with the Gaussians of the longest run (m_max from attempts)
 // and of the run that leaves the final state (g_final in all, m_final from attempts), the control record, the default
 // final state and the raw key blocks.
 __device__ __forceinline__ void lg_stream(const GaussArgs &g, long long m_max, long long g_final, long long m_final)
 {
-    __shared__ uint32_t key[2][MT_N];
     const int tid = threadIdx.x;
     const long long need = (m_max + 1) / 2;
     long long n_att = lg_attempt_bound(need);
@@ -83,15 +97,7 @@ __device__ __forceinline__ void lg_stream(const GaussArgs &g, long long m_max, l
         g.state_out[MT_N] = (uint32_t)g.pos0;
         g.state_out[MT_N + 1] = g_final == 0 ? LG_GAUSS_AS_START : LG_NO_GAUSS;     // (the cached one was used)
     }
-    const int n_blocks = (int)lg_stream_blocks(g.pos0, n_att);
-    for (int t = tid; t < MT_N; t += MT_TPB) key[0][t] = g.stream[t] = g.key[t];
-    __syncthreads();
-    for (int k = 1; k < n_blocks; k++) {
-        const uint32_t *o = key[(k - 1) & 1];
-        uint32_t *nw = key[k & 1];
-        mt_gen_block(o, nw, tid);
-        for (int t = tid; t < MT_N; t += MT_TPB) g.stream[(int64_t)k * MT_N + t] = nw[t];
-    }
+    lg_key_blocks(g.key, g.stream, (int)lg_stream_blocks(g.pos0, n_att));
 }
 
 __device__ __forceinline__ double lg_double(const uint32_t *stream, int64_t raw)
@@ -100,15 +106,23 @@ __device__ __forceinline__ double lg_double(const uint32_t *stream, int64_t raw)
     return ((double)a * 67108864.0 + (double)b) / 9007199254740992.0;
 }
 
-// attempt j: x1, x2, r2 as NumPy computes them; returns whether it is accepted
-__device__ __forceinline__ bool lg_attempt(const GaussArgs &g, int64_t j, double &x1, double &x2, double &r2)
+// the attempt that starts at raw word `raw`: x1, x2, r2 as NumPy computes them; returns whether it is accepted
+__device__ __forceinline__ bool lg_attempt_at(const uint32_t *stream, int64_t raw, double &x1, double &x2, double &r2)
 {
-    const int64_t raw = (int64_t)g.pos0 + 4 * j;
-    x1 = __dadd_rn(__dmul_rn(2.0, lg_double(g.stream, raw)), -1.0);
-    x2 = __dadd_rn(__dmul_rn(2.0, lg_double(g.stream, raw + 2)), -1.0);
+    x1 = __dadd_rn(__dmul_rn(2.0, lg_double(stream, raw)), -1.0);
+    x2 = __dadd_rn(__dmul_rn(2.0, lg_double(stream, raw + 2)), -1.0);
     r2 = __dadd_rn(__dmul_rn(x1, x1), __dmul_rn(x2, x2));
     return r2 < 1.0 && r2 != 0.0;
 }
+
+// attempt j of a run from the start state
+__device__ __forceinline__ bool lg_attempt(const GaussArgs &g, int64_t j, double &x1, double &x2, double &r2)
+{
+    return lg_attempt_at(g.stream, (int64_t)g.pos0 + 4 * j, x1, x2, r2);
+}
+
+// f = sqrt(-2 log r2 / r2) of an accepted attempt; its Gaussians are f x2 (first) and f x1 (second, the cached one)
+__device__ __forceinline__ double lg_polar_f(double r2) { return sqrt(__ddiv_rn(__dmul_rn(-2.0, log(r2)), r2)); }
 
 __global__ void __launch_bounds__(LG_TILE) k_lg_flags(GaussArgs g)
 {
@@ -131,7 +145,7 @@ __global__ void __launch_bounds__(LG_TILE) k_lg_accept(GaussArgs g)
     const bool acc = j < n_att && lg_attempt(g, j, x1, x2, r2);
     const int k = seg_rank<1, LG_TILE>(acc ? 0 : -1, g.att, 0, tile);
     if (k < 0 || k >= need) return;
-    const double f = sqrt(__ddiv_rn(__dmul_rn(-2.0, log(r2)), r2));
+    const double f = lg_polar_f(r2);
     g.pair[2 * (int64_t)k] = __dmul_rn(f, x2);
     g.pair[2 * (int64_t)k + 1] = __dmul_rn(f, x1);
     if (m_final > 0 && k == (m_final - 1) / 2) {

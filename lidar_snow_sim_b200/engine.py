@@ -969,6 +969,53 @@ class SnowfallEngine:
             _set_mt_state(start, state)
         return out
 
+    def lisa_average_block_batch(self, points, cloud_offsets, model, alpha, p_min, choices, rate_candidate=None,
+                                 r_min=0.9, range_accuracy=0.09, range_scale=None, counts=None):
+        """
+        The dataset's whole LISA block (dense_dataset.py:713-746) with average_augment or goodin_augment on a batch of
+        device-resident float32 clouds, its per-sample draws included (lss_lisa_average_block_batch, current stream):
+        each cloud draws its coin flip np.random.choice(choices), then, when applied and rate_candidate is given, the
+        rain rate np.random.choice(rainfall_rates), then its detected rows' Gaussians, all from NumPy's global
+        generator in batch order.  alpha (and Goodin's range_scale): one value per candidate rate (at most 64);
+        rate_candidate: for each entry of the rate list the candidate its value maps to (None: no rate is drawn, the
+        dataset's sampling other than 'uniform', and every applied cloud takes candidate 0).  points, counts, r_min,
+        range_accuracy and p_min as lisa_average_cloud_batch.  Synchronises once and sets NumPy's global state as B
+        calls of the block leave it.  Returns dict(points (N, F) float32: each cloud's kept rows at the front of its
+        slot; counts (B,) int32; n_lost (B,) int32; draws: host int64 (B, 4), per cloud the rate index drawn (-1 not
+        applied, 0 without a rate draw), the raw word its Gaussians start at (from word 0 of the start key), whether
+        a cached Gaussian waited there, and the Gaussians it took).
+        """
+        off, B, N = _cloud_offsets(cloud_offsets)
+        _check_tensor('points', points, self.device, torch.float32, (N, None), min_cols=5)
+        _check_tensor('counts', counts, self.device, torch.int32, (B,), optional=True)
+        ch = np.ascontiguousarray(np.asarray(choices).reshape(-1) != 0, dtype=np.uint8)
+        if not 1 <= ch.shape[0] <= 64:
+            raise ValueError(f'choices: expected 1 to 64 entries, got {ch.shape[0]}')
+        K = np.asarray(alpha).size
+        if not 1 <= K <= 64:
+            raise ValueError(f'alpha: expected 1 to 64 candidate rates, got {K}')
+        rc = None if rate_candidate is None else np.ascontiguousarray(rate_candidate, dtype=np.int32).reshape(-1)
+        if rc is not None and (rc.shape[0] == 0 or rc.min() < 0 or rc.max() >= K):
+            raise ValueError(f'rate_candidate: expected a non-empty list of candidates in [0, {K})')
+        al, sc, start, words = self._lisa_average_params(K, model, alpha, range_scale, False)
+        F = points.shape[1]
+        out = _outputs(None, self.device, points=((N, F), torch.float32), counts=((B,), torch.int32),
+                       n_lost=((B,), torch.int32))
+        host = torch.empty(MT_GAUSS_WORDS // 2 + 4 * B, dtype=torch.int64, device=self.device)   # state, then draws
+        n_rates = 0 if rc is None else rc.shape[0]
+        ws = self._scratch('lisa_block', self.lib.lss_lisa_average_block_batch_workspace_bytes(N, B, K, n_rates))
+        self._call('lss_lisa_average_block_batch', points, F, _ptr(off), counts, B, _ptr(ch), ch.shape[0], _ptr(rc),
+                   n_rates, int(model), _ptr(al), _ptr(sc), K, float(p_min), float(r_min), float(range_accuracy),
+                   _ptr(words), out['points'], out['counts'], out['n_lost'], host[MT_GAUSS_WORDS // 2:],
+                   host[:MT_GAUSS_WORDS // 2], ws, ws.numel())
+        draws = np.zeros((0, 4), np.int64)
+        if B > 0:
+            host = host.cpu()                                      # the one synchronisation: state and draws
+            _set_mt_state(start, host[:MT_GAUSS_WORDS // 2].view(torch.int32))
+            draws = host[MT_GAUSS_WORDS // 2:].numpy().reshape(B, 4)
+        out['draws'] = draws
+        return out
+
     def _pa_args(self, points, cloud_offsets, planes, nparts, box_offsets, counts):
         """(off, B, boff, M) of the arguments pa_partition_batch and pa_apply_batch share, checked"""
         off, B, N = _cloud_offsets(cloud_offsets)

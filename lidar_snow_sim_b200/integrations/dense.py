@@ -230,15 +230,18 @@ def _no_pair_message(rainfall_rate):
 _LISA_CHANCES = {'8in9': [1, 1, 1, 1, 1, 1, 1, 1, 0], '1in10': [1, 0, 0, 0, 0, 0, 0, 0, 0, 0]}   # dense_dataset.py:717-722
 
 
+def _lisa_choices(method):
+    """the coin flip's list of the LISA key `method` (dense_dataset.py:717-722)"""
+    for key, c in _LISA_CHANCES.items():
+        if key in method:
+            return c
+    return [0]
+
+
 def _lisa_draws(method, rainfall_rates):
     """The block's draws from NumPy's global generator for one sample: the coin flip, then the rain rate under 'uniform'
     (dense_dataset.py:717-730).  Returns (applied, rain rate)."""
-    choices = [0]
-    for key, c in _LISA_CHANCES.items():
-        if key in method:
-            choices = c
-            break
-    if not np.random.choice(choices):
+    if not np.random.choice(_lisa_choices(method)):
         return False, 0
     rainfall_rate = 0
     if 'uniform' in method:
@@ -270,18 +273,28 @@ def lisa_block(points, dataset_cfg, lisa, rainfall_rates, training=True):
     return points[np.where(points[:, 4] != 0)]
 
 
-def lisa_block_batch(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, counts=None, training=True):
+def lisa_block_batch(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, counts=None, training=True,
+                     all_modes=False):
     """`lisa_block` for a batch of device-resident clouds in one LISA.augment_batch call: points CUDA float32 (N, F),
     F >= 5; cloud b = rows cloud_offsets[b]:cloud_offsets[b+1] (the first counts[b] with `counts`).  The draws are taken
     sample by sample in batch order -- coin flip, rain rate, and for an applied sample the generator key augment would
     draw -- so every cloud's rows and NumPy's global state afterwards equal B lisa_block calls in turn.  Returns
     dict(points (N, F) float32, each cloud's rows at the front of its slot; counts (B,) int32; n_lost (B,) int32).
-    Only LISA's Monte-Carlo modes: the others draw NumPy's Gaussians on the device, which the per-sample host draws
-    (coin flip, rain rate) would have to interleave with; lisa_block takes them one sample at a time."""
+    Without all_modes, only LISA's Monte-Carlo modes: the others draw NumPy's Gaussians on the device, which the
+    per-sample host draws (coin flip, rain rate) would have to interleave with; lisa_block takes them one sample at a
+    time.
+    all_modes=True also takes the fog, haze and spray modes and 'goodin et al.' (a LISA built with all_modes=True): the
+    coin flips and rain rates are then drawn on the device, between the clouds' Gaussians, on one replay of NumPy's
+    stream (SnowfallEngine.lisa_average_block_batch), and the call synchronises once, at the end.  Rows, counts, the
+    decisions and NumPy's whole state equal B lisa_block calls in turn.  With all_modes the result also holds
+    applied (B,) host bool and rainfall_rate (B,) host float64 (0 where not applied), for every mode."""
     import torch
     if not getattr(lisa, 'monte_carlo', True):
-        raise NotImplementedError(f"lisa_block_batch runs LISA's Monte-Carlo modes only, not '{lisa.atm_model}': their "
-                                  f"Gaussians interleave with the per-sample host draws; use lisa_block per sample")
+        if not all_modes:
+            raise NotImplementedError(f"lisa_block_batch runs LISA's Monte-Carlo modes only, not '{lisa.atm_model}': "
+                                      f"their Gaussians interleave with the per-sample host draws; use lisa_block per "
+                                      f"sample, or pass all_modes=True")
+        return _lisa_block_batch_device(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, counts, training)
     off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
     B = off.shape[0] - 1
     if points.dim() != 2 or points.shape[1] < 5:
@@ -295,9 +308,55 @@ def lisa_block_batch(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, c
             if apply[b]:
                 seeds[b] = lisa.draw_seed()
     if not apply.any():
+        res = dict(points=points, counts=_slot_counts(off, points.device) if counts is None else counts,
+                   n_lost=torch.zeros(B, dtype=torch.int32, device=points.device))
+    else:
+        res = lisa.augment_batch(points, off, rates, counts=counts, apply=apply, seeds=seeds)
+    if all_modes:
+        res.update(applied=apply, rainfall_rate=rates)
+    return res
+
+
+def _lisa_block_batch_device(points, cloud_offsets, dataset_cfg, lisa, rainfall_rates, counts, training):
+    """lisa_block_batch(all_modes=True) of the average modes and Goodin: the candidate rates are the distinct values of
+    rainfall_rates under 'uniform' (else the one rate 0, as lisa_block passes it); the average modes' detection does not
+    depend on the rate, so they have one candidate."""
+    import torch
+    off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
+    B = off.shape[0] - 1
+    if points.dim() != 2 or points.shape[1] < 5:
+        raise ValueError('lisa_block_batch needs (N, >= 5) float32 rows (the F = 4 branch builds a float64 array)')
+    applied, rainfall_rate = np.zeros(B, dtype=bool), np.zeros(B)
+    if not (training and 'LISA' in dataset_cfg):
         return dict(points=points, counts=_slot_counts(off, points.device) if counts is None else counts,
-                    n_lost=torch.zeros(B, dtype=torch.int32, device=points.device))
-    return lisa.augment_batch(points, off, rates, counts=counts, apply=apply, seeds=seeds)
+                    n_lost=torch.zeros(B, dtype=torch.int32, device=points.device), applied=applied,
+                    rainfall_rate=rainfall_rate)
+    method = dataset_cfg['LISA']
+    rates, rate_candidate, values = None, None, [0]
+    if 'uniform' in method:
+        rates = np.asarray(rainfall_rates)
+        if rates.size == 0:
+            raise ValueError("lisa_block_batch: 'uniform' sampling needs a non-empty rainfall_rates")
+        values, rate_candidate = np.unique(rates, return_inverse=True)
+    goodin = lisa.atm_model == 'goodin et al.'
+    if not goodin:
+        values, rate_candidate = [None], None if rate_candidate is None else np.zeros_like(rate_candidate)
+    if len(values) > 64:
+        raise ValueError(f'lisa_block_batch: {len(values)} distinct rain rates; at most 64 are supported')
+    params = [lisa._average_params(v) for v in values]
+    model, p_min = params[0][0], params[0][3]
+    engine = lisa.engine or default_engine()
+    res = engine.lisa_average_block_batch(points, off, model, [q[1] for q in params], p_min, _lisa_choices(method),
+                                          rate_candidate=rate_candidate, r_min=float(lisa.r_min),
+                                          range_accuracy=float(lisa.range_accuracy),
+                                          range_scale=[q[2] for q in params] if goodin else None, counts=counts)
+    engine.check()
+    idx = res.pop('draws')[:, 0]
+    applied = idx >= 0
+    if rates is not None:
+        rainfall_rate[applied] = rates[idx[applied]]
+    res.update(applied=applied, rainfall_rate=rainfall_rate)
+    return res
 
 
 def foggify_cvl(points, alpha, dataset_cfg, engine=None, lut_dir=None, rng=None, lut=None):
