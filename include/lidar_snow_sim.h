@@ -435,6 +435,55 @@ LSS_API lss_status lss_lisa_cloud_batch(lss_engine *e, const float *d_points, in
                                         void *d_workspace, int64_t workspace_bytes, void *stream);
 LSS_API int64_t lss_lisa_cloud_batch_workspace_bytes(int64_t n_total, int n_clouds);
 
+/* ---- LISA's C++ core (the reference's `pylisa`: lib/LISA/src Lisa.cpp, MiniLisa.cpp, Utils.cpp) --------------------------
+ * lss_pylisa_qext: Utils.cpp calc_qext(x, m) for every size parameter h_x[j] (float64[n] host, finite and > 0) and one
+ * complex refractive index m = m_re + i m_im: the extinction efficiency from S1(0), Wiscombe's n_stop = round(x +
+ * 4 x^0.3333 + 2) and n_mx = round(max(n_stop, |m| x) + 15) (half away from zero, computed on the host with libm), the
+ * logarithmic derivative downward from 0, psi / chi upward from sin x / cos x, complex arithmetic as libgcc's __muldc3 /
+ * __divdc3.  One thread per size parameter, longest series first.
+ *   d_out        float64[n] device: qext(h_x[j])
+ *   d_workspace  lss_pylisa_qext_workspace_bytes(...) bytes (D_0 .. D_(n_stop - 1) of every series: about 200 MB for the
+ *                reference's 2000 diameters logspace(-6, 1.5) mm at 0.903 um).  No allocation, no synchronisation.
+ * LSS_ERR_INVALID_ARG for a non-finite m, a bad x, or a series longer than LSS_MIE_MAX_ORDER; the query returns -1.     */
+LSS_API lss_status lss_pylisa_qext(lss_engine *e, const double *h_x, int n, double m_re, double m_im, double *d_out,
+                                   void *d_workspace, int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_pylisa_qext_workspace_bytes(const double *h_x, int n, double m_re, double m_im);
+/* lss_pylisa_batch: Lisa::augment(pc, Rr) (5 columns: x, y, z, reflectance, label 0 lost / 1 scattered / 2 original) or,
+ * with LSS_PYLISA_MINI, MiniLisa::augment(pc, Rr) (4 columns) on a batch of device-resident float64 clouds, one call of
+ * the augmenter per cloud.  Each row keeps every quirk of the reference (the dead rounding draw, ceil(Nt) ranges from the
+ * unrounded Nt, pow(u, 0.3333), diameters only when a range was kept, the first maximum, three branches against
+ * p_min = 0.9 / max_range^2, lost rows as zeros, a Gaussian only for rows kept).  Random numbers: Philox-4x32-10 of the
+ * counter (draw, row, call lo, call hi) under key (seed lo, seed hi), generate_canonical's two-word mapping:
+ * augmenter draws under (h_aug_key[b], h_aug_call[b]), diameter draws under (h_dist_key[b], h_dist_call[b]) at the kept
+ * rank.
+ *   d_points          float64[n_total * n_features], n_features >= 4 (x, y, z, reflectance, ...)
+ *   h_cloud_offsets   int64[n_clouds + 1] host; d_cloud_counts int32[n_clouds] device or NULL: valid rows per slot
+ *   h_rain_rate       float64[n_clouds] host: Rr [mm/h] of each cloud (Marshall-Palmer N_total for the particle count)
+ *   h_alpha           float64[n_clouds] host, or NULL: then each cloud's alpha is MiniLisa::calc_alpha with the
+ *                     Marshall-Palmer N_model over d_qext_table (float64[n_diameters * 2] device: d [mm], qext; 2 to 6144
+ *                     diameters), Utils.cpp trapz summed in order on the device
+ *   h_aug_key, h_aug_call, h_dist_key, h_dist_call   uint64[n_clouds] host (the dist pair may be NULL with LSS_PYLISA_MINI)
+ *   ran_uncer, min_range, max_range, b_div   the Lidar's values; ref_r  Lisa's Fresnel term |(m - 1) / (m + 1)|^2
+ *   d_out_points      float64[n_total * (5 or 4)]: rows of the valid rows of each slot; rows behind them untouched
+ *   d_out_alpha       float64[n_clouds]: the alpha each cloud used
+ *   d_out_status      int32[n_clouds]: 0; 1 where a row's particle count Nt is NaN (a NaN coordinate: the reference's
+ *                     std::vector::reserve throws); 2 where Nt is infinite or above 2^31 - 1 (an infinite range: the
+ *                     reference never returns).  Those clouds' rows are unspecified.
+ *   d_out_record      int32[n_total * 3] device or NULL: per row, ranges drawn, ranges kept, Gaussian pairs rejected (-1:
+ *                     no Gaussian drawn)
+ *   d_workspace       lss_pylisa_batch_workspace_bytes(n_clouds) bytes.  1 staging launch and 2 kernels; no allocation, no
+ *                     synchronisation.                                                                                 */
+#define LSS_PYLISA_MINI 0x1
+LSS_API lss_status lss_pylisa_batch(lss_engine *e, const double *d_points, int n_features, const int64_t *h_cloud_offsets,
+                                    const int32_t *d_cloud_counts, int n_clouds, int flags, const double *h_rain_rate,
+                                    const double *h_alpha, const double *d_qext_table, int n_diameters,
+                                    const uint64_t *h_aug_key, const uint64_t *h_aug_call, const uint64_t *h_dist_key,
+                                    const uint64_t *h_dist_call, double ran_uncer, double min_range, double max_range,
+                                    double b_div, double ref_r, double *d_out_points, double *d_out_alpha,
+                                    int32_t *d_out_status, int32_t *d_out_record, void *d_workspace,
+                                    int64_t workspace_bytes, void *stream);
+LSS_API int64_t lss_pylisa_batch_workspace_bytes(int n_clouds);
+
 /* ---- LISA's fog / haze / spray modes and Goodin et al.'s rain model -----------------------------------------------------
  * LISA.average_augment (lib/LISA/python/lisa.py:340-388: chu_hogg_fog, strong_advection_fog, moderate_advection_fog,
  * coast_haze, continental_haze, moderate_spray, strong_spray) and LISA.goodin_augment (:391-443: 'goodin et al.') on a

@@ -28,6 +28,7 @@ FLAG_DEVICE_PREPASS = 0x4
 FLAG_ASSUME_SORTED = 0x8
 FOG_HARD, FOG_SOFT, FOG_GAIN = 0x1, 0x2, 0x4
 DROR_CUBE, DROR_WORK_STATS = 0x1, 0x100
+PYLISA_MINI = 0x1
 
 
 
@@ -115,6 +116,12 @@ SIGNATURES = [
                                         _c.c_double, _c.c_double, _c.c_double, _c.c_double, _c.c_int, _P, _c.c_int, _P, _P,
                                         _P, _P, _c.c_int64, _P]),
     ('lss_lisa_cloud_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),
+    ('lss_pylisa_qext', _c.c_int, [_P, _P, _c.c_int, _c.c_double, _c.c_double, _P, _P, _c.c_int64, _P]),
+    ('lss_pylisa_qext_workspace_bytes', _c.c_int64, [_P, _c.c_int, _c.c_double, _c.c_double]),
+    ('lss_pylisa_batch', _c.c_int, [_P, _P, _c.c_int, _P, _P, _c.c_int, _c.c_int, _P, _P, _P, _c.c_int, _P, _P, _P, _P,
+                                    _c.c_double, _c.c_double, _c.c_double, _c.c_double, _c.c_double, _P, _P, _P, _P, _P,
+                                    _c.c_int64, _P]),
+    ('lss_pylisa_batch_workspace_bytes', _c.c_int64, [_c.c_int]),
     ('lss_lisa_average_batch', _c.c_int, [_P, _P, _c.c_int, _P, _c.c_int, _c.c_int, _P, _P, _c.c_double, _c.c_double,
                                           _c.c_double, _c.c_int, _P, _P, _P, _P, _c.c_int64, _P]),
     ('lss_lisa_average_batch_workspace_bytes', _c.c_int64, [_c.c_int64, _c.c_int]),

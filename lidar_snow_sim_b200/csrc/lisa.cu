@@ -20,6 +20,7 @@
 //   * otherwise the reference is not reproducible itself (a thread pool shares the global generator, :333-339); the kernel
 //     uses a counter-based generator (Philox-4x32-10) keyed by (seed, return index), restated in NumPy by
 //     tests/lisa_stream.py: tests/test_lisa_stream_gpu.py holds both kernels to the oracle replayed on that stream.
+#include "philox.cuh"
 #include "segments.cuh"
 #include <algorithm>
 #include <cmath>
@@ -39,14 +40,7 @@ struct LisaArgs {
     int *status;
 };
 
-// ---- Philox-4x32-10 ----------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void philox_round(unsigned &c0, unsigned &c1, unsigned &c2, unsigned &c3, unsigned k0, unsigned k1)
-{
-    const unsigned long long p0 = (unsigned long long)0xD2511F53u * c0, p1 = (unsigned long long)0xCD9E8D57u * c2;
-    const unsigned n0 = (unsigned)(p1 >> 32) ^ c1 ^ k0, n1 = (unsigned)p1, n2 = (unsigned)(p0 >> 32) ^ c3 ^ k1, n3 = (unsigned)p0;
-    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-}
-
+// ---- Philox-4x32-10 (philox.cuh) -----------------------------------------------------------------------------------------
 __device__ double philox_double(unsigned long long seed, unsigned long long point, unsigned long long draw)
 {
     unsigned c0 = (unsigned)draw, c1 = (unsigned)(draw >> 32), c2 = (unsigned)point, c3 = (unsigned)(point >> 32);
