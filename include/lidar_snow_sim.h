@@ -302,7 +302,14 @@ LSS_API int64_t lss_wet_ground_poly_workspace_bytes(int64_t n_total, int n_cloud
  *   d_out        float64[n_total*n_features]  augmented rows in input order (float32 valued when only LSS_FOG_HARD)
  *   d_out_fog_mask uint8[n_total]             1 = the fog response replaced the return (simulated_fog_pc = rows with 1)
  *   d_out_rank   int32[n_total] or NULL       rank of each fog point among its cloud's fog points, -1 elsewhere
- *   d_out_info   float64[n_clouds*3]          min_fog_response (inf if none), max_fog_response, num_fog_responses
+ *   d_out_info   float64[n_clouds*3]          min_fog_response (inf if none), max_fog_response (0 if none or all
+ *                                             below 0), num_fog_responses.  A negative count flags a cloud where the
+ *                                             reference raises inside its loop (with LSS_FOG_SOFT): -1 - (2 * fog points
+ *                                             before the first such row + kind), kind 0 = a NaN range (KeyError(nan):
+ *                                             the row is not fog), kind 1 = a fog point of infinite range with v1 noise
+ *                                             (Generator.uniform's OverflowError); the other outputs are then undefined
+ * NaN handling: a NaN fog response is never fog (builtin min(NaN, 255) is NaN); LSS_FOG_GAIN takes builtin max's
+ * maximum -- NaN only when row 0's intensity is NaN, else the largest non-NaN one, the first of equal values (-0 / +0).
  * Parity: masks, ranks, counts and the random stream are exact; intensities / coordinates agree to float64 rounding
  * except where the reference itself is host-defined (float32 np.exp, scalar float32 power, pow): DESIGN.md 8.          */
 #define LSS_FOG_HARD 0x1u

@@ -14,6 +14,11 @@
 //   k_fog_apply   everything: hard, soft, noise (k-th PCG64 output by jump-ahead), min / max response, max intensity,
 //                 num_fog_responses
 //   k_fog_gain    intensity *= 255 / ceil(max intensity)                                            (:282-285)
+// Where the reference raises inside its loop, after the draws of the fog points before the row: a NaN range has no
+// table key (KeyError(nan), :214; the row is not fog here), and with v1 noise a fog point at an infinite range asks
+// Generator.uniform for an infinite interval (OverflowError, :241).  The cloud's info carries the first such row's kind
+// and the number of fog points before it, so the host mirrors can raise with the caller's generator where the
+// reference leaves it.
 // k_fog_count / k_fog_apply take their fog parameters (alpha, beta, beta_0, table) either once for the whole batch
 // (lss_fog_batch) or per cloud (lss_fog_batch_params, PER_CLOUD = true); the arithmetic is the same.
 //
@@ -28,6 +33,7 @@ namespace {
 constexpr int FOG_TILE = 256;                     // points per CTA; rows are staged through shared memory (coalesced I/O)
 constexpr int FOG_STAGE_F = 8;                    // ... for up to this many features; wider rows are accessed in place
 constexpr int LUT_N = 2001;
+constexpr int FOG_INFO = 6;                       // workspace info words per cloud (FogArgs::info)
 
 struct FogArgs {
     const float *pts;            // [N * F]
@@ -45,8 +51,16 @@ struct FogArgs {
     uint8_t *mask;               // [N]
     int32_t *rank;               // [N] or null
     SegTiles seg;                // tiles of FOG_TILE rows, one class: fog points
-    unsigned long long *info;    // [B * 4] zero-filled; bit patterns: ~min response, max response, count, max intensity
-                                 // (ordered; the minimum is kept complemented so that 0 is the neutral value of both)
+    unsigned long long *info;    // [B * FOG_INFO] zero-filled; bit patterns: ~min response, max response, count,
+                                 // gain maximum, ~first zero intensity, ~first NaN range (ordered; minima are kept
+                                 // complemented so that 0 is the neutral value of every word):
+                                 //   gain maximum  ord_of of the largest non-NaN output intensity with -0 read as +0,
+                                 //                 all ones (a NaN) when row 0's is NaN (builtin max keeps a first NaN
+                                 //                 and skips every later one)
+                                 //   first zero    (row << 1) | sign bit of the first row whose output intensity is +-0
+                                 //                 (builtin max keeps the first of equal values: the sign of a zero max)
+                                 //   first raise   (row << 32) | (fog points before that row) << 1 | kind of the first
+                                 //                 row where the reference raises: 0 NaN range, 1 v1 noise at inf
 };
 
 // correctly rounded float32 exp via float64 (np.exp on float32 is a host SIMD kernel, < 1 ulp but host defined)
@@ -64,7 +78,7 @@ __device__ __forceinline__ double ord_to(unsigned long long o)
     return __longlong_as_double((long long)b);
 }
 
-struct Soft { bool fog; double resp, fog_distance; float r0, hard_i; };
+struct Soft { bool fog, nan_key; double resp, fog_distance; float r0, hard_i; };
 
 struct FogCloud { const double *lut; double alpha, beta, beta_0; };
 
@@ -89,8 +103,10 @@ __device__ __forceinline__ Soft soft_target(const FogArgs &a, const FogCloud &c,
         s.hard_i = rintf(__fmul_rn(exp32(__fmul_rn(coef, s.r0)), I));
     }
     s.fog = false; s.resp = 0.0; s.fog_distance = 0.0;
-    if (a.soft) {
-        // key = float(str(round(r_0, 1))), min(key, 200): index rint(float32(r_0 * 10)) capped at 2000   (:212-214)
+    s.nan_key = a.soft && isnan(s.r0);                                      // integral_dict[nan]: KeyError (:214)
+    if (a.soft && !s.nan_key) {
+        // key = float(str(round(r_0, 1))), min(key, 200): index rint(float32(r_0 * 10)) capped at 2000, an infinite
+        // range (or r_0 * 10 overflowing) included   (:212-214)
         const float k10 = rintf(__fmul_rn(s.r0, 10.0f));
         int k = (k10 >= (float)(LUT_N - 1)) ? LUT_N - 1 : (int)k10;
         k = k < 0 ? 0 : k;
@@ -98,7 +114,7 @@ __device__ __forceinline__ Soft soft_target(const FogArgs &a, const FogCloud &c,
         double r = __dmul_rn(c.lut[2 * k + 1], (double)I);                  // * original intensity       (:216)
         r = __dmul_rn(r, (double)__fmul_rn(s.r0, s.r0));                    // * r_0 ** 2 (float32)
         r = __ddiv_rn(__dmul_rn(r, c.beta), c.beta_0);
-        s.resp = fmin(r, 255.0);                                            // :219
+        s.resp = 255.0 < r ? 255.0 : r;                                     // builtin min(r, 255) keeps a NaN (:219)
         s.fog = s.resp > (double)s.hard_i;                                  // :221
     }
     return s;
@@ -178,12 +194,12 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
 {
     __shared__ float s_in[FOG_TILE * FOG_STAGE_F];
     __shared__ double s_out[FOG_TILE * FOG_STAGE_F];
-    __shared__ unsigned long long s_min, s_max, s_imax;
+    __shared__ unsigned long long s_min, s_max, s_imax, s_zero, s_nan;
     const int b = blockIdx.y, tile = blockIdx.x;
     const int64_t beg = a.cloud_off[b];
     const int n = (int)(a.cloud_off[b + 1] - beg);
     if (tile * FOG_TILE >= n) return;
-    if (threadIdx.x == 0) { s_min = ~0ull; s_max = 0ull; s_imax = 0ull; }
+    if (threadIdx.x == 0) { s_min = ~0ull; s_max = 0ull; s_imax = 0ull; s_zero = 0ull; s_nan = 0ull; }
     const int i = tile * FOG_TILE + threadIdx.x;
     const bool active = i < n;
     const int rows = min(FOG_TILE, n - tile * FOG_TILE);
@@ -251,7 +267,18 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
             atomicMin(&s_min, ord_of(s.resp));
             atomicMax(&s_max, ord_of(s.resp));
         }
-        if (a.gain) atomicMax(&s_imax, ord_of(out_i));
+        const bool inf_v1 = s.fog && a.noise > 0 && a.variant == 1 && isinf(s.r0);
+        if (s.nan_key || inf_v1) atomicMax(&s_nan, ~(((unsigned long long)threadIdx.x << 1) | (inf_v1 ? 1ull : 0ull)));
+        if (a.gain) {
+            // max(augmented_pc[:, 3]) (:283): NaN only from row 0, otherwise the largest other value, the first of equal
+            if (!isnan(out_i)) {
+                atomicMax(&s_imax, ord_of(out_i == 0.0 ? 0.0 : out_i));
+                if (out_i == 0.0)
+                    atomicMax(&s_zero, ~(((unsigned long long)i << 1) | (unsigned long long)(signbit(out_i) ? 1 : 0)));
+            } else if (i == 0) {
+                atomicMax(&s_imax, ~0ull);
+            }
+        }
     }
     __syncthreads();
     if (staged) {                                                  // coalesced store of the tile's float64 rows
@@ -260,9 +287,17 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_apply(FogArgs a)
         for (int f = threadIdx.x; f < nf; f += FOG_TILE) __stcs(dst + f, s_out[f]);
     }
     if (threadIdx.x == 0) {
-        if (s_min != ~0ull) { atomicMax(&a.info[4 * b], ~s_min); atomicMax(&a.info[4 * b + 1], s_max); }
-        if (a.gain) atomicMax(&a.info[4 * b + 3], s_imax);
-        if (a.soft && tile == 0) a.info[4 * b + 2] = (unsigned long long)a.seg.total[0][b];   // (0 for an empty cloud)
+        unsigned long long *info = a.info + (int64_t)FOG_INFO * b;
+        if (s_min != ~0ull) { atomicMax(&info[0], ~s_min); atomicMax(&info[1], s_max); }
+        if (a.gain) { atomicMax(&info[3], s_imax); atomicMax(&info[4], s_zero); }
+        if (a.soft && tile == 0) info[2] = (unsigned long long)a.seg.total[0][b];   // (0 for an empty cloud)
+        if (s_nan) {        // the tile's first raising row: row, fog points before it (the tile's masks), kind
+            const int t = (int)(~s_nan >> 1);
+            int before = a.seg.tile[a.seg.tile_base[b] + tile];
+            for (int k = 0; k < t; k++) before += a.mask[beg + tile * FOG_TILE + k];
+            atomicMax(&info[5], ~(((unsigned long long)(tile * FOG_TILE + t) << 32) |
+                                  ((unsigned long long)before << 1) | (~s_nan & 1ull)));
+        }
     }
 }
 
@@ -274,21 +309,27 @@ __global__ void __launch_bounds__(FOG_TILE) k_fog_gain(FogArgs a)
     const int i = blockIdx.x * FOG_TILE + threadIdx.x;
     if (i >= n) return;
     // max_intensity = np.ceil(max(augmented_pc[:, 3])); gain_factor = 255 / max_intensity; column *= gain_factor
-    const double gain_factor = __ddiv_rn(255.0, ceil(ord_to(a.info[4 * b + 3])));
+    const unsigned long long *info = a.info + (int64_t)FOG_INFO * b;
+    double m = ord_to(info[3]);
+    if (m == 0.0 && (~info[4] & 1ull)) m = -0.0;                   // the first zero was -0: ceil(-0) = -0, gain -inf
+    const double gain_factor = __ddiv_rn(255.0, ceil(m));
     double *o = a.out + (beg + i) * a.F + 3;
     *o = __dmul_rn(*o, gain_factor);
 }
 
 // info: ordered bit patterns -> (min response, max response, count) as doubles; a cloud without fog points reports
-// (inf, 0, 0) like the reference's initial values (:201-203)
+// (inf, 0, 0) like the reference's initial values (:201-203), and a maximum below 0 stays 0.  A cloud where the reference raises reports
+// -1 - (2 * fog points before the first raising row + its kind) as its count.
 __global__ void k_fog_info(FogArgs a, int B, double *info_out)
 {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const unsigned long long cnt = a.info[4 * b + 2];
-    info_out[3 * b] = cnt ? ord_to(~a.info[4 * b]) : __longlong_as_double(0x7ff0000000000000LL);
-    info_out[3 * b + 1] = cnt ? ord_to(a.info[4 * b + 1]) : 0.0;
-    info_out[3 * b + 2] = (double)cnt;
+    const unsigned long long *info = a.info + (int64_t)FOG_INFO * b;
+    const unsigned long long cnt = info[2];
+    info_out[3 * b] = cnt ? ord_to(~info[0]) : __longlong_as_double(0x7ff0000000000000LL);
+    const double mx = ord_to(info[1]);
+    info_out[3 * b + 1] = cnt && mx > 0.0 ? mx : 0.0;             // max_fog_response starts at 0 (:202)
+    info_out[3 * b + 2] = info[5] ? -1.0 - (double)(unsigned)~info[5] : (double)cnt;   // (low 32 bits)
 }
 
 // The workspace, region by region; returns the noise generators' region.  per_cloud: room for the per-cloud parameters
@@ -298,7 +339,7 @@ unsigned long long *fog_carve(WsCarve &c, FogArgs &a, int64_t n_total, int n_clo
     a.cloud_off = c.take<int64_t>(n_clouds + 1);
     a.seg = seg_take(c, n_total, n_clouds, FOG_TILE, 1);
     a.seg.total[0] = c.take<int32_t>(n_clouds);
-    a.info = c.take<unsigned long long>((int64_t)n_clouds * 4);
+    a.info = c.take<unsigned long long>((int64_t)n_clouds * FOG_INFO);
     unsigned long long *rng = c.take<unsigned long long>((int64_t)n_clouds * 4);
     char *par = c.take<char>(per_cloud ? (int64_t)n_clouds * (3 * 8 + 4) : 0);
     a.cloud_par = per_cloud ? (const double *)par : nullptr;
@@ -377,7 +418,7 @@ lss_status fog_run(lss_engine *e, const float *d_points, int n_features, const i
         l.upload(rng, h_rng_state, sizeof(uint64_t) * 4 * B);
         a.rng = rng;
     }
-    l.zero(a.info, (size_t)B * 4 * 8);
+    l.zero(a.info, (size_t)B * FOG_INFO * 8);
     LSS_CUDA_CHECK(e, lss_stage(e, l, st));
     const dim3 grid((unsigned)((g.max_n + FOG_TILE - 1) / FOG_TILE), B);
     if (N > 0) {

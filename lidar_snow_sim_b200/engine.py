@@ -478,7 +478,9 @@ class SnowfallEngine:
         Batched simulate_fog() (lib/LiDAR_fog_sim/fog_simulation.py:299-316) on device-resident clouds (current stream,
         no synchronisation).  points: CUDA float32 (N, F), F >= 4; lut: CUDA float64 (2001, 2) integral look-up table;
         rng_states: host uint64 (B, 4) PCG64 states (variants 1-3) or ext_noise: CUDA float64 (N,) values by rank.
-        Returns dict(points float64 (N, F), fog_mask uint8 (N,), info float64 (B, 3) [, rank int32 (N,)]).
+        Returns dict(points float64 (N, F), fog_mask uint8 (N,), info float64 (B, 3) [, rank int32 (N,)]); info[b] =
+        (min response, max response, count), count -1 - (2 * fog points before the row + kind) for a cloud where the
+        reference raises (kind 0: a NaN range, KeyError; 1: v1 noise at an infinite range, OverflowError).
         """
         off, B, N = _cloud_offsets(cloud_offsets)
         _check_tensor('lut', lut, self.device, torch.float64, (2001, 2), optional=True)

@@ -212,6 +212,26 @@ def _pcg64_advance(rng, delta):
     rng.bit_generator.state = st
 
 
+def _raise_like_reference(rng, n_rows, count, gain, variant, draws):
+    """Raise what P_R_fog_soft raises for a cloud of n_rows rows whose fog pass reported `count`, after its `integers`
+    draw.  A negative count is -1 - (2 * fog points before the first raising row + kind): KeyError(nan) at a NaN range
+    (kind 0, fog_simulation.py:214) or Generator.uniform's OverflowError at a v1 fog point of infinite range (kind 1,
+    :241), both after the noise draws of the fog points before the row.  Gain on an empty cloud raises builtin max's
+    ValueError (:283)."""
+    if count < 0:
+        before, kind = divmod(-1 - int(count), 2)
+        if draws and before:
+            if variant == 4:
+                rng.beta(a=2, b=20, size=before)
+            else:
+                _pcg64_advance(rng, before)
+        if kind:
+            raise OverflowError('high - low range exceeds valid bounds')
+        raise KeyError(math.nan)
+    if gain and n_rows == 0:
+        raise ValueError('max() iterable argument is empty')
+
+
 def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=True, *, engine=None, lut=None,
                  lut_dir=None, rng=None):
     """
@@ -220,6 +240,9 @@ def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=T
     the input's float32 when only `hard`.
     lut: None = the pickled table of the nearest shipped alpha (LSS_FOG_LUT_DIR / lut_dir), a (2001, 2) array, or
     'device' = the table of exactly p.alpha (and p's pulse width and geometry) generated on the device.
+    Raises where the soft target of the reference raises, with `rng` where the reference leaves it: KeyError(nan) for
+    a cloud with a NaN range and OverflowError for v1 noise at an infinite range (after the draws of the fog points
+    before the row), ValueError for gain on an empty cloud.
     """
     variants = {'v1': 1, 'v2': 2, 'v3': 3, 'v4': 4}
     if soft and noise > 0 and noise_variant not in variants:
@@ -243,10 +266,18 @@ def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=T
     variant = variants.get(noise_variant, 1)
     kw = dict(hard=hard, soft=soft, gain=gain, noise=int(noise), noise_variant=variant)
     draws = soft and noise > 0
+    if soft and gain and N == 0:
+        _raise_like_reference(rng, N, 0, gain, variant, draws)
+    if N == 0:                                              # the reference's loop does not run: nothing to compute
+        if not soft:
+            return pc32.copy(), None, None
+        return pc32.astype(np.float64), None, {'min_fog_response': np.inf, 'max_fog_response': 0, 'num_fog_responses': 0}
     if draws and variant == 4:
-        # Generator.beta is rejection sampling (no jump-ahead): first pass for ranks and the count, draw, second pass
-        first = eng.fog_batch(d_pts, off, d_lut, p.alpha, p.beta, p.beta_0, **dict(kw, noise=0))
+        # Generator.beta is rejection sampling (no jump-ahead): first pass for ranks and the count (without the
+        # external values the noise is not applied), draw, second pass
+        first = eng.fog_batch(d_pts, off, d_lut, p.alpha, p.beta, p.beta_0, **kw)
         cnt = int(first['info'][0, 2].item())
+        _raise_like_reference(rng, N, cnt, gain, variant, draws)
         ext = torch.zeros((max(N, 1),), dtype=torch.float64)
         if cnt:
             ext[:cnt] = torch.from_numpy(rng.beta(a=2, b=20, size=cnt))
@@ -260,6 +291,7 @@ def simulate_fog(p, pc, noise, gain=False, noise_variant='v1', hard=True, soft=T
         return aug.astype(np.float32), None, None           # P_R_fog_hard keeps the input's dtype (:183-189)
     info = res['info'].cpu().numpy()[0]
     cnt = int(info[2])
+    _raise_like_reference(rng, N, cnt, gain, variant, draws and variant != 4)
     if draws and variant != 4 and cnt:
         _pcg64_advance(rng, cnt)
     mask = res['fog_mask'].cpu().numpy().astype(bool)
@@ -277,7 +309,10 @@ def simulate_fog_batch(ps, pcs, noise, gain=False, noise_variant='v1', hard=True
     Generators (None: the module-level RNG for every cloud).  The integral tables are generated on the device, one per
     distinct parameter set, as with lut='device'.  Returns B triples, each identical to
     simulate_fog(ps[b], pcs[b], noise, ..., rng=rngs[b], lut='device') called for b = 0, 1, ... in turn -- the generators
-    are left where those calls leave them, also when clouds share one.
+    are left where those calls leave them, also when clouds share one.  Like those calls, the first cloud with a NaN
+    range raises KeyError(nan) (OverflowError for v1 noise at an infinite range), and with gain the first empty cloud
+    ValueError: the generators of earlier clouds
+    stepped in full, the failing cloud's where the reference leaves it, later ones untouched.
     """
     B = len(pcs)
     ps, rngs = _batch_args(ps, B, noise, noise_variant, soft, rngs)
@@ -329,7 +364,8 @@ def simulate_fog_batch_device(ps, points, cloud_offsets, noise, gain=False, nois
     The engine call of simulate_fog_batch on device-resident clouds: points CUDA float32 (N, F), cloud b at rows
     cloud_offsets[b] .. cloud_offsets[b + 1].  Steps the generators exactly as simulate_fog_batch (one integers draw
     per cloud, then one draw per fog point; the fog counts come from a first pass that draws nothing, one synchronising
-    copy) and returns fog_batch_params' dict (points float64 (N, F), fog_mask, info; None for an empty batch).
+    copy; without draws the counts are copied back after the call, for the errors) and raises as simulate_fog_batch.
+    Returns fog_batch_params' dict (points float64 (N, F), fog_mask, info; None for an empty batch).
     """
     off = np.ascontiguousarray(cloud_offsets, dtype=np.int64)
     B = off.shape[0] - 1
@@ -359,19 +395,25 @@ def simulate_fog_batch_device(ps, points, cloud_offsets, noise, gain=False, nois
         return eng.fog_batch_params(d_pts, off, luts, alpha, beta, beta_0, index, **dict(kw, **extra))
 
     draws = soft and noise > 0
+    rows = np.diff(off)
     if not draws:
         res = run()
         if soft:
-            for g in rngs:
+            eng.check()
+            cnt = res['info'][:, 2].cpu().numpy().astype(np.int64)
+            for b, g in enumerate(rngs):
                 g.integers(low=1, high=20, size=1)          # :207, one per call
+                _raise_like_reference(g, rows[b], cnt[b], gain, variant, False)
     else:
         # the fog counts do not depend on the noise: a first pass gives every cloud's count, so each generator can be
-        # stepped exactly as the sequential calls step it (integers draw, then one draw per fog point), shared or not
-        cnt = run(noise=0)['info'][:, 2].cpu().numpy().astype(np.int64)
+        # stepped exactly as the sequential calls step it (integers draw, then one draw per fog point), shared or not.
+        # (Without generator states or external values the noise is not applied; the pass still flags where it raises.)
+        cnt = run()['info'][:, 2].cpu().numpy().astype(np.int64)
         if variant == 4:
             ext = torch.zeros((max(N, 1),), dtype=torch.float64)
             for b, g in enumerate(rngs):
                 g.integers(low=1, high=20, size=1)
+                _raise_like_reference(g, rows[b], cnt[b], gain, variant, True)
                 if cnt[b]:
                     ext[off[b]:off[b] + cnt[b]] = torch.from_numpy(g.beta(a=2, b=20, size=int(cnt[b])))
             res = run(ext_noise=ext.to(eng.device))
@@ -379,6 +421,7 @@ def simulate_fog_batch_device(ps, points, cloud_offsets, noise, gain=False, nois
             states = np.zeros((B, 4), dtype=np.uint64)
             for b, g in enumerate(rngs):
                 g.integers(low=1, high=20, size=1)
+                _raise_like_reference(g, rows[b], cnt[b], gain, variant, True)
                 states[b] = _pcg64_state(g)
                 if cnt[b]:
                     _pcg64_advance(g, int(cnt[b]))

@@ -4,6 +4,7 @@ Tables: fog_distance exact and responses within 1e-13 relative of the reference'
 and of the oracle.  Per-cloud batch: bit-identical to one simulate_fog(lut='device') call per cloud, generators
 included."""
 import os
+import re
 
 import numpy as np
 import pytest
@@ -127,10 +128,11 @@ def _same(a, b):
     return a.dtype == b.dtype and np.array_equal(a, b)
 
 
+# (gain is test_batch_gain_equals_sequential_calls: with gain the batch's empty cloud raises; the ids stay as they were)
 @pytest.mark.parametrize('cfg', [dict(noise=10, noise_variant='v1'), dict(noise=10, noise_variant='v2'),
                                  dict(noise=4, noise_variant='v3'), dict(noise=3, noise_variant='v4'),
-                                 dict(noise=10, noise_variant='v1', gain=True), dict(noise=0),
-                                 dict(noise=10, soft=False), dict(noise=10, noise_variant='v2', hard=False)])
+                                 dict(noise=0), dict(noise=10, soft=False), dict(noise=10, noise_variant='v2', hard=False)],
+                         ids=['cfg0', 'cfg1', 'cfg2', 'cfg3', 'cfg5', 'cfg6', 'cfg7'])
 @pytest.mark.parametrize('shared', [False, True])
 def test_batch_equals_sequential_calls(engine, cfg, shared):
     from lidar_snow_sim_b200.fog import simulate_fog, simulate_fog_batch
@@ -164,6 +166,56 @@ def test_batch_equals_sequential_calls(engine, cfg, shared):
         for x, y in zip(w, g):
             assert _same(x, y), (b, cfg)
     for s, t in zip(keep_seq, keep_bat):                   # the generators end where the sequential calls leave them
+        assert np.array_equal(s.random(3), t.random(3))
+
+
+@pytest.mark.parametrize('shared', [False, True])
+def test_batch_gain_equals_sequential_calls(engine, shared):
+    """gain (v1 noise): a batch with an empty cloud raises builtin max's ValueError like the sequential calls, after
+    that cloud's `integers` draw, with every generator where those calls leave it (later clouds untouched); without the
+    empty cloud the batch is bit-identical to one simulate_fog(lut='device') call per cloud"""
+    from lidar_snow_sim_b200.fog import simulate_fog, simulate_fog_batch
+    cfg = dict(noise=10, noise_variant='v1', gain=True)
+    clouds = _clouds()
+    ps = [P(alpha=a) for a in ALPHA_MIX]
+    ps[4] = P(alpha=0.005, tau_h=1.5e-8)
+    empty = [b for b in range(len(clouds)) if clouds[b].shape[0] == 0]
+    assert empty == [2]
+
+    def gens(n):
+        if shared:
+            g = np.random.default_rng(7)
+            return [g] * n, [g]
+        gs = [np.random.default_rng(70 + b) for b in range(n)]
+        return gs, gs
+
+    # with the empty cloud: the sequential calls raise at cloud 2
+    g_seq, keep_seq = gens(len(clouds))
+    with pytest.raises(ValueError, match=re.escape('max() iterable argument is empty')):
+        for b in range(len(clouds)):
+            simulate_fog(ps[b], clouds[b], engine=engine, rng=g_seq[b], lut='device', **cfg)
+    g_bat, keep_bat = gens(len(clouds))
+    with pytest.raises(ValueError, match=re.escape('max() iterable argument is empty')):
+        simulate_fog_batch(ps, clouds, engine=engine, rngs=g_bat, **cfg)
+    if not shared:                                          # clouds after the failing one: generators untouched
+        for b in range(3, len(clouds)):
+            assert np.array_equal(g_bat[b].bit_generator.state['state'],
+                                  np.random.default_rng(70 + b).bit_generator.state['state'])
+    for s, t in zip(keep_seq, keep_bat):
+        assert np.array_equal(s.random(3), t.random(3))
+
+    # without it: bit-identical results
+    keep = [b for b in range(len(clouds)) if b not in empty]
+    cs, qs = [clouds[b] for b in keep], [ps[b] for b in keep]
+    g_seq, keep_seq = gens(len(cs))
+    want = [simulate_fog(qs[b], cs[b], engine=engine, rng=g_seq[b], lut='device', **cfg) for b in range(len(cs))]
+    g_bat, keep_bat = gens(len(cs))
+    got = simulate_fog_batch(qs, cs, engine=engine, rngs=g_bat, **cfg)
+    assert len(got) == len(want)
+    for b, (w, g) in enumerate(zip(want, got)):
+        for x, y in zip(w, g):
+            assert _same(x, y), b
+    for s, t in zip(keep_seq, keep_bat):
         assert np.array_equal(s.random(3), t.random(3))
 
 
